@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- throughput of the APT decode hot path on B200 (BASELINE.json metric: input Msamples/s decoded).
+"""bench.py -- throughput of the APT decode hot path on H100 (BASELINE.json metric: input Msamples/s decoded).
 
 One "step" = one pass of decode() (resample -> envelope -> low-pass -> sync -> rows) over one batch of synthetic
 recordings per GPU.  Default workload at every N: BASELINE.json configs[3] -- a batch of 64 independent 48 kHz, 15-min,
@@ -11,6 +11,7 @@ configuration (configs[1], the one the roofline kernel is quoted on) is measured
     python bench.py --gpus 1 --steps 20 --warmup 3
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference        # CPU arm: the oracle port of the Rust reference on the host cores
+    python bench.py --dump-outputs DIR      # also write the rows / sync positions of the last timed step as DIR/*.npy
 
 JSON keys beyond the base contract: roofline (dominant kernel, CUDA-event timed on the decoder's stream), cpu_baseline
 (oracle on the host cores), e2e (pageable host buffers through the C-ABI batch call), e2e_apt_decode (one apt_decode()
@@ -58,6 +59,9 @@ def parse_args():
     ap.add_argument("--seed-base", type=int, default=0,
                     help="first recording seed of rank 0 (rank r uses seed-base + 4r ...); 12 puts the tied recording, seed 15, on one GPU")
     ap.add_argument("--no-extras", action="store_true", help="skip the single-recording and other-rate measurements")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed device-resident path returned in its last step as DIR/<name>.npy "
+                         "(float32 / float64, at most 64 MB in all; rows: a fixed, seeded sample)")
     return ap.parse_args()
 
 
@@ -69,11 +73,11 @@ def measured_peaks():
                 return float(json.load(f)["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet (HBM3), not a measurement"
 
 
 class ClockSampler:
-    """SM clock and clock-event (throttle) reasons sampled WHILE a timed region runs (B200_PROFILING.md): NVML through
+    """SM clock and clock-event (throttle) reasons sampled WHILE a timed region runs: NVML through
     nvidia_ml_py polled at 20 Hz by a thread that only records while `active` is set (timed() sets it around each
     timed region); `nvidia-smi -lms` as the fallback when NVML cannot be loaded."""
 
@@ -262,6 +266,31 @@ def run_reference(args, rank, world):
     print(json.dumps(line), flush=True)
 
 
+DUMP_BYTES = 60_000_000            # rows + sync positions + counts: under 64 MB with the .npy headers
+
+
+def dump_outputs(path, rows, produced, syncs):
+    """Writes what the B decoders of the timed path returned in its last step: values_returned.npy (B,) the number of
+    f32 values each decoder wrote, sync_positions.npy (B, P) its sync positions (NaN-padded), and of the rows
+    (2080 values each) rows.npy (B, R, 2080) at the R row indices in row_index.npy -- every row when they all fit the
+    64 MB budget, otherwise the same seeded sample of indices for every recording."""
+    import torch
+    os.makedirs(path, exist_ok=True)
+    B = len(rows)
+    counts = np.array([float(p) for p in produced])
+    sync = np.full((B, max(1, max(s.size for s in syncs))), np.nan)
+    for k, s in enumerate(syncs):
+        sync[k, : s.size] = s
+    nrows = min(int(p) // 2080 for p in produced)
+    fit = max(1, (DUMP_BYTES - sync.nbytes - counts.nbytes) // (B * (2080 * 4 + 8)))
+    idx = np.arange(nrows) if nrows <= fit else np.sort(np.random.default_rng(0).choice(nrows, size=fit, replace=False))
+    sel = torch.from_numpy(idx).to(rows[0].device)
+    sample = np.stack([r[: nrows * 2080].view(-1, 2080).index_select(0, sel).cpu().numpy() for r in rows])
+    for name, a in (("rows", sample.astype(np.float32)), ("row_index", idx.astype(np.float64)),
+                    ("values_returned", counts), ("sync_positions", sync)):
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
 def nerr(got, ref):
     scale = float(np.max(np.abs(ref))) if ref.size else 1.0
     return float(np.max(np.abs(got.astype(np.float64) - ref.astype(np.float64)))) / (scale or 1.0)
@@ -367,6 +396,9 @@ def run_b200(args, rank, local_rank, world):
     ms_step = ms_total / K
     sync_dev = [decs[k].last_sync() for k in range(n_seeds)]
     rows_dev = [out_devs[k][: produced[k]].cpu().numpy() for k in range(n_seeds)]
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs if world == 1 else os.path.join(args.dump_outputs, f"rank{rank}"), out_devs,
+                     produced, [d.last_sync() for d in decs])
 
     # ---- end-to-end arm ("e2e"): the reference-facing batch call on ordinary PAGEABLE host buffers, H2D + D2H inside ----
     outs = [np.zeros(bound, dtype=np.float32) for _ in range(B)]        # zeros: the pages exist before the timed region
@@ -448,21 +480,11 @@ def run_b200(args, rank, local_rank, world):
     dom = "resample_envelope"
     alg_bytes = 4 * n + 4 * n_work                      # SURVEY.md §8(d): read every input once, write every e once
     achieved = alg_bytes / (kernel_ms[dom] * 1e-3) / 1e9 if dom in kernel_ms else None
-    traffic, traffic_source = None, None
-    try:   # dram__bytes_read.sum + dram__bytes_write.sum of that kernel from the committed ncu --set full capture
-        tp = os.path.join("profiles", "r02_ncu_kernels_metrics.json")
-        with open(os.path.join(ROOT, tp)) as f:
-            for m in json.load(f):
-                if "k_polyphase_ut" in m["kernel"] and abs(args.seconds - 900.0) < 1e-6 and rate == 48000 and repeat == 1:
-                    traffic = (m["dram__bytes_read.sum"] + m["dram__bytes_write.sum"]) * 1e6
-                    traffic_source = tp + " (committed ncu capture of the same kernel and input, not this run)"
-    except Exception:
-        pass
     step_bytes = 4 * n + 4 * int(produced[0])
     roofline = {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak if achieved else None, "traffic": traffic, "traffic_source": traffic_source,
+                "frac": achieved / peak if achieved else None,
                 "peak_source": peak_kind, "algorithmic_bytes": alg_bytes, "kernel_ms": kernel_ms.get(dom),
-                "kernel_name": "k_polyphase_ut" if 12480 // math.gcd(rate, 12480) == 13 else "k_polyphase_ph / k_polyphase_ws",
+                "kernel_name": "k_polyphase_ws" if 12480 // math.gcd(rate, 12480) == 13 else "k_polyphase_ph / k_polyphase_ws",
                 "all_kernels_ms": kernel_ms,
                 "whole_decode": {"algorithmic_bytes": step_bytes, "ms": sum(kernel_ms.values()),
                                  "frac_of_peak": step_bytes / (sum(kernel_ms.values()) * 1e-3) / 1e9 / peak}}
@@ -536,6 +558,7 @@ def run_b200(args, rank, local_rank, world):
 
     line = None
     if rank == 0:
+        l2_mb = getattr(torch.cuda.get_device_properties(local_rank), "L2_cache_size", 0) / 1e6
         cpu = None
         if not args.no_cpu_baseline and world == 1:
             threads, jobs = cpu_setup(args, B)
@@ -556,7 +579,8 @@ def run_b200(args, rank, local_rank, world):
             "config": {"workload": workload_string(args, B, repeat),
                        "profile": "standard", "recordings_per_gpu": B, "samples_per_recording": int(n),
                        "work_samples": int(n_work), "rows": int(produced[0] // 2080), "sync_roots": int(counts["n_roots"]),
-                       "l2": f"inputs_exceed_l2 ({4 * n * B / 1e6:.1f} MB of f32 input per GPU and step > 126 MB L2)",
+                       "l2": f"{4 * n * B / 1e6:.1f} MB of f32 input per GPU and step, {l2_mb:.0f} MB L2",
+                       "device": torch.cuda.get_device_name(local_rank),
                        "sharding": "independent recordings, no collective; recording -> stream of its rank's GPU",
                        "numa_bound": numa_bound},
             "e2e": {"value": e2e_value, "unit": UNIT, "ms_per_step": e2e_total / K, "h2d_bytes_per_step": int(4 * n * B),

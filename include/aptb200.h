@@ -1,5 +1,5 @@
 /*
- * aptb200.h -- C ABI of the B200-native APT decode path.
+ * aptb200.h -- C ABI of the H100-native APT decode path.
  *
  * Drop-in boundary for the signal-to-image hot path of martinber/noaa-apt
  * v1.4.1 (src/{dsp,filters,decode,resample}.rs).  The reference has no FFI
@@ -291,7 +291,7 @@ int apt_memcpy_d2h(int device, void *dst, const void *src, size_t bytes);
 
 /* ----------------------------------------------------------- introspection */
 
-/* Geometry of the tiled sm_100a resampler for a ratio L/M and a tap set (DESIGN.md "Tiled polyphase
+/* Geometry of the tiled sm_90a resampler for a ratio L/M and a tap set (DESIGN.md "Tiled polyphase
  * kernel"); host code, no GPU.  usable == 0: the shape falls back to the generic kernel.  Optional
  * outputs: tile_taps (groups*group_stride floats; per group one sub-table per slice lane, slice_stride floats
  * apart, holding per loop iteration a 32-float record: taps of half A [4 samples][4 outputs], then half B) and

@@ -1,4 +1,4 @@
-"""noaa-apt_b200 -- B200-native APT decode path behind the reference's own surface.
+"""noaa-apt_b200 -- H100-native APT decode path behind the reference's own surface.
 
 Mirrors the module layout of martinber/noaa-apt's hot path:
 
@@ -8,7 +8,7 @@ Mirrors the module layout of martinber/noaa-apt's hot path:
     noaa_apt_b200.Context, noaa_apt_b200.Settings, noaa_apt_b200.err
 
 Every compute call goes through the C ABI of libaptb200.so (include/aptb200.h) into hand-written
-sm_100a CUDA kernels.  There is no CPU path: importing works anywhere, computing needs a GPU.
+sm_90a CUDA kernels.  There is no CPU path: importing works anywhere, computing needs a GPU.
 """
 from . import _lib, config, context, dsp, err, filters, frequency, image, wav  # noqa: F401
 from . import decode as _decode_mod

@@ -163,7 +163,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} has not been built. Run `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). There is no CPU fallback.")
+            "(nvcc, sm_90a). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (restype, argtypes) in SIGNATURES.items():
         fn = getattr(lib, name)   # AttributeError here means the ABI and the header have diverged

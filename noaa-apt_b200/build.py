@@ -1,4 +1,4 @@
-"""Builds libaptb200.so (CUDA kernels + C ABI) in-tree with nvcc for sm_100a.
+"""Builds libaptb200.so (CUDA kernels + C ABI) in-tree with nvcc for sm_90a (H100).
 
 The library is the product: every compute entry point lives in it and there is
 no CPU fallback.  nvcc cross-compiles without a GPU, so this also runs on the
@@ -15,7 +15,7 @@ LIB = os.path.join(HERE, "libaptb200.so")
 
 NVCC_FLAGS = [
     "-O3", "-std=c++17",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-Xcompiler", "-fPIC,-ffp-contract=off,-fno-fast-math,-Wall",
     "-cudart", "static",

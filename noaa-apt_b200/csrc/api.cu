@@ -59,6 +59,14 @@ int require_device() {
     return APT_OK;
 }
 
+// Launch context of the one-shot stage entry points: default stream, SM count of the current device.
+LaunchCtx stage_ctx() {
+    int dev = 0, sms = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    return LaunchCtx{nullptr, std::max(sms, 1)};
+}
+
 int free_decoder_buffers(apt_decoder *d) {
     cudaSetDevice(d->device);
     if (d->stream) cudaStreamSynchronize(d->stream);
@@ -284,7 +292,7 @@ extern "C" int apt_resample_with_filter(const float *signal, uint64_t n, uint32_
     APT_TRY(dy.alloc(rp.nout * sizeof(float)));
     APT_CUDA(cudaMemcpy(dx.p, signal, n * sizeof(float), cudaMemcpyHostToDevice));
     APT_CUDA(cudaMemcpy(dh.p, rp.taps.data(), rp.taps.size() * sizeof(float), cudaMemcpyHostToDevice));
-    const LaunchCtx c{nullptr, 148};
+    const LaunchCtx c = stage_ctx();
     if (rp.polyphase) {
         const uint64_t off2 = 2 * ((static_cast<uint64_t>(rp.taps.size()) - 1) / 2);
         TilePlan tp{};
@@ -292,10 +300,8 @@ extern "C" int apt_resample_with_filter(const float *signal, uint64_t n, uint32_
         std::vector<u32> xs;
         UtPlan up{};
         std::vector<float> us;
-        if (!getenv("APTB200_GENERIC_RESAMPLER") && make_ut_plan(rp.r.l, rp.r.m, rp.taps, up, us)) {
-            APT_TRY(launch_polyphase_ut(c, dx.as<float>(), n, dh.as<float>(), up, us, rp.nout, 0, 0, false, 0.f, 1.f, dy.as<float>()));
-            APT_CUDA(cudaDeviceSynchronize());
-        } else if (!getenv("APTB200_GENERIC_RESAMPLER") && make_tile_plan(rp.r.l, rp.r.m, rp.taps, tp, tt, xs)) {
+        // kernel preference as in make_plan: tiled, then uniform-tap, then phase-major
+        if (!getenv("APTB200_GENERIC_RESAMPLER") && make_tile_plan(rp.r.l, rp.r.m, rp.taps, tp, tt, xs)) {
             DevBuf dt, dg;
             APT_TRY(dt.alloc(tt.size() * sizeof(float)));
             APT_TRY(dg.alloc(xs.size() * sizeof(u32)));
@@ -303,6 +309,9 @@ extern "C" int apt_resample_with_filter(const float *signal, uint64_t n, uint32_
             APT_CUDA(cudaMemcpy(dg.p, xs.data(), xs.size() * sizeof(u32), cudaMemcpyHostToDevice));
             APT_TRY(launch_polyphase_tiled(c, dx.as<float>(), n, dt.as<float>(), dg.as<u32>(), tp, rp.nout, 0, 0, false, 0.f,
                                            1.f, dy.as<float>()));
+            APT_CUDA(cudaDeviceSynchronize());
+        } else if (!getenv("APTB200_GENERIC_RESAMPLER") && make_ut_plan(rp.r.l, rp.r.m, rp.taps, up, us)) {
+            APT_TRY(launch_polyphase_ut(c, dx.as<float>(), n, dh.as<float>(), up, us, rp.nout, 0, 0, false, 0.f, 1.f, dy.as<float>()));
             APT_CUDA(cudaDeviceSynchronize());
         } else {
             PhPlan pp{};
@@ -353,7 +362,7 @@ extern "C" int apt_demodulate(const float *signal, uint64_t n, float carrier_pi,
     APT_TRY(dx.alloc(n * sizeof(float)));
     APT_TRY(dy.alloc(n * sizeof(float)));
     APT_CUDA(cudaMemcpy(dx.p, signal, n * sizeof(float), cudaMemcpyHostToDevice));
-    APT_TRY(launch_envelope(LaunchCtx{nullptr, 148}, dx.as<float>(), n, cosphi2, sinphi, dy.as<float>()));
+    APT_TRY(launch_envelope(stage_ctx(), dx.as<float>(), n, cosphi2, sinphi, dy.as<float>()));
     APT_CUDA(cudaMemcpy(out, dy.p, n * sizeof(float), cudaMemcpyDeviceToHost));
     return APT_OK;
 }
@@ -369,7 +378,7 @@ extern "C" int apt_filter_taps(const float *signal, uint64_t n, const float *coe
     APT_TRY(dy.alloc(n * sizeof(float)));
     APT_CUDA(cudaMemcpy(dx.p, signal, n * sizeof(float), cudaMemcpyHostToDevice));
     if (ncoeff) APT_CUDA(cudaMemcpy(dc.p, coeff, ncoeff * sizeof(float), cudaMemcpyHostToDevice));
-    APT_TRY(launch_fir_decimate(LaunchCtx{nullptr, 148}, dx.p, APT_F32, dc.as<float>(), static_cast<u32>(ncoeff), 1, n,
+    APT_TRY(launch_fir_decimate(stage_ctx(), dx.p, APT_F32, dc.as<float>(), static_cast<u32>(ncoeff), 1, n,
                                 dy.as<float>()));
     APT_CUDA(cudaMemcpy(out, dy.p, n * sizeof(float), cudaMemcpyDeviceToHost));
     return APT_OK;
@@ -1082,7 +1091,7 @@ int image_stage_host(const float *signal, uint64_t n, int contrast, float percen
         APT_TRY(dbounds.alloc(2 * sizeof(float)));
         APT_CUDA(cudaMemcpy(dbounds.p, bounds, 2 * sizeof(float), cudaMemcpyHostToDevice));
     }
-    const LaunchCtx c{nullptr, 148};
+    const LaunchCtx c = stage_ctx();
     // a partial last row cannot occur in an image; min/max, percent and the map treat the signal as one row of n pixels then
     const u32 nrows = whole ? static_cast<u32>(rows) : 1u;
     const u32 px = whole ? kPxPerRow : static_cast<u32>(n);
@@ -1147,7 +1156,7 @@ extern "C" int apt_quantize_i16(const float *signal, uint64_t n, int16_t *out) {
     APT_TRY(dctl.alloc(sizeof(PostCtl)));
     APT_TRY(dout.alloc(n * sizeof(int16_t)));
     APT_CUDA(cudaMemcpy(dx.p, signal, n * sizeof(float), cudaMemcpyHostToDevice));
-    APT_TRY(launch_quantize_i16(LaunchCtx{nullptr, 148}, dx.as<float>(), n, dctl.as<PostCtl>(), dout.as<short>()));
+    APT_TRY(launch_quantize_i16(stage_ctx(), dx.as<float>(), n, dctl.as<PostCtl>(), dout.as<short>()));
     APT_CUDA(cudaMemcpy(out, dout.p, n * sizeof(int16_t), cudaMemcpyDeviceToHost));
     return APT_OK;
 }

@@ -55,7 +55,10 @@ int make_plan(uint32_t input_rate, const apt_settings &s, Plan &p) {
     p.off2 = 2 * ((static_cast<uint64_t>(p.h.size()) - 1) / 2);
     p.tiled = p.first_polyphase && !getenv("APTB200_GENERIC_RESAMPLER") &&
               make_tile_plan(p.first.l, p.first.m, p.h, p.tile, p.tile_taps, p.tile_xs);
-    p.ut = p.first_polyphase && !getenv("APTB200_GENERIC_RESAMPLER") &&
+    // the uniform-tap kernel only where the tiled one does not fit: without a packed fp32 FMA (sm_90) its one uniform
+    // tap load per FMA pair makes it the slower of the two (48 kHz x 900 s: 214 us against
+    // 125 us on an H100 SXM at 700 W)
+    p.ut = p.first_polyphase && !p.tiled && !getenv("APTB200_GENERIC_RESAMPLER") &&
            make_ut_plan(p.first.l, p.first.m, p.h, p.utp, p.ut_stream);
     p.ph = p.first_polyphase && !p.ut && !p.tiled && !getenv("APTB200_GENERIC_RESAMPLER") &&
            make_ph_plan(p.first.l, p.first.m, p.h, p.php, p.ph_table, p.ph_xs);
@@ -371,13 +374,12 @@ static int enqueue_front(apt_decoder *d, const void *in, int format, uint64_t n,
 std::atomic<int> g_jobs_in_flight[64];      // per CUDA device: decodes submitted and not yet waited for
 
 // The envelope e (4 N_w bytes, 45 MB for 15 min) is written by the resampler and read by the record and the gather
-// kernels; between those, the resampler's 173 MB input stream pushes most of it out of the 126 MB L2, so e goes to DRAM
-// and comes back (ncu in application order: 273 MB of DRAM traffic per decode against 188 MB algorithmic).  When this is the
-// only decode on the device, e can get a PERSISTING access-policy window on the decoder's stream (everything else the
-// stream touches is treated as streaming): 201 MB per decode, same speed (the kernels that read e are not memory bound).
+// kernels; between those, the resampler's 173 MB input stream pushes it out of the 50 MB L2, so e goes to DRAM and comes
+// back.  When this is the only decode on the device, e can get a PERSISTING access-policy window on the decoder's stream
+// (everything else the stream touches is treated as streaming) for as much of it as the set-aside holds.
 // With several decodes in flight the set-aside would only shrink the cache, so the window is dropped then.
-// OPT-IN (APTB200_L2_WINDOW=1): measured on one GPU only; the 4-GPU run that would have validated it next to NCCL and in
-// a multi-device process did not complete, and a device-wide L2 carve-out is not something to switch on unverified.
+// OPT-IN (APTB200_L2_WINDOW=1): not validated next to NCCL or in a multi-device process, and a device-wide L2 carve-out
+// is not something to switch on unverified.
 static void set_envelope_l2_window(apt_decoder *d, uint64_t nwork, bool alone) {
     static const bool disabled = getenv("APTB200_L2_WINDOW") == nullptr;
     static std::atomic<int> setaside[64];              // per device: bytes set aside (0 not tried yet, -1 unsupported)

@@ -38,7 +38,7 @@ struct Plan {
     uint32_t dec = 0;              // work_rate / 4160 when work_multiple
     Ratio last{};                  // work_rate -> 4160 for the final NoFilter resample
     std::vector<int8_t> guard;     // sync template (empty unless work_multiple)
-    bool tiled = false;            // the tiled sm_100a resampler fits this (L, M, taps)
+    bool tiled = false;            // the tiled sm_90a resampler fits this (L, M, taps)
     TilePlan tile{};
     std::vector<float> tile_taps;
     std::vector<u32> tile_xs;
@@ -61,7 +61,7 @@ uint64_t plan_out_bound(const Plan &p, uint64_t n);
 
 struct apt_decoder {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 0;              // of `device`, set by apt_decoder_create
     cudaStream_t stream = nullptr;
     aptb200::Plan plan;
 

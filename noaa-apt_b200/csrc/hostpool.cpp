@@ -142,7 +142,7 @@ HostStager::HostStager(int device, size_t chunk_bytes, int ring, int threads)
     ok_ = true;
     for (int i = 0; i < ring; ++i) {
         // write-combined pinned staging: the copy threads only ever write it (streaming stores) and only the DMA engine
-        // reads it -- 4.3 ms instead of 5.2 ms per 172.8 MB recording through apt_decode (APTB200_COPY_NO_WC=1 reverts)
+        // reads it (APTB200_COPY_NO_WC=1 reverts)
         static const bool wc = getenv("APTB200_COPY_NO_WC") == nullptr;
         if (cudaHostAlloc(reinterpret_cast<void **>(&ring_[i]), chunk_, wc ? cudaHostAllocWriteCombined : cudaHostAllocDefault) != cudaSuccess ||
             cudaEventCreateWithFlags(&ev_[i], cudaEventDisableTiming) != cudaSuccess) {

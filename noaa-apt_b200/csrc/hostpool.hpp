@@ -1,8 +1,8 @@
 // Host-side plumbing of the reference-facing entry points: a small pool of copy threads that moves a caller's
 // PAGEABLE buffer (the reference hands over an ordinary Vec<f32>, decode.rs:43-49) through a ring of pinned staging
-// buffers so that the H2D DMA of chunk c overlaps the memcpy of chunk c+1 -- cudaMemcpy from pageable memory reaches
-// ~11 GB/s on the B200 boxes, this pipeline ~49 GB/s (profiles/r02_hostcopy_microbench.txt), the PCIe limit being ~55.
-// Also: CPU affinity of our own threads to the NUMA node the GPU hangs off (GPU0-3 <-> node 0, GPU4-7 <-> node 1 there).
+// buffers so that the H2D DMA of chunk c overlaps the memcpy of chunk c+1 -- cudaMemcpy from pageable memory is far
+// below the PCIe limit (tools/hostcopy_bench.cu measures both).
+// Also: CPU affinity of our own threads to the NUMA node the GPU hangs off.
 #pragma once
 
 #include <atomic>

@@ -1,7 +1,6 @@
 // Tiled polyphase resampler fused with the envelope demodulator (fast_resampling dsp.rs:186-289 + demodulate
-// dsp.rs:350-383), written for sm_100a.  It served L = 13 until kernels_ut.cuh replaced it there (92 -> 62 us) and
-// still serves other small interpolation factors (L <= 13 groups, e.g. L = 26); the mbarrier / TMA / packed-fp32
-// helpers below are shared by both.
+// dsp.rs:350-383).  It served L = 13 until kernels_ut.cuh replaced it there and still serves other small
+// interpolation factors (L <= 13 groups, e.g. L = 26); the mbarrier / TMA / fp32-pair helpers below are shared by both.
 //
 // Formulation.  y[k] = sum_x h[x*L - k*M] * X[x].  Outputs k and k + P_out (P_out = lcm(8, L)) use the
 // same taps on inputs shifted by P_in = P_out*M/L, so per "group" g (outputs 8g..8g+7 of a super-period)
@@ -14,11 +13,11 @@
 //   producer warp  : 1-D TMA bulk copies (cp.async.bulk -> UBLKCP) of the next tile's 32 input rows + one
 //                    halo row into the free row stage (2 stages), completion on an mbarrier;
 //   G compute warps: one per group.  A warp's 32 lanes are KS=4 interleaved slices of the sample axis x 8 row
-//                    lanes; a thread owns 8 outputs x 4 rows as 16 packed fp32x2 accumulators.  Per loop
+//                    lanes; a thread owns 8 outputs x 4 rows as 16 fp32 accumulator pairs.  Per loop
 //                    iteration: 4 LDS.128 of samples (the 8 row lanes of a quarter-warp hit 8 distinct 16-byte
 //                    bank groups because the row pitch/4 is odd), 8 warp-broadcast LDS.128 of taps (4 distinct
-//                    addresses skewed across bank groups) and 64 FFMA2 (fma.rn.f32x2: tap pair x broadcast
-//                    sample).  The four slices' partial sums go to shared-memory planes;
+//                    addresses skewed across bank groups) and 64 pair FMAs (tap pair x broadcast sample).
+//                    The four slices' partial sums go to shared-memory planes;
 //   E epilogue warps: sum the planes, turn (r[k-1], r[k]) into the envelope (dsp.rs:373) and store float4 --
 //                    while the compute warps are already on the next tile.  The resampled signal itself never
 //                    reaches HBM.  r[K0-1] comes from the halo row (window of the last group of the previous
@@ -73,7 +72,8 @@ constexpr int kTileR = 8, kTileH = 4, kTileQ = 4, kTileKS = 4;
 constexpr int kTileRowLanes = 32 / kTileKS;           // 8
 constexpr int kTileQT = kTileRowLanes * kTileQ;       // 32 rows per tile
 
-// ---- packed fp32x2 helpers: one FFMA2 issue slot does two FMAs (each half rounded on its own) ----
+// ---- fp32 pair helpers: a register pair holding two independent accumulators.  sm_90 has no packed fp32 FMA,
+// so fma2 is two FFMAs, each half rounded on its own (the pack / unpack moves are register-pair aliases in SASS) ----
 typedef unsigned long long f32x2;
 __device__ __forceinline__ f32x2 pack2(float lo, float hi) {
     f32x2 r;
@@ -84,9 +84,11 @@ __device__ __forceinline__ void unpack2(f32x2 v, float &lo, float &hi) {
     asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-    f32x2 d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
+    float a0, a1, b0, b1, c0, c1;
+    unpack2(a, a0, a1);
+    unpack2(b, b0, b1);
+    unpack2(c, c0, c1);
+    return pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ float4 lds128(u32 addr) {
     float4 v;

@@ -1,6 +1,6 @@
 // Generic (any L/M/tap-count) kernels of the decode path.  One thread per output,
 // summation in the reference's order with one FMA per tap.  They are the
-// correctness baseline for every configuration; the tiled sm_100a fast paths in
+// correctness baseline for every configuration; the tiled sm_90a fast paths in
 // kernels_fast.cuh take over for the shapes the standard profiles produce.
 #pragma once
 

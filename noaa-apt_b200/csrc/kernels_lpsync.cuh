@@ -9,15 +9,15 @@
 // per output instead of 114.  The summation order differs from the reference's sequential loop, i.e. the
 // values agree to fp32 rounding (~1e-7 relative), not bit for bit; the generic kernel keeps the exact order.
 //
-// One CTA handles 1856 consecutive positions: e tile -> f tile -> box sums -> correlation, all with packed fp32x2
-// arithmetic (one issue slot = two FMAs / adds):
+// One CTA handles 1856 consecutive positions: e tile -> f tile -> box sums -> correlation, all on fp32 register pairs
+// (fma2: two FMAs / adds):
 //   low-pass   : a thread owns 8 outputs of ONE parity (even warps the even positions, odd warps the odd ones), so
 //                that for every output the window pairs (e[2t], e[2t+1]) -- the register pairs an LDS.128 delivers --
-//                meet the tap pairs (c[j], c[j-1]) with j of a fixed parity: FFMA2(window pair, tap pair) with the
-//                tap pair a warp-uniform kernel-parameter operand; f = lo + hi.  19 FFMA2 + 1 FADD instead of 37 FFMA.
+//                meet the tap pairs (c[j], c[j-1]) with j of a fixed parity: fma2(window pair, tap pair) with the
+//                tap pair a warp-uniform kernel-parameter operand; f = lo + hi.
 //   box sums   : pair sums P[k] = f[2k] + f[2k+1] shared by neighbouring outputs: PW + 2 adds per two outputs.
 //   correlation: output pairs (v, v+1), v even, accumulate box pairs (B[m], B[m+1]), m even (2*PW is even), with
-//                FFMA2 by (+-1, +-1): 19 per output pair.
+//                fma2 by (+-1, +-1): 19 per output pair.
 // f and corr go to HBM once each (coalesced float4 from the shared tiles); e is read once (+7 % halo).  Shared-memory
 // tiles are skewed by 4 floats every 32 so that 8- and 16-float-strided LDS.128 stay conflict-free.
 #pragma once

@@ -8,9 +8,9 @@
 // WARP-UNIFORM.  Four consecutive phases (a group) read nearly the same samples, so a group shares ONE 16-byte aligned
 // window of WIN samples per lane (every period's input span sits in its own shared-memory row, pitch = 4 mod 32 floats:
 // the 32 lanes' LDS.128 are conflict-free) and the table stores the group's taps laid out AGAINST that window (zero where
-// a phase does not reach): element i of the window meets the four phases' taps as one broadcast LDS.128 and two packed
-// FFMA2, with compile-time register indices -- no shift variants, a quarter of the shared-memory window traffic of a
-// per-phase formulation (which measured smem-bandwidth-bound at 131 us for 11025 Hz x 900 s).  Ascending window index is
+// a phase does not reach): element i of the window meets the four phases' taps as one broadcast LDS.128 and two pair
+// FMAs, with compile-time register indices -- no shift variants, a quarter of the shared-memory window traffic of a
+// per-phase formulation (which is shared-memory-bandwidth bound).  Ascending window index is
 // ascending tap index for every phase: the reference's summation order.  PCM16 input is converted while the rows are
 // staged (wav.rs:37 fused into the load).
 //
@@ -48,7 +48,7 @@ __device__ __forceinline__ void ph_cp_async4(float *dst, const float *src, bool 
 // rows of a tile: f32 samples by 4-byte cp.async (a row starts at an arbitrary sample; all copies of a tile are in flight
 // together), PCM16 samples through registers, eight loads at a time, converted on the way (wav.rs:37)
 __device__ __forceinline__ void ph_stage_row(const float *signal, u64 len, long long gx0, u32 row_len, float *row, u32 lane) {
-    // (aligned 16-byte loads through registers + scalar stores at the shifted positions measured slower: 69 vs 62 us)
+    // (aligned 16-byte loads through registers + scalar stores at the shifted positions measured slower)
     if (gx0 >= 0 && static_cast<u64>(gx0) + row_len <= len) {
         const float *src = signal + gx0;
         for (u32 i = lane; i < row_len; i += 32) ph_cp_async4(row + i, src + i, true);
@@ -76,7 +76,7 @@ __device__ __forceinline__ void ph_stage_row(const int16_t *signal, u64 len, lon
 
 // Four consecutive phases (one group) of this lane's period from ONE aligned window of WIN samples: window element i
 // meets the four taps tg[i] = (T'[4g][i], .., T'[4g+3][i]) -- the group's taps laid out against the common window, zero
-// where a phase does not reach -- as two packed FFMA2 (sample broadcast x tap pair).  Ascending i = ascending tap index
+// where a phase does not reach -- as two pair FMAs (sample broadcast x tap pair).  Ascending i = ascending tap index
 // for every phase: the reference's summation order.
 template <int WIN>
 __device__ __forceinline__ void ph_group(const float *row, u32 xa, const float4 *tg, float (&y)[4]) {
@@ -141,7 +141,7 @@ k_polyphase_ph(const InT *__restrict__ signal, u64 len, const float *__restrict_
 
     const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     // the 80-KB table by 16-byte cp.async: every copy in flight at once (a load-then-store loop costs one L2 round trip per
-    // iteration, 20 of them: 10 of the kernel's 57 us in the first capture); completion is awaited with the first tile's rows
+    // iteration, 20 of them); completion is awaited with the first tile's rows
     for (u32 i = tid; i < ngroups * WIN; i += blockDim.x)
         asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(static_cast<u32>(__cvta_generic_to_shared(s_table + 4 * i))),
                      "l"(table_g + 4 * i) : "memory");

@@ -491,8 +491,7 @@ k_pick_links(u64 ncorr, u64 nwork, u32 row, u32 dist, const RootIndex ri, u32 *_
 // k_pick_cluster: the same orbit walk inside ONE thread-block cluster.  The jump tables live in the distributed
 // shared memory of the cluster's CTAs (node c in CTA c / per), every level ends in a hardware cluster barrier
 // instead of a global-memory grid barrier, and nothing but the root lists, the orbit and the positions touches
-// global memory: ~11 levels of (one DSMEM gather per node + barrier.cluster) instead of 11 grid barriers at
-// ~3.5 us each.  Recordings whose candidates do not fit the cluster's shared memory run the identical code on
+// global memory: ~11 levels of (one DSMEM gather per node + barrier.cluster) instead of 11 grid barriers.  Recordings whose candidates do not fit the cluster's shared memory run the identical code on
 // the global ping-pong tables (slower, still parallel); beyond the scratch capacity: the one-thread walk.
 // ---------------------------------------------------------------------------------------------
 constexpr u32 kPickClusterPer = 24576;       // nodes per CTA: 2 tables x 96 KB of dynamic shared memory
@@ -517,7 +516,7 @@ __device__ __forceinline__ void pick_node(u32 c, u32 nr, u32 ncand, u64 ncorr, u
 }
 
 // J0 for every node, one thread each over the WHOLE GPU (the chains of dependent loads behind F -- root list binary
-// searches -- are latency-bound: 8 CTAs of a cluster would need several rounds of them, 148 SMs need one).
+// searches -- are latency-bound: 8 CTAs of a cluster would need several rounds of them, the whole GPU needs one).
 __global__ void __launch_bounds__(256)
 k_pick_j0(u64 ncorr, u32 row, u32 dist, const RootIndex ri, u32 *__restrict__ positions, u32 max_positions,
           SyncResult *__restrict__ result, PickScratch sc) {
@@ -656,7 +655,7 @@ k_pick_cluster(u64 ncorr, u64 nwork, u32 row, u32 dist, const RootIndex ri, u32 
 //   k_pick_final (ONE CTA) : compact the flagged nodes (K of them), E restricted to them in SHARED memory, pointer doubling
 //                            over K nodes with __syncthreads only (orbit in steps of 8), expansion of every 8-step by a walk
 //                            through J0, events -> positions, counts.
-// No grid barrier, no cluster: ~20 us instead of 39 us (11 grid barriers) for a 15-minute recording, and the single CTA
+// No grid barrier, no cluster: about half the time of the 11 grid barriers for a 15-minute recording, and the single CTA
 // leaves the GPU to the other streams of a batch.  Falls back to the one-thread walk when K exceeds the shared-memory table.
 // ---------------------------------------------------------------------------------------------
 constexpr u32 kPickR = 8;

@@ -86,7 +86,7 @@ __device__ __forceinline__ u32 warp_excl_sum(u32 v, u32 lane, u32 &total) {
 //   stage   : e[i0 - EOFF, i0 + 32*TB) -> rows (logical index m <-> e[i0 - EOFF + m]); samples with index < 1 or >= n
 //             are zero (dsp.rs:399: signal[0] is never read)
 //   phase 1 : lane = one row of 32 consecutive outputs f[i0 + 32r ..]: the 32+EOFF window in registers as packed pairs,
-//             four passes (two parities x two halves) of 8 outputs x NPAIR FFMA2 with warp-uniform tap pairs (the
+//             four passes (two parities x two halves) of 8 outputs x NPAIR pair FMAs with warp-uniform tap pairs (the
 //             index algebra of kernels_lpsync.cuh); box sums B[n] = f[n] + ... + f[n+BOX-1] of the row straight from the
 //             registers (the BOX-1 values of the next row come from the neighbouring lane by shuffle; rounds run from the
 //             last row block to the first so that lane 31 gets them from the block done before) -> B rows
@@ -105,8 +105,8 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 
 // NW = 1 (what is instantiated): every warp is its own CTA.  NW > 1: the NW warps of a CTA take NW consecutive tiles and
 // meet at a CTA barrier before every phase, so that they share the fetched instruction lines (the kernel is ~3900
-// straight-line instructions per tile, 46 KB of code).  Measured at NW = 4 / 8 / 10 / 16 / 20: 49.5 / 49.5 / 55.6 / 65.9 /
-// 59.7 us against 47.6 us for NW = 1 -- instruction supply is not what bounds the kernel; kept as a template parameter only.
+// straight-line instructions per tile, 46 KB of code).  Every NW > 1 measured slower than NW = 1 -- instruction supply is
+// not what bounds the kernel; kept as a template parameter only.
 template <int NT, int PW, int TB, int NBUF = 2, int NW = 1>
 __global__ void __launch_bounds__(32 * NW, rec_ctas_per_sm(TB, NT, NBUF) / NW > 0 ? rec_ctas_per_sm(TB, NT, NBUF) / NW : 1)
 k_lowpass_records(const float *__restrict__ e, u64 n, u64 ncorr, const __grid_constant__ LpTaps taps, SyncCtl *__restrict__ ctl,
@@ -159,7 +159,7 @@ k_lowpass_records(const float *__restrict__ e, u64 n, u64 ncorr, const __grid_co
     };
     // Tiles are dealt out statically (every tile costs the same): CTA b takes the tile groups b, b + gridDim.x, ...; a group
     // is NW consecutive tiles, one per warp.  No tickets: two same-address atomics per tile (ticket + pool cursor, 11.7 k of
-    // them on one cache line) were what kept the first version at ~52 us whatever the occupancy.
+    // them on one cache line) bounded the first version whatever the occupancy.
     auto phase_barrier = [&]() {
         if (LOCK) __syncthreads();
     };
@@ -193,9 +193,7 @@ k_lowpass_records(const float *__restrict__ e, u64 n, u64 ncorr, const __grid_co
             phase_barrier();
             const u32 r = 32 * rb + lane;
             const float *row = s + r * PITCH;
-            // One window sample x the taps of two neighbouring outputs: FFMA2 R.F32 (broadcast) x UR.pair + R.pair, the form that
-            // runs at 2.9 clk per sub-partition; the packed-window form (R.pair x UR.pair) used here before takes 5.0 clk
-            // and made this phase the kernel's bound (profiles/r02_fma_rate_bench.txt).
+            // One window sample x the taps of two neighbouring outputs: broadcast sample x uniform tap pair + accumulator pair.
             float w[WN];
 #pragma unroll
             for (int k = 0; k < WN / 4; ++k) {
@@ -261,9 +259,7 @@ k_lowpass_records(const float *__restrict__ e, u64 n, u64 ncorr, const __grid_co
             const u32 q = 32 * rd + lane;
             const u32 qa = q < NI ? q : NI - 1;             // idle lanes of the last round re-read the last item
             const float *brow = s + (qa + kRecShift) * PITCH;
-            // Packed adds (FFMA2 with an immediate +-1: 5.0 clk per warp instruction for 64 adds; scalar FADD would be 1.16 clk
-            // for 32) on purpose: the kernel is bound by instruction issue, not by the FMA pipe, and the scalar variant -- twice
-            // the instructions -- measured 6 us slower (profiles/r02_fma_rate_bench.txt, DESIGN.md 3.2).
+            // Pair adds written as FMAs by +-1 on the accumulator pairs (fma2): each is one correctly rounded add.
             const f32x2 plus1 = pack2(1.f, 1.f), minus1 = pack2(-1.f, -1.f);
             f32x2 acc[16];
 #pragma unroll
@@ -577,9 +573,8 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 
 // Four pixels of one thread: the window starts OFF samples into the 16-byte aligned floats at `src` (OFF = the row position's
 // alignment, compile time: the register indices are fixed per variant).  One window sample x the taps it has in two
-// neighbouring pixels (DEC samples apart): FFMA2 R.F32 (broadcast) x UR.pair + R.pair, NT + DEC of them per pixel pair --
-// half the instructions of the scalar form and 2.9 clk each (the packed-window form R.pair x UR.pair takes 5.0;
-// profiles/r02_fma_rate_bench.txt).
+// neighbouring pixels (DEC samples apart): broadcast sample x uniform tap pair + accumulator pair, NT + DEC of them per
+// pixel pair.
 template <int NT, int DEC, int OFF>
 __device__ __forceinline__ void gather_quad(const float *src, const LpTaps &lp, float (&acc)[4]) {
     constexpr int EOFF = (NT - 1 + 3) / 4 * 4;

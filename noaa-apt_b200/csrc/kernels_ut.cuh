@@ -8,9 +8,8 @@
 // A thread owns Q rows x the output PAIRS (2p, 2p+1) of its role (one packed fp32x2 accumulator per pair and row);
 // the 32 lanes of a warp are 32 consecutive rows.  The tap pair (T[u][2p], T[u][2p+1]) is therefore warp-uniform:
 // it is read with LDCU from the kernel-parameter constant bank into uniform registers and used directly as the
-// packed operand of FFMA2 (`FFMA2 R, R.F32, UR.F32x2, R`); the only shared-memory traffic is the thread's own
-// samples (one chunk of CH = 8 samples per row per loop iteration).  In isolation the form reaches 104-107 FMA/clk/SM,
-// the FFMA2 pipe limit, against 70-84 for shared-memory tap operands (profiles/r01_microbench_uniform_taps.txt).
+// tap operands of the pair's two FFMAs; the only shared-memory traffic is the thread's own samples (one chunk of
+// CH = 8 samples per row per loop iteration), so the taps cost no shared-memory bandwidth at all.
 //
 // Zero padding.  Pair p only sees samples fx(2p) .. lx(2p+1); the loop over 8-sample chunks is cut into
 // segments with a fixed set of active pairs: ramp-up (pairs 0..a-1 for a = 1..NP-1), steady (all), ramp-down

@@ -256,7 +256,7 @@ int launch_lowpass_corr(const LaunchCtx &c, const float *e, u64 n, const float *
     const u64 ntiles = (n + kLpTile - 1) / kLpTile;
     // persistent: exactly the resident CTAs, each walks its tiles with the next tile's loads in flight
     auto launch = [&](auto kern) {
-        static const int per_sm = [&] {          // per instantiation (generic lambda); the same on every B200
+        static const int per_sm = [&] {          // per instantiation (generic lambda); one GPU model per process
             int v = 0;
             if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, kern, 256, 0) != cudaSuccess || v < 1) v = 2;
             return v;
@@ -306,8 +306,8 @@ int launch_pick(const LaunchCtx &c, u64 ncorr, u64 nwork, u32 row, u32 dist, con
     int &nk = kernels_launched ? *kernels_launched : dummy;
     nk = 1;
     // Which parallel orbit walk: APTB200_PICK = compress | cluster | grid forces one; by default the whole-GPU cooperative
-    // walk (39 us, but it needs every SM) when the device is otherwise idle, the 8-CTA cluster walk (60 us on 8 SMs) when
-    // other recordings are in flight on other streams (batch: 338 k vs 280 k Msamples/s at 64 streams).
+    // walk (faster, but it needs every SM) when the device is otherwise idle, the 8-CTA cluster walk (8 SMs) when
+    // other recordings are in flight on other streams (the batch workload runs faster with it).
     static const int forced = [] {
         const char *e = getenv("APTB200_PICK");
         if (getenv("APTB200_GRID_PICK")) return 2;

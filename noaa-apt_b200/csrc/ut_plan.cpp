@@ -70,8 +70,8 @@ bool make_ut_plan(u32 l, u32 m, const std::vector<float> &taps, UtPlan &up, std:
     bool ok = false;
     u32 want_q = 0;
     if (const char *e = getenv("APTB200_UT_Q")) want_q = static_cast<u32>(atoi(e));
-    // rows per thread: 2 measured best (48 kHz: 71 us against 76 for q = 4, which leaves room for only 12 warps;
-    // 96 kHz: 142 us against 181 for q = 1, whose one uniform load per FFMA2 saturates the uniform-load port);
+    // rows per thread: 2 measured best (q = 4 leaves room for only 12 warps; q = 1 issues one uniform load per pair
+    // of FMAs);
     // q = 1 only when two rows per thread do not fit shared memory (192 kHz); q = 4 on request (APTB200_UT_Q)
     for (u32 q : {2u, 1u, 4u}) {
         if (want_q ? q != want_q : q == 4) continue;

@@ -1,5 +1,5 @@
 //! Replacement body for `src/decode.rs::decode` (decode.rs:43-162) of martinber/noaa-apt: same signature,
-//! the work is done by libaptb200 on a B200.  SOURCE ONLY (never compiled here: no Rust toolchain in the
+//! the work is done by libaptb200 on an H100.  SOURCE ONLY (never compiled here: no Rust toolchain in the
 //! image).  `find_sync`, `generate_sync_frame` and the constants of decode.rs stay as they are.
 
 use std::ffi::CStr;

@@ -1,7 +1,7 @@
 """Cuts two excerpts (60 s in total) out of the reference's own test recording
-`/root/reference/test/test_11025hz.wav` (11025 Hz, 16-bit mono, 822 s; sha256 50160851becd5997...) and stores the
+`test/test_11025hz.wav` (11025 Hz, 16-bit mono, 822 s; sha256 50160851becd5997...) and stores the
 raw PCM16 samples in tests/golden/test_11025hz_excerpts.npz, so that the one real-world input the reference
-ships (test/test.sh:45-46) reaches the CUDA kernels on the GPU box, where /root/reference does not exist.
+ships (test/test.sh:45-46) reaches the CUDA kernels and the tests without the reference checkout.
 
     [0 s, 40 s)     the recording starts in noise: sync spacings from 1122 to 13454 work samples, the seed peak is
                     refined, several frames are skipped (decode.rs:241-253)
@@ -11,7 +11,7 @@ ships (test/test.sh:45-46) reaches the CUDA kernels on the GPU box, where /root/
 The file holds reference-owned DATA (a fixture), no reference code.  The sync positions the CPU oracle finds are
 stored next to the samples as a drift guard; the GPU tests recompute them with the oracle on the box.
 
-    python tests/golden/make_wav_excerpt.py
+    python tests/golden/make_wav_excerpt.py <reference checkout>/test/test_11025hz.wav
 """
 import hashlib
 import os
@@ -22,15 +22,14 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
-WAV = "/root/reference/test/test_11025hz.wav"
 EXCERPTS = {"start": (0, 40), "dup": (230, 250)}
 
 
-def main():
+def main(wav_path):
     import oracle
-    with open(WAV, "rb") as f:
+    with open(wav_path, "rb") as f:
         digest = hashlib.sha256(f.read()).hexdigest()
-    with wave.open(WAV) as w:
+    with wave.open(wav_path) as w:
         assert (w.getnchannels(), w.getsampwidth(), w.getframerate()) == (1, 2, 11025)
         pcm = np.frombuffer(w.readframes(w.getnframes()), dtype="<i2")
     out = {"rate": np.int64(11025), "sha256": np.array(digest)}
@@ -45,4 +44,4 @@ def main():
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1])
