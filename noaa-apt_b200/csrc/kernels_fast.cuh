@@ -13,11 +13,14 @@
 //   producer warp  : 1-D TMA bulk copies (cp.async.bulk -> UBLKCP) of the next tiles' 32 input rows + one
 //                    halo row into the free row stages (3 where shared memory allows, else 2: up to stages-1
 //                    tiles in flight while one is computed), completion on an mbarrier;
-//   G compute warps: one per group.  A warp's 32 lanes are KS=4 interleaved slices of the sample axis x 8 row
+//   compute warps  : one per group, except that with G = 13 there are 12 and warps 0..3 also compute 8 rows each
+//                    of group 12 (see the warp roles below).  A warp's 32 lanes are KS=4 interleaved slices of the sample axis x 8 row
 //                    lanes; a thread owns 8 outputs x 4 rows as 16 fp32 accumulator pairs.  Per loop
 //                    iteration: 4 LDS.128 of samples (the 8 row lanes of a quarter-warp hit 8 distinct 16-byte
 //                    bank groups because the row pitch/4 is odd), 8 warp-broadcast LDS.128 of taps (4 distinct
-//                    addresses skewed across bank groups) and 64 pair FMAs (tap pair x broadcast sample).
+//                    addresses skewed across bank groups) and 64 pair FMAs (tap pair x broadcast sample).  For
+//                    the loop shapes of the plans in use the loop is fully unrolled (tile_main_fixed), with the
+//                    next iteration's sample loads in flight during the current one's FMAs.
 //                    After the loop the four slices' partial sums are reduced by two shuffle rounds, and each
 //                    lane turns 4 consecutive outputs of 2 rows into the envelope (dsp.rs:373) and stores them
 //                    as float4.  The resampled signal itself never reaches HBM.  The output before a group's
@@ -28,6 +31,7 @@
 #pragma once
 
 #include <cstdint>
+#include <type_traits>
 #include <cuda_runtime.h>
 
 #include "kernels_generic.cuh"
@@ -98,21 +102,81 @@ __device__ __forceinline__ float4 lds128(u32 addr) {
     return v;
 }
 
-// One half (4 outputs, as two packed pairs) x 4 rows x the 4 consecutive samples of one 16-byte chunk.
+// One half (4 outputs, as two packed pairs) x Q rows x the 4 consecutive samples of one 16-byte chunk.
 // acc[p][j] packs outputs (2p, 2p+1) of row j; the tap pair comes straight out of the LDS.128 register quad,
 // the sample is duplicated into both lanes of the packed operand.
-__device__ __forceinline__ void half_fma2(f32x2 (&acc)[2][kTileQ], u32 tap_addr, const float4 (&s)[kTileQ]) {
+template <int Q>
+__device__ __forceinline__ void half_fma2(f32x2 (&acc)[2][Q], u32 tap_addr, const float4 (&s)[Q]) {
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
         const float4 tp = lds128(tap_addr + 16 * u);  // taps of outputs r = 0..3 for sample u of the chunk
         const f32x2 t01 = pack2(tp.x, tp.y), t23 = pack2(tp.z, tp.w);
 #pragma unroll
-        for (int j = 0; j < kTileQ; ++j) {
+        for (int j = 0; j < Q; ++j) {
             const float sv = u == 0 ? s[j].x : u == 1 ? s[j].y : u == 2 ? s[j].z : s[j].w;
             const f32x2 sv2 = pack2(sv, sv);
             acc[0][j] = fma2(t01, sv2, acc[0][j]);
             acc[1][j] = fma2(t23, sv2, acc[1][j]);
         }
+    }
+}
+
+// The main loop of one group over Q rows of a tile (row j at row_addr[j]): iterations [0, it_b_begin) run half A only,
+// [it_b_begin, it_a_end) both halves, [it_a_end, iters) half B only.  Any plan shape.
+template <int Q>
+__device__ __forceinline__ void tile_main_runtime(f32x2 (&acc_a)[2][Q], f32x2 (&acc_b)[2][Q], u32 tap_addr,
+                                                  const u32 (&row_addr)[Q], u32 it_b_begin, u32 it_a_end, u32 iters,
+                                                  u32 rec_bytes) {
+    u32 row_off = 0, it = 0;
+    for (; it < it_b_begin; ++it) {                        // half A only
+        float4 s[Q];
+#pragma unroll
+        for (int j = 0; j < Q; ++j) s[j] = lds128(row_addr[j] + row_off);
+        half_fma2(acc_a, tap_addr, s);
+        row_off += kTileKS * 16;
+        tap_addr += rec_bytes;
+    }
+    for (; it < it_a_end; ++it) {                          // both halves
+        float4 s[Q];
+#pragma unroll
+        for (int j = 0; j < Q; ++j) s[j] = lds128(row_addr[j] + row_off);
+        half_fma2(acc_a, tap_addr, s);
+        half_fma2(acc_b, tap_addr + 64, s);
+        row_off += kTileKS * 16;
+        tap_addr += rec_bytes;
+    }
+    for (; it < iters; ++it) {                             // half B only
+        float4 s[Q];
+#pragma unroll
+        for (int j = 0; j < Q; ++j) s[j] = lds128(row_addr[j] + row_off);
+        half_fma2(acc_b, tap_addr + 64, s);
+        row_off += kTileKS * 16;
+        tap_addr += rec_bytes;
+    }
+}
+
+// The same loop for a plan shape known at compile time: ITERS iterations, half B active from BB on, half A up to AE,
+// HALVES tap records per (iteration, slice lane).  Fully unrolled, every shared-memory address is a register plus an
+// immediate, so there is no loop-carried register renaming.  The Q sample quads are double-buffered in registers and
+// those of iteration it+1 are requested before the FMAs of iteration it, which hides the LDS latency behind them.  The
+// tap quads are loaded in source order next to the FMAs that use them; how far ahead of those FMAs they are issued is
+// left to ptxas's scheduling of the unrolled body.  Each accumulator sees the same FMAs in the same order as in
+// tile_main_runtime, so the results are bit-identical.
+template <int Q, int ITERS, int BB, int AE, int HALVES>
+__device__ __forceinline__ void tile_main_fixed(f32x2 (&acc_a)[2][Q], f32x2 (&acc_b)[2][Q], u32 tap_addr,
+                                                const u32 (&row_addr)[Q]) {
+    constexpr u32 rec_bytes = HALVES * 64;
+    float4 s[2][Q];
+#pragma unroll
+    for (int j = 0; j < Q; ++j) s[0][j] = lds128(row_addr[j]);
+#pragma unroll
+    for (int it = 0; it < ITERS; ++it) {
+        if (it + 1 < ITERS) {
+#pragma unroll
+            for (int j = 0; j < Q; ++j) s[(it + 1) & 1][j] = lds128(row_addr[j] + (it + 1) * kTileKS * 16);
+        }
+        if (it < AE) half_fma2(acc_a, tap_addr + it * rec_bytes, s[it & 1]);
+        if (it >= BB) half_fma2(acc_b, tap_addr + it * rec_bytes + 64, s[it & 1]);
     }
 }
 
@@ -124,9 +188,11 @@ __device__ __forceinline__ void named_bar_sync(u32 id, u32 nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// group_xs[g] = w0_g, the (4-aligned) first input sample of group g relative to its row.
-template <bool ENVELOPE>
-__global__ void __launch_bounds__(32 * (13 + 1), 1)
+// group_xs[g] = w0_g, the (4-aligned) first input sample of group g relative to its row.  ITERS > 0: the plan's loop
+// shape (tp.iters, first iteration of half B, end of half A, halves) is <ITERS, BB, AE, HALVES> and the main loop is
+// tile_main_fixed; ITERS == 0: any shape, runtime loop bounds.  The block is tp.compute_warps + 1 warps, at most 13.
+template <bool ENVELOPE, int ITERS, int BB, int AE, int HALVES>
+__global__ void __launch_bounds__(32 * (kTileMaxComputeWarps + 1), 1)
 k_polyphase_ws(const float *__restrict__ signal, u64 len, const float *__restrict__ tile_taps,
                const u32 *__restrict__ group_xs, TilePlan tp, u64 nout, u64 tile_begin, u64 ntiles, float cosphi2,
                float sinphi, float *__restrict__ out, unsigned long long *__restrict__ prof) {
@@ -150,23 +216,26 @@ k_polyphase_ws(const float *__restrict__ signal, u64 len, const float *__restric
     float *s_xch = s_stage0 + tp.stages * tp.stage_floats;
 
     const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const u32 G = tp.groups;
+    const u32 G = tp.groups, CW = tp.compute_warps;
     const u32 tile_out = QT * tp.p_out;
 
     if (tid == 0) {
         mbar_init(bar_taps, 1);
         for (u32 s = 0; s < tp.stages; ++s) {
             mbar_init(full_rows + s, 1);
-            mbar_init(empty_rows + s, G);
+            mbar_init(empty_rows + s, CW);
         }
         fence_mbar_init();
     }
     __syncthreads();
 
-    // Warp roles: compute warps 0..G-1, then the producer.  Warps are spread over the 4 SM sub-partitions
-    // round-robin (warp % 4); with 13 compute warps sub-partition 0 gets four of them, and the producer (warp 13)
-    // goes to sub-partition 1.
-    const bool is_producer = warp == G;
+    // Warp roles: compute warps 0..CW-1, then the producer.  Warps are spread over the 4 SM sub-partitions round-robin
+    // (warp % 4).  With G <= 12 groups compute warp g owns group g.  With G = 13 there are 12 compute warps, 3 per
+    // sub-partition: warp g owns group g < 12, and the 32 rows of group 12 are split over warps 0..3, one on each
+    // sub-partition, 8 rows each (one per row lane).  Each sub-partition then carries 3.25 groups per tile instead of 4
+    // on one and 3 on the others.  The producer (warp 12) lands on sub-partition 0, the halo dot product on warp 6
+    // (sub-partition 2); both are light next to a group.
+    const bool is_producer = warp == CW;
     if (is_producer) {
         // ======================================= producer =======================================
         const bool aligned16 = (reinterpret_cast<uintptr_t>(signal) & 15) == 0;
@@ -263,21 +332,31 @@ k_polyphase_ws(const float *__restrict__ signal, u64 len, const float *__restric
     } else {
         // ======================================= compute ========================================
         const u32 ks = lane >> 3, ql = lane & 7;
-        const u32 w0 = group_xs[warp];
         const u32 it_a_end = tp.half_taps / 16;       // half A is active for iterations [0, it_a_end)
         const u32 it_b_begin = tp.halves == 2 ? tp.shift / 16 : tp.iters;   // half B for [it_b_begin, iters)
         const u32 rec_bytes = tp.halves * 64;         // one (iteration, slice lane) tap record
         const u32 R = 4 * tp.halves;
-        const u32 tap_base = smem_u32(s_taps) + (warp * tp.group_stride + ks * tp.slice_stride) * 4;
-        // row r lives at pair r/2, half r%2; this thread reads rows ql, ql+8, ql+16, ql+24
-        const u32 row_off = (tp.rows_per_copy == 2 ? (ql >> 1) * tp.pair_pitch + (ql & 1) * tp.p_in : ql * tp.pair_pitch) * 4 +
-                            (w0 + ks * 4) * 4;
         const u32 row_step8 = (8 / tp.rows_per_copy) * tp.pair_pitch * 4;
+        // row r lives at pair r/2, half r%2; this thread reads rows ql, ql+8, ql+16, ql+24 of its group
+        const u32 lane_row = (tp.rows_per_copy == 2 ? (ql >> 1) * tp.pair_pitch + (ql & 1) * tp.p_in : ql * tp.pair_pitch) * 4;
+        const u32 row_off = lane_row + (group_xs[warp] + ks * 4) * 4;
+        const u32 tap_base = smem_u32(s_taps) + (warp * tp.group_stride + ks * tp.slice_stride) * 4;
+        // G > CW: warps 0..3 also compute group G-1 in row qx = ql + 8*warp (one row per row lane)
+        const bool split = G > CW && warp < 4;
+        const u32 gx = G - 1, qx = ql + 8 * warp;
+        const u32 row_off_x = lane_row + (group_xs[gx] + ks * 4) * 4 + warp * row_step8;
+        const u32 tap_base_x = smem_u32(s_taps) + (gx * tp.group_stride + ks * tp.slice_stride) * 4;
         // after the reduction this lane holds outputs 4*hsel..4*hsel+3 of the group in rows q0 and q0 + 8
         const u32 hsel = ks & 1, rsel = ks >> 1, q0 = ql + 16 * rsel;
-        const u32 halo_warp = G > 2 ? 2 : G - 1;
+        const u32 halo_warp = G > CW ? 6 : G > 2 ? 2 : G - 1;
         const float inv_sinphi = 1.f / sinphi;
         const bool out_aligned = (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+        // one group's main loop over the Q rows at row_addr
+        auto main_loop = [&](auto &acc_a, auto &acc_b, u32 tap_addr, const auto &row_addr) {
+            constexpr int NQ = static_cast<int>(std::extent_v<std::remove_reference_t<decltype(row_addr)>>);
+            if constexpr (ITERS > 0) tile_main_fixed<NQ, ITERS, BB, AE, HALVES>(acc_a, acc_b, tap_addr, row_addr);
+            else tile_main_runtime<NQ>(acc_a, acc_b, tap_addr, row_addr, it_b_begin, it_a_end, tp.iters, rec_bytes);
+        };
         mbar_wait(bar_taps, 0);
         u32 n = 0, st = 0, ph = 0;
         for (u64 tile = tile_begin + blockIdx.x; tile < ntiles; tile += gridDim.x, ++n) {
@@ -285,43 +364,24 @@ k_polyphase_ws(const float *__restrict__ signal, u64 len, const float *__restric
             PROF_MARK();
             mbar_wait(full_rows + st, ph);
             PROF_ADD(0);
-            f32x2 acc_a[2][Q], acc_b[2][Q];
+            f32x2 acc_a[2][Q], acc_b[2][Q], xa[2][1], xb[2][1];
 #pragma unroll
-            for (int p = 0; p < 2; ++p)
+            for (int p = 0; p < 2; ++p) {
 #pragma unroll
                 for (int j = 0; j < Q; ++j) acc_a[p][j] = acc_b[p][j] = 0ull;
+                xa[p][0] = xb[p][0] = 0ull;
+            }
             if (tp.debug != 1 && tp.debug < 5) {
-                u32 tap_addr = tap_base;
-                u32 row_addr = smem_u32(rows) + row_off;
-                u32 it = 0;
-                for (; it < it_b_begin; ++it) {                        // half A only
-                    float4 s[Q];
-#pragma unroll
-                    for (int j = 0; j < Q; ++j) s[j] = lds128(row_addr + j * row_step8);
-                    half_fma2(acc_a, tap_addr, s);
-                    row_addr += KS * 16;
-                    tap_addr += rec_bytes;
-                }
-                for (; it < it_a_end; ++it) {                          // both halves
-                    float4 s[Q];
-#pragma unroll
-                    for (int j = 0; j < Q; ++j) s[j] = lds128(row_addr + j * row_step8);
-                    half_fma2(acc_a, tap_addr, s);
-                    half_fma2(acc_b, tap_addr + 64, s);
-                    row_addr += KS * 16;
-                    tap_addr += rec_bytes;
-                }
-                for (; it < tp.iters; ++it) {                          // half B only
-                    float4 s[Q];
-#pragma unroll
-                    for (int j = 0; j < Q; ++j) s[j] = lds128(row_addr + j * row_step8);
-                    half_fma2(acc_b, tap_addr + 64, s);
-                    row_addr += KS * 16;
-                    tap_addr += rec_bytes;
+                const u32 rbase = smem_u32(rows) + row_off;
+                const u32 row_addr[Q] = {rbase, rbase + row_step8, rbase + 2 * row_step8, rbase + 3 * row_step8};
+                main_loop(acc_a, acc_b, tap_base, row_addr);
+                if (split) {
+                    const u32 row_addr_x[1] = {smem_u32(rows) + row_off_x};
+                    main_loop(xa, xb, tap_base_x, row_addr_x);
                 }
             }
-            // r[K0 - 1]: the last output of the last group, applied to the halo row -- by warp 2, which shares its
-            // sub-partition with two compute warps instead of three (warp G-1 = 12 is on the busiest one)
+            // r[K0 - 1]: the last output of the last group, applied to the halo row -- by a warp that owns no rows of
+            // group G-1 and shares its sub-partition only with other compute warps
             float halo = 0.f;
             if (ENVELOPE && warp == halo_warp && tile > 0) {
                 const float *vrow = rows + tp.rows_floats;
@@ -365,53 +425,78 @@ k_polyphase_ws(const float *__restrict__ signal, u64 len, const float *__restric
                     const float send = rsel ? w[jj][e] : w[2 + jj][e];
                     r[jj][e] = (rsel ? w[2 + jj][e] : w[jj][e]) + __shfl_xor_sync(0xffffffffu, send, 16);
                 }
-            float prev[2] = {0.f, 0.f};
+            // the same for the row of group G-1: lanes with rsel == 0 hold its outputs 4*hsel..4*hsel+3
+            float rx[4] = {0.f, 0.f, 0.f, 0.f};
+            if (split) {
+                float vx[2][4];
+                unpack2(xa[0][0], vx[0][0], vx[0][1]);
+                unpack2(xa[1][0], vx[0][2], vx[0][3]);
+                unpack2(xb[0][0], vx[1][0], vx[1][1]);
+                unpack2(xb[1][0], vx[1][2], vx[1][3]);
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const float send = hsel ? vx[0][e] : vx[1][e];
+                    const float wx = (hsel ? vx[1][e] : vx[0][e]) + __shfl_xor_sync(0xffffffffu, send, 8);
+                    rx[e] = wx + __shfl_xor_sync(0xffffffffu, wx, 16);
+                }
+            }
+            float prev[2] = {0.f, 0.f}, prev_x = 0.f;
             if (ENVELOPE) {
                 // Previous output of each lane's first one: output 3 of half A in the neighbouring lane (half B), else the
                 // last output of the previous group in the same row, of the last group in the previous row, or the halo.
-                // The exchange array [tile parity][warp][1 + row] holds each warp's last output per row (row -1: halo).
+                // The exchange array [tile parity][group][1 + row] holds each group's last output per row (row -1: halo).
                 float *xch = s_xch + (n & 1) * G * (QT + 1);
                 if (hsel == tp.halves - 1) {
                     xch[warp * (QT + 1) + 1 + q0] = r[0][3];
                     xch[warp * (QT + 1) + 9 + q0] = r[1][3];
+                    if (split && rsel == 0) xch[gx * (QT + 1) + 1 + qx] = rx[3];
                 }
                 if (warp == halo_warp && lane == 0) xch[(G - 1) * (QT + 1)] = halo;
-                named_bar_sync(1, 32 * G);
+                named_bar_sync(1, 32 * CW);
 #pragma unroll
                 for (int jj = 0; jj < 2; ++jj) {
                     const float left = __shfl_xor_sync(0xffffffffu, r[jj][3], 8);
                     const u32 q = q0 + 8 * jj;
                     prev[jj] = hsel ? left : warp > 0 ? xch[(warp - 1) * (QT + 1) + 1 + q] : xch[(G - 1) * (QT + 1) + q];
                 }
-            }
-            if (hsel < tp.halves) {                                 // one half only: lanes of half B store nothing
-                const u64 k_base = tile * tile_out;
-                const bool full_tile = k_base + tile_out <= nout && out_aligned;
-#pragma unroll
-                for (int jj = 0; jj < 2; ++jj) {
-                    const u32 kl = (q0 + 8 * jj) * tp.p_out + warp * R + 4 * hsel;   // output index inside the tile
-                    float4 res = make_float4(r[jj][0], r[jj][1], r[jj][2], r[jj][3]);
-                    if (ENVELOPE) {
-                        res.x = envelope2_fast(prev[jj], r[jj][0], cosphi2, inv_sinphi);
-                        res.y = envelope2_fast(r[jj][0], r[jj][1], cosphi2, inv_sinphi);
-                        res.z = envelope2_fast(r[jj][1], r[jj][2], cosphi2, inv_sinphi);
-                        res.w = envelope2_fast(r[jj][2], r[jj][3], cosphi2, inv_sinphi);
-                        if (kl == 0 && k_base == 0) res.x = 0.f;     // output[0] = 0 (dsp.rs:357)
-                    }
-                    if (full_tile) {
-                        *reinterpret_cast<float4 *>(out + k_base + kl) = res;
-                    } else {
-                        const u64 k = k_base + kl;
-                        if (k < nout) out[k] = res.x;
-                        if (k + 1 < nout) out[k + 1] = res.y;
-                        if (k + 2 < nout) out[k + 2] = res.z;
-                        if (k + 3 < nout) out[k + 3] = res.w;
-                    }
+                if (split) {
+                    const float left = __shfl_xor_sync(0xffffffffu, rx[3], 8);
+                    prev_x = hsel ? left : xch[(gx - 1) * (QT + 1) + 1 + qx];
                 }
+            }
+            // envelope and store of outputs 4*hsel..4*hsel+3 of group g in row q (one half only: lanes of half B store
+            // nothing)
+            const u64 k_base = tile * tile_out;
+            const bool full_tile = k_base + tile_out <= nout && out_aligned;
+            auto finish = [&](u32 g, u32 q, const float (&y)[4], float before) {
+                const u32 kl = q * tp.p_out + g * R + 4 * hsel;   // output index inside the tile
+                float4 res = make_float4(y[0], y[1], y[2], y[3]);
+                if (ENVELOPE) {
+                    res.x = envelope2_fast(before, y[0], cosphi2, inv_sinphi);
+                    res.y = envelope2_fast(y[0], y[1], cosphi2, inv_sinphi);
+                    res.z = envelope2_fast(y[1], y[2], cosphi2, inv_sinphi);
+                    res.w = envelope2_fast(y[2], y[3], cosphi2, inv_sinphi);
+                    if (kl == 0 && k_base == 0) res.x = 0.f;     // output[0] = 0 (dsp.rs:357)
+                }
+                if (full_tile) {
+                    *reinterpret_cast<float4 *>(out + k_base + kl) = res;
+                } else {
+                    const u64 k = k_base + kl;
+                    if (k < nout) out[k] = res.x;
+                    if (k + 1 < nout) out[k + 1] = res.y;
+                    if (k + 2 < nout) out[k + 2] = res.z;
+                    if (k + 3 < nout) out[k + 3] = res.w;
+                }
+            };
+            if (hsel < tp.halves) {
+                finish(warp, q0, r[0], prev[0]);
+                finish(warp, q0 + 8, r[1], prev[1]);
+                if (split && rsel == 0) finish(gx, qx, rx, prev_x);
             }
             PROF_ADD(2);
         }
         if (profiling && warp == 0) { prof[2] = pt[0]; prof[3] = pt[1]; prof[4] = pt[2]; prof[8] = n; }
+        if (profiling && warp < 4) prof[9 + warp] = pt[1];   // main loops of warps 0..3, one per SM sub-partition
         if (prof != nullptr && warp == 0 && lane == 0) {   // per-CTA wall time of the whole kernel body + SM id
             u32 smid;
             asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));

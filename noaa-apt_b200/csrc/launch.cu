@@ -60,6 +60,29 @@ int launch_polyphase(const LaunchCtx &c, const void *signal, int format, u64 len
     return APT_OK;
 }
 
+// Launches k_polyphase_ws for the plan's loop shape: (iterations, first iteration of half B, end of half A, halves).
+// The standard plans at 48 kHz (7, 1, 6, 2) and 96 kHz (11, 11, 11, 1) and the 48 kHz fast profile (3, 0, 3, 2) get an
+// unrolled main loop; other plans keep the runtime loop.
+template <bool ENV>
+static int launch_ws_shape(const TilePlan &tp, unsigned grid, unsigned block, cudaStream_t stream, const float *signal,
+                            u64 len, const float *tile_taps, const u32 *group_xs, u64 nout, u64 tile_begin, u64 ntiles,
+                            float cosphi2, float sinphi, float *out, unsigned long long *prof) {
+    auto run = [&](auto kern) -> int {
+        APT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tp.smem_bytes)));
+        kern<<<grid, block, tp.smem_bytes, stream>>>(signal, len, tile_taps, group_xs, tp, nout, tile_begin, ntiles, cosphi2,
+                                                     sinphi, out, prof);
+        return APT_OK;
+    };
+    const u32 b_begin = tp.halves == 2 ? tp.shift / 16 : tp.iters, a_end = tp.half_taps / 16;
+    auto shape = [&](u32 it, u32 bb, u32 ae, u32 halves) {
+        return tp.iters == it && b_begin == bb && a_end == ae && tp.halves == halves;
+    };
+    if (shape(7, 1, 6, 2)) return run(k_polyphase_ws<ENV, 7, 1, 6, 2>);
+    if (shape(11, 11, 11, 1)) return run(k_polyphase_ws<ENV, 11, 11, 11, 1>);
+    if (shape(3, 0, 3, 2)) return run(k_polyphase_ws<ENV, 3, 0, 3, 2>);
+    return run(k_polyphase_ws<ENV, 0, 0, 0, 0>);
+}
+
 int launch_polyphase_tiled(const LaunchCtx &c, const float *signal, u64 len, const float *tile_taps,
                            const u32 *group_xs, const TilePlan &tp, u64 nout, u64 tile_begin, u64 tile_end,
                            bool envelope, float cosphi2, float sinphi, float *out) {
@@ -69,23 +92,17 @@ int launch_polyphase_tiled(const LaunchCtx &c, const float *signal, u64 len, con
     if (tile_end != 0) ntiles = std::min(ntiles, tile_end);
     if (tile_begin >= ntiles) return APT_OK;
     const unsigned grid = static_cast<unsigned>(std::min<u64>(ntiles - tile_begin, static_cast<u64>(c.sm_count)));
-    const unsigned block = 32 * (tp.groups + 1);   // compute warps + producer warp
+    const unsigned block = 32 * (tp.compute_warps + 1);   // compute warps + producer warp
     unsigned long long *prof = nullptr;
     if (getenv("APTB200_TILE_PROFILE")) {
         APT_CUDA(cudaMalloc(&prof, 512 * sizeof(unsigned long long)));
         APT_CUDA(cudaMemsetAsync(prof, 0, 512 * sizeof(unsigned long long), c.stream));
     }
-    if (envelope) {
-        auto kern = k_polyphase_ws<true>;
-        APT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tp.smem_bytes)));
-        kern<<<grid, block, tp.smem_bytes, c.stream>>>(signal, len, tile_taps, group_xs, tp, nout, tile_begin, ntiles,
-                                                        cosphi2, sinphi, out, prof);
-    } else {
-        auto kern = k_polyphase_ws<false>;
-        APT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tp.smem_bytes)));
-        kern<<<grid, block, tp.smem_bytes, c.stream>>>(signal, len, tile_taps, group_xs, tp, nout, tile_begin, ntiles,
-                                                        cosphi2, sinphi, out, prof);
-    }
+    const int rc = envelope ? launch_ws_shape<true>(tp, grid, block, c.stream, signal, len, tile_taps, group_xs, nout, tile_begin,
+                                                    ntiles, cosphi2, sinphi, out, prof)
+                            : launch_ws_shape<false>(tp, grid, block, c.stream, signal, len, tile_taps, group_xs, nout, tile_begin,
+                                                     ntiles, cosphi2, sinphi, out, prof);
+    if (rc != APT_OK) return rc;
     APT_CUDA(cudaGetLastError());
     if (prof) {
         unsigned long long h[512];
@@ -95,6 +112,8 @@ int launch_polyphase_tiled(const LaunchCtx &c, const float *signal, u64 len, con
         fprintf(stderr, "[tile profile, CTA 0, %llu tiles, %u stages, cycles] producer: wait_empty %llu issue %llu | compute warp 0: "
                         "wait_full %llu main %llu exchange+store %llu\n",
                 h[8], tp.stages, h[0], h[1], h[2], h[3], h[4]);
+        fprintf(stderr, "[tile profile] main loops of warps 0..3 (SM sub-partitions 0..3; with 13 groups they include group 12's rows): %llu %llu %llu %llu\n", h[9], h[10],
+                h[11], h[12]);
         unsigned long long mn = ~0ull, mx = 0, sum = 0;
         for (unsigned b = 0; b < grid; ++b) { mn = std::min(mn, h[16 + 2 * b]); mx = std::max(mx, h[16 + 2 * b]); sum += h[16 + 2 * b]; }
         fprintf(stderr, "[tile profile] per-CTA kernel-body cycles: min %llu avg %llu max %llu; first 12:", mn, sum / grid, mx);

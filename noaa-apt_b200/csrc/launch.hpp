@@ -79,11 +79,15 @@ struct PickScratch {
     u32 cap;           // candidate capacity
 };
 
+// Compute warps of the tiled kernel's block (+ 1 producer warp: 416 threads).  A plan of 13 groups splits the rows of
+// group 12 over compute warps 0..3 (kernels_fast.cuh).
+constexpr u32 kTileMaxComputeWarps = 12;
 // Geometry of the tiled kernel for one (L, M, taps) triple; built on the host (make_tile_plan).
 struct TilePlan {
     u32 l, m;          // resampling ratio
     u32 halves;        // 2: groups of 8 outputs in two half windows; 1: groups of 4 outputs (one window)
-    u32 groups;        // G = L / gcd(R, L), R = 4*halves (= compute warps per CTA); group g owns outputs R*g..R*g+R-1
+    u32 groups;        // G = L / gcd(R, L), R = 4*halves; group g owns outputs R*g..R*g+R-1
+    u32 compute_warps; // min(G, kTileMaxComputeWarps): G = 13 splits group 12 over compute warps 0..3
     u32 p_out, p_in;   // outputs / inputs per super-period (p_out = 8G)
     u32 usteps;        // samples a group reads per row (= half_taps + shift), multiple of 16
     u32 half_taps;     // padded taps of one half (4 outputs), multiple of 16

@@ -9,7 +9,7 @@ namespace aptb200 {
 
 namespace {
 constexpr u32 kH = 4, kQ = 4, kKS = 4, kQT = (32 / kKS) * kQ;
-constexpr u32 kMaxGroups = 13;                 // compute warps per CTA the kernel is compiled for (+ 1 producer: 448 threads)
+constexpr u32 kMaxGroups = kTileMaxComputeWarps + 1;   // the kernel splits one group's rows over four compute warps
 constexpr u32 kSmemTwoCtas = (233472 - 2 * 1024) / 2 - 512;   // dynamic bytes that still let two CTAs share an SM
 constexpr u32 kSmemOneCta = 227 * 1024;
 constexpr u32 kIterSamples = 4 * kKS;          // samples consumed per loop iteration (one 16-byte chunk per slice lane)
@@ -136,6 +136,7 @@ static bool try_tile_plan(u32 halves, u32 stages, u32 l, u32 m, const std::vecto
     tp.l = l;
     tp.m = m;
     tp.groups = groups;
+    tp.compute_warps = std::min(groups, kTileMaxComputeWarps);
     tp.p_out = static_cast<u32>(p_out);
     tp.p_in = static_cast<u32>(p_in);
     tp.usteps = static_cast<u32>(span);
