@@ -192,7 +192,10 @@ int apt_resample_wav(const char *input_path, const char *output_path, uint32_t o
 typedef enum apt_contrast {
     APT_CONTRAST_MINMAX = 0,      /* Contrast::MinMax: dsp::get_min / get_max             noaa_apt.rs:157-163, dsp.rs:20-54  */
     APT_CONTRAST_PERCENT = 1,     /* Contrast::Percent(p): misc::percent, 1000 buckets    misc.rs:119-175                    */
-    APT_CONTRAST_TELEMETRY = 2    /* Contrast::Telemetry: wedges 9 / 8 of the best frame  noaa_apt.rs:141-149, telemetry.rs  */
+    APT_CONTRAST_TELEMETRY = 2,   /* Contrast::Telemetry: wedges 9 / 8 of the best frame  noaa_apt.rs:141-149, telemetry.rs  */
+    APT_CONTRAST_HISTOGRAM = 3    /* Contrast::Histogram: MinMax bounds, then grey histogram equalisation per channel half
+                                     (processing.rs:87-103, imageext.rs:23-46,95-119).  Only apt_process,
+                                     apt_decode_image and apt_decoder_set_process_mode accept it. */
 } apt_contrast;
 
 typedef struct apt_image_info {
@@ -217,6 +220,35 @@ int apt_map_signal_u8(const float *signal, uint64_t n, float low, float high, ui
 int apt_contrast_bounds(const float *signal, uint64_t n, int contrast, float percent, apt_image_info *info);
 /* telemetry.rs:147-170: per-row means of the two telemetry bands and their pooled variance (n / 2080 values each). */
 int apt_telemetry_rows(const float *signal, uint64_t n, float *mean_a, float *mean_b, float *variance);
+
+/* The rest of noaa_apt::process (noaa_apt.rs:140-240) apart from the map overlay, on the device: contrast bounds ->
+ * map_signal_u8 -> into_rgba8 -> false colour (processing.rs:108-157) -> grey histogram equalisation (processing.rs:87-103)
+ * -> Rotate::Yes (processing.rs:21-37: both 909-px image rectangles turned by 180 degrees, sync / space / telemetry columns
+ * kept).  Given the same f32 rows the image is bit-identical to the reference's.
+ *   contrast  apt_contrast (APT_CONTRAST_HISTOGRAM included); percent is read for APT_CONTRAST_PERCENT only, in [0, 1]
+ *   palette   NULL, or 256*256*3 bytes: the palette image after into_rgb8, row = channel B value, column = channel A value
+ *   tune      ColorSettings::{ch_a_tune_start, ch_a_tune_end, ch_b_tune_start, ch_b_tune_end}
+ *   rgba      0: grey output, 1 B/px (no palette allowed); 1: RGBA output, 4 B/px (alpha 255)
+ * Colour + APT_CONTRAST_HISTOGRAM (the Lab branch, imageext.rs:50-63) is not available: APT_ERR_BAD_ARG.  The argument
+ * rules are checked before any device is touched. */
+typedef struct apt_process_settings {
+    int contrast;
+    float percent;
+    int rotate;                   /* 0: Rotate::No, else Rotate::Yes */
+    const uint8_t *palette;       /* 256*256*3 RGB or NULL */
+    float tune[4];                /* ch_a start, ch_a end, ch_b start, ch_b end */
+    int rgba;
+} apt_process_settings;
+
+/* process() on host rows (rows = decode()'s output, n = rows*2080 values): out receives rows*2080*(rgba ? 4 : 1) bytes,
+ * *nout that count; cap in bytes. */
+int apt_process(const float *rows, uint64_t n, const apt_process_settings *ps, uint8_t *out, uint64_t cap, uint64_t *nout,
+                apt_image_info *info);
+/* decode() + process() in one call; only the finished pixels leave the GPU.  cap in bytes >= apt_decode_len_bound * (rgba ? 4 : 1);
+ * *nout receives the byte count.  Errors as apt_decode_image_u8. */
+int apt_decode_image(const void *signal, int format, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
+                     const apt_process_settings *ps, uint8_t *out, uint64_t cap, uint64_t *nout, apt_image_info *info,
+                     apt_status_cb cb, void *user);
 
 /* ----------------------------------------------- decoder object (streams) */
 
@@ -243,6 +275,10 @@ int apt_decoder_submit_host(apt_decoder *dec, const void *signal, int format, ui
 /* Image mode of a decoder: contrast >= 0 (apt_contrast) makes every following submit produce the u8 image instead of the
  * f32 rows -- `out` is then a uint8_t buffer and `cap` / *nout count bytes; contrast < 0 switches back to f32 rows. */
 int apt_decoder_set_image_mode(apt_decoder *dec, int contrast, float percent);
+/* Process mode of a decoder: every following submit produces the image apt_process describes -- `out` is a uint8_t buffer,
+ * `cap` and *nout count bytes (rows*2080*(rgba ? 4 : 1)).  The palette is copied to the device here, once.  NULL switches
+ * back to f32 rows; apt_decoder_set_image_mode also leaves process mode. */
+int apt_decoder_set_process_mode(apt_decoder *dec, const apt_process_settings *ps);
 /* Contrast bounds / telemetry of the last image job (after apt_decoder_wait). */
 int apt_decoder_image_info(apt_decoder *dec, apt_image_info *info);
 /* 1 if the decoder's job has finished (apt_decoder_wait will not block) or none is in flight, else 0. */

@@ -62,7 +62,13 @@ class CImageInfo(C.Structure):
                 ("wedges_a", C.c_float * 16), ("wedges_b", C.c_float * 16)]
 
 
-CONTRAST_MINMAX, CONTRAST_PERCENT, CONTRAST_TELEMETRY = 0, 1, 2
+CONTRAST_MINMAX, CONTRAST_PERCENT, CONTRAST_TELEMETRY, CONTRAST_HISTOGRAM = 0, 1, 2, 3
+
+
+class CProcessSettings(C.Structure):
+    _fields_ = [("contrast", C.c_int), ("percent", C.c_float), ("rotate", C.c_int), ("palette", C.c_void_p),
+                ("tune", C.c_float * 4), ("rgba", C.c_int)]
+
 
 class CWavInfo(C.Structure):
     _fields_ = [("sample_rate", C.c_uint32), ("channels", C.c_uint32), ("bits_per_sample", C.c_uint32), ("is_float", C.c_uint32),
@@ -115,7 +121,13 @@ SIGNATURES = {
     "apt_map_signal_u8": (C.c_int, [C.c_void_p, C.c_uint64, C.c_float, C.c_float, C.c_void_p]),
     "apt_contrast_bounds": (C.c_int, [C.c_void_p, C.c_uint64, C.c_int, C.c_float, C.POINTER(CImageInfo)]),
     "apt_telemetry_rows": (C.c_int, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "apt_process": (C.c_int, [C.c_void_p, C.c_uint64, C.POINTER(CProcessSettings), C.c_void_p, C.c_uint64, _u64p,
+                              C.POINTER(CImageInfo)]),
+    "apt_decode_image": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64, C.c_uint32, C.POINTER(CSettings), C.c_int,
+                                   C.POINTER(CProcessSettings), C.c_void_p, C.c_uint64, _u64p, C.POINTER(CImageInfo),
+                                   STATUS_CB, C.c_void_p]),
     "apt_decoder_set_image_mode": (C.c_int, [C.c_void_p, C.c_int, C.c_float]),
+    "apt_decoder_set_process_mode": (C.c_int, [C.c_void_p, C.POINTER(CProcessSettings)]),
     "apt_decoder_image_info": (C.c_int, [C.c_void_p, C.POINTER(CImageInfo)]),
     "apt_decoder_create": (C.c_int, [C.c_int, C.c_uint32, C.POINTER(CSettings), C.c_uint64, C.POINTER(C.c_void_p)]),
     "apt_decoder_destroy": (None, [C.c_void_p]),

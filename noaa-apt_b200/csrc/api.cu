@@ -78,7 +78,7 @@ int free_decoder_buffers(apt_decoder *d) {
     if (d->h_res) cudaFreeHost(d->h_res);
     if (d->h_out) cudaFreeHost(d->h_out);
     if (d->h_post) cudaFreeHost(d->h_post);
-    for (void *p : {(void *)d->d_post, (void *)d->d_tel, (void *)d->d_out8})
+    for (void *p : {(void *)d->d_post, (void *)d->d_tel, (void *)d->d_out8, (void *)d->d_palette, (void *)d->d_proc, (void *)d->d_grey})
         if (p) cudaFree(p);
     d->own_stager.reset();
     for (auto e : d->ev_begin) cudaEventDestroy(e);
@@ -541,6 +541,36 @@ int enqueue_image_stage(apt_decoder *d, unsigned char *out8) {
     const u32 max_rows = static_cast<u32>(std::max<uint64_t>(d->max_out / kPxPerRow, 1));
     const u32 fixed = d->job_sync ? 0u : static_cast<u32>(d->job_fixed_out / kPxPerRow);
     (void)p;
+    if (d->proc_active) {
+        struct Hook : KernelHook {
+            apt_decoder *d;
+            int slot = -1;
+            explicit Hook(apt_decoder *dec) : d(dec) {}
+            void begin(const char *name) override { slot = prof_begin(d, name); }
+            void end() override { prof_end(d, slot); }
+        } hook(d);
+        ProcessLaunch a{};
+        a.rows = d->d_out;
+        a.result = d->job_sync ? d->d_res : nullptr;
+        a.fixed_rows = fixed;
+        a.max_rows = max_rows;
+        a.contrast = d->proc.contrast;
+        a.percent = d->proc.percent;
+        a.rotate = d->proc.rotate != 0;
+        a.rgba = d->proc.rgba != 0;
+        a.palette = d->proc_palette ? d->d_palette : nullptr;
+        memcpy(a.tune, d->proc.tune, sizeof(a.tune));
+        a.ctl = d->d_post;
+        a.tel_a = d->d_tel;
+        a.tel_b = d->d_tel + max_rows;
+        a.tel_v = d->d_tel + 2 * static_cast<size_t>(max_rows);
+        a.proc = d->d_proc;
+        a.grey = d->d_grey;
+        a.out = out8;
+        APT_TRY(launch_process_stage(c, a, &hook));
+        APT_CUDA(cudaMemcpyAsync(d->h_post, d->d_post, offsetof(PostCtl, buckets), cudaMemcpyDeviceToHost, d->stream));
+        return APT_OK;
+    }
     APT_TRY(launch_image_stage(c, d->d_out, d->job_sync ? d->d_res : nullptr, fixed, max_rows, kPxPerRow, d->image_contrast,
                                d->image_percent, d->d_post, d->d_tel, d->d_tel + max_rows, d->d_tel + 2 * static_cast<size_t>(max_rows),
                                nullptr, out8, false));
@@ -579,9 +609,12 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
         return fail(APT_ERR_BAD_ARG, "work_rate %u is too high for the sync picker (min_distance %u > 16384); decode without "
                                      "sync or use a work_rate <= 37440", p.st.work_rate, p.dist);
     const uint64_t need = d->job_sync ? (nwork / p.row) * kPxPerRow : plan_out_bound(p, n);
-    if (!out || cap < need) return fail(APT_ERR_CAPACITY, "output needs room for %llu %s", (unsigned long long)need,
-                                        d->image_contrast >= 0 ? "bytes" : "floats");
+    // bytes per output pixel of an image job: RGBA in process mode, else grey
+    const uint64_t bpp = d->image_contrast >= 0 && d->proc_active && d->proc.rgba ? 4 : 1;
+    if (!out || cap < need * bpp) return fail(APT_ERR_CAPACITY, "output needs room for %llu %s", (unsigned long long)(need * bpp),
+                                              d->image_contrast >= 0 ? "bytes" : "floats");
     d->job_image = d->image_contrast >= 0;
+    d->job_bpp = bpp;
     if (d->job_image) {
         if (!p.work_multiple) return fail(APT_ERR_BAD_ARG, "the image stage needs rows of 2080 pixels (work_rate multiple of 4160)");
         const uint64_t max_rows = std::max<uint64_t>(d->max_out / kPxPerRow, 1);
@@ -591,9 +624,20 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
             APT_CUDA(cudaMalloc(&d->d_tel, 3 * max_rows * sizeof(float)));
         }
         if (!d->d_out) APT_CUDA(cudaMalloc(&d->d_out, std::max<uint64_t>(d->max_out, 1) * sizeof(float)));
-        if (host && !d->d_out8) APT_CUDA(cudaMalloc(&d->d_out8, std::max<uint64_t>(d->max_out, 1)));
+        const uint64_t out8_need = std::max<uint64_t>(d->max_out, 1) * bpp;
+        if (host && d->out8_bytes < out8_need) {
+            if (d->d_out8) APT_CUDA(cudaFree(d->d_out8));
+            d->d_out8 = nullptr;
+            d->out8_bytes = 0;
+            APT_CUDA(cudaMalloc(&d->d_out8, out8_need));
+            d->out8_bytes = out8_need;
+        }
+        if (d->proc_active) {
+            if (!d->d_proc) APT_CUDA(cudaMalloc(&d->d_proc, sizeof(ProcCtl)));
+            if (!d->d_grey) APT_CUDA(cudaMalloc(&d->d_grey, std::max<uint64_t>(d->max_out, 1)));
+        }
     }
-    const size_t elem = d->job_image ? 1 : sizeof(float);
+    const size_t elem = d->job_image ? bpp : sizeof(float);
 
     const void *dev_in = signal;
     float *rows_dst = out;
@@ -709,7 +753,7 @@ extern "C" int apt_decoder_wait(apt_decoder *d, uint64_t *nout) {
             if (d->job_host && d->job_d2h_floats)
                 APT_CUDA(cudaMemcpyAsync(d->job_out_pageable ? static_cast<void *>(d->h_out) : static_cast<void *>(d->job_out),
                                          d->job_image ? static_cast<const void *>(d->d_out8) : static_cast<const void *>(d->d_out),
-                                         d->job_d2h_floats * (d->job_image ? 1 : sizeof(float)), cudaMemcpyDeviceToHost, d->stream));
+                                         d->job_d2h_floats * (d->job_image ? d->job_bpp : sizeof(float)), cudaMemcpyDeviceToHost, d->stream));
             APT_CUDA(cudaStreamSynchronize(d->stream));
             d->last_fused = false;
         }
@@ -722,7 +766,7 @@ extern "C" int apt_decoder_wait(apt_decoder *d, uint64_t *nout) {
         }
         produced = static_cast<uint64_t>(res.n_rows) * kPxPerRow;
     }
-    const size_t elem = d->job_image ? 1 : sizeof(float);
+    const size_t elem = d->job_image ? d->job_bpp : sizeof(float);
     if (d->job_host && d->job_out_pageable && produced) {
         if (d->stager) d->stager->scatter(d->job_out, d->h_out, produced * elem);
         else memcpy(d->job_out, d->h_out, produced * elem);
@@ -752,7 +796,7 @@ extern "C" int apt_decoder_wait(apt_decoder *d, uint64_t *nout) {
         d->kernel_ms.assign(d->ev_used, 0.f);
         for (int i = 0; i < d->ev_used; ++i) cudaEventElapsedTime(&d->kernel_ms[i], d->ev_begin[i], d->ev_end[i]);
     }
-    if (nout) *nout = produced;
+    if (nout) *nout = d->job_image ? produced * d->job_bpp : produced;
     return APT_OK;
 }
 
@@ -764,6 +808,56 @@ extern "C" int apt_decoder_set_image_mode(apt_decoder *d, int contrast, float pe
         return fail(APT_ERR_BAD_ARG, "Percent given should be between 0 and 1");      // misc.rs:120-124
     d->image_contrast = contrast;
     d->image_percent = percent;
+    d->proc_active = false;
+    return APT_OK;
+}
+
+namespace {
+
+// The argument rules of the process entry points; no device needed.
+int check_process_settings(const apt_process_settings *ps) {
+    if (!ps) return fail(APT_ERR_BAD_ARG, "null process settings");
+    if (ps->contrast < 0 || ps->contrast > APT_CONTRAST_HISTOGRAM) return fail(APT_ERR_BAD_ARG, "unknown contrast mode %d", ps->contrast);
+    if (ps->contrast == APT_CONTRAST_PERCENT && !(ps->percent >= 0.f && ps->percent <= 1.f))
+        return fail(APT_ERR_BAD_ARG, "Percent given should be between 0 and 1");      // misc.rs:120-124
+    if (ps->palette && !ps->rgba) return fail(APT_ERR_BAD_ARG, "false colour needs RGBA output");
+    if (ps->palette && ps->contrast == APT_CONTRAST_HISTOGRAM)
+        return fail(APT_ERR_BAD_ARG, "colour histogram equalisation is not available");
+    return APT_OK;
+}
+
+// 256*256*3 RGB -> 256*256 u32 with R in the low byte and alpha 255 (Rgb::to_rgba), one 4-byte load per coloured pixel
+std::vector<u32> pack_palette(const uint8_t *rgb) {
+    std::vector<u32> p(256 * 256);
+    for (size_t i = 0; i < p.size(); ++i)
+        p[i] = static_cast<u32>(rgb[3 * i]) | (static_cast<u32>(rgb[3 * i + 1]) << 8) | (static_cast<u32>(rgb[3 * i + 2]) << 16) | 0xFF000000u;
+    return p;
+}
+
+}  // namespace
+
+extern "C" int apt_decoder_set_process_mode(apt_decoder *d, const apt_process_settings *ps) {
+    if (!d) return fail(APT_ERR_BAD_ARG, "null decoder");
+    if (d->in_flight) return fail(APT_ERR_BAD_ARG, "decoder has a job in flight");
+    if (!ps) {
+        d->proc_active = false;
+        d->image_contrast = -1;
+        return APT_OK;
+    }
+    APT_TRY(check_process_settings(ps));
+    if (ps->palette) {
+        APT_CUDA(cudaSetDevice(d->device));
+        if (!d->d_palette) APT_CUDA(cudaMalloc(&d->d_palette, 256 * 256 * sizeof(u32)));
+        const std::vector<u32> packed = pack_palette(ps->palette);
+        APT_CUDA(cudaMemcpyAsync(d->d_palette, packed.data(), packed.size() * sizeof(u32), cudaMemcpyHostToDevice, d->stream));
+        APT_CUDA(cudaStreamSynchronize(d->stream));
+    }
+    d->proc = *ps;
+    d->proc.palette = nullptr;
+    d->proc_palette = ps->palette != nullptr;
+    d->proc_active = true;
+    d->image_contrast = ps->contrast;
+    d->image_percent = ps->percent;
     return APT_OK;
 }
 
@@ -996,7 +1090,7 @@ void cache_put_multi(int device, uint32_t rate, const apt_settings &st, apt_deco
 
 int decode_oneshot(const void *signal, int format, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
                    float *out, uint64_t cap, uint64_t *nout, apt_status_cb cb, void *user, int contrast = -1,
-                   float percent = 0.f, apt_image_info *info = nullptr) {
+                   float percent = 0.f, apt_image_info *info = nullptr, const apt_process_settings *ps = nullptr) {
     if (!s || !nout) return fail(APT_ERR_BAD_ARG, "null argument");
     *nout = 0;
     if (n == 0 || !signal) return fail(APT_ERR_BAD_ARG, "empty signal");
@@ -1022,10 +1116,12 @@ int decode_oneshot(const void *signal, int format, uint64_t n, uint32_t input_ra
     d->cb_user = user;
     d->image_contrast = contrast;
     d->image_percent = percent;
-    int st = apt_decoder_submit_host(d, signal, format, n, sync, out, cap);
+    int st = ps ? apt_decoder_set_process_mode(d, ps) : APT_OK;
+    if (st == APT_OK) st = apt_decoder_submit_host(d, signal, format, n, sync, out, cap);
     if (st == APT_OK) st = apt_decoder_wait(d, nout);
     if (st == APT_OK && info) *info = d->last_image;
     d->image_contrast = -1;
+    d->proc_active = false;
     d->cb = nullptr;
     d->cb_user = nullptr;
     if (use_cache) cache_put(device, input_rate, *s, d);
@@ -1069,6 +1165,14 @@ extern "C" int apt_decode_image_u8(const void *signal, int format, uint64_t n, u
         return fail(APT_ERR_BAD_ARG, "Percent given should be between 0 and 1");
     return decode_oneshot(signal, format, n, input_rate, s, sync, reinterpret_cast<float *>(out), cap, nout, cb, user, contrast,
                           percent, info);
+}
+
+extern "C" int apt_decode_image(const void *signal, int format, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
+                                const apt_process_settings *ps, uint8_t *out, uint64_t cap, uint64_t *nout, apt_image_info *info,
+                                apt_status_cb cb, void *user) {
+    APT_TRY(check_process_settings(ps));
+    return decode_oneshot(signal, format, n, input_rate, s, sync, reinterpret_cast<float *>(out), cap, nout, cb, user,
+                          ps->contrast, ps->percent, info, ps);
 }
 
 namespace {
@@ -1143,6 +1247,67 @@ extern "C" int apt_contrast_bounds(const float *signal, uint64_t n, int contrast
 extern "C" int apt_telemetry_rows(const float *signal, uint64_t n, float *mean_a, float *mean_b, float *variance) {
     if (!mean_a || !mean_b || !variance) return fail(APT_ERR_BAD_ARG, "null argument");
     return image_stage_host(signal, n, APT_CONTRAST_MINMAX, 0.f, nullptr, nullptr, nullptr, mean_a, mean_b, variance);
+}
+
+extern "C" int apt_process(const float *rows, uint64_t n, const apt_process_settings *ps, uint8_t *out, uint64_t cap,
+                           uint64_t *nout, apt_image_info *info) {
+    APT_TRY(check_process_settings(ps));
+    if (!nout) return fail(APT_ERR_BAD_ARG, "null argument");
+    *nout = 0;
+    if (!rows || n == 0) return fail(APT_ERR_BAD_ARG, "empty signal");   // get_min of an empty vector is an error, dsp.rs:21-25
+    const uint64_t nrows = n / kPxPerRow;
+    if (nrows * kPxPerRow != n) return fail(APT_ERR_BAD_ARG, "not a whole number of 2080-px rows");
+    if (nrows >= (1ull << 32) / kPxPerRow) return fail(APT_ERR_BAD_ARG, "image too large");
+    const uint64_t bytes = n * (ps->rgba ? 4 : 1);
+    if (!out || cap < bytes) return fail(APT_ERR_CAPACITY, "output needs room for %llu bytes", (unsigned long long)bytes);
+    APT_TRY(require_device());
+    DevBuf dx, dctl, dtel, dproc, dgrey, dout, dpal;
+    APT_TRY(dx.alloc(n * sizeof(float)));
+    APT_TRY(dctl.alloc(sizeof(PostCtl)));
+    APT_TRY(dtel.alloc(3 * nrows * sizeof(float)));
+    APT_TRY(dproc.alloc(sizeof(ProcCtl)));
+    APT_TRY(dgrey.alloc(n));
+    APT_TRY(dout.alloc(bytes));
+    APT_CUDA(cudaMemcpy(dx.p, rows, n * sizeof(float), cudaMemcpyHostToDevice));
+    if (ps->palette) {
+        APT_TRY(dpal.alloc(256 * 256 * sizeof(u32)));
+        const std::vector<u32> packed = pack_palette(ps->palette);
+        APT_CUDA(cudaMemcpy(dpal.p, packed.data(), packed.size() * sizeof(u32), cudaMemcpyHostToDevice));
+    }
+    ProcessLaunch a{};
+    a.rows = dx.as<float>();
+    a.result = nullptr;
+    a.fixed_rows = a.max_rows = static_cast<u32>(nrows);
+    a.contrast = ps->contrast;
+    a.percent = ps->percent;
+    a.rotate = ps->rotate != 0;
+    a.rgba = ps->rgba != 0;
+    a.palette = ps->palette ? dpal.as<u32>() : nullptr;
+    memcpy(a.tune, ps->tune, sizeof(a.tune));
+    a.ctl = dctl.as<PostCtl>();
+    a.tel_a = dtel.as<float>();
+    a.tel_b = a.tel_a + nrows;
+    a.tel_v = a.tel_a + 2 * nrows;
+    a.proc = dproc.as<ProcCtl>();
+    a.grey = dgrey.as<unsigned char>();
+    a.out = dout.p;
+    APT_TRY(launch_process_stage(stage_ctx(), a, nullptr));
+    APT_CUDA(cudaDeviceSynchronize());
+    PostCtl pc;
+    APT_CUDA(cudaMemcpy(&pc, dctl.p, offsetof(PostCtl, buckets), cudaMemcpyDeviceToHost));
+    if (pc.status == 3) return fail(APT_ERR_TOO_SHORT, "Recording too short for telemetry decoding");
+    if (pc.status != 0) return fail(APT_ERR_BAD_ARG, "image stage failed (status %u)", pc.status);
+    APT_CUDA(cudaMemcpy(out, dout.p, bytes, cudaMemcpyDeviceToHost));
+    if (info) {
+        info->low = pc.low;
+        info->high = pc.high;
+        info->rows = nrows;
+        info->telemetry_row = pc.telemetry_row;
+        memcpy(info->wedges_a, pc.wedges_a, sizeof(info->wedges_a));
+        memcpy(info->wedges_b, pc.wedges_b, sizeof(info->wedges_b));
+    }
+    *nout = bytes;
+    return APT_OK;
 }
 
 // ======================================================================= resample tool (WAV -> WAV)
@@ -1325,6 +1490,7 @@ extern "C" int apt_decode_batch(const void *const *signals, int format, const ui
                         d->stager = decs[0]->stager;
                     }
                     d->image_contrast = -1;
+                    d->proc_active = false;
                     decs.push_back(d);
                     job_of.push_back(-1);
                 }

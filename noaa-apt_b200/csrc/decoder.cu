@@ -102,29 +102,34 @@ uint64_t plan_out_bound(const Plan &p, uint64_t n) {
 
 // ---------------------------------------------------------------------------------- helpers
 
+int prof_begin(apt_decoder *d, const char *name) {
+    d->launches++;
+    if (!d->profiling) return -1;
+    const int slot = d->ev_used++;
+    if (slot >= static_cast<int>(d->ev_begin.size())) {
+        cudaEvent_t a, b;
+        cudaEventCreate(&a);
+        cudaEventCreate(&b);
+        d->ev_begin.push_back(a);
+        d->ev_end.push_back(b);
+        d->kernel_names.emplace_back();
+    }
+    d->kernel_names[slot] = name;
+    cudaEventRecord(d->ev_begin[slot], d->stream);
+    return slot;
+}
+
+void prof_end(apt_decoder *d, int slot) {
+    if (slot >= 0) cudaEventRecord(d->ev_end[slot], d->stream);
+}
+
 namespace {
 
 struct Prof {
     apt_decoder *d;
     int slot;
-    Prof(apt_decoder *dec, const char *name) : d(dec), slot(-1) {
-        d->launches++;
-        if (!d->profiling) return;
-        slot = d->ev_used++;
-        if (slot >= static_cast<int>(d->ev_begin.size())) {
-            cudaEvent_t a, b;
-            cudaEventCreate(&a);
-            cudaEventCreate(&b);
-            d->ev_begin.push_back(a);
-            d->ev_end.push_back(b);
-            d->kernel_names.emplace_back();
-        }
-        d->kernel_names[slot] = name;
-        cudaEventRecord(d->ev_begin[slot], d->stream);
-    }
-    ~Prof() {
-        if (slot >= 0) cudaEventRecord(d->ev_end[slot], d->stream);
-    }
+    Prof(apt_decoder *dec, const char *name) : d(dec), slot(prof_begin(dec, name)) {}
+    ~Prof() { prof_end(d, slot); }
 };
 
 }  // namespace

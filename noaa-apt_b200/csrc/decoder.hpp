@@ -57,6 +57,11 @@ uint64_t plan_work_len(const Plan &p, uint64_t n);
 // decode() output length for no-sync / upper bound for sync.
 uint64_t plan_out_bound(const Plan &p, uint64_t n);
 
+// Kernel accounting of a decoder: counts the launch and, when profiling, records the begin event of slot `name`;
+// returns the slot to close with prof_end (-1: none).
+int prof_begin(apt_decoder *d, const char *name);
+void prof_end(apt_decoder *d, int slot);
+
 }  // namespace aptb200
 
 struct apt_decoder {
@@ -122,8 +127,17 @@ struct apt_decoder {
     aptb200::PostCtl *d_post = nullptr, *h_post = nullptr;   // device block; pinned copy of its head for the host
     float *d_tel = nullptr;        // 3 * max_rows floats: telemetry band means and variance per row
     unsigned char *d_out8 = nullptr;
+    uint64_t out8_bytes = 0;       // size of d_out8 (max_out, or 4 * max_out once an RGBA process job ran)
     bool job_image = false;
     apt_image_info last_image{};
+    // process mode (apt_decoder_set_process_mode): the image stage is the whole of process() but the map overlay
+    bool proc_active = false;
+    apt_process_settings proc{};   // palette field unused: the palette lives in d_palette
+    bool proc_palette = false;
+    aptb200::u32 *d_palette = nullptr;      // 256*256 packed RGBA
+    aptb200::ProcCtl *d_proc = nullptr;
+    unsigned char *d_grey = nullptr;        // max_out B intermediate grey plane
+    uint64_t job_bpp = 1;          // output bytes per pixel of the image job in flight
 
     // job in flight
     bool in_flight = false;

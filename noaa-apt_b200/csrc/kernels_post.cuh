@@ -5,7 +5,10 @@
 //   misc::percent (1000-bucket histogram)       misc.rs:119-175
 //   telemetry::read_telemetry / from_bands      telemetry.rs:125-243, :30-66
 //   noaa_apt::map_signal_u8                     noaa_apt.rs:249-259
-// Given the same f32 rows these kernels reproduce the reference's u8 image and contrast bounds bit for bit.
+//   grey histogram equalisation                 processing.rs:87-103, imageext.rs:23-46, :95-119
+//   processing::false_color                     processing.rs:108-157
+//   processing::rotate (Rotate::Yes)            processing.rs:21-37
+// Given the same f32 rows these kernels reproduce the reference's u8 / RGBA image and contrast bounds bit for bit.
 #pragma once
 
 #include <cstdint>
@@ -248,6 +251,136 @@ k_post_map_u8(const float *__restrict__ rows, const SyncResult *__restrict__ res
     } else {
         for (u64 i = static_cast<u64>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<u64>(gridDim.x) * blockDim.x)
             out[i] = map_u8(rows[i], low, range);
+    }
+}
+
+// ------------------------------------------------ the rest of noaa_apt::process (noaa_apt.rs:140-240), map overlay excepted
+// Column layout, decode.rs:16-35: channel A is x in [0, 1040), B is x in [1040, 2080); the image data of a channel is its
+// columns [86, 995) (sync 39 px + space 47 px in front, telemetry 45 px behind).
+constexpr u32 kProcRowPx = 2080, kProcChannelPx = 1040, kProcImageX0 = 86, kProcImageEnd = 995;
+
+// map_signal_u8 (as k_post_map_u8) and, in the same pass, the grey-value histogram of each channel half for
+// Contrast::Histogram (imageext.rs:95-119).  Counts are privatised per warp in shared memory.  APT images have long runs
+// of one value (sync bars, the space band, telemetry wedges, pixels clipped at 0 / 255), so lanes holding the same
+// (channel, value) are first merged with __match_any_sync: a run costs one shared atomic per warp, not one per lane.
+// Rows of 2080 px and 16-byte aligned rows / 4-byte aligned output (the launcher checks): every float4 lies in one channel.
+__global__ void __launch_bounds__(256)
+k_post_map_u8_hist(const float *__restrict__ rows, const SyncResult *__restrict__ result, u32 fixed_rows,
+                   const PostCtl *__restrict__ ctl, unsigned char *__restrict__ out, ProcCtl *__restrict__ proc) {
+    __shared__ u32 s_h[8][512];
+    for (u32 i = threadIdx.x; i < 8 * 512; i += blockDim.x) (&s_h[0][0])[i] = 0u;
+    __syncthreads();
+    const u32 lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    u32 *h = s_h[warp];
+    const u64 n4 = static_cast<u64>(post_rows(ctl, result, fixed_rows)) * (kProcRowPx / 4);
+    const float low = ctl->low, range = __fsub_rn(ctl->high, low);
+    const u64 stride = static_cast<u64>(gridDim.x) * blockDim.x;
+    // the loop bound is per warp, so that every lane reaches the __match_any_sync calls
+    for (u64 base = static_cast<u64>(blockIdx.x) * blockDim.x + (warp << 5); base < n4; base += stride) {
+        const u64 i = base + lane;
+        u32 key[4] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
+        if (i < n4) {
+            const float4 v = reinterpret_cast<const float4 *>(rows)[i];
+            uchar4 o;
+            o.x = map_u8(v.x, low, range); o.y = map_u8(v.y, low, range); o.z = map_u8(v.z, low, range); o.w = map_u8(v.w, low, range);
+            reinterpret_cast<uchar4 *>(out)[i] = o;
+            const u32 ch = static_cast<u32>(i % (kProcRowPx / 4)) >= kProcChannelPx / 4 ? 256u : 0u;
+            key[0] = ch + o.x; key[1] = ch + o.y; key[2] = ch + o.z; key[3] = ch + o.w;
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const u32 peers = __match_any_sync(0xffffffffu, key[j]);
+            if (key[j] != 0xFFFFFFFFu && lane == static_cast<u32>(__ffs(peers) - 1)) atomicAdd(&h[key[j]], static_cast<u32>(__popc(peers)));
+        }
+    }
+    __syncthreads();
+    for (u32 b = threadIdx.x; b < 512; b += blockDim.x) {
+        u32 s = 0;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) s += s_h[w][b];
+        if (s) atomicAdd(&proc->hist[0][0] + b, s);
+    }
+}
+
+// imageext.rs:23-46, :95-119 for both channel halves: cumulative u32 histogram, total = hist[255] as f32, and
+// v -> (255.0 * (hist[v] as f32 / total)) as u8.  The u32 -> f32 conversions round to nearest (they are inexact above 2^24
+// pixels per half, about 16 000 rows); `as u8` truncates and saturates (NaN -> 0).  One CTA, one thread per (channel, value).
+__global__ void __launch_bounds__(512)
+k_post_eq_lut(ProcCtl *__restrict__ proc) {
+    __shared__ u32 s[512];
+    const u32 t = threadIdx.x, bin = t & 255u;
+    s[t] = (&proc->hist[0][0])[t];
+    __syncthreads();
+    for (u32 o = 1; o < 256; o <<= 1) {
+        const u32 v = bin >= o ? s[t - o] : 0u;
+        __syncthreads();
+        s[t] += v;
+        __syncthreads();
+    }
+    const float total = __uint2float_rn(s[t | 255u]);
+    const float v = __fmul_rn(255.f, __fdiv_rn(__uint2float_rn(s[t]), total));
+    (&proc->lut[0][0])[t] = !(v >= 0.f) ? 0 : (v >= 255.f ? 255 : static_cast<unsigned char>(static_cast<u32>(v)));
+}
+
+// processing.rs:125-140 tune_input_values for one channel: (in * ((1 + e) - s) - s * 255).clamp(0, 255) as u32 with
+// s = start * 0.3, e = end * 0.3, every f32 operation rounded on its own (no FMA).
+__device__ __forceinline__ unsigned char tune_value(u32 in, float start, float end) {
+    const float s = __fmul_rn(start, 0.3f), e = __fmul_rn(end, 0.3f);
+    const float o = __fsub_rn(__fmul_rn(static_cast<float>(in), __fsub_rn(__fadd_rn(1.f, e), s)), __fmul_rn(s, 255.f));
+    return !(o >= 0.f) ? 0 : (o >= 255.f ? 255 : static_cast<unsigned char>(static_cast<u32>(o)));   // f32::clamp keeps NaN; `as u32` -> 0
+}
+
+// The finishing pass over the grey plane: rotation (processing.rs:21-37, Rotate::Yes) as a gather of source coordinates
+// -- (x0 + i, y) <- (x0 + 908 - i, rows - 1 - y) inside the two 909-px image rectangles -- then
+//   mode 0  the grey value
+//   mode 1  the equalisation table of the pixel's channel half (Contrast::Histogram)
+//   mode 2  false colour (processing.rs:108-157): in channel A's image columns palette[val_b][val_a] with the tuned values
+//           of a = grey(x, y) and b = grey(x + 1040, y); everywhere else the grey value
+// and writes grey (1 B/px, 4-byte stores) or RGBA (R = G = B = grey, A = 255 outside the colour region; 16-byte stores).
+// One thread per 4 consecutive output pixels of a row.  Both per-value tables (equalisation, or the two tune maps) sit in
+// shared memory; the palette, 256 KB packed as u32, is read through the read-only path (__ldg, L1 / L2).
+template <bool RGBA>
+__global__ void __launch_bounds__(256)
+k_post_finish(const unsigned char *__restrict__ grey, const PostCtl *__restrict__ ctl, const ProcCtl *__restrict__ proc, int mode,
+              int rotate, const u32 *__restrict__ palette, float4 tune, void *__restrict__ out) {
+    __shared__ unsigned char s_tab[2][256];
+    for (u32 i = threadIdx.x; i < 512; i += blockDim.x) {
+        const u32 ch = i >> 8, v = i & 255u;
+        unsigned char t = static_cast<unsigned char>(v);
+        if (mode == 1) t = proc->lut[ch][v];
+        else if (mode == 2) t = ch == 0 ? tune_value(v, tune.x, tune.y) : tune_value(v, tune.z, tune.w);
+        s_tab[ch][v] = t;
+    }
+    __syncthreads();
+    const u32 rows = ctl->rows;
+    const u64 nq = static_cast<u64>(rows) * (kProcRowPx / 4);
+    for (u64 q = static_cast<u64>(blockIdx.x) * blockDim.x + threadIdx.x; q < nq; q += static_cast<u64>(gridDim.x) * blockDim.x) {
+        const u32 y = static_cast<u32>(q / (kProcRowPx / 4));
+        const u32 x0 = static_cast<u32>(q % (kProcRowPx / 4)) * 4;
+        u32 px[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const u32 x = x0 + k;
+            const u32 chb = x >= kProcChannelPx ? 1u : 0u;
+            const u32 xc = x - chb * kProcChannelPx;                          // column within the channel
+            const bool img = xc >= kProcImageX0 && xc < kProcImageEnd;
+            u32 sx = x, sy = y;
+            if (rotate && img) {
+                sx = x - xc + (kProcImageX0 + kProcImageEnd - 1) - xc;        // x0 + 908 - i
+                sy = rows - 1 - y;
+            }
+            const unsigned char *line = grey + static_cast<u64>(sy) * kProcRowPx;
+            const u32 g = line[sx];
+            if (RGBA && mode == 2 && img && !chb) {
+                const u32 b = line[sx + kProcChannelPx];
+                px[k] = __ldg(palette + (static_cast<u32>(s_tab[1][b]) << 8) + s_tab[0][g]);
+            } else {
+                const u32 v = mode == 1 ? s_tab[chb][g] : g;
+                px[k] = RGBA ? (v * 0x010101u) | 0xFF000000u : v;
+            }
+        }
+        if (RGBA) reinterpret_cast<uint4 *>(out)[q] = make_uint4(px[0], px[1], px[2], px[3]);
+        else reinterpret_cast<u32 *>(out)[q] = px[0] | (px[1] << 8) | (px[2] << 16) | (px[3] << 24);
     }
 }
 

@@ -54,6 +54,11 @@ struct PostCtl {
     float wedges_a[16], wedges_b[16];
     u32 buckets[1000];       // misc::percent histogram
 };
+// Histogram equalisation of the process stage (kernels_post.cuh); hist is zeroed before each histogram-mode job.
+struct ProcCtl {
+    u32 hist[2][256];              // grey-value counts of channel A (x < 1040) and channel B
+    unsigned char lut[2][256];     // equalised value of each grey value, per channel
+};
 
 // Where the picker finds the roots: per block of `block` positions an ascending list.
 struct RootIndex {
@@ -202,6 +207,31 @@ int launch_gather(const LaunchCtx &c, const float *f, const u32 *positions, cons
 int launch_image_stage(const LaunchCtx &c, const float *rows, const SyncResult *result, u32 fixed_rows, u32 max_rows, u32 px,
                        int contrast, float percent, PostCtl *ctl, float *tel_a, float *tel_b, float *tel_v,
                        const float *bounds_dev, unsigned char *out, bool stats_only);
+
+// Called around every kernel of a stage (profiling events and launch counting of a decoder).
+struct KernelHook {
+    virtual void begin(const char *name) = 0;
+    virtual void end() = 0;
+};
+
+// The rest of noaa_apt::process (kernels_post.cuh, aptb200.h apt_process_settings) on rows of 2080 pixels.  All pointers are
+// device pointers; rows counted by `result` (sync decode) or fixed_rows, as in launch_image_stage.
+struct ProcessLaunch {
+    const float *rows;
+    const SyncResult *result;
+    u32 fixed_rows, max_rows;
+    int contrast;                  // apt_contrast, APT_CONTRAST_HISTOGRAM included
+    float percent;
+    bool rotate, rgba;
+    const u32 *palette;            // 256*256 packed RGBA (R in the low byte, alpha 255), row = channel B value; nullptr: none
+    float tune[4];
+    PostCtl *ctl;
+    float *tel_a, *tel_b, *tel_v;  // per-row scratch, max_rows floats each
+    ProcCtl *proc;                 // histograms + equalisation table (histogram mode)
+    unsigned char *grey;           // max_rows * 2080 B intermediate grey plane (unused when the output is that plane)
+    void *out;                     // max_rows * 2080 * (rgba ? 4 : 1) B
+};
+int launch_process_stage(const LaunchCtx &c, const ProcessLaunch &a, KernelHook *hook);
 
 // wav.rs:71-85: normalise by the maximum and quantise to i16 (x, out: device; ctl: scratch control block).
 int launch_quantize_i16(const LaunchCtx &c, const float *x, u64 n, PostCtl *ctl, short *out);

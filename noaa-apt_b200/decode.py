@@ -97,6 +97,7 @@ class Decoder:
         raise_for(self._lib.apt_decoder_create(self.device, self.input_rate, C.byref(s), self.max_samples, C.byref(h)))
         self._h = h
         self._keep = None
+        self._bpp = None       # bytes per pixel of the process mode's image; None: f32 rows
 
     def close(self):
         if getattr(self, "_h", None):
@@ -121,12 +122,35 @@ class Decoder:
     def submit_host_ptr(self, signal_ptr, fmt, n, sync, out_ptr, cap):
         raise_for(self._lib.apt_decoder_submit_host(self._h, signal_ptr, fmt, n, int(bool(sync)), out_ptr, cap))
 
+    # --- process mode (image.process on every job) ---
+    def set_process_mode(self, contrast=None, percent=0.98, rotate=False, palette=None, tune=(0, 0, 0, 0), rgba=None):
+        """contrast=None: back to f32 rows.  Otherwise the numpy submit()/wait()/decode() return the image of
+        image.process: (rows, 2080) u8 grey or (rows, 2080, 4) u8 RGBA; image_info() gives the contrast info."""
+        from . import image
+        if contrast is None:
+            raise_for(self._lib.apt_decoder_set_process_mode(self._h, None))
+            self._bpp = None
+            return
+        ps, bpp, _pal = image.process_settings(contrast, percent, rotate, palette, tune, rgba)
+        raise_for(self._lib.apt_decoder_set_process_mode(self._h, C.byref(ps)))   # the palette is copied here
+        self._bpp = bpp
+
+    def image_info(self):
+        from . import image
+        ci = _lib.CImageInfo()
+        raise_for(self._lib.apt_decoder_image_info(self._h, C.byref(ci)))
+        return image._info(ci)
+
     # --- numpy interface ---
     def submit(self, signal, sync=True, out=None):
         x = np.ascontiguousarray(signal)
         fmt = _fmt_of(x)
+        bpp = self._bpp
         if out is None:
-            out = np.empty(max(self.out_bound(x.size), 1), dtype=np.float32)
+            if bpp:
+                out = np.empty(max(self.out_bound(x.size) * bpp, 1), dtype=np.uint8)
+            else:
+                out = np.empty(max(self.out_bound(x.size), 1), dtype=np.float32)
         self._keep = (x, out)
         self.submit_host_ptr(x.ctypes.data, fmt, x.size, sync, out.ctypes.data, out.size)
         return out
@@ -137,6 +161,10 @@ class Decoder:
         keep, self._keep = self._keep, None
         raise_for(st)
         if keep is not None:
+            bpp = self._bpp
+            if bpp:
+                flat = keep[1][: n.value]
+                return flat.reshape(-1, PX_PER_ROW, 4) if bpp == 4 else flat.reshape(-1, PX_PER_ROW)
             return keep[1][: n.value]
         return n.value
 

@@ -1,15 +1,90 @@
-"""The front of noaa_apt::process (noaa_apt.rs:132-190) on the device: contrast bounds (MinMax / misc::percent /
-telemetry wedges) and map_signal_u8 -- the decoded rows become the u8 image before they leave the GPU."""
+"""noaa_apt::process (noaa_apt.rs:132-240) on the device, the map overlay excepted: contrast bounds (MinMax /
+misc::percent / telemetry wedges), map_signal_u8, false colour, grey histogram equalisation and rotation -- the decoded
+rows become the finished image before they leave the GPU."""
 import ctypes as C
 
 import numpy as np
 
 from . import _lib
 from .config import Settings
-from .err import raise_for
+from .err import InvalidInput, raise_for
 from .frequency import _rate_hz
 
-MINMAX, PERCENT, TELEMETRY = _lib.CONTRAST_MINMAX, _lib.CONTRAST_PERCENT, _lib.CONTRAST_TELEMETRY
+MINMAX, PERCENT, TELEMETRY, HISTOGRAM = (_lib.CONTRAST_MINMAX, _lib.CONTRAST_PERCENT, _lib.CONTRAST_TELEMETRY,
+                                         _lib.CONTRAST_HISTOGRAM)
+
+
+def load_palette(path):
+    """A false-colour palette image as (256, 256, 3) u8 RGB: the image crate's into_rgb8 drops alpha, and any size but
+    256x256 is InvalidInput (processing.rs:110-116)."""
+    from PIL import Image
+    with Image.open(path) as im:
+        rgb = np.asarray(im.convert("RGB"), dtype=np.uint8)
+    if rgb.shape != (256, 256, 3):
+        raise InvalidInput(_lib.ERR_BAD_ARG, "Invalid palette image dimensions")
+    return np.ascontiguousarray(rgb)
+
+
+def process_settings(contrast, percent=0.98, rotate=False, palette=None, tune=(0, 0, 0, 0), rgba=None):
+    """(apt_process_settings, bytes per pixel, palette array to keep alive).  rgba=None: RGBA with a palette, else grey."""
+    pal = None
+    if palette is not None:
+        pal = np.ascontiguousarray(palette, dtype=np.uint8)
+        if pal.shape != (256, 256, 3):
+            raise InvalidInput(_lib.ERR_BAD_ARG, "Invalid palette image dimensions")
+    if rgba is None:
+        rgba = pal is not None
+    ps = _lib.CProcessSettings()
+    ps.contrast = int(contrast)
+    ps.percent = float(percent)
+    ps.rotate = int(bool(rotate))
+    ps.palette = pal.ctypes.data if pal is not None else None
+    ps.tune = (C.c_float * 4)(*[float(t) for t in tune])
+    ps.rgba = int(bool(rgba))
+    return ps, (4 if rgba else 1), pal
+
+
+def _shape(flat, bpp):
+    return flat.reshape(-1, 2080, 4) if bpp == 4 else flat.reshape(-1, 2080)
+
+
+def process(rows, contrast, percent=0.98, rotate=False, palette=None, tune=(0, 0, 0, 0), rgba=None):
+    """The image process() returns for decode()'s rows (noaa_apt.rs:140-240 without the map): (rows, 2080) u8 grey or
+    (rows, 2080, 4) u8 RGBA, plus the contrast info."""
+    x = np.ascontiguousarray(rows, dtype=np.float32).ravel()
+    ps, bpp, _pal = process_settings(contrast, percent, rotate, palette, tune, rgba)
+    out = np.empty(max(x.size * bpp, 1), dtype=np.uint8)
+    n = C.c_uint64(0)
+    ci = _lib.CImageInfo()
+    raise_for(_lib.load().apt_process(x.ctypes.data, x.size, C.byref(ps), out.ctypes.data, out.size, C.byref(n), C.byref(ci)))
+    return _shape(out[: n.value], bpp), _info(ci)
+
+
+def decode_image(context, settings, signal, input_rate, sync=True, contrast=MINMAX, percent=0.98, rotate=False,
+                 palette=None, tune=(0, 0, 0, 0), rgba=None):
+    """decode() + process() in one call -> (image of shape (rows, 2080) or (rows, 2080, 4), info)."""
+    lib = _lib.load()
+    x = np.ascontiguousarray(signal)
+    fmt = _lib.PCM16 if x.dtype == np.int16 else _lib.F32
+    if fmt == _lib.F32:
+        x = np.ascontiguousarray(x, dtype=np.float32)
+    ps, bpp, _pal = process_settings(contrast, percent, rotate, palette, tune, rgba)
+    s = (settings or Settings()).to_c()
+    rate = _rate_hz(input_rate)
+    bound = C.c_uint64(0)
+    raise_for(lib.apt_decode_len_bound(x.size, rate, C.byref(s), C.byref(bound)))
+    out = np.empty(max(bound.value * bpp, 1), dtype=np.uint8)
+    n = C.c_uint64(0)
+    ci = _lib.CImageInfo()
+
+    def _cb(progress, desc, _user):
+        if context is not None:
+            context.status(progress, desc.decode())
+
+    cb = _lib.STATUS_CB(_cb)
+    raise_for(lib.apt_decode_image(x.ctypes.data, fmt, x.size, rate, C.byref(s), int(bool(sync)), C.byref(ps),
+                                   out.ctypes.data, out.size, C.byref(n), C.byref(ci), cb, None))
+    return _shape(out[: n.value].copy(), bpp), _info(ci)
 
 
 def _info(ci):

@@ -81,6 +81,13 @@ extern "C" {
                                info: *mut apt_image_info) -> c_int;
     pub fn apt_telemetry_rows(signal: *const c_float, n: u64, mean_a: *mut c_float, mean_b: *mut c_float,
                               variance: *mut c_float) -> c_int;
+
+    // the rest of noaa_apt::process (false colour, histogram equalisation, rotation), map overlay excepted
+    pub fn apt_process(rows: *const c_float, n: u64, ps: *const apt_process_settings, out: *mut u8, cap: u64, nout: *mut u64,
+                       info: *mut apt_image_info) -> c_int;
+    pub fn apt_decode_image(signal: *const c_void, format: c_int, n: u64, input_rate: u32, s: *const apt_settings, sync: c_int,
+                            ps: *const apt_process_settings, out: *mut u8, cap: u64, nout: *mut u64, info: *mut apt_image_info,
+                            cb: apt_status_cb, user: *mut c_void) -> c_int;
 }
 
 pub const APT_F32: c_int = 0;
@@ -88,6 +95,7 @@ pub const APT_PCM16: c_int = 1;
 pub const APT_CONTRAST_MINMAX: c_int = 0;
 pub const APT_CONTRAST_PERCENT: c_int = 1;
 pub const APT_CONTRAST_TELEMETRY: c_int = 2;
+pub const APT_CONTRAST_HISTOGRAM: c_int = 3;
 pub const APT_ERR_IO: c_int = 11;
 
 #[repr(C)]
@@ -98,3 +106,8 @@ pub struct apt_wav_info { pub sample_rate: u32, pub channels: u32, pub bits_per_
 #[derive(Default, Clone, Copy)]
 pub struct apt_image_info { pub low: f32, pub high: f32, pub rows: u64, pub telemetry_row: u64,
                             pub wedges_a: [f32; 16], pub wedges_b: [f32; 16] }
+
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct apt_process_settings { pub contrast: c_int, pub percent: c_float, pub rotate: c_int,
+                                  pub palette: *const u8 /* 256*256*3 RGB or null */, pub tune: [c_float; 4], pub rgba: c_int }
