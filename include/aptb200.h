@@ -381,6 +381,55 @@ int apt_decode_batch(const void *const *signals, int format, const uint64_t *len
                      float *const *outs, const uint64_t *caps, uint64_t *nouts, int *statuses,
                      const int *devices, int ndevices, int streams_per_device);
 
+/* ------------------------------------------------------------------ streaming decoder */
+
+/* Live decoding: push audio as it arrives, get finished image rows back.
+ *
+ * The rows returned by the pushes plus apt_stream_finish, concatenated, are bit-identical to apt_decode /
+ * apt_decode_pcm16 on the whole recording with the same settings and `sync`, however the recording is split into pushes
+ * (any sizes, f32 and PCM16 mixed).  After finish, apt_stream_sync_positions equals apt_decoder_last_sync.  finish returns
+ * the status apt_decode would return (APT_ERR_TOO_SHORT, APT_ERR_FEW_SYNC_FRAMES); the rows already returned are then
+ * not an image apt_decode would produce and the caller discards them.
+ *
+ * Emission rule: rows leave as soon as they are final, within `latency_work` work-rate samples.  With sync, after a push
+ * every row k with max(p_k + row, p_{k+1} + G) + latency_work <= work_final has been returned (p_k: sync position k,
+ * row: samples per row, G: template length); without sync, every row r with (r+1)*row + latency_work <= work_final.
+ *
+ * All device memory is allocated by apt_stream_create and depends only on (input_rate, settings, max_push); push and
+ * finish allocate nothing.  Pushes are synchronous (the rows are in `rows` on return) and take pageable host pointers;
+ * pushes larger than max_push are split into steps of max_push samples.  Supported: the standard, fast and slow
+ * profiles (any settings whose demodulation low-pass has 37, 43 or 61 taps) at every input rate apt_decode accepts,
+ * with a work rate that is a multiple of 4160.  sync with another work rate fails with APT_ERR_WORK_RATE, sync = 0
+ * with APT_ERR_BAD_ARG. */
+typedef struct apt_stream apt_stream;
+typedef struct apt_stream_info {
+    uint64_t samples_in;      /* input samples pushed so far */
+    uint64_t work_final;      /* envelope samples that no later input can change */
+    uint64_t rows_out;        /* rows returned so far */
+    uint64_t peaks;           /* sync positions decided so far */
+    uint64_t latency_work;    /* slack of the emission rule, in work-rate samples (constant per stream) */
+    uint64_t max_push;        /* samples one internal step takes; larger pushes are split */
+    uint64_t device_bytes;    /* device memory the stream owns (constant from create to destroy) */
+} apt_stream_info;
+
+int apt_stream_create(int device, uint32_t input_rate, const apt_settings *s, int sync, uint64_t max_push, apt_stream **st);
+void apt_stream_destroy(apt_stream *st);
+/* rows * 2080: the floats one push of n samples can return at most (the `cap` that push needs). */
+int apt_stream_push_bound(apt_stream *st, uint64_t n, uint64_t *cap_floats);
+/* format: APT_F32 or APT_PCM16.  APT_ERR_CAPACITY (cap below apt_stream_push_bound) leaves the stream unchanged, so the
+ * push can be retried.  A push after finish (before reset), or one that takes the work-rate index past 2^32 - 1, is
+ * APT_ERR_BAD_ARG. */
+int apt_stream_push(apt_stream *st, const void *samples, int format, uint64_t n, float *rows, uint64_t cap, uint64_t *nout);
+/* End of the recording: the remaining rows (cap: apt_stream_push_bound(st, 0)) and the status of the whole decode. */
+int apt_stream_finish(apt_stream *st, float *rows, uint64_t cap, uint64_t *nout);
+/* Start a new recording with the same plan and buffers. */
+int apt_stream_reset(apt_stream *st);
+/* Sync positions decided so far (positions == NULL: count only; APT_ERR_CAPACITY when cap is too small). */
+int apt_stream_sync_positions(apt_stream *st, uint64_t *positions, size_t cap, size_t *n);
+int apt_stream_get_info(apt_stream *st, apt_stream_info *info);
+/* Host only, no device: the geometry a stream of these parameters would have (latency_work, max_push, device_bytes). */
+int apt_stream_geometry(uint32_t input_rate, const apt_settings *s, int sync, uint64_t max_push, apt_stream_info *info);
+
 #ifdef __cplusplus
 }
 #endif

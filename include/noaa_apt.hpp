@@ -200,4 +200,49 @@ inline std::vector<uint64_t> find_sync(Context &, const Signal &signal, Rate wor
     return pos;
 }
 
+// Live decoding (apt_stream_*): push audio as it arrives, get the rows that became final.  The rows of all pushes plus
+// finish() equal decode() on the whole recording bit for bit.  Owns the device memory from construction to destruction.
+class Stream {
+  public:
+    Stream(Rate input_rate, const config::Settings &settings, bool sync = true, uint64_t max_push = 48000, int device = 0) {
+        const apt_settings s = settings.to_c();
+        err::check(apt_stream_create(device, input_rate.get_hz(), &s, sync ? 1 : 0, max_push, &st_));
+    }
+    ~Stream() { apt_stream_destroy(st_); }
+    Stream(const Stream &) = delete;
+    Stream &operator=(const Stream &) = delete;
+
+    Signal push(const float *samples, size_t n) { return rows(n, [&](float *o, uint64_t c, uint64_t *k) {
+        return apt_stream_push(st_, samples, APT_F32, n, o, c, k); }); }
+    Signal push(const int16_t *samples, size_t n) { return rows(n, [&](float *o, uint64_t c, uint64_t *k) {
+        return apt_stream_push(st_, samples, APT_PCM16, n, o, c, k); }); }
+    Signal push(const Signal &samples) { return push(samples.data(), samples.size()); }
+    Signal finish() { return rows(0, [&](float *o, uint64_t c, uint64_t *k) { return apt_stream_finish(st_, o, c, k); }); }
+    void reset() { err::check(apt_stream_reset(st_)); }
+    std::vector<uint64_t> positions() const {
+        size_t n = 0;
+        err::check(apt_stream_sync_positions(st_, nullptr, 0, &n));
+        std::vector<uint64_t> pos(n);
+        if (n) err::check(apt_stream_sync_positions(st_, pos.data(), pos.size(), &n));
+        return pos;
+    }
+    apt_stream_info info() const {
+        apt_stream_info i{};
+        err::check(apt_stream_get_info(st_, &i));
+        return i;
+    }
+
+  private:
+    template <typename F>
+    Signal rows(uint64_t n, F call) {
+        uint64_t cap = 0, got = 0;
+        err::check(apt_stream_push_bound(st_, n, &cap));
+        Signal out(cap ? cap : 1);
+        err::check(call(out.data(), out.size(), &got));
+        out.resize(got);
+        return out;
+    }
+    apt_stream *st_ = nullptr;
+};
+
 }  // namespace noaa_apt

@@ -14,11 +14,12 @@ from . import _lib, config, context, dsp, err, filters, frequency, image, wav  #
 from . import decode as _decode_mod
 from .config import Settings
 from .context import Context
-from .decode import (CARRIER_FREQ, FINAL_RATE, PX_PER_ROW, Decoder, decode, decode_batch, decode_len_bound,
-                     find_sync, generate_sync_frame)
+from .decode import (CARRIER_FREQ, FINAL_RATE, PX_PER_ROW, Decoder, Stream, decode, decode_batch, decode_len_bound,
+                     find_sync, generate_sync_frame, stream_geometry)
 from .frequency import Freq, Rate
 
-__all__ = ["decode", "decode_batch", "decode_len_bound", "find_sync", "generate_sync_frame", "Decoder",
+__all__ = ["decode", "decode_batch", "decode_len_bound", "find_sync", "generate_sync_frame", "Decoder", "Stream",
+           "stream_geometry",
            "Settings", "Context", "Freq", "Rate", "dsp", "filters", "err", "config", "frequency", "image", "wav",
            "FINAL_RATE", "PX_PER_ROW", "CARRIER_FREQ"]
 

@@ -79,6 +79,11 @@ class CPhInfo(C.Structure):
     _fields_ = [(n, C.c_uint32) for n in ("usable", "l", "m", "j", "jpad", "pitch", "row_len", "smem_bytes")]
 
 
+class CStreamInfo(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("samples_in", "work_final", "rows_out", "peaks", "latency_work", "max_push",
+                                          "device_bytes")]
+
+
 STATUS_CB = C.CFUNCTYPE(None, C.c_float, C.c_char_p, C.c_void_p)
 
 # name -> (restype, argtypes); every symbol include/aptb200.h declares.
@@ -162,6 +167,15 @@ SIGNATURES = {
     "apt_decode_batch": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, _u64p, C.c_int, C.c_uint32, C.POINTER(CSettings),
                                    C.c_int, C.POINTER(C.c_void_p), _u64p, _u64p, C.POINTER(C.c_int),
                                    C.POINTER(C.c_int), C.c_int, C.c_int]),
+    "apt_stream_create": (C.c_int, [C.c_int, C.c_uint32, C.POINTER(CSettings), C.c_int, C.c_uint64, C.POINTER(C.c_void_p)]),
+    "apt_stream_destroy": (None, [C.c_void_p]),
+    "apt_stream_push_bound": (C.c_int, [C.c_void_p, C.c_uint64, _u64p]),
+    "apt_stream_push": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_uint64, C.c_void_p, C.c_uint64, _u64p]),
+    "apt_stream_finish": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, _u64p]),
+    "apt_stream_reset": (C.c_int, [C.c_void_p]),
+    "apt_stream_sync_positions": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, _szp]),
+    "apt_stream_get_info": (C.c_int, [C.c_void_p, C.POINTER(CStreamInfo)]),
+    "apt_stream_geometry": (C.c_int, [C.c_uint32, C.POINTER(CSettings), C.c_int, C.c_uint64, C.POINTER(CStreamInfo)]),
 }
 
 _lib = None

@@ -67,7 +67,9 @@ LaunchCtx stage_ctx() {
     return LaunchCtx{nullptr, std::max(sms, 1)};
 }
 
-int free_decoder_buffers(apt_decoder *d) {
+}  // namespace
+
+int aptb200::free_decoder_buffers(apt_decoder *d) {
     cudaSetDevice(d->device);
     if (d->stream) cudaStreamSynchronize(d->stream);
     for (void *p : {(void *)d->d_h, (void *)d->d_lp, (void *)d->d_one, (void *)d->d_guard, d->d_in, (void *)d->d_r,
@@ -91,6 +93,8 @@ int free_decoder_buffers(apt_decoder *d) {
     if (d->stream) cudaStreamDestroy(d->stream);
     return APT_OK;
 }
+
+namespace {
 
 // Allocates what find_sync needs for up to max_work work-rate samples: the picker's buffers always, the fused stage's
 // record pool when the plan has one (the legacy f / corr / per-block root lists come on first use: ensure_legacy_sync).
@@ -454,6 +458,40 @@ extern "C" int apt_decode_len_bound(uint64_t n, uint32_t input_rate, const apt_s
     return APT_OK;
 }
 
+namespace aptb200 {
+
+int upload_plan(apt_decoder *d) {
+    const Plan &p = d->plan;
+    const float one = 1.f;
+    APT_CUDA(cudaMalloc(&d->d_h, p.h.size() * sizeof(float)));
+    APT_CUDA(cudaMemcpy(d->d_h, p.h.data(), p.h.size() * sizeof(float), cudaMemcpyHostToDevice));
+    APT_CUDA(cudaMalloc(&d->d_lp, p.lp.size() * sizeof(float)));
+    APT_CUDA(cudaMemcpy(d->d_lp, p.lp.data(), p.lp.size() * sizeof(float), cudaMemcpyHostToDevice));
+    APT_CUDA(cudaMalloc(&d->d_one, sizeof(float)));
+    APT_CUDA(cudaMemcpy(d->d_one, &one, sizeof(float), cudaMemcpyHostToDevice));
+    if (p.ph) {
+        APT_CUDA(cudaMalloc(&d->d_ph_table, p.ph_table.size() * sizeof(float)));
+        APT_CUDA(cudaMemcpy(d->d_ph_table, p.ph_table.data(), p.ph_table.size() * sizeof(float), cudaMemcpyHostToDevice));
+        APT_CUDA(cudaMalloc(&d->d_ph_xs, p.ph_xs.size() * sizeof(unsigned short)));
+        APT_CUDA(cudaMemcpy(d->d_ph_xs, p.ph_xs.data(), p.ph_xs.size() * sizeof(unsigned short), cudaMemcpyHostToDevice));
+    }
+    if (p.tiled) {
+        APT_CUDA(cudaMalloc(&d->d_tile_taps, p.tile_taps.size() * sizeof(float)));
+        APT_CUDA(cudaMemcpy(d->d_tile_taps, p.tile_taps.data(), p.tile_taps.size() * sizeof(float), cudaMemcpyHostToDevice));
+        APT_CUDA(cudaMalloc(&d->d_tile_xs, p.tile_xs.size() * sizeof(u32)));
+        APT_CUDA(cudaMemcpy(d->d_tile_xs, p.tile_xs.data(), p.tile_xs.size() * sizeof(u32), cudaMemcpyHostToDevice));
+    }
+    return APT_OK;
+}
+
+uint64_t plan_table_bytes(const Plan &p) {
+    return (p.h.size() + p.lp.size() + 1) * sizeof(float) +
+           (p.ph ? p.ph_table.size() * sizeof(float) + p.ph_xs.size() * sizeof(unsigned short) : 0) +
+           (p.tiled ? p.tile_taps.size() * sizeof(float) + p.tile_xs.size() * sizeof(u32) : 0);
+}
+
+}  // namespace aptb200
+
 extern "C" int apt_decoder_create(int device, uint32_t input_rate, const apt_settings *s, uint64_t max_samples,
                                   apt_decoder **dec) {
     if (!s || !dec) return fail(APT_ERR_BAD_ARG, "null argument");
@@ -493,25 +531,7 @@ extern "C" int apt_decoder_create(int device, uint32_t input_rate, const apt_set
         return fail(APT_ERR_BAD_ARG, "recording too long: %llu work-rate samples (limit 2^32-1)",
                     (unsigned long long)d->max_work);
 
-    const float one = 1.f;
-    APT_CUDA(cudaMalloc(&d->d_h, p.h.size() * sizeof(float)));
-    APT_CUDA(cudaMemcpy(d->d_h, p.h.data(), p.h.size() * sizeof(float), cudaMemcpyHostToDevice));
-    APT_CUDA(cudaMalloc(&d->d_lp, p.lp.size() * sizeof(float)));
-    APT_CUDA(cudaMemcpy(d->d_lp, p.lp.data(), p.lp.size() * sizeof(float), cudaMemcpyHostToDevice));
-    APT_CUDA(cudaMalloc(&d->d_one, sizeof(float)));
-    APT_CUDA(cudaMemcpy(d->d_one, &one, sizeof(float), cudaMemcpyHostToDevice));
-    if (p.ph) {
-        APT_CUDA(cudaMalloc(&d->d_ph_table, p.ph_table.size() * sizeof(float)));
-        APT_CUDA(cudaMemcpy(d->d_ph_table, p.ph_table.data(), p.ph_table.size() * sizeof(float), cudaMemcpyHostToDevice));
-        APT_CUDA(cudaMalloc(&d->d_ph_xs, p.ph_xs.size() * sizeof(unsigned short)));
-        APT_CUDA(cudaMemcpy(d->d_ph_xs, p.ph_xs.data(), p.ph_xs.size() * sizeof(unsigned short), cudaMemcpyHostToDevice));
-    }
-    if (p.tiled) {
-        APT_CUDA(cudaMalloc(&d->d_tile_taps, p.tile_taps.size() * sizeof(float)));
-        APT_CUDA(cudaMemcpy(d->d_tile_taps, p.tile_taps.data(), p.tile_taps.size() * sizeof(float), cudaMemcpyHostToDevice));
-        APT_CUDA(cudaMalloc(&d->d_tile_xs, p.tile_xs.size() * sizeof(u32)));
-        APT_CUDA(cudaMemcpy(d->d_tile_xs, p.tile_xs.data(), p.tile_xs.size() * sizeof(u32), cudaMemcpyHostToDevice));
-    }
+    APT_TRY(upload_plan(d.get()));
     const size_t work_bytes = std::max<uint64_t>(d->max_work, 1) * sizeof(float);
     if (!p.first_polyphase) APT_CUDA(cudaMalloc(&d->d_r, work_bytes));
     APT_CUDA(cudaMalloc(&d->d_e, work_bytes));

@@ -222,29 +222,73 @@ int materialise_stages(apt_decoder *d) {
 static bool fast_front(const apt_decoder *d) { return d->plan.ut || (d->plan.tiled && d->d_tile_taps); }
 static bool ph_front(const apt_decoder *d) { return d->plan.ph && d->d_ph_table; }
 
+FrontUnits front_units(const Plan &p) {
+    const uint64_t l = p.first.l, m = p.first.m;
+    FrontUnits u;
+    u.tiled = p.ut || p.tiled || p.ph;   // apt_decoder_create uploads the tables of whichever the plan chose
+    if (p.ut) {
+        u.unit_in = static_cast<uint64_t>(p.utp.rb) * m;
+        u.unit_out = static_cast<uint64_t>(p.utp.rb) * l;
+        u.before = p.utp.back;
+        u.after = p.utp.slot_floats - p.utp.back;           // a block's span beyond its first row's first sample
+    } else if (p.ph) {
+        u.unit_in = static_cast<uint64_t>(kPhTilePeriods) * m;              // a tile = 32 periods of m samples
+        u.unit_out = static_cast<uint64_t>(kPhTilePeriods) * l;
+        u.before = m + 4;                                                   // the period in front of the tile (+4 alignment)
+        u.after = static_cast<uint64_t>(kPhTilePeriods - 1) * m + p.php.row_len;
+    } else if (u.tiled) {
+        u.unit_in = static_cast<uint64_t>(p.tile.qt) * p.tile.p_in;
+        u.unit_out = static_cast<uint64_t>(p.tile.qt) * p.tile.p_out;
+        u.before = p.tile.p_in - p.tile_xs.back();       // halo row: window of the last group one super-period back
+        u.after = static_cast<uint64_t>(p.tile.qt - 1) * p.tile.p_in + p.tile.row_len;
+    } else {
+        u.unit_out = 1;                                  // one output of the generic kernel (or of filter + decimate)
+    }
+    return u;
+}
+
+void front_span(const Plan &p, const FrontUnits &fu, uint64_t u0, uint64_t u1, uint64_t n, uint64_t &xa, uint64_t &xb) {
+    const uint64_t l = p.first.l, m = p.first.m;
+    if (!p.first_polyphase) {                           // out[k] = sum_j x[k*m - j] c[j] (k > j), and e[k] reads r[k-1]
+        const uint64_t ntaps = p.h.size();
+        const uint64_t kfirst = u0 == 0 ? 0 : u0 - 1;
+        xa = kfirst * m > ntaps ? kfirst * m - ntaps : 0;
+        xb = std::min<uint64_t>(n, u1 * m);             // output k exists once (k+1)*m samples do (decimate, dsp.rs:299-301)
+    } else if (fu.tiled) {
+        xa = u0 == 0 ? 0 : u0 * fu.unit_in - fu.before;
+        xb = std::min<uint64_t>(n, (u1 - 1) * fu.unit_in + fu.after);
+    } else {
+        const uint64_t kfirst = u0 == 0 ? 0 : u0 - 1;                    // the envelope needs r[k0 - 1]
+        xa = (kfirst * m + l - 1) / l;
+        xa &= ~static_cast<uint64_t>(7);                                  // keep 16-byte alignment of PCM16 chunks
+        xb = std::min<uint64_t>(n, ((u1 - 1) * m + p.off2) / l + 1);
+    }
+}
+
 // fast_resampling + demodulate of outputs produced from a device-resident (or staged) chunk.
-// `in` is the address sample 0 of the recording would have (a biased pointer for chunk buffers).
-static int launch_front_polyphase(apt_decoder *d, const void *in, int format, uint64_t n, uint64_t nwork,
-                                  uint64_t tile_begin, uint64_t tile_end, uint64_t k_begin, uint64_t k_end,
-                                  float *conv_base /* f32 view of a PCM16 chunk (already biased) or nullptr */) {
+// `in` is the address sample 0 of the recording would have (a biased pointer for chunk buffers), `e` the address of
+// envelope sample 0.
+int launch_front_polyphase(apt_decoder *d, const void *in, int format, uint64_t n, uint64_t nwork,
+                           uint64_t tile_begin, uint64_t tile_end, uint64_t k_begin, uint64_t k_end,
+                           float *conv_base /* f32 view of a PCM16 chunk (already biased) or nullptr */, float *e) {
     const Plan &p = d->plan;
     const LaunchCtx c{d->stream, d->sm_count};
     if (p.ut && (format == APT_F32 || conv_base)) {
         const float *fin = format == APT_F32 ? static_cast<const float *>(in) : conv_base;
         if ((reinterpret_cast<uintptr_t>(fin) & 15) == 0)
             return launch_polyphase_ut(c, fin, n, d->d_h, p.utp, p.ut_stream, nwork, tile_begin, tile_end, true, p.cosphi2,
-                                       p.sinphi, d->d_e);
+                                       p.sinphi, e);
     }
     if (p.tiled && d->d_tile_taps && (format == APT_F32 || conv_base)) {
         const float *fin = format == APT_F32 ? static_cast<const float *>(in) : conv_base;
         return launch_polyphase_tiled(c, fin, n, d->d_tile_taps, d->d_tile_xs, p.tile, nwork, tile_begin, tile_end, true,
-                                      p.cosphi2, p.sinphi, d->d_e);
+                                      p.cosphi2, p.sinphi, e);
     }
     if (ph_front(d))   // large L: phase-major kernel, f32 or PCM16 samples (the cast is part of its row staging)
         return launch_polyphase_ph(c, in, format, n, d->d_ph_table, d->d_ph_xs, p.php, nwork, tile_begin, tile_end, true, p.cosphi2,
-                                   p.sinphi, d->d_e);
+                                   p.sinphi, e);
     return launch_polyphase(c, in, format, n, d->d_h, p.first.l, p.first.m, p.off2, k_begin, k_end ? k_end : nwork, true,
-                            p.cosphi2, p.sinphi, d->d_e);
+                            p.cosphi2, p.sinphi, e);
 }
 
 // Long host recording: upload in chunks (with the filter-length overlap each chunk needs) on the copy stream while
@@ -254,32 +298,14 @@ static int enqueue_front_chunked(apt_decoder *d, const void *host, int format, u
     const LaunchCtx c{d->stream, d->sm_count};
     const size_t sb = format == APT_PCM16 ? 2 : 4;
     const uint64_t cap = d->chunk_samples;
-    const bool tiled = fast_front(d) || ph_front(d);
     const uint64_t l = p.first.l, m = p.first.m;
+    const FrontUnits fu = front_units(p);
+    const bool tiled = fu.tiled;
     uint64_t units, per_chunk;            // tiles / blocks or outputs
-    // a unit (tile of the warp-specialised kernel, block of the uniform-tap kernel) reads unit_in new samples,
-    // plus `before` samples in front of the first unit of a chunk and `after` beyond the start of the last one
-    uint64_t unit_in = 0, unit_out = 0, before = 0, after = 0;
-    if (p.ut) {
-        unit_in = static_cast<uint64_t>(p.utp.rb) * m;
-        unit_out = static_cast<uint64_t>(p.utp.rb) * l;
-        before = p.utp.back;
-        after = p.utp.slot_floats - p.utp.back;           // a block's span beyond its first row's first sample
-    } else if (ph_front(d)) {
-        unit_in = static_cast<uint64_t>(kPhTilePeriods) * m;              // a tile = 32 periods of m samples
-        unit_out = static_cast<uint64_t>(kPhTilePeriods) * l;
-        before = m + 4;                                                   // the period in front of the tile (+4 alignment)
-        after = static_cast<uint64_t>(kPhTilePeriods - 1) * m + p.php.row_len;
-    } else if (tiled) {
-        unit_in = static_cast<uint64_t>(p.tile.qt) * p.tile.p_in;
-        unit_out = static_cast<uint64_t>(p.tile.qt) * p.tile.p_out;
-        before = p.tile.p_in - d->plan.tile_xs.back();    // halo row: window of the last group one super-period back
-        after = static_cast<uint64_t>(p.tile.qt - 1) * p.tile.p_in + p.tile.row_len;
-    }
     if (tiled) {
-        units = (nwork + unit_out - 1) / unit_out;
-        if (cap < before + after + unit_in + 64) return fail(APT_ERR_BAD_ARG, "chunk too small for one tile");
-        per_chunk = (cap - before - after - 64) / unit_in + 1;
+        units = (nwork + fu.unit_out - 1) / fu.unit_out;
+        if (cap < fu.before + fu.after + fu.unit_in + 64) return fail(APT_ERR_BAD_ARG, "chunk too small for one tile");
+        per_chunk = (cap - fu.before - fu.after - 64) / fu.unit_in + 1;
     } else {
         units = nwork;
         const uint64_t halo = p.off2 / l + 4;
@@ -293,15 +319,7 @@ static int enqueue_front_chunked(apt_decoder *d, const void *host, int format, u
         const uint64_t u1 = std::min(units, u0 + per_chunk);
         const int b = static_cast<int>(chunk & 1);
         uint64_t xa, xb;
-        if (tiled) {
-            xa = u0 == 0 ? 0 : u0 * unit_in - before;
-            xb = std::min<uint64_t>(n, (u1 - 1) * unit_in + after);
-        } else {
-            const uint64_t kfirst = u0 == 0 ? 0 : u0 - 1;                    // the envelope needs r[k0 - 1]
-            xa = (kfirst * m + l - 1) / l;
-            xa &= ~static_cast<uint64_t>(7);                                  // keep 16-byte alignment of PCM16 chunks
-            xb = std::min<uint64_t>(n, ((u1 - 1) * m + p.off2) / l + 1);
-        }
+        front_span(p, fu, u0, u1, n, xa, xb);
         if (xb <= xa || xb - xa > cap) return fail(APT_ERR_BAD_ARG, "internal: chunk geometry (%llu..%llu, cap %llu)",
                                                    (unsigned long long)xa, (unsigned long long)xb, (unsigned long long)cap);
         // copy stream: wait until the compute stream has finished with this buffer, then upload
@@ -323,7 +341,7 @@ static int enqueue_front_chunked(apt_decoder *d, const void *host, int format, u
         }
         d->launches++;
         APT_TRY(launch_front_polyphase(d, in_biased, format, n, nwork, tiled ? u0 : 0, tiled ? u1 : 0, tiled ? 0 : u0,
-                                       tiled ? 0 : u1, conv_biased));
+                                       tiled ? 0 : u1, conv_biased, d->d_e));
         APT_CUDA(cudaEventRecord(d->ev_free[b], d->stream));
     }
     d->job_chunks = chunk;
@@ -359,7 +377,7 @@ static int enqueue_front(apt_decoder *d, const void *in, int format, uint64_t n,
                 d->launches++;
                 conv = d->d_conv;
             }
-            APT_TRY(launch_front_polyphase(d, in, format, n, nwork, 0, 0, 0, 0, conv));
+            APT_TRY(launch_front_polyphase(d, in, format, n, nwork, 0, 0, 0, 0, conv, d->d_e));
         }
         if (d->cb) d->cb(0.4f, "Demodulating", d->cb_user);                 // decode.rs:87
     } else {

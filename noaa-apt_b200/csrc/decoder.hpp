@@ -57,6 +57,28 @@ uint64_t plan_work_len(const Plan &p, uint64_t n);
 // decode() output length for no-sync / upper bound for sync.
 uint64_t plan_out_bound(const Plan &p, uint64_t n);
 
+// First-stage units (decoder.cu): a unit (tile of the tiled / phase-major kernel, block of the uniform-tap kernel) makes
+// unit_out envelope outputs from unit_in new samples, plus `before` samples in front of the first unit of a run and
+// `after` beyond the start of the last one.  The generic polyphase kernel and filter + decimate work per output
+// (tiled == false, unit_out == 1).  Shared by the chunked upload and the stream.
+struct FrontUnits {
+    bool tiled = false;
+    uint64_t unit_in = 0, unit_out = 0, before = 0, after = 0;
+};
+FrontUnits front_units(const Plan &p);
+// Input samples [xa, xb) units [u0, u1) read from a recording of n samples.
+void front_span(const Plan &p, const FrontUnits &fu, uint64_t u0, uint64_t u1, uint64_t n, uint64_t &xa, uint64_t &xb);
+// Resample + envelope of tiles / blocks [tile_begin, tile_end) or generic outputs [k_begin, k_end) into e (biased pointers).
+int launch_front_polyphase(apt_decoder *d, const void *in, int format, uint64_t n, uint64_t nwork, uint64_t tile_begin,
+                           uint64_t tile_end, uint64_t k_begin, uint64_t k_end, float *conv_base, float *e);
+
+// Uploads the plan's filter taps and resampler tables (apt_decoder_create and apt_stream_create); plan_table_bytes is
+// the device memory that takes.
+int upload_plan(apt_decoder *d);
+uint64_t plan_table_bytes(const Plan &p);
+// Frees every buffer, event and stream the decoder owns (the object itself stays).
+int free_decoder_buffers(apt_decoder *d);
+
 // Kernel accounting of a decoder: counts the launch and, when profiling, records the begin event of slot `name`;
 // returns the slot to close with prof_end (-1: none).
 int prof_begin(apt_decoder *d, const char *name);

@@ -96,22 +96,22 @@ k_pcm16_to_f32(const int16_t *__restrict__ in, u64 n, float *__restrict__ out) {
     if (blockIdx.x == 0 && threadIdx.x < n - n8 * 8) out[n8 * 8 + threadIdx.x] = static_cast<float>(in[n8 * 8 + threadIdx.x]);
 }
 
-// demodulate alone (stage entry point, and the L == 1 decode path).
+// demodulate alone (stage entry point, and the L == 1 decode path): outputs [begin, n), indices absolute.
 __global__ void __launch_bounds__(256)
-k_envelope(const float *__restrict__ x, u64 n, float cosphi2, float sinphi, float *__restrict__ out) {
-    for (u64 i = static_cast<u64>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+k_envelope(const float *__restrict__ x, u64 begin, u64 n, float cosphi2, float sinphi, float *__restrict__ out) {
+    for (u64 i = begin + static_cast<u64>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
          i += static_cast<u64>(gridDim.x) * blockDim.x)
         out[i] = i == 0 ? 0.f : envelope2(__ldg(x + i - 1), __ldg(x + i), cosphi2, sinphi);
 }
 
 // dsp::filter (dsp.rs:396-404) followed by decimate (dsp.rs:299-303):
-//   out[i] = sum_{j < ntaps, j < i*m} x[i*m - j] * c[j],  i < nout  (m == 1: plain filter)
+//   out[i] = sum_{j < ntaps, j < i*m} x[i*m - j] * c[j],  begin <= i < nout  (m == 1: plain filter)
 // ZERO_FIRST reproduces what NoFilter does to element 0 in the final stage of decode().
 template <typename InT>
 __global__ void __launch_bounds__(256)
-k_fir_decimate_generic(const InT *__restrict__ x, const float *__restrict__ c, u32 ntaps, u32 m, u64 nout,
+k_fir_decimate_generic(const InT *__restrict__ x, const float *__restrict__ c, u32 ntaps, u32 m, u64 begin, u64 nout,
                        float *__restrict__ out) {
-    for (u64 i = static_cast<u64>(blockIdx.x) * blockDim.x + threadIdx.x; i < nout;
+    for (u64 i = begin + static_cast<u64>(blockIdx.x) * blockDim.x + threadIdx.x; i < nout;
          i += static_cast<u64>(gridDim.x) * blockDim.x) {
         const u64 pos = i * m;
         const u32 jn = pos < ntaps ? static_cast<u32>(pos) : ntaps;   // strict i > j

@@ -9,6 +9,8 @@
 // per output instead of 114.  The summation order differs from the reference's sequential loop, i.e. the
 // values agree to fp32 rounding (~1e-7 relative), not bit for bit; the generic kernel keeps the exact order.
 //
+// Tiles start at `base` (BASED instantiations only; a multiple of 16, so every position keeps the parity and the 16-byte alignment it has with
+// base 0 and the values are those of a run from 0); there f_out == nullptr skips storing f.
 // One CTA handles 1856 consecutive positions: e tile -> f tile -> box sums -> correlation, all on fp32 register pairs
 // (fma2: two FMAs / adds):
 //   low-pass   : a thread owns 8 outputs of ONE parity (even warps the even positions, odd warps the odd ones), so
@@ -80,10 +82,11 @@ __device__ __forceinline__ void lp_outputs(const LpTaps &taps, const float *s_e,
     }
 }
 
-template <int NT, int PW>
-__global__ void __launch_bounds__(256, NT <= 37 ? 4 : 2)
-k_lowpass_corr(const float *__restrict__ e, u64 n, u64 ncorr, const __grid_constant__ LpTaps taps, float *__restrict__ f_out,
+template <int NT, int PW, bool BASED>
+__global__ void __launch_bounds__(256, NT <= 37 && !BASED ? 4 : 2)
+k_lowpass_corr(const float *__restrict__ e, u64 base_arg, u64 n, u64 ncorr, const __grid_constant__ LpTaps taps, float *__restrict__ f_out,
                float *__restrict__ corr_out) {
+    const u64 base = BASED ? base_arg : 0;     // the whole-recording instantiations keep their register budget
     constexpr int T = kLpTile;
     constexpr int G = 38 * PW;                 // template length
     constexpr int BOX = 2 * PW;                // run length
@@ -104,7 +107,7 @@ k_lowpass_corr(const float *__restrict__ e, u64 n, u64 ncorr, const __grid_const
     constexpr int NPRE = (ENP / 4 + 255) / 256;
     float4 pre[NPRE];
     auto fetch = [&](u64 tile_idx) {
-        const u64 i0f = tile_idx * T;
+        const u64 i0f = base + tile_idx * T;
 #pragma unroll
         for (int r = 0; r < NPRE; ++r) {
             const u32 m4 = 4 * (tid + 256 * r);
@@ -124,8 +127,8 @@ k_lowpass_corr(const float *__restrict__ e, u64 n, u64 ncorr, const __grid_const
         }
     };
     fetch(blockIdx.x);
-    for (u64 tile = blockIdx.x; tile * T < n; tile += gridDim.x) {
-        const u64 i0 = tile * T;
+    for (u64 tile = blockIdx.x; base + tile * T < n; tile += gridDim.x) {
+        const u64 i0 = base + tile * T;
         // ---- e tile: s_e[skew(m)] = e[i0 - EOFF + m] ----
 #pragma unroll
         for (int r = 0; r < NPRE; ++r) {
@@ -145,7 +148,7 @@ k_lowpass_corr(const float *__restrict__ e, u64 n, u64 ncorr, const __grid_const
         if (tid < BOX + 16) s_f[skew(FNP + tid)] = 0.f;   // tail read by the last box sums, never used
         __syncthreads();
         // ---- the tile's own f values go to HBM (f_out is 16-byte aligned, T a multiple of 4) ----
-        for (u32 i4 = tid; i4 < T / 4; i4 += 256) {
+        for (u32 i4 = tid; (!BASED || f_out != nullptr) && i4 < T / 4; i4 += 256) {
             const u64 gi = i0 + 4 * i4;
             if (gi >= n) break;
             const float4 v = *reinterpret_cast<const float4 *>(s_f + skew(4 * i4));

@@ -607,7 +607,7 @@ __device__ __forceinline__ void gather_quad(const float *src, const LpTaps &lp, 
 template <int NT, int DEC>
 __global__ void __launch_bounds__(kGatherLpThreads)
 k_gather_rows_lp(const float *__restrict__ e, u64 n, const u32 *__restrict__ positions, const SyncResult *__restrict__ result,
-                 u32 fixed_rows, u32 row, u32 px, const __grid_constant__ LpTaps lp, float *__restrict__ out) {
+                 u32 fixed_rows, u32 first_row, u32 row, u32 px, const __grid_constant__ LpTaps lp, float *__restrict__ out) {
     constexpr int EOFF = (NT - 1 + 3) / 4 * 4;
     constexpr int PARTS = 2;
     extern __shared__ __align__(16) float g_smem[];
@@ -620,7 +620,7 @@ k_gather_rows_lp(const float *__restrict__ e, u64 n, const u32 *__restrict__ pos
     // sample index of buf[0] of an item, and the offset of the row's window in it
     auto origin = [&](u32 item, long long &a0) -> u32 {
         const u32 j = item / PARTS, part = item % PARTS;
-        const u64 p = positions ? positions[j] : static_cast<u64>(j) * row;
+        const u64 p = positions ? positions[j] : static_cast<u64>(first_row + j) * row;
         const long long g0 = static_cast<long long>(p) + static_cast<long long>(DEC) * (part * part_px) - EOFF;
         a0 = g0 & ~3ll;                                            // floor to a multiple of 4 (also for negative g0)
         return static_cast<u32>(g0 - a0);
@@ -664,7 +664,7 @@ k_gather_rows_lp(const float *__restrict__ e, u64 n, const u32 *__restrict__ pos
             }
             const u32 c = c_begin + c4;
             float *dst = out + static_cast<u64>(j) * px + c;
-            if (j == 0 && c == 0) acc[0] = 0.f;
+            if (first_row + j == 0 && c == 0) acc[0] = 0.f;
             if (out_aligned && c + 3 < c_end) {
                 *reinterpret_cast<float4 *>(dst) = make_float4(acc[0], acc[1], acc[2], acc[3]);
             } else {

@@ -16,6 +16,7 @@
 #include "kernels_ph.cuh"
 #include "kernels_sync.cuh"
 #include "kernels_sync2.cuh"
+#include "kernels_stream.cuh"
 #include "kernels_post.cuh"
 #include "kernels_ut.cuh"
 
@@ -225,13 +226,13 @@ int launch_polyphase_ph(const LaunchCtx &c, const void *signal, int format, u64 
 }
 
 int launch_fir_decimate(const LaunchCtx &c, const void *signal, int format, const float *coeff, u32 ntaps, u32 m,
-                        u64 nout, float *out) {
-    if (nout == 0) return APT_OK;
-    const unsigned grid = grid_for(nout, 256, c.sm_count);
+                        u64 nout, float *out, u64 begin) {
+    if (nout <= begin) return APT_OK;
+    const unsigned grid = grid_for(nout - begin, 256, c.sm_count);
     if (format == APT_PCM16)
-        k_fir_decimate_generic<int16_t><<<grid, 256, 0, c.stream>>>(static_cast<const int16_t *>(signal), coeff, ntaps, m, nout, out);
+        k_fir_decimate_generic<int16_t><<<grid, 256, 0, c.stream>>>(static_cast<const int16_t *>(signal), coeff, ntaps, m, begin, nout, out);
     else
-        k_fir_decimate_generic<float><<<grid, 256, 0, c.stream>>>(static_cast<const float *>(signal), coeff, ntaps, m, nout, out);
+        k_fir_decimate_generic<float><<<grid, 256, 0, c.stream>>>(static_cast<const float *>(signal), coeff, ntaps, m, begin, nout, out);
     APT_CUDA(cudaGetLastError());
     return APT_OK;
 }
@@ -243,9 +244,9 @@ int launch_pcm16_to_f32(const LaunchCtx &c, const int16_t *in, u64 n, float *out
     return APT_OK;
 }
 
-int launch_envelope(const LaunchCtx &c, const float *x, u64 n, float cosphi2, float sinphi, float *out) {
-    if (n == 0) return APT_OK;
-    k_envelope<<<grid_for(n, 256, c.sm_count), 256, 0, c.stream>>>(x, n, cosphi2, sinphi, out);
+int launch_envelope(const LaunchCtx &c, const float *x, u64 n, float cosphi2, float sinphi, float *out, u64 begin) {
+    if (n <= begin) return APT_OK;
+    k_envelope<<<grid_for(n - begin, 256, c.sm_count), 256, 0, c.stream>>>(x, begin, n, cosphi2, sinphi, out);
     APT_CUDA(cudaGetLastError());
     return APT_OK;
 }
@@ -262,8 +263,9 @@ bool lowpass_corr_supported(u32 ntaps, u32 pw) {
 }
 
 int launch_lowpass_corr(const LaunchCtx &c, const float *e, u64 n, const float *taps_host, u32 ntaps, u32 pw, float *f,
-                        float *corr) {
-    if (n == 0) return APT_OK;
+                        float *corr, u64 base) {
+    if (n <= base) return APT_OK;
+    if (base % 16) return fail(APT_ERR_BAD_ARG, "low-pass/correlation: start %llu is not a multiple of 16", (unsigned long long)base);
     LpTaps t{};
     auto tap = [&](long long j) { return j >= 0 && j < static_cast<long long>(ntaps) ? taps_host[j] : 0.f; };
     for (int i = 0; i < 32; ++i) {
@@ -272,7 +274,7 @@ int launch_lowpass_corr(const LaunchCtx &c, const float *e, u64 n, const float *
     }
     for (int j = -1; j < 63; ++j) t.p[j + 1] = make_float2(tap(j), tap(j + 1));
     const u64 ncorr = n > 38ull * pw ? n - 38ull * pw : 0;
-    const u64 ntiles = (n + kLpTile - 1) / kLpTile;
+    const u64 ntiles = (n - base + kLpTile - 1) / kLpTile;
     // persistent: exactly the resident CTAs, each walks its tiles with the next tile's loads in flight
     auto launch = [&](auto kern) {
         static const int per_sm = [&] {          // per instantiation (generic lambda); one GPU model per process
@@ -281,11 +283,12 @@ int launch_lowpass_corr(const LaunchCtx &c, const float *e, u64 n, const float *
             return v;
         }();
         const unsigned grid = static_cast<unsigned>(std::min<u64>(ntiles, static_cast<u64>(c.sm_count) * per_sm));
-        kern<<<grid, 256, 0, c.stream>>>(e, n, ncorr, t, f, corr);
+        kern<<<grid, 256, 0, c.stream>>>(e, base, n, ncorr, t, f, corr);
     };
-    if (ntaps == 37 && pw == 3) launch(k_lowpass_corr<37, 3>);
-    else if (ntaps == 43 && pw == 4) launch(k_lowpass_corr<43, 4>);
-    else if (ntaps == 61 && pw == 5) launch(k_lowpass_corr<61, 5>);
+    const bool based = base != 0 || f == nullptr;   // the based instantiations take a start and may skip f
+    if (ntaps == 37 && pw == 3) based ? launch(k_lowpass_corr<37, 3, true>) : launch(k_lowpass_corr<37, 3, false>);
+    else if (ntaps == 43 && pw == 4) based ? launch(k_lowpass_corr<43, 4, true>) : launch(k_lowpass_corr<43, 4, false>);
+    else if (ntaps == 61 && pw == 5) based ? launch(k_lowpass_corr<61, 5, true>) : launch(k_lowpass_corr<61, 5, false>);
     else return fail(APT_ERR_BAD_ARG, "no fused low-pass/correlation kernel for %u taps, pixel width %u", ntaps, pw);
     APT_CUDA(cudaGetLastError());
     return APT_OK;
@@ -476,7 +479,8 @@ int launch_resolve_roots(const LaunchCtx &c, const TileDesc *desc, const Rec *po
 }
 
 int launch_gather_lp(const LaunchCtx &c, const float *e, u64 n, const u32 *positions, const SyncResult *result,
-                     u32 fixed_rows, u32 max_rows, u32 row, u32 px, u32 dec, const float *taps_host, u32 ntaps, float *out) {
+                     u32 fixed_rows, u32 max_rows, u32 row, u32 px, u32 dec, const float *taps_host, u32 ntaps, float *out,
+                     u32 first_row) {
     if (max_rows == 0) return APT_OK;
     const LpTaps lp = make_lp_taps(taps_host, ntaps, static_cast<int>(dec));
     const u32 part_px = (px / 2 + 3) / 4 * 4;
@@ -494,13 +498,24 @@ int launch_gather_lp(const LaunchCtx &c, const float *e, u64 n, const u32 *posit
         const u64 slots = static_cast<u64>(c.sm_count) * per_sm;
         const u64 rounds = (items + slots - 1) / slots;
         const unsigned grid = static_cast<unsigned>((items + rounds - 1) / rounds);
-        kern<<<grid, kGatherLpThreads, smem, c.stream>>>(e, n, positions, result, fixed_rows, row, px, lp, out);
+        kern<<<grid, kGatherLpThreads, smem, c.stream>>>(e, n, positions, result, fixed_rows, first_row, row, px, lp, out);
     };
     if (ntaps == 37 && dec == 3) launch(k_gather_rows_lp<37, 3>);
     else if (ntaps == 43 && dec == 4) launch(k_gather_rows_lp<43, 4>);
     else if (ntaps == 61 && dec == 5) launch(k_gather_rows_lp<61, 5>);
     else return fail(APT_ERR_BAD_ARG, "no fused gather kernel for %u taps, decimation %u", ntaps, dec);
     static_assert(kGatherLpThreads * 4 >= 1040, "one pass of a half row");
+    APT_CUDA(cudaGetLastError());
+    return APT_OK;
+}
+
+int launch_stream_sync(const LaunchCtx &c, const StreamSyncArgs &a) {
+    if (a.dist == 0 || a.dist > static_cast<u32>(kStreamThreads * kStreamChunk))
+        return fail(APT_ERR_BAD_ARG, "streamed picker: min_distance %u outside [1, %d]", a.dist, kStreamThreads * kStreamChunk);
+    const size_t smem = 2ull * a.dist * sizeof(float);
+    auto kern = k_stream_sync<kStreamChunk>;
+    APT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    kern<<<1, kStreamThreads, smem, c.stream>>>(a);
     APT_CUDA(cudaGetLastError());
     return APT_OK;
 }

@@ -166,17 +166,19 @@ int launch_polyphase(const LaunchCtx &c, const void *signal, int format, u64 len
 // wav.rs:37: PCM16 -> f32 (both pointers 16-byte aligned).
 int launch_pcm16_to_f32(const LaunchCtx &c, const int16_t *in, u64 n, float *out);
 // dsp::filter + decimate (dsp.rs:396-404, 299-303).
+// Outputs [begin, nout), absolute indices (`signal` and `out` are the addresses index 0 would have).
 int launch_fir_decimate(const LaunchCtx &c, const void *signal, int format, const float *coeff, u32 ntaps, u32 m,
-                        u64 nout, float *out);
-// dsp::demodulate (dsp.rs:350-383).
-int launch_envelope(const LaunchCtx &c, const float *x, u64 n, float cosphi2, float sinphi, float *out);
+                        u64 nout, float *out, u64 begin = 0);
+// dsp::demodulate (dsp.rs:350-383), outputs [begin, n) (out[0] = 0; out[i] reads x[i-1] and x[i]).
+int launch_envelope(const LaunchCtx &c, const float *x, u64 n, float cosphi2, float sinphi, float *out, u64 begin = 0);
 // sync cross-correlation (decode.rs:225-233).
 int launch_corr(const LaunchCtx &c, const float *f, u64 ncorr, const int8_t *guard, u32 glen, float *corr);
 // Fused low-pass + sync correlation (kernels_lpsync.cuh).  Returns false when (ntaps, pixel width) has no
-// instantiation -- the caller then uses launch_fir_decimate + launch_corr.  corr == nullptr: low-pass only.
+// instantiation -- the caller then uses launch_fir_decimate + launch_corr.  corr == nullptr: low-pass only; f == nullptr:
+// correlation only.  Positions [base, n) (corr: [base, n - 38*pixel_width)); base is an absolute index, a multiple of 16.
 bool lowpass_corr_supported(u32 ntaps, u32 pixel_width);
 int launch_lowpass_corr(const LaunchCtx &c, const float *e, u64 n, const float *taps_host, u32 ntaps, u32 pixel_width,
-                        float *f, float *corr);
+                        float *f, float *corr, u64 base = 0);
 // roots of the correlation (see kernels_sync.cuh).
 int launch_roots(const LaunchCtx &c, const float *corr, u64 ncorr, u32 dist, u32 *root_list, u32 *root_count,
                  SyncResult *result, const PickScratch *scratch /* nullptr: no dense numbering */);
@@ -192,8 +194,42 @@ int launch_resolve_roots(const LaunchCtx &c, const TileDesc *desc, const Rec *po
                          u64 ncorr, u32 *root_list, u32 *root_count, u32 *tile_base, u32 *by_id, SyncCtl *ctl,
                          SyncResult *result);
 // aligned rows + final decimation with the low-pass evaluated per pixel from the envelope (f never exists in HBM).
+// first_row: global index of the first row written (pixel 0 of global row 0 is zeroed; no-sync rows start at
+// first_row * row).
 int launch_gather_lp(const LaunchCtx &c, const float *e, u64 n, const u32 *positions, const SyncResult *result,
-                     u32 fixed_rows, u32 max_rows, u32 row, u32 px, u32 dec, const float *taps_host, u32 ntaps, float *out);
+                     u32 fixed_rows, u32 max_rows, u32 row, u32 px, u32 dec, const float *taps_host, u32 ntaps, float *out,
+                     u32 first_row = 0);
+// Carry of the streamed peak picker (kernels_stream.cuh), device resident; zeroed when a recording starts.
+struct StreamCarry {
+    u64 decided;          // root flags of the correlation positions [0, decided) are known
+    u64 s;                // next start of the walk (seed_state == 2)
+    u64 root_head, root_tail;   // live roots: ring entries [root_head, root_tail) (running counters)
+    u64 gathered;         // rows listed for the gather so far
+    u64 first_gather;     // global index of the first row of the last list
+    u64 run_head, run_tail;     // pending peaks: runs [run_head, run_tail) of the run ring (running counters)
+    u32 head_used;        // rows of the head run listed already
+    u32 seed_state;       // 0: corr[0..D] not final yet; 1: seed known; 2: peak 0 pushed
+    u32 seed;             // first i <= D with corr[i] > 0, or 0xFFFFFFFF
+    u32 len;              // peaks pushed
+    u32 more;             // another round can make progress (row list full, or run ring entries freed)
+    u32 status;           // 0 ok; 1 the root ring overflowed
+    SyncResult gres;      // n_rows = rows of the last list (what k_gather_rows_lp reads), status 0
+};
+struct StreamSyncArgs {
+    const float *corr;    // address correlation index 0 would have
+    u64 c_end;            // corr[.. c_end) is final
+    u64 ncorr;            // at the end of the recording: N_w - template length
+    u64 work_final;       // e[.. work_final) is final (N_w at the end)
+    u32 finish, row, dist;
+    u32 run_cap;          // run ring: run r is (run_pos, run_cnt)[r % run_cap]
+    u32 gather_cap;       // entries of gpos
+    u32 root_cap;         // root ring
+    u32 *roots, *run_pos, *run_cnt, *gpos;
+    StreamCarry *carry;
+};
+// One step of the streamed picker: roots of the newly final correlation, seed, orbit walk, rows to gather.
+int launch_stream_sync(const LaunchCtx &c, const StreamSyncArgs &a);
+
 // Bytes of scratch k_pick_parallel needs, and carving of one allocation into a PickScratch.
 size_t pick_scratch_bytes(u32 max_blocks, u32 max_positions, u32 cap);
 PickScratch pick_scratch_carve(void *base, u32 max_blocks, u32 max_positions, u32 cap);

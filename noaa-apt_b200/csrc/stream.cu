@@ -1,0 +1,469 @@
+// Streaming decoder (include/aptb200.h apt_stream_*, DESIGN.md §9): decode() carried across pushes of audio.
+//
+// Every step (one slice of at most max_push samples) runs on the stream's own CUDA stream:
+//   upload -> resample + envelope of the first-stage units whose input is complete -> low-pass + correlation of the newly
+//   final range -> k_stream_sync (roots, seed, orbit walk, rows to gather) -> k_gather_rows_lp -> one copy back.
+// The input, envelope and correlation live in windows that keep only what a later step can still read; a window is
+// compacted by moving its tail to the front when the tail is shorter than the part dropped (so the move never overlaps).
+#include <algorithm>
+#include <cstring>
+#include <memory>
+#include <new>
+#include <vector>
+
+#include "aptb200.h"
+#include "common.hpp"
+#include "decoder.hpp"
+#include "filters_host.hpp"
+#include "launch.hpp"
+
+using namespace aptb200;
+
+namespace {
+
+constexpr uint64_t kHalo = 80;      // envelope samples in front of a low-pass output: 60 taps + the gather's 4-alignment
+constexpr uint32_t kRunRing = 256;  // pending peaks as (position, count) runs: a handful are pending in practice
+
+inline uint64_t floor16(uint64_t x) { return x & ~static_cast<uint64_t>(15); }
+
+// Everything the buffers depend on: (plan, sync, max_push).
+struct Geom {
+    FrontUnits fu;
+    uint64_t G = 0, D = 0, row = 0;
+    uint64_t cap_in = 0, cap_e = 0, cap_c = 0, root_cap = 0, gather_cap = 0;
+    uint64_t latency = 0, bytes = 0;
+};
+
+int check_stream_args(uint32_t input_rate, const apt_settings *s, int sync, uint64_t max_push, Plan &p) {
+    if (!s) return fail(APT_ERR_BAD_ARG, "null settings");
+    if (max_push == 0 || max_push > (1ull << 28)) return fail(APT_ERR_BAD_ARG, "max_push %llu outside [1, 2^28]", (unsigned long long)max_push);
+    APT_TRY(make_plan(input_rate, *s, p));
+    if (!p.work_multiple) {
+        if (sync) return fail(APT_ERR_WORK_RATE, "work_rate is not multiple of FINAL_RATE");   // decode.rs:172-176
+        return fail(APT_ERR_BAD_ARG, "the stream needs a work rate that is a multiple of 4160 (the final NoFilter resample is "
+                                     "not streamed)");
+    }
+    if (!lowpass_corr_supported(static_cast<u32>(p.lp.size()), p.dec))
+        return fail(APT_ERR_BAD_ARG, "the stream supports the standard, fast and slow demodulation low-pass (37/43/61 taps), "
+                                     "not %zu taps at %u samples per pixel", p.lp.size(), p.dec);
+    if (sync && p.dist > 16384)
+        return fail(APT_ERR_BAD_ARG, "work_rate %u is too high for the sync picker (min_distance %u > 16384)", p.st.work_rate, p.dist);
+    return APT_OK;
+}
+
+Geom make_geom(const Plan &p, int sync, uint64_t max_push) {
+    Geom g;
+    g.fu = front_units(p);
+    g.G = p.guard.size();
+    g.D = p.dist;
+    g.row = p.row;
+    const uint64_t l = p.first.l, m = p.first.m;
+    // input tail: from the next unit's first sample to the end of what was pushed (less than one unit span)
+    uint64_t t_in;
+    if (!p.first_polyphase) t_in = p.h.size() + 2 * m + 32;
+    else if (g.fu.tiled) t_in = g.fu.before + g.fu.after + g.fu.unit_in + 32;
+    else t_in = (2 * p.off2 + 2 * m) / l + 32;
+    // envelope outputs one step can finalise (finish: the units the input tail still held)
+    const uint64_t w_new = (max_push + t_in) * l / m + 2 * g.fu.unit_out + 64;
+    // envelope tail: a pending row (< row + 1 before work_final) or a pending peak (>= decided >= c_end - D), plus the
+    // low-pass halo and the 16-sample alignment of the window start
+    const uint64_t t_e = g.row + g.D + g.G + kHalo + 64;
+    const uint64_t t_c = g.D + 64;
+    g.cap_in = 2 * t_in + max_push + 64;
+    g.cap_e = 2 * t_e + w_new + 64;
+    g.cap_c = sync ? 2 * t_c + w_new + 64 : 0;
+    g.root_cap = sync ? w_new + 2 * g.D + 1024 : 0;
+    g.gather_cap = w_new / g.row + 4;
+    g.latency = sync ? g.D + 1 : 0;
+    const uint64_t rows_floats = (g.gather_cap + 1) * kPxPerRow;
+    g.bytes = plan_table_bytes(p) + g.cap_in * 4 + max_push * (2 + 4) + g.cap_e * 4 * (p.first_polyphase ? 1 : 2) +
+              (sync ? g.cap_c * 4 + g.root_cap * 4 + kRunRing * 8 + sizeof(StreamCarry) : sizeof(StreamCarry)) +
+              g.gather_cap * 4 + rows_floats * 4;
+    return g;
+}
+
+}  // namespace
+
+struct apt_stream {
+    apt_decoder dec;                // plan, device, CUDA stream and filter tables (the other members stay unused)
+    int sync = 0;
+    uint64_t max_push = 0;
+    Geom g;
+    float *d_in = nullptr, *d_conv = nullptr, *d_e = nullptr, *d_r = nullptr, *d_corr = nullptr, *d_rows = nullptr;
+    int16_t *d_pcm = nullptr;
+    u32 *d_roots = nullptr, *d_gpos = nullptr;
+    char *d_carry = nullptr;        // StreamCarry, then the run ring (kRunRing positions, kRunRing counts)
+    char *h_carry = nullptr;        // pinned copy of the same
+    float *h_rows = nullptr;        // pinned rows of one round
+    // recording state
+    uint64_t samples_in = 0, in_base = 0, units_done = 0, work_final = 0, e_base = 0, c_base = 0, c_end = 0;
+    uint64_t rows_out = 0, gathered = 0, held_slot = 0;
+    bool finished = false;
+    std::vector<uint64_t> positions;
+    uint64_t runs_seen = 0;         // runs whose peaks are in `positions`
+
+    const StreamCarry &carry() const { return *reinterpret_cast<const StreamCarry *>(h_carry); }
+    const u32 *run_pos() const { return reinterpret_cast<const u32 *>(h_carry + sizeof(StreamCarry)); }
+    const u32 *run_cnt() const { return run_pos() + kRunRing; }
+};
+
+namespace {
+
+void free_stream(apt_stream *st) {
+    cudaSetDevice(st->dec.device);
+    if (st->dec.stream) cudaStreamSynchronize(st->dec.stream);
+    for (void *p : {(void *)st->d_in, (void *)st->d_conv, (void *)st->d_e, (void *)st->d_r, (void *)st->d_corr,
+                    (void *)st->d_rows, (void *)st->d_pcm, (void *)st->d_roots, (void *)st->d_gpos, (void *)st->d_carry})
+        if (p) cudaFree(p);
+    if (st->h_carry) cudaFreeHost(st->h_carry);
+    if (st->h_rows) cudaFreeHost(st->h_rows);
+    free_decoder_buffers(&st->dec);
+}
+
+int reset_state(apt_stream *st) {
+    st->samples_in = st->in_base = st->units_done = st->work_final = st->e_base = st->c_base = st->c_end = 0;
+    st->rows_out = st->gathered = st->held_slot = st->runs_seen = 0;
+    st->finished = false;
+    st->positions.clear();
+    APT_CUDA(cudaSetDevice(st->dec.device));
+    APT_CUDA(cudaMemsetAsync(st->d_carry, 0, sizeof(StreamCarry), st->dec.stream));
+    APT_CUDA(cudaMemsetAsync(st->d_in, 0, st->g.cap_in * sizeof(float), st->dec.stream));
+    APT_CUDA(cudaStreamSynchronize(st->dec.stream));
+    memset(st->h_carry, 0, sizeof(StreamCarry));
+    return APT_OK;
+}
+
+// Moves the tail [keep, end) of a window based at `base` to its front when that does not overlap.
+int compact(apt_stream *st, float *buf, uint64_t &base, uint64_t keep, uint64_t end) {
+    keep = floor16(std::min(keep, end));
+    if (keep <= base) return APT_OK;
+    const uint64_t drop = keep - base, tail = end - keep;
+    if (tail > drop) return APT_OK;
+    if (tail) APT_CUDA(cudaMemcpyAsync(buf, buf + drop, tail * sizeof(float), cudaMemcpyDeviceToDevice, st->dec.stream));
+    base = keep;
+    return APT_OK;
+}
+
+// First envelope sample a later step can still read.
+uint64_t envelope_keep(const apt_stream *st) {
+    if (!st->sync) return st->rows_out * st->g.row;
+    const StreamCarry &cy = st->carry();
+    uint64_t row_lb;
+    if (cy.run_head < cy.run_tail) row_lb = st->run_pos()[cy.run_head % kRunRing];   // known peak, envelope not final yet
+    else if (cy.seed_state < 2) row_lb = 0;
+    else row_lb = cy.s >= st->c_end ? cy.s : std::max<uint64_t>(cy.s, cy.decided);   // the next peak is >= this
+    return std::min(row_lb, floor16(st->c_end));   // the next low-pass / correlation run starts at floor16(c_end)
+}
+
+int compact_all(apt_stream *st) {
+    const Plan &p = st->dec.plan;
+    uint64_t xa, xb;
+    front_span(p, st->g.fu, st->units_done, st->units_done + 1, ~0ull, xa, xb);
+    APT_TRY(compact(st, st->d_in, st->in_base, xa, st->samples_in));
+    const uint64_t ek = envelope_keep(st);
+    const uint64_t ekeep = ek > kHalo ? ek - kHalo : 0;
+    uint64_t eb = st->e_base;
+    APT_TRY(compact(st, st->d_e, eb, ekeep, st->work_final));
+    if (st->d_r && eb != st->e_base) {
+        uint64_t rb = st->e_base;
+        APT_TRY(compact(st, st->d_r, rb, ekeep, st->work_final));
+    }
+    st->e_base = eb;
+    if (st->sync) {
+        const StreamCarry &cy = st->carry();
+        APT_TRY(compact(st, st->d_corr, st->c_base, cy.seed_state == 0 ? 0 : cy.decided, st->c_end));
+    }
+    return APT_OK;
+}
+
+// Copies rows [rows_out, rel_hi) out of the pinned round buffer (slot 0 = row rows_out) and remembers a row that was
+// gathered but is not released yet (its peak is the last one).
+void take_rows(apt_stream *st, uint64_t rel_hi, float *rows, uint64_t &nout) {
+    const uint64_t n = rel_hi - st->rows_out;
+    if (n) memcpy(rows + nout, st->h_rows, n * kPxPerRow * sizeof(float));
+    nout += n * kPxPerRow;
+    st->held_slot = st->gathered > rel_hi ? st->gathered - 1 - st->rows_out : 0;
+    st->rows_out = rel_hi;
+}
+
+// One step: `n` new samples (maybe none) and, when `finish`, the end of the recording.
+int step(apt_stream *st, const void *host, int format, uint64_t n, bool finish, float *rows, uint64_t &nout, int &status) {
+    apt_decoder &d = st->dec;
+    const Plan &p = d.plan;
+    const Geom &g = st->g;
+    const LaunchCtx c{d.stream, d.sm_count};
+    APT_TRY(compact_all(st));
+    // ---- upload (PCM16 is cast into the f32 window: pushes may mix formats) ----
+    if (n) {
+        const uint64_t off = st->samples_in - st->in_base;
+        if (off + n > g.cap_in) return fail(APT_ERR_BAD_ARG, "internal: input window overflow");
+        if (format == APT_PCM16) {
+            APT_CUDA(cudaMemcpyAsync(st->d_pcm, host, n * 2, cudaMemcpyHostToDevice, d.stream));
+            APT_TRY(launch_pcm16_to_f32(c, st->d_pcm, n, st->d_conv));
+            APT_CUDA(cudaMemcpyAsync(st->d_in + off, st->d_conv, n * 4, cudaMemcpyDeviceToDevice, d.stream));
+        } else {
+            APT_CUDA(cudaMemcpyAsync(st->d_in + off, host, n * 4, cudaMemcpyHostToDevice, d.stream));
+        }
+        st->samples_in += n;
+    }
+    const uint64_t N = st->samples_in;
+    const uint64_t nw = plan_work_len(p, N);
+    if (finish && nw < 10ull * p.row) {    // decode.rs:79-83
+        status = fail(APT_ERR_TOO_SHORT, "Got less than 10 rows of samples, audio file is too short");
+        return APT_OK;
+    }
+    // ---- first stage: the units whose input span is complete (all of them at the end) ----
+    const uint64_t l = p.first.l, m = p.first.m;
+    uint64_t u_hi;
+    if (!p.first_polyphase) u_hi = nw;                                       // output k needs samples [.., (k+1)m)
+    else if (g.fu.tiled) {
+        const uint64_t total = (nw + g.fu.unit_out - 1) / g.fu.unit_out;
+        u_hi = finish ? total : std::min(N >= g.fu.after ? (N - g.fu.after) / g.fu.unit_in + 1 : 0, nw / g.fu.unit_out);
+    } else {
+        u_hi = finish ? nw : std::min(N * l > p.off2 ? (N * l - p.off2 - 1) / m + 1 : 0, nw);   // (k*m + off2)/l < N
+    }
+    const uint64_t work_before = st->work_final;
+    if (u_hi > st->units_done) {
+        const uint64_t work_hi = finish ? nw : std::min(nw, u_hi * g.fu.unit_out);
+        if (work_hi - st->e_base > g.cap_e) return fail(APT_ERR_BAD_ARG, "internal: envelope window overflow");
+        const float *in = st->d_in - st->in_base;
+        float *e = st->d_e - st->e_base;
+        if (p.first_polyphase) {
+            const bool t = g.fu.tiled;
+            APT_TRY(launch_front_polyphase(&d, in, APT_F32, N, nw, t ? st->units_done : 0, t ? u_hi : 0, t ? 0 : st->units_done,
+                                           t ? 0 : u_hi, nullptr, e));
+        } else {
+            float *r = st->d_r - st->e_base;
+            APT_TRY(launch_fir_decimate(c, in, APT_F32, d.d_h, static_cast<u32>(p.h.size()), p.first.m, u_hi, r, st->units_done));
+            APT_TRY(launch_envelope(c, r, u_hi, p.cosphi2, p.sinphi, e, st->units_done));
+        }
+        st->units_done = u_hi;
+        st->work_final = work_hi;
+    }
+    const u32 ntaps = static_cast<u32>(p.lp.size());
+    float *e = st->d_e - st->e_base;
+    if (!st->sync) {   // rows r with (r+1)*row <= work_final (decode.rs:141-147)
+        const uint64_t r_hi = st->work_final / p.row;
+        while (st->rows_out < r_hi) {
+            const uint64_t cnt = std::min<uint64_t>(r_hi - st->rows_out, g.gather_cap);
+            APT_TRY(launch_gather_lp(c, e, st->work_final, nullptr, nullptr, static_cast<u32>(cnt), static_cast<u32>(cnt), p.row, kPxPerRow,
+                                     p.dec, p.lp.data(), ntaps, st->d_rows, static_cast<u32>(st->rows_out)));
+            APT_CUDA(cudaMemcpyAsync(st->h_rows, st->d_rows, cnt * kPxPerRow * sizeof(float), cudaMemcpyDeviceToHost, d.stream));
+            APT_CUDA(cudaStreamSynchronize(d.stream));
+            st->gathered = st->rows_out + cnt;
+            take_rows(st, st->rows_out + cnt, rows, nout);
+        }
+        return APT_OK;
+    }
+    // ---- low-pass + correlation of the newly final range ----
+    const uint64_t c_new = finish ? nw - g.G : (st->work_final > g.G ? st->work_final - g.G : 0);
+    if (!finish && c_new <= st->c_end && st->work_final == work_before) return APT_OK;   // nothing became final
+    if (c_new > st->c_end) {
+        const uint64_t lp_base = floor16(st->c_end);
+        if (c_new - st->c_base > g.cap_c || (lp_base >= kHalo && lp_base - kHalo < st->e_base))
+            return fail(APT_ERR_BAD_ARG, "internal: correlation window overflow");
+        APT_TRY(launch_lowpass_corr(c, e, st->work_final, p.lp.data(), ntaps, p.dec, nullptr, st->d_corr - st->c_base, lp_base));
+        st->c_end = c_new;
+    }
+    // ---- picker + gather, in rounds until the walk has gone as far as the final data allow ----
+    const size_t carry_bytes = sizeof(StreamCarry) + 2 * kRunRing * sizeof(u32);
+    StreamCarry *dcy = reinterpret_cast<StreamCarry *>(st->d_carry);
+    for (;;) {
+        if (st->held_slot)
+            APT_CUDA(cudaMemcpyAsync(st->d_rows, st->d_rows + st->held_slot * kPxPerRow, kPxPerRow * sizeof(float),
+                                     cudaMemcpyDeviceToDevice, d.stream));
+        st->held_slot = 0;
+        const uint64_t held = st->gathered - st->rows_out;
+        const StreamCarry before = st->carry();
+        StreamSyncArgs a{};
+        a.corr = st->d_corr - st->c_base;
+        a.c_end = st->c_end;
+        a.ncorr = st->c_end;
+        a.work_final = st->work_final;
+        a.finish = finish ? 1 : 0;
+        a.row = p.row;
+        a.dist = p.dist;
+        a.run_cap = kRunRing;
+        a.gather_cap = static_cast<u32>(g.gather_cap);
+        a.root_cap = static_cast<u32>(g.root_cap);
+        a.roots = st->d_roots;
+        a.run_pos = reinterpret_cast<u32 *>(st->d_carry + sizeof(StreamCarry));
+        a.run_cnt = a.run_pos + kRunRing;
+        a.gpos = st->d_gpos;
+        a.carry = dcy;
+        APT_TRY(launch_stream_sync(c, a));
+        APT_TRY(launch_gather_lp(c, e, st->work_final, st->d_gpos, &dcy->gres, 0, static_cast<u32>(g.gather_cap), p.row, kPxPerRow,
+                                 p.dec, p.lp.data(), ntaps, st->d_rows + held * kPxPerRow, static_cast<u32>(st->gathered)));
+        APT_CUDA(cudaMemcpyAsync(st->h_carry, st->d_carry, carry_bytes, cudaMemcpyDeviceToHost, d.stream));
+        APT_CUDA(cudaMemcpyAsync(st->h_rows, st->d_rows, (held + g.gather_cap) * kPxPerRow * sizeof(float), cudaMemcpyDeviceToHost,
+                                 d.stream));
+        APT_CUDA(cudaStreamSynchronize(d.stream));
+        const StreamCarry &cy = st->carry();
+        if (cy.status != 0) return fail(APT_ERR_BAD_ARG, "internal: root ring overflow");
+        // runs pushed by this launch: their ring entries cannot have been reused yet (a launch pushes at most
+        // kRunRing - pending runs, and the pending ones start at or after runs_seen)
+        for (; st->runs_seen < cy.run_tail; ++st->runs_seen)
+            st->positions.insert(st->positions.end(), st->run_cnt()[st->runs_seen % kRunRing], st->run_pos()[st->runs_seen % kRunRing]);
+        if (st->positions.size() != cy.len) return fail(APT_ERR_BAD_ARG, "internal: peak runs and peak count disagree");
+        st->gathered = cy.gathered;
+        // released: rows whose next peak exists; a failed decode (fewer than 5 peaks at the end) releases nothing more
+        const bool failed = finish && cy.len < 5;
+        const uint64_t rel_hi = failed ? st->rows_out : std::min<uint64_t>(st->gathered, cy.len > 0 ? cy.len - 1 : 0);
+        take_rows(st, std::max(rel_hi, st->rows_out), rows, nout);
+        if (!cy.more) break;
+        if (cy.len == before.len && cy.gathered == before.gathered && cy.run_head == before.run_head)
+            return fail(APT_ERR_BAD_ARG, "internal: the picker made no progress");   // never loop on an unchanged carry
+    }
+    if (finish && st->carry().len < 5)   // decode.rs:112-118
+        status = fail(APT_ERR_FEW_SYNC_FRAMES, "Found less than 5 sync frames, audio file is too short or too noisy");
+    return APT_OK;
+}
+
+uint64_t rows_bound(const apt_stream *st, uint64_t n) {
+    const uint64_t nw = plan_work_len(st->dec.plan, st->samples_in + n);
+    const uint64_t most = nw / st->g.row + 1;
+    return most > st->rows_out ? (most - st->rows_out) * kPxPerRow : 0;
+}
+
+}  // namespace
+
+extern "C" int apt_stream_geometry(uint32_t input_rate, const apt_settings *s, int sync, uint64_t max_push, apt_stream_info *info) {
+    if (!info) return fail(APT_ERR_BAD_ARG, "null argument");
+    Plan p;
+    APT_TRY(check_stream_args(input_rate, s, sync, max_push, p));
+    const Geom g = make_geom(p, sync, max_push);
+    *info = apt_stream_info{};
+    info->latency_work = g.latency;
+    info->max_push = max_push;
+    info->device_bytes = g.bytes;
+    return APT_OK;
+}
+
+extern "C" int apt_stream_create(int device, uint32_t input_rate, const apt_settings *s, int sync, uint64_t max_push, apt_stream **out) {
+    if (!out) return fail(APT_ERR_BAD_ARG, "null argument");
+    *out = nullptr;
+    std::unique_ptr<apt_stream> st(new (std::nothrow) apt_stream);
+    if (!st) return fail(APT_ERR_NOMEM, "out of host memory");
+    APT_TRY(check_stream_args(input_rate, s, sync, max_push, st->dec.plan));
+    int count = 0;
+    if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0) {
+        cudaGetLastError();
+        return fail(APT_ERR_CUDA, "no usable CUDA device; this library has no CPU fallback");
+    }
+    const Plan &p = st->dec.plan;
+    st->sync = sync ? 1 : 0;
+    st->max_push = max_push;
+    st->g = make_geom(p, st->sync, max_push);
+    const Geom &g = st->g;
+    apt_decoder &d = st->dec;
+    d.device = device;
+    APT_CUDA(cudaSetDevice(device));
+    APT_CUDA(cudaDeviceGetAttribute(&d.sm_count, cudaDevAttrMultiProcessorCount, device));
+    struct Rollback {
+        apt_stream *st;
+        bool armed = true;
+        ~Rollback() {
+            if (armed) free_stream(st);
+        }
+    } rollback{st.get()};
+    APT_CUDA(cudaStreamCreateWithFlags(&d.stream, cudaStreamNonBlocking));
+    APT_TRY(upload_plan(&d));
+    const uint64_t rows_floats = (g.gather_cap + 1) * kPxPerRow;
+    APT_CUDA(cudaMalloc(&st->d_in, g.cap_in * sizeof(float)));
+    APT_CUDA(cudaMalloc(&st->d_pcm, max_push * sizeof(int16_t)));
+    APT_CUDA(cudaMalloc(&st->d_conv, max_push * sizeof(float)));
+    APT_CUDA(cudaMalloc(&st->d_e, g.cap_e * sizeof(float)));
+    if (!p.first_polyphase) APT_CUDA(cudaMalloc(&st->d_r, g.cap_e * sizeof(float)));
+    const size_t carry_bytes = sizeof(StreamCarry) + (st->sync ? 2 * kRunRing * sizeof(u32) : 0);
+    APT_CUDA(cudaMalloc(&st->d_carry, carry_bytes));
+    if (st->sync) {
+        APT_CUDA(cudaMalloc(&st->d_corr, g.cap_c * sizeof(float)));
+        APT_CUDA(cudaMalloc(&st->d_roots, g.root_cap * sizeof(u32)));
+    }
+    APT_CUDA(cudaMalloc(&st->d_gpos, g.gather_cap * sizeof(u32)));
+    APT_CUDA(cudaMalloc(&st->d_rows, rows_floats * sizeof(float)));
+    APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&st->h_carry), sizeof(StreamCarry) + 2 * kRunRing * sizeof(u32), cudaHostAllocDefault));
+    APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&st->h_rows), rows_floats * sizeof(float), cudaHostAllocDefault));
+    APT_TRY(reset_state(st.get()));
+    rollback.armed = false;
+    *out = st.release();
+    return APT_OK;
+}
+
+extern "C" void apt_stream_destroy(apt_stream *st) {
+    if (!st) return;
+    free_stream(st);
+    delete st;
+}
+
+extern "C" int apt_stream_push_bound(apt_stream *st, uint64_t n, uint64_t *cap_floats) {
+    if (!st || !cap_floats) return fail(APT_ERR_BAD_ARG, "null argument");
+    *cap_floats = rows_bound(st, n);
+    return APT_OK;
+}
+
+extern "C" int apt_stream_push(apt_stream *st, const void *samples, int format, uint64_t n, float *rows, uint64_t cap, uint64_t *nout) {
+    if (nout) *nout = 0;
+    if (!st) return fail(APT_ERR_BAD_ARG, "null stream");
+    if (st->finished) return fail(APT_ERR_BAD_ARG, "push after finish: call apt_stream_reset to start a new recording");
+    if (format != APT_F32 && format != APT_PCM16) return fail(APT_ERR_BAD_ARG, "unknown sample format %d", format);
+    if (n == 0) return APT_OK;
+    if (!samples) return fail(APT_ERR_BAD_ARG, "null samples");
+    if (plan_work_len(st->dec.plan, st->samples_in + n) >= (1ull << 32))
+        return fail(APT_ERR_BAD_ARG, "recording too long: the work-rate index would pass 2^32-1");
+    const uint64_t need = rows_bound(st, n);
+    if (need && (!rows || cap < need)) return fail(APT_ERR_CAPACITY, "rows needs room for %llu floats", (unsigned long long)need);
+    APT_CUDA(cudaSetDevice(st->dec.device));
+    uint64_t got = 0;
+    const size_t sb = format == APT_PCM16 ? 2 : 4;
+    int status = APT_OK;
+    for (uint64_t done = 0; done < n;) {
+        const uint64_t k = std::min(st->max_push, n - done);
+        APT_TRY(step(st, static_cast<const char *>(samples) + done * sb, format, k, false, rows, got, status));
+        done += k;
+    }
+    if (nout) *nout = got;
+    return status;
+}
+
+extern "C" int apt_stream_finish(apt_stream *st, float *rows, uint64_t cap, uint64_t *nout) {
+    if (nout) *nout = 0;
+    if (!st) return fail(APT_ERR_BAD_ARG, "null stream");
+    if (st->finished) return fail(APT_ERR_BAD_ARG, "the stream is already finished");
+    if (st->samples_in == 0) return fail(APT_ERR_BAD_ARG, "empty signal");   // signal[0] panics in demodulate, dsp.rs:367
+    const uint64_t need = rows_bound(st, 0);
+    if (need && (!rows || cap < need)) return fail(APT_ERR_CAPACITY, "rows needs room for %llu floats", (unsigned long long)need);
+    APT_CUDA(cudaSetDevice(st->dec.device));
+    uint64_t got = 0;
+    int status = APT_OK;
+    APT_TRY(step(st, nullptr, APT_F32, 0, true, rows, got, status));
+    st->finished = true;
+    if (nout) *nout = got;
+    return status;
+}
+
+extern "C" int apt_stream_reset(apt_stream *st) {
+    if (!st) return fail(APT_ERR_BAD_ARG, "null stream");
+    return reset_state(st);
+}
+
+extern "C" int apt_stream_sync_positions(apt_stream *st, uint64_t *positions, size_t cap, size_t *n) {
+    if (!st || !n) return fail(APT_ERR_BAD_ARG, "null argument");
+    *n = st->positions.size();
+    if (!positions) return APT_OK;
+    std::copy_n(st->positions.begin(), std::min(cap, st->positions.size()), positions);
+    if (cap < st->positions.size()) return fail(APT_ERR_CAPACITY, "positions needs %zu entries", st->positions.size());
+    return APT_OK;
+}
+
+extern "C" int apt_stream_get_info(apt_stream *st, apt_stream_info *info) {
+    if (!st || !info) return fail(APT_ERR_BAD_ARG, "null argument");
+    info->samples_in = st->samples_in;
+    info->work_final = st->work_final;
+    info->rows_out = st->rows_out;
+    info->peaks = st->positions.size();
+    info->latency_work = st->g.latency;
+    info->max_push = st->max_push;
+    info->device_bytes = st->g.bytes;
+    return APT_OK;
+}

@@ -224,6 +224,79 @@ class Decoder:
         return int(self._lib.apt_decoder_launch_count(self._h))
 
 
+def _stream_info(ci):
+    return {n: int(getattr(ci, n)) for n, _ in _lib.CStreamInfo._fields_}
+
+
+def stream_geometry(input_rate, settings=None, sync=True, max_push=48000):
+    """apt_stream_geometry: latency_work, max_push and device_bytes of a stream, computed on the host (no device)."""
+    s = (settings or Settings()).to_c()
+    ci = _lib.CStreamInfo()
+    raise_for(_lib.load().apt_stream_geometry(_rate_hz(input_rate), C.byref(s), int(bool(sync)), int(max_push), C.byref(ci)))
+    return _stream_info(ci)
+
+
+class Stream:
+    """apt_stream: live decoding.  push() audio as it arrives and get back the image rows that became final; the rows
+    of all pushes plus finish() are bit-identical to decode() on the whole recording."""
+
+    def __init__(self, input_rate, settings=None, sync=True, max_push=48000, device=0):
+        self._lib = _lib.load()
+        s = (settings or Settings()).to_c()
+        h = C.c_void_p(None)
+        raise_for(self._lib.apt_stream_create(int(device), _rate_hz(input_rate), C.byref(s), int(bool(sync)), int(max_push),
+                                              C.byref(h)))
+        self._h = h
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.apt_stream_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def _rows(self, n, call):
+        cap = C.c_uint64(0)
+        raise_for(self._lib.apt_stream_push_bound(self._h, n, C.byref(cap)))
+        out = np.empty(max(cap.value, PX_PER_ROW), dtype=np.float32)
+        got = C.c_uint64(0)
+        raise_for(call(out, got))
+        return out[: got.value].reshape(-1, PX_PER_ROW).copy()
+
+    def push(self, samples):
+        """float32 or int16 samples -> (k, 2080) float32 rows that became final."""
+        x = np.ascontiguousarray(samples).ravel()
+        fmt = _fmt_of(x)
+        return self._rows(x.size, lambda out, got: self._lib.apt_stream_push(self._h, x.ctypes.data, fmt, x.size, out.ctypes.data,
+                                                                             out.size, C.byref(got)))
+
+    def finish(self):
+        """The remaining rows; raises the error decode() would raise (too short, too few sync frames)."""
+        return self._rows(0, lambda out, got: self._lib.apt_stream_finish(self._h, out.ctypes.data, out.size, C.byref(got)))
+
+    def reset(self):
+        raise_for(self._lib.apt_stream_reset(self._h))
+
+    def positions(self):
+        n = C.c_size_t(0)
+        raise_for(self._lib.apt_stream_sync_positions(self._h, None, 0, C.byref(n)))
+        pos = np.empty(n.value, dtype=np.uint64)
+        if n.value:
+            raise_for(self._lib.apt_stream_sync_positions(self._h, pos.ctypes.data, pos.size, C.byref(n)))
+        return pos
+
+    def info(self):
+        ci = _lib.CStreamInfo()
+        raise_for(self._lib.apt_stream_get_info(self._h, C.byref(ci)))
+        return _stream_info(ci)
+
+
 def decode_batch(signals, input_rate, settings=None, sync=True, devices=None, streams_per_device=4):
     """Independent recordings sharded recording i -> devices[i % G], no collective (SURVEY §8e).
     Returns (list of row arrays or None, list of status codes)."""

@@ -88,7 +88,27 @@ extern "C" {
     pub fn apt_decode_image(signal: *const c_void, format: c_int, n: u64, input_rate: u32, s: *const apt_settings, sync: c_int,
                             ps: *const apt_process_settings, out: *mut u8, cap: u64, nout: *mut u64, info: *mut apt_image_info,
                             cb: apt_status_cb, user: *mut c_void) -> c_int;
+    // live decoding (apt_stream_*): push audio as it arrives, get the rows that became final
+    pub fn apt_stream_create(device: c_int, input_rate: u32, s: *const apt_settings, sync: c_int, max_push: u64,
+                             st: *mut *mut apt_stream) -> c_int;
+    pub fn apt_stream_destroy(st: *mut apt_stream);
+    pub fn apt_stream_push_bound(st: *mut apt_stream, n: u64, cap_floats: *mut u64) -> c_int;
+    pub fn apt_stream_push(st: *mut apt_stream, samples: *const c_void, format: c_int, n: u64, rows: *mut c_float, cap: u64,
+                           nout: *mut u64) -> c_int;
+    pub fn apt_stream_finish(st: *mut apt_stream, rows: *mut c_float, cap: u64, nout: *mut u64) -> c_int;
+    pub fn apt_stream_reset(st: *mut apt_stream) -> c_int;
+    pub fn apt_stream_sync_positions(st: *mut apt_stream, pos: *mut u64, cap: usize, n: *mut usize) -> c_int;
+    pub fn apt_stream_get_info(st: *mut apt_stream, info: *mut apt_stream_info) -> c_int;
+    pub fn apt_stream_geometry(input_rate: u32, s: *const apt_settings, sync: c_int, max_push: u64, info: *mut apt_stream_info) -> c_int;
 }
+
+#[repr(C)]
+pub struct apt_stream { _private: [u8; 0] }
+
+#[repr(C)]
+#[derive(Default, Clone, Copy)]
+pub struct apt_stream_info { pub samples_in: u64, pub work_final: u64, pub rows_out: u64, pub peaks: u64, pub latency_work: u64,
+                             pub max_push: u64, pub device_bytes: u64 }
 
 pub const APT_F32: c_int = 0;
 pub const APT_PCM16: c_int = 1;
