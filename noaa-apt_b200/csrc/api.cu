@@ -72,10 +72,10 @@ LaunchCtx stage_ctx() {
 int aptb200::free_decoder_buffers(apt_decoder *d) {
     cudaSetDevice(d->device);
     if (d->stream) cudaStreamSynchronize(d->stream);
-    for (void *p : {(void *)d->d_h, (void *)d->d_lp, (void *)d->d_one, (void *)d->d_guard, d->d_in, (void *)d->d_r,
+    d->front.release();
+    for (void *p : {(void *)d->d_lp, (void *)d->d_one, (void *)d->d_guard, d->d_in, (void *)d->d_r,
                     (void *)d->d_e, (void *)d->d_f, (void *)d->d_corr, (void *)d->d_aligned, (void *)d->d_root_list,
-                    (void *)d->d_root_count, (void *)d->d_pos, (void *)d->d_res, (void *)d->d_out, d->d_pick, (void *)d->d_tile_taps, (void *)d->d_tile_xs, (void *)d->d_conv,
-                    (void *)d->d_ph_table, (void *)d->d_ph_xs, (void *)d->d_ctl, (void *)d->d_desc, (void *)d->d_pool, (void *)d->d_roots2, (void *)d->d_tile_base, (void *)d->d_by_id})
+                    (void *)d->d_root_count, (void *)d->d_pos, (void *)d->d_res, (void *)d->d_out, d->d_pick, (void *)d->d_conv, (void *)d->d_ctl, (void *)d->d_desc, (void *)d->d_pool, (void *)d->d_roots2, (void *)d->d_tile_base, (void *)d->d_by_id})
         if (p) cudaFree(p);
     if (d->h_res) cudaFreeHost(d->h_res);
     if (d->h_out) cudaFreeHost(d->h_out);
@@ -246,27 +246,23 @@ extern "C" int apt_generate_sync_frame(uint32_t work_rate, int8_t *out, size_t c
 
 namespace {
 
-struct ResamplePlan {
-    Ratio r{};
-    bool polyphase = false;
-    std::vector<float> taps;
-    uint64_t nout = 0;
-};
-
-int plan_resample(uint64_t n, uint32_t in_rate, uint32_t out_rate, const apt_filter *f, ResamplePlan &rp) {
+// The first stage of dsp::resample_with_filter (dsp.rs:62-98) for the caller's filter, and its output length.
+int plan_resample(uint64_t n, uint32_t in_rate, uint32_t out_rate, const apt_filter *f, FrontPlan &fp, uint64_t &nout) {
     if (!f) return fail(APT_ERR_BAD_ARG, "null filter");
-    int st = resample_ratio(in_rate, out_rate, rp.r);
+    Ratio r{};
+    int st = resample_ratio(in_rate, out_rate, r);
     if (st == APT_ERR_RESAMPLE_TO_ZERO) return fail(st, "Can't resample to 0Hz");
     if (st == APT_ERR_RATE_OVERFLOW)
         return fail(st, "Can't resample, looks like the sample rates do not have a big divisor in common. "
-                        "input_rate: %u, output_rate: %u, l: %u, m: %u", in_rate, out_rate, rp.r.l, rp.r.m);
+                        "input_rate: %u, output_rate: %u, l: %u, m: %u", in_rate, out_rate, r.l, r.m);
     if (st != APT_OK) return fail(st, "invalid input rate");
-    rp.polyphase = rp.r.l > 1;
     apt_filter ff = *f;
-    if (rp.polyphase) resample_filter(ff, in_rate, in_rate * rp.r.l);
-    st = design(ff, rp.taps);
+    if (r.l > 1) resample_filter(ff, in_rate, in_rate * r.l);   // dsp.rs:93
+    std::vector<float> taps;
+    st = design(ff, taps);
     if (st != APT_OK) return fail(st, "filter cannot be designed");
-    rp.nout = rp.polyphase ? polyphase_len(n, rp.r.l, rp.r.m, rp.taps.size()) : n / rp.r.m;
+    fp = make_front(r, std::move(taps));
+    nout = fp.work_len(n);
     return APT_OK;
 }
 
@@ -275,71 +271,28 @@ int plan_resample(uint64_t n, uint32_t in_rate, uint32_t out_rate, const apt_fil
 extern "C" int apt_resample_len(uint64_t n, uint32_t input_rate, uint32_t output_rate, const apt_filter *f,
                                 uint64_t *nout) {
     if (!nout) return fail(APT_ERR_BAD_ARG, "null argument");
-    ResamplePlan rp;
-    APT_TRY(plan_resample(n, input_rate, output_rate, f, rp));
-    *nout = rp.nout;
-    return APT_OK;
+    FrontPlan fp;
+    return plan_resample(n, input_rate, output_rate, f, fp, *nout);
 }
 
 extern "C" int apt_resample_with_filter(const float *signal, uint64_t n, uint32_t input_rate, uint32_t output_rate,
                                         const apt_filter *f, float *out, uint64_t cap, uint64_t *nout) {
     if (!nout || (!signal && n)) return fail(APT_ERR_BAD_ARG, "null argument");
-    ResamplePlan rp;
-    APT_TRY(plan_resample(n, input_rate, output_rate, f, rp));
-    *nout = rp.nout;
-    if (rp.nout > cap || (!out && rp.nout)) return fail(APT_ERR_CAPACITY, "output needs %llu floats", (unsigned long long)rp.nout);
-    if (rp.nout == 0) return APT_OK;
+    FrontPlan fp;
+    APT_TRY(plan_resample(n, input_rate, output_rate, f, fp, *nout));
+    const uint64_t ny = *nout;
+    if (ny > cap || (!out && ny)) return fail(APT_ERR_CAPACITY, "output needs %llu floats", (unsigned long long)ny);
+    if (ny == 0) return APT_OK;
     APT_TRY(require_device());
-    DevBuf dx, dh, dy;
+    FrontTables tables;
+    DevBuf dx, dy;
     APT_TRY(dx.alloc(n * sizeof(float)));
-    APT_TRY(dh.alloc(rp.taps.size() * sizeof(float)));
-    APT_TRY(dy.alloc(rp.nout * sizeof(float)));
+    APT_TRY(dy.alloc(ny * sizeof(float)));
     APT_CUDA(cudaMemcpy(dx.p, signal, n * sizeof(float), cudaMemcpyHostToDevice));
-    APT_CUDA(cudaMemcpy(dh.p, rp.taps.data(), rp.taps.size() * sizeof(float), cudaMemcpyHostToDevice));
-    const LaunchCtx c = stage_ctx();
-    if (rp.polyphase) {
-        const uint64_t off2 = 2 * ((static_cast<uint64_t>(rp.taps.size()) - 1) / 2);
-        TilePlan tp{};
-        std::vector<float> tt;
-        std::vector<u32> xs;
-        UtPlan up{};
-        std::vector<float> us;
-        // kernel preference as in make_plan: tiled, then uniform-tap, then phase-major
-        if (!getenv("APTB200_GENERIC_RESAMPLER") && make_tile_plan(rp.r.l, rp.r.m, rp.taps, tp, tt, xs)) {
-            DevBuf dt, dg;
-            APT_TRY(dt.alloc(tt.size() * sizeof(float)));
-            APT_TRY(dg.alloc(xs.size() * sizeof(u32)));
-            APT_CUDA(cudaMemcpy(dt.p, tt.data(), tt.size() * sizeof(float), cudaMemcpyHostToDevice));
-            APT_CUDA(cudaMemcpy(dg.p, xs.data(), xs.size() * sizeof(u32), cudaMemcpyHostToDevice));
-            APT_TRY(launch_polyphase_tiled(c, dx.as<float>(), n, dt.as<float>(), dg.as<u32>(), tp, rp.nout, 0, 0, false, 0.f,
-                                           1.f, dy.as<float>()));
-            APT_CUDA(cudaDeviceSynchronize());
-        } else if (!getenv("APTB200_GENERIC_RESAMPLER") && make_ut_plan(rp.r.l, rp.r.m, rp.taps, up, us)) {
-            APT_TRY(launch_polyphase_ut(c, dx.as<float>(), n, dh.as<float>(), up, us, rp.nout, 0, 0, false, 0.f, 1.f, dy.as<float>()));
-            APT_CUDA(cudaDeviceSynchronize());
-        } else {
-            PhPlan pp{};
-            std::vector<float> ptab;
-            std::vector<unsigned short> pxs;
-            if (!getenv("APTB200_GENERIC_RESAMPLER") && make_ph_plan(rp.r.l, rp.r.m, rp.taps, pp, ptab, pxs)) {
-                DevBuf dt, dg;
-                APT_TRY(dt.alloc(ptab.size() * sizeof(float)));
-                APT_TRY(dg.alloc(pxs.size() * sizeof(unsigned short)));
-                APT_CUDA(cudaMemcpy(dt.p, ptab.data(), ptab.size() * sizeof(float), cudaMemcpyHostToDevice));
-                APT_CUDA(cudaMemcpy(dg.p, pxs.data(), pxs.size() * sizeof(unsigned short), cudaMemcpyHostToDevice));
-                APT_TRY(launch_polyphase_ph(c, dx.p, APT_F32, n, dt.as<float>(), dg.as<unsigned short>(), pp, rp.nout, 0, 0, false, 0.f,
-                                            1.f, dy.as<float>()));
-                APT_CUDA(cudaDeviceSynchronize());
-            } else {
-                APT_TRY(launch_polyphase(c, dx.p, APT_F32, n, dh.as<float>(), rp.r.l, rp.r.m, off2, 0, rp.nout, false, 0.f, 1.f,
-                                         dy.as<float>()));
-            }
-        }
-    } else {
-        APT_TRY(launch_fir_decimate(c, dx.p, APT_F32, dh.as<float>(), static_cast<u32>(rp.taps.size()), rp.r.m,
-                                    rp.nout, dy.as<float>()));
-    }
-    APT_CUDA(cudaMemcpy(out, dy.p, rp.nout * sizeof(float), cudaMemcpyDeviceToHost));
+    APT_TRY(tables.upload(fp));
+    APT_TRY(front_launch(stage_ctx(), fp, tables, dx.p, APT_F32, nullptr, n, ny, 0, fp.units(ny), false, 0.f, 1.f, nullptr,
+                         dy.as<float>(), nullptr));
+    APT_CUDA(cudaMemcpy(out, dy.p, ny * sizeof(float), cudaMemcpyDeviceToHost));
     return APT_OK;
 }
 
@@ -463,32 +416,15 @@ namespace aptb200 {
 int upload_plan(apt_decoder *d) {
     const Plan &p = d->plan;
     const float one = 1.f;
-    APT_CUDA(cudaMalloc(&d->d_h, p.h.size() * sizeof(float)));
-    APT_CUDA(cudaMemcpy(d->d_h, p.h.data(), p.h.size() * sizeof(float), cudaMemcpyHostToDevice));
+    APT_TRY(d->front.upload(p.front));
     APT_CUDA(cudaMalloc(&d->d_lp, p.lp.size() * sizeof(float)));
     APT_CUDA(cudaMemcpy(d->d_lp, p.lp.data(), p.lp.size() * sizeof(float), cudaMemcpyHostToDevice));
     APT_CUDA(cudaMalloc(&d->d_one, sizeof(float)));
     APT_CUDA(cudaMemcpy(d->d_one, &one, sizeof(float), cudaMemcpyHostToDevice));
-    if (p.ph) {
-        APT_CUDA(cudaMalloc(&d->d_ph_table, p.ph_table.size() * sizeof(float)));
-        APT_CUDA(cudaMemcpy(d->d_ph_table, p.ph_table.data(), p.ph_table.size() * sizeof(float), cudaMemcpyHostToDevice));
-        APT_CUDA(cudaMalloc(&d->d_ph_xs, p.ph_xs.size() * sizeof(unsigned short)));
-        APT_CUDA(cudaMemcpy(d->d_ph_xs, p.ph_xs.data(), p.ph_xs.size() * sizeof(unsigned short), cudaMemcpyHostToDevice));
-    }
-    if (p.tiled) {
-        APT_CUDA(cudaMalloc(&d->d_tile_taps, p.tile_taps.size() * sizeof(float)));
-        APT_CUDA(cudaMemcpy(d->d_tile_taps, p.tile_taps.data(), p.tile_taps.size() * sizeof(float), cudaMemcpyHostToDevice));
-        APT_CUDA(cudaMalloc(&d->d_tile_xs, p.tile_xs.size() * sizeof(u32)));
-        APT_CUDA(cudaMemcpy(d->d_tile_xs, p.tile_xs.data(), p.tile_xs.size() * sizeof(u32), cudaMemcpyHostToDevice));
-    }
     return APT_OK;
 }
 
-uint64_t plan_table_bytes(const Plan &p) {
-    return (p.h.size() + p.lp.size() + 1) * sizeof(float) +
-           (p.ph ? p.ph_table.size() * sizeof(float) + p.ph_xs.size() * sizeof(unsigned short) : 0) +
-           (p.tiled ? p.tile_taps.size() * sizeof(float) + p.tile_xs.size() * sizeof(u32) : 0);
-}
+uint64_t plan_table_bytes(const Plan &p) { return FrontTables::bytes(p.front) + (p.lp.size() + 1) * sizeof(float); }
 
 }  // namespace aptb200
 
@@ -522,10 +458,10 @@ extern "C" int apt_decoder_create(int device, uint32_t input_rate, const apt_set
         uint64_t chunk = 32ull << 20;
         if (const char *e = getenv("APTB200_CHUNK_SAMPLES")) chunk = std::max<uint64_t>(strtoull(e, nullptr, 10), 1u << 16);
         chunk &= ~7ull;   // both staging halves stay 16-byte aligned for f32 and PCM16 samples
-        d->chunk_samples = (max_samples > 2 * chunk && p.first_polyphase) ? chunk : 0;
-        if (getenv("APTB200_CHUNK_SAMPLES") && max_samples > chunk && p.first_polyphase) d->chunk_samples = chunk;
+        d->chunk_samples = (max_samples > 2 * chunk && p.front.chunkable()) ? chunk : 0;
+        if (getenv("APTB200_CHUNK_SAMPLES") && max_samples > chunk && p.front.chunkable()) d->chunk_samples = chunk;
     }
-    d->max_work = plan_work_len(p, max_samples);
+    d->max_work = p.front.work_len(max_samples);
     d->max_out = plan_out_bound(p, max_samples);
     if (d->max_work >= (1ull << 32))
         return fail(APT_ERR_BAD_ARG, "recording too long: %llu work-rate samples (limit 2^32-1)",
@@ -533,7 +469,7 @@ extern "C" int apt_decoder_create(int device, uint32_t input_rate, const apt_set
 
     APT_TRY(upload_plan(d.get()));
     const size_t work_bytes = std::max<uint64_t>(d->max_work, 1) * sizeof(float);
-    if (!p.first_polyphase) APT_CUDA(cudaMalloc(&d->d_r, work_bytes));
+    if (p.front.needs_scratch()) APT_CUDA(cudaMalloc(&d->d_r, work_bytes));
     APT_CUDA(cudaMalloc(&d->d_e, work_bytes));
     APT_TRY(alloc_sync_buffers(d.get()));
     if (!d->use_records) APT_TRY(ensure_legacy_sync(d.get()));
@@ -556,19 +492,11 @@ namespace {
 
 // contrast bounds + u8 map of the rows the job leaves in d_out; the head of the control block follows the job to the host
 int enqueue_image_stage(apt_decoder *d, unsigned char *out8) {
-    const Plan &p = d->plan;
     const LaunchCtx c{d->stream, d->sm_count};
     const u32 max_rows = static_cast<u32>(std::max<uint64_t>(d->max_out / kPxPerRow, 1));
     const u32 fixed = d->job_sync ? 0u : static_cast<u32>(d->job_fixed_out / kPxPerRow);
-    (void)p;
     if (d->proc_active) {
-        struct Hook : KernelHook {
-            apt_decoder *d;
-            int slot = -1;
-            explicit Hook(apt_decoder *dec) : d(dec) {}
-            void begin(const char *name) override { slot = prof_begin(d, name); }
-            void end() override { prof_end(d, slot); }
-        } hook(d);
+        DecoderHook hook(d);
         ProcessLaunch a{};
         a.rows = d->d_out;
         a.result = d->job_sync ? d->d_res : nullptr;
@@ -619,7 +547,7 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
     d->job_cap = cap;
     d->job_fixed_out = 0;
 
-    const uint64_t nwork = plan_work_len(p, n);
+    const uint64_t nwork = p.front.work_len(n);
     d->job_work = nwork;
     if (nwork < 10ull * p.row) {   // decode.rs:79-83
         d->job_status = fail(APT_ERR_TOO_SHORT, "Got less than 10 rows of samples, audio file is too short");
@@ -678,7 +606,7 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
                                    cudaHostAllocDefault));   // sized for f32 rows: also holds the u8 image
         // Recordings longer than the chunk size are uploaded in chunks that overlap the resampling; shorter ones
         // (and the L == 1 first stage) are staged whole.
-        const bool chunked = d->chunk_samples != 0 && n > d->chunk_samples && p.first_polyphase;
+        const bool chunked = d->chunk_samples != 0 && n > d->chunk_samples && p.front.chunkable();
         if (d->chunk_samples != 0 && n > d->chunk_samples && !chunked)
             return fail(APT_ERR_BAD_ARG, "recording longer than the staging buffer and the first stage is not polyphase");
         const uint64_t stage_samples = d->chunk_samples ? 2 * d->chunk_samples : d->max_samples;
@@ -692,13 +620,7 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
                     APT_CUDA(cudaEventCreateWithFlags(&d->ev_free[i], cudaEventDisableTiming));
                 }
             }
-            if (format == APT_PCM16 && d->conv_cap < d->chunk_samples) {
-                if (d->d_conv) APT_CUDA(cudaFree(d->d_conv));
-                d->d_conv = nullptr;
-                d->conv_cap = 0;
-                APT_CUDA(cudaMalloc(&d->d_conv, d->chunk_samples * sizeof(float)));
-                d->conv_cap = d->chunk_samples;
-            }
+            if (format == APT_PCM16) APT_TRY(ensure_conv(d, d->chunk_samples, d->chunk_samples));
             host_chunked = signal;
             dev_in = nullptr;
         } else if (d->job_in_pageable && d->stager) {
@@ -1119,7 +1041,7 @@ int decode_oneshot(const void *signal, int format, uint64_t n, uint32_t input_ra
         // errors that do not need a device come first, in the reference's order
         Plan p;
         APT_TRY(make_plan(input_rate, *s, p));
-        if (plan_work_len(p, n) < 10ull * p.row)
+        if (p.front.work_len(n) < 10ull * p.row)
             return fail(APT_ERR_TOO_SHORT, "Got less than 10 rows of samples, audio file is too short");
         if (sync && !p.work_multiple) return fail(APT_ERR_WORK_RATE, "work_rate is not multiple of FINAL_RATE");
     }

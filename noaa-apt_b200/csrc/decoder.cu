@@ -37,31 +37,23 @@ int make_plan(uint32_t input_rate, const apt_settings &s, Plan &p) {
         return fail(APT_ERR_BAD_ARG, "work_rate %u is too large", s.work_rate);
 
     // decode.rs:65-77 -> dsp::resample_with_filter (dsp.rs:62-98)
-    int st = resample_ratio(input_rate, s.work_rate, p.first);
+    Ratio first{};
+    int st = resample_ratio(input_rate, s.work_rate, first);
     if (st == APT_ERR_RESAMPLE_TO_ZERO) return fail(st, "Can't resample to 0Hz");
     if (st == APT_ERR_RATE_OVERFLOW)
         return fail(st, "Can't resample, looks like the sample rates do not have a big divisor in common. "
                         "input_rate: %u, output_rate: %u, l: %u, m: %u",
-                    input_rate, s.work_rate, p.first.l, p.first.m);
+                    input_rate, s.work_rate, first.l, first.m);
     if (st != APT_OK) return fail(st, "invalid input rate %u", input_rate);
-    p.first_polyphase = p.first.l > 1;
 
     apt_filter rf{APT_FILTER_LOWPASS_DC, Freq::hz(s.resample_cutout, input_rate).get_pi_rad(), s.resample_atten,
                   Freq::hz(s.resample_delta_freq, input_rate).get_pi_rad()};
-    if (p.first_polyphase) resample_filter(rf, input_rate, input_rate * p.first.l);   // dsp.rs:93
-    st = design(rf, p.h);
+    if (first.l > 1) resample_filter(rf, input_rate, input_rate * first.l);   // dsp.rs:93
+    std::vector<float> h;
+    st = design(rf, h);
     if (st != APT_OK) return fail(st, "resampling filter cannot be designed (atten %g, delta_w %g)",
                                   (double)rf.atten, (double)rf.delta_w_pi);
-    p.off2 = 2 * ((static_cast<uint64_t>(p.h.size()) - 1) / 2);
-    p.tiled = p.first_polyphase && !getenv("APTB200_GENERIC_RESAMPLER") &&
-              make_tile_plan(p.first.l, p.first.m, p.h, p.tile, p.tile_taps, p.tile_xs);
-    // the uniform-tap kernel only where the tiled one does not fit: without a packed fp32 FMA (sm_90) its one uniform
-    // tap load per FMA pair makes it the slower of the two (48 kHz x 900 s: 214 us against
-    // 125 us on an H100 SXM at 700 W)
-    p.ut = p.first_polyphase && !p.tiled && !getenv("APTB200_GENERIC_RESAMPLER") &&
-           make_ut_plan(p.first.l, p.first.m, p.h, p.utp, p.ut_stream);
-    p.ph = p.first_polyphase && !p.ut && !p.tiled && !getenv("APTB200_GENERIC_RESAMPLER") &&
-           make_ph_plan(p.first.l, p.first.m, p.h, p.php, p.ph_table, p.ph_xs);
+    p.front = make_front(first, std::move(h));
 
     // decode.rs:95-100
     const float cut = static_cast<float>(kFinalRate) / static_cast<float>(s.work_rate);
@@ -87,13 +79,8 @@ int make_plan(uint32_t input_rate, const apt_settings &s, Plan &p) {
     return APT_OK;
 }
 
-uint64_t plan_work_len(const Plan &p, uint64_t n) {
-    if (p.first_polyphase) return polyphase_len(n, p.first.l, p.first.m, p.h.size());
-    return n / p.first.m;   // decimate, dsp.rs:299-301
-}
-
 uint64_t plan_out_bound(const Plan &p, uint64_t n) {
-    const uint64_t nw = plan_work_len(p, n);
+    const uint64_t nw = p.front.work_len(n);
     if (p.row == 0) return 0;
     const uint64_t rows = nw / p.row;
     if (p.work_multiple) return rows * kPxPerRow;
@@ -125,11 +112,9 @@ void prof_end(apt_decoder *d, int slot) {
 
 namespace {
 
-struct Prof {
-    apt_decoder *d;
-    int slot;
-    Prof(apt_decoder *dec, const char *name) : d(dec), slot(prof_begin(dec, name)) {}
-    ~Prof() { prof_end(d, slot); }
+struct Prof : DecoderHook {   // a slot around a scope
+    Prof(apt_decoder *dec, const char *name) : DecoderHook(dec) { begin(name); }
+    ~Prof() { end(); }
 };
 
 }  // namespace
@@ -218,108 +203,35 @@ int materialise_stages(apt_decoder *d) {
     return APT_OK;
 }
 
-// one of the two TMA-staged resamplers serves this decoder's first stage (they take f32 samples only)
-static bool fast_front(const apt_decoder *d) { return d->plan.ut || (d->plan.tiled && d->d_tile_taps); }
-static bool ph_front(const apt_decoder *d) { return d->plan.ph && d->d_ph_table; }
-
-FrontUnits front_units(const Plan &p) {
-    const uint64_t l = p.first.l, m = p.first.m;
-    FrontUnits u;
-    u.tiled = p.ut || p.tiled || p.ph;   // apt_decoder_create uploads the tables of whichever the plan chose
-    if (p.ut) {
-        u.unit_in = static_cast<uint64_t>(p.utp.rb) * m;
-        u.unit_out = static_cast<uint64_t>(p.utp.rb) * l;
-        u.before = p.utp.back;
-        u.after = p.utp.slot_floats - p.utp.back;           // a block's span beyond its first row's first sample
-    } else if (p.ph) {
-        u.unit_in = static_cast<uint64_t>(kPhTilePeriods) * m;              // a tile = 32 periods of m samples
-        u.unit_out = static_cast<uint64_t>(kPhTilePeriods) * l;
-        u.before = m + 4;                                                   // the period in front of the tile (+4 alignment)
-        u.after = static_cast<uint64_t>(kPhTilePeriods - 1) * m + p.php.row_len;
-    } else if (u.tiled) {
-        u.unit_in = static_cast<uint64_t>(p.tile.qt) * p.tile.p_in;
-        u.unit_out = static_cast<uint64_t>(p.tile.qt) * p.tile.p_out;
-        u.before = p.tile.p_in - p.tile_xs.back();       // halo row: window of the last group one super-period back
-        u.after = static_cast<uint64_t>(p.tile.qt - 1) * p.tile.p_in + p.tile.row_len;
-    } else {
-        u.unit_out = 1;                                  // one output of the generic kernel (or of filter + decimate)
-    }
-    return u;
-}
-
-void front_span(const Plan &p, const FrontUnits &fu, uint64_t u0, uint64_t u1, uint64_t n, uint64_t &xa, uint64_t &xb) {
-    const uint64_t l = p.first.l, m = p.first.m;
-    if (!p.first_polyphase) {                           // out[k] = sum_j x[k*m - j] c[j] (k > j), and e[k] reads r[k-1]
-        const uint64_t ntaps = p.h.size();
-        const uint64_t kfirst = u0 == 0 ? 0 : u0 - 1;
-        xa = kfirst * m > ntaps ? kfirst * m - ntaps : 0;
-        xb = std::min<uint64_t>(n, u1 * m);             // output k exists once (k+1)*m samples do (decimate, dsp.rs:299-301)
-    } else if (fu.tiled) {
-        xa = u0 == 0 ? 0 : u0 * fu.unit_in - fu.before;
-        xb = std::min<uint64_t>(n, (u1 - 1) * fu.unit_in + fu.after);
-    } else {
-        const uint64_t kfirst = u0 == 0 ? 0 : u0 - 1;                    // the envelope needs r[k0 - 1]
-        xa = (kfirst * m + l - 1) / l;
-        xa &= ~static_cast<uint64_t>(7);                                  // keep 16-byte alignment of PCM16 chunks
-        xb = std::min<uint64_t>(n, ((u1 - 1) * m + p.off2) / l + 1);
-    }
-}
-
-// fast_resampling + demodulate of outputs produced from a device-resident (or staged) chunk.
-// `in` is the address sample 0 of the recording would have (a biased pointer for chunk buffers), `e` the address of
-// envelope sample 0.
-int launch_front_polyphase(apt_decoder *d, const void *in, int format, uint64_t n, uint64_t nwork,
-                           uint64_t tile_begin, uint64_t tile_end, uint64_t k_begin, uint64_t k_end,
-                           float *conv_base /* f32 view of a PCM16 chunk (already biased) or nullptr */, float *e) {
-    const Plan &p = d->plan;
-    const LaunchCtx c{d->stream, d->sm_count};
-    if (p.ut && (format == APT_F32 || conv_base)) {
-        const float *fin = format == APT_F32 ? static_cast<const float *>(in) : conv_base;
-        if ((reinterpret_cast<uintptr_t>(fin) & 15) == 0)
-            return launch_polyphase_ut(c, fin, n, d->d_h, p.utp, p.ut_stream, nwork, tile_begin, tile_end, true, p.cosphi2,
-                                       p.sinphi, e);
-    }
-    if (p.tiled && d->d_tile_taps && (format == APT_F32 || conv_base)) {
-        const float *fin = format == APT_F32 ? static_cast<const float *>(in) : conv_base;
-        return launch_polyphase_tiled(c, fin, n, d->d_tile_taps, d->d_tile_xs, p.tile, nwork, tile_begin, tile_end, true,
-                                      p.cosphi2, p.sinphi, e);
-    }
-    if (ph_front(d))   // large L: phase-major kernel, f32 or PCM16 samples (the cast is part of its row staging)
-        return launch_polyphase_ph(c, in, format, n, d->d_ph_table, d->d_ph_xs, p.php, nwork, tile_begin, tile_end, true, p.cosphi2,
-                                   p.sinphi, e);
-    return launch_polyphase(c, in, format, n, d->d_h, p.first.l, p.first.m, p.off2, k_begin, k_end ? k_end : nwork, true,
-                            p.cosphi2, p.sinphi, e);
+int ensure_conv(apt_decoder *d, uint64_t need, uint64_t alloc) {
+    if (d->conv_cap >= need) return APT_OK;
+    if (d->d_conv) APT_CUDA(cudaFree(d->d_conv));
+    d->d_conv = nullptr;
+    d->conv_cap = 0;
+    APT_CUDA(cudaMalloc(&d->d_conv, alloc * sizeof(float)));
+    d->conv_cap = alloc;
+    return APT_OK;
 }
 
 // Long host recording: upload in chunks (with the filter-length overlap each chunk needs) on the copy stream while
-// the previous chunk is resampled on the compute stream.  Only the polyphase first stage is chunked.
+// the previous chunk is resampled on the compute stream.  Only a polyphase first stage is chunked.
 static int enqueue_front_chunked(apt_decoder *d, const void *host, int format, uint64_t n, uint64_t nwork) {
     const Plan &p = d->plan;
+    const FrontPlan &f = p.front;
     const LaunchCtx c{d->stream, d->sm_count};
     const size_t sb = format == APT_PCM16 ? 2 : 4;
     const uint64_t cap = d->chunk_samples;
-    const uint64_t l = p.first.l, m = p.first.m;
-    const FrontUnits fu = front_units(p);
-    const bool tiled = fu.tiled;
-    uint64_t units, per_chunk;            // tiles / blocks or outputs
-    if (tiled) {
-        units = (nwork + fu.unit_out - 1) / fu.unit_out;
-        if (cap < fu.before + fu.after + fu.unit_in + 64) return fail(APT_ERR_BAD_ARG, "chunk too small for one tile");
-        per_chunk = (cap - fu.before - fu.after - 64) / fu.unit_in + 1;
-    } else {
-        units = nwork;
-        const uint64_t halo = p.off2 / l + 4;
-        if (cap < 2 * halo + 1024) return fail(APT_ERR_BAD_ARG, "chunk too small for the filter");
-        per_chunk = (cap - 2 * halo) * l / m;
-    }
-    if (per_chunk == 0) return fail(APT_ERR_BAD_ARG, "chunk too small");
+    const uint64_t units = f.units(nwork);
+    uint64_t per_chunk;
+    APT_TRY(f.chunk_units(cap, per_chunk));
     char *stage[2] = {static_cast<char *>(d->d_in), static_cast<char *>(d->d_in) + cap * 4};
     uint64_t chunk = 0;
+    Prof pr(d, kFrontSlot);
     for (uint64_t u0 = 0; u0 < units; u0 += per_chunk, ++chunk) {
         const uint64_t u1 = std::min(units, u0 + per_chunk);
         const int b = static_cast<int>(chunk & 1);
         uint64_t xa, xb;
-        front_span(p, fu, u0, u1, n, xa, xb);
+        f.span(u0, u1, n, xa, xb);
         if (xb <= xa || xb - xa > cap) return fail(APT_ERR_BAD_ARG, "internal: chunk geometry (%llu..%llu, cap %llu)",
                                                    (unsigned long long)xa, (unsigned long long)xb, (unsigned long long)cap);
         // copy stream: wait until the compute stream has finished with this buffer, then upload
@@ -331,17 +243,16 @@ static int enqueue_front_chunked(apt_decoder *d, const void *host, int format, u
                                      d->copy_stream));
         APT_CUDA(cudaEventRecord(d->ev_copied[b], d->copy_stream));
         APT_CUDA(cudaStreamWaitEvent(d->stream, d->ev_copied[b], 0));
-        // compute stream: (cast,) resample + envelope of this chunk's outputs
-        const void *in_biased = stage[b] - xa * sb;
+        // compute stream: (cast,) resample + envelope of this chunk's units
         float *conv_biased = nullptr;
-        if (format == APT_PCM16 && fast_front(d)) {
+        if (format == APT_PCM16 && f.wants_f32()) {
             APT_TRY(launch_pcm16_to_f32(c, reinterpret_cast<const int16_t *>(stage[b]), xb - xa, d->d_conv));
             d->launches++;
             conv_biased = d->d_conv - xa;
         }
         d->launches++;
-        APT_TRY(launch_front_polyphase(d, in_biased, format, n, nwork, tiled ? u0 : 0, tiled ? u1 : 0, tiled ? 0 : u0,
-                                       tiled ? 0 : u1, conv_biased, d->d_e));
+        APT_TRY(front_launch(c, f, d->front, stage[b] - xa * sb, format, conv_biased, n, nwork, u0, u1, true, p.cosphi2, p.sinphi,
+                             nullptr, d->d_e, nullptr));
         APT_CUDA(cudaEventRecord(d->ev_free[b], d->stream));
     }
     d->job_chunks = chunk;
@@ -357,38 +268,23 @@ static int enqueue_front(apt_decoder *d, const void *in, int format, uint64_t n,
         d->cb(0.1f, msg, d->cb_user);                                       // decode.rs:63
     }
     d->job_chunks = 0;
-    if (p.first_polyphase) {
-        // fast_resampling + demodulate fused: r is never written (decode.rs:77,89)
-        Prof pr(d, "resample_envelope");
-        if (host_chunked) {
-            APT_TRY(enqueue_front_chunked(d, host_chunked, format, n, nwork));
-        } else {
-            float *conv = nullptr;
-            if (format == APT_PCM16 && fast_front(d) && (reinterpret_cast<uintptr_t>(in) & 15) == 0) {
-                // the WAV's int16 samples: `as f32` (wav.rs:37) on the device, then the same tiled kernel
-                if (d->conv_cap < n) {
-                    if (d->d_conv) APT_CUDA(cudaFree(d->d_conv));
-                    d->d_conv = nullptr;
-                    d->conv_cap = 0;
-                    APT_CUDA(cudaMalloc(&d->d_conv, std::max<uint64_t>(d->max_samples, n) * sizeof(float)));
-                    d->conv_cap = std::max<uint64_t>(d->max_samples, n);
-                }
-                APT_TRY(launch_pcm16_to_f32(c, static_cast<const int16_t *>(in), n, d->d_conv));
-                d->launches++;
-                conv = d->d_conv;
-            }
-            APT_TRY(launch_front_polyphase(d, in, format, n, nwork, 0, 0, 0, 0, conv, d->d_e));
-        }
-        if (d->cb) d->cb(0.4f, "Demodulating", d->cb_user);                 // decode.rs:87
+    if (host_chunked) {
+        APT_TRY(enqueue_front_chunked(d, host_chunked, format, n, nwork));
     } else {
-        {
-            Prof pr(d, "filter_decimate");
-            APT_TRY(launch_fir_decimate(c, in, format, d->d_h, static_cast<u32>(p.h.size()), p.first.m, nwork, d->d_r));
+        const float *conv = nullptr;
+        if (format == APT_PCM16 && p.front.wants_f32() && (reinterpret_cast<uintptr_t>(in) & 15) == 0) {
+            // the WAV's int16 samples: `as f32` (wav.rs:37) on the device, then the f32 kernel
+            APT_TRY(ensure_conv(d, n, std::max<uint64_t>(d->max_samples, n)));
+            APT_TRY(launch_pcm16_to_f32(c, static_cast<const int16_t *>(in), n, d->d_conv));
+            d->launches++;
+            conv = d->d_conv;
         }
-        if (d->cb) d->cb(0.4f, "Demodulating", d->cb_user);
-        Prof pr(d, "envelope");
-        APT_TRY(launch_envelope(c, d->d_r, nwork, p.cosphi2, p.sinphi, d->d_e));
+        // resample (decode.rs:77) + demodulate (decode.rs:89)
+        DecoderHook hook(d);
+        APT_TRY(front_launch(c, p.front, d->front, in, format, conv, n, nwork, 0, p.front.units(nwork), true, p.cosphi2, p.sinphi,
+                             d->d_r, d->d_e, &hook));
     }
+    if (d->cb) d->cb(0.4f, "Demodulating", d->cb_user);                     // decode.rs:87
     if (d->cb) d->cb(0.42f, "Filtering", d->cb_user);                       // decode.rs:93
     return APT_OK;
 }
@@ -442,7 +338,7 @@ int decoder_enqueue(apt_decoder *d, const void *in, int format, uint64_t n, int 
     const Plan &p = d->plan;
     LaunchCtx c{d->stream, d->sm_count};
     c.busy = d->device >= 0 && d->device < 64 && g_jobs_in_flight[d->device].load(std::memory_order_relaxed) > 0 ? 1 : 0;
-    const uint64_t nwork = plan_work_len(p, n);
+    const uint64_t nwork = p.front.work_len(n);
     d->job_work = nwork;
     d->ev_used = 0;
     set_envelope_l2_window(d, nwork, c.busy == 0);

@@ -12,6 +12,7 @@
 #include <memory>
 
 #include "filters_host.hpp"
+#include "front.hpp"
 #include "hostpool.hpp"
 #include "launch.hpp"
 
@@ -26,10 +27,7 @@ constexpr uint32_t kCarrierHz = 2400;
 struct Plan {
     uint32_t input_rate = 0;
     apt_settings st{};
-    Ratio first{};                 // input_rate -> work_rate (dsp.rs:73-75)
-    bool first_polyphase = false;  // L > 1: fast_resampling; else filter + decimate
-    std::vector<float> h;          // resampling filter taps (LowpassDcRemoval, decode.rs:65-76)
-    uint64_t off2 = 0;             // 2 * ((N-1)/2): highest tap index fast_resampling touches
+    FrontPlan front;               // input_rate -> work_rate with the LowpassDcRemoval filter (decode.rs:65-89)
     std::vector<float> lp;         // demodulation low-pass taps (Lowpass, decode.rs:95-100)
     float cosphi2 = 0.f, sinphi = 1.f;   // dsp.rs:360-363
     uint32_t row = 0;              // samples_per_work_row (decode.rs:55)
@@ -38,39 +36,11 @@ struct Plan {
     uint32_t dec = 0;              // work_rate / 4160 when work_multiple
     Ratio last{};                  // work_rate -> 4160 for the final NoFilter resample
     std::vector<int8_t> guard;     // sync template (empty unless work_multiple)
-    bool tiled = false;            // the tiled sm_90a resampler fits this (L, M, taps)
-    TilePlan tile{};
-    std::vector<float> tile_taps;
-    std::vector<u32> tile_xs;
-    bool ph = false;               // the phase-major resampler (large L: 11025 / 22050 / 44100 Hz) fits
-    PhPlan php{};
-    std::vector<float> ph_table;
-    std::vector<unsigned short> ph_xs;
-    bool ut = false;               // the uniform-tap resampler (taps as a kernel parameter) fits: preferred
-    UtPlan utp{};
-    std::vector<float> ut_stream;
 };
 
 int make_plan(uint32_t input_rate, const apt_settings &s, Plan &plan);
-// N_w for n input samples.
-uint64_t plan_work_len(const Plan &p, uint64_t n);
 // decode() output length for no-sync / upper bound for sync.
 uint64_t plan_out_bound(const Plan &p, uint64_t n);
-
-// First-stage units (decoder.cu): a unit (tile of the tiled / phase-major kernel, block of the uniform-tap kernel) makes
-// unit_out envelope outputs from unit_in new samples, plus `before` samples in front of the first unit of a run and
-// `after` beyond the start of the last one.  The generic polyphase kernel and filter + decimate work per output
-// (tiled == false, unit_out == 1).  Shared by the chunked upload and the stream.
-struct FrontUnits {
-    bool tiled = false;
-    uint64_t unit_in = 0, unit_out = 0, before = 0, after = 0;
-};
-FrontUnits front_units(const Plan &p);
-// Input samples [xa, xb) units [u0, u1) read from a recording of n samples.
-void front_span(const Plan &p, const FrontUnits &fu, uint64_t u0, uint64_t u1, uint64_t n, uint64_t &xa, uint64_t &xb);
-// Resample + envelope of tiles / blocks [tile_begin, tile_end) or generic outputs [k_begin, k_end) into e (biased pointers).
-int launch_front_polyphase(apt_decoder *d, const void *in, int format, uint64_t n, uint64_t nwork, uint64_t tile_begin,
-                           uint64_t tile_end, uint64_t k_begin, uint64_t k_end, float *conv_base, float *e);
 
 // Uploads the plan's filter taps and resampler tables (apt_decoder_create and apt_stream_create); plan_table_bytes is
 // the device memory that takes.
@@ -78,11 +48,20 @@ int upload_plan(apt_decoder *d);
 uint64_t plan_table_bytes(const Plan &p);
 // Frees every buffer, event and stream the decoder owns (the object itself stays).
 int free_decoder_buffers(apt_decoder *d);
+// Grows the f32 copy of a PCM16 input to `alloc` samples when it holds fewer than `need`.
+int ensure_conv(apt_decoder *d, uint64_t need, uint64_t alloc);
 
 // Kernel accounting of a decoder: counts the launch and, when profiling, records the begin event of slot `name`;
 // returns the slot to close with prof_end (-1: none).
 int prof_begin(apt_decoder *d, const char *name);
 void prof_end(apt_decoder *d, int slot);
+struct DecoderHook : KernelHook {
+    apt_decoder *d;
+    int slot = -1;
+    explicit DecoderHook(apt_decoder *dec) : d(dec) {}
+    void begin(const char *name) override { slot = prof_begin(d, name); }
+    void end() override { prof_end(d, slot); }
+};
 
 }  // namespace aptb200
 
@@ -95,14 +74,11 @@ struct apt_decoder {
     uint64_t max_samples = 0, max_work = 0, max_corr = 0, max_out = 0;
     uint32_t max_blocks = 0, max_positions = 0;
 
-    float *d_h = nullptr, *d_lp = nullptr, *d_one = nullptr;
-    float *d_ph_table = nullptr;
-    unsigned short *d_ph_xs = nullptr;
-    float *d_tile_taps = nullptr;
-    aptb200::u32 *d_tile_xs = nullptr;
+    aptb200::FrontTables front;    // the first stage's taps and tables
+    float *d_lp = nullptr, *d_one = nullptr;
     int8_t *d_guard = nullptr;
     void *d_in = nullptr;          // staging for submit_host (f32 sized)
-    float *d_conv = nullptr;       // f32 copy of a PCM16 input for the tiled resampler (allocated on first use)
+    float *d_conv = nullptr;       // f32 copy of a PCM16 input for a first stage that wants one (allocated on first use)
     // chunked upload of long host recordings (BASELINE configs[2]): two staging buffers of chunk_samples each,
     // a copy stream and events so that the H2D of chunk c+1 overlaps the resampling of chunk c
     uint64_t chunk_samples = 0;    // 0: the whole recording is staged at once
@@ -110,7 +86,7 @@ struct apt_decoder {
     cudaEvent_t ev_copied[2] = {nullptr, nullptr}, ev_free[2] = {nullptr, nullptr};
     uint64_t job_chunks = 0;
     uint64_t conv_cap = 0;         // samples d_conv holds
-    float *d_r = nullptr;          // resampled signal, only for the L == 1 first stage
+    float *d_r = nullptr;          // resampled signal, only for a first stage that needs the scratch
     float *d_e = nullptr;          // envelope           ("demodulation_result")
     uint64_t l2_window_bytes = 0;  // bytes of d_e covered by a persisting L2 access-policy window on `stream` (0: none)
     // fused sync stage (kernels_sync2.cuh): f and corr never reach HBM; per-tile records -> roots

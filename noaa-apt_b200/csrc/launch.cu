@@ -89,8 +89,7 @@ int launch_polyphase_tiled(const LaunchCtx &c, const float *signal, u64 len, con
                            bool envelope, float cosphi2, float sinphi, float *out) {
     if (nout == 0) return APT_OK;
     const u64 tile_out = static_cast<u64>(tp.qt) * tp.p_out;
-    u64 ntiles = (nout + tile_out - 1) / tile_out;
-    if (tile_end != 0) ntiles = std::min(ntiles, tile_end);
+    const u64 ntiles = std::min((nout + tile_out - 1) / tile_out, tile_end);
     if (tile_begin >= ntiles) return APT_OK;
     const unsigned grid = static_cast<unsigned>(std::min<u64>(ntiles - tile_begin, static_cast<u64>(c.sm_count)));
     const unsigned block = 32 * (tp.compute_warps + 1);   // compute warps + producer warp
@@ -182,8 +181,7 @@ int launch_polyphase_ut(const LaunchCtx &c, const float *signal, u64 len, const 
                         float cosphi2, float sinphi, float *out) {
     if (nout == 0) return APT_OK;
     const u64 blk_out = static_cast<u64>(up.rb) * up.l;
-    u64 nblk = (nout + blk_out - 1) / blk_out;
-    if (blk_end != 0) nblk = std::min(nblk, blk_end);
+    const u64 nblk = std::min((nout + blk_out - 1) / blk_out, blk_end);
     if (blk_begin >= nblk) return APT_OK;
     if ((reinterpret_cast<uintptr_t>(signal) & 15) || (reinterpret_cast<uintptr_t>(out) & 15) || stream.size() != 4ull * up.nvec)
         return fail(APT_ERR_BAD_ARG, "uniform-tap resampler: misaligned buffers or inconsistent plan");
@@ -202,8 +200,7 @@ int launch_polyphase_ph(const LaunchCtx &c, const void *signal, int format, u64 
                         float cosphi2, float sinphi, float *out) {
     if (nout == 0) return APT_OK;
     const u64 tile_out = static_cast<u64>(kPhPeriods) * pp.l;
-    u64 ntiles = (nout + tile_out - 1) / tile_out;
-    if (tile_end != 0) ntiles = std::min(ntiles, tile_end);
+    const u64 ntiles = std::min((nout + tile_out - 1) / tile_out, tile_end);
     if (tile_begin >= ntiles) return APT_OK;
     const PhGeom g{pp.l, pp.m, pp.j, pp.pitch, pp.row_len, pp.smem_bytes};
     const unsigned grid = static_cast<unsigned>(std::min<u64>(ntiles - tile_begin, static_cast<u64>(c.sm_count)));

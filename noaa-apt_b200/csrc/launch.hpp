@@ -277,7 +277,7 @@ int launch_quantize_i16(const LaunchCtx &c, const float *x, u64 n, PostCtl *ctl,
 bool make_tile_plan(u32 l, u32 m, const std::vector<float> &taps, TilePlan &tp, std::vector<float> &tile_taps,
                     std::vector<u32> &group_xs);
 // Tiled fast_resampling (+ envelope).  f32 samples only.
-// Tiles [tile_begin, tile_end) (tile_end == 0: all); `signal` is the address sample 0 would have.
+// Tiles [tile_begin, tile_end); `signal` is the address sample 0 would have.
 int launch_polyphase_tiled(const LaunchCtx &c, const float *signal, u64 len, const float *tile_taps,
                            const u32 *group_xs, const TilePlan &tp, u64 nout, u64 tile_begin, u64 tile_end,
                            bool envelope, float cosphi2, float sinphi, float *out);
@@ -287,7 +287,7 @@ int launch_polyphase_tiled(const LaunchCtx &c, const float *signal, u64 len, con
 // xs = [l/4] window starts (row index), both go to HBM.
 bool make_ph_plan(u32 l, u32 m, const std::vector<float> &taps, PhPlan &pp, std::vector<float> &table,
                   std::vector<unsigned short> &xs);
-// Tiles of 32 periods (32*l outputs) [tile_begin, tile_end) (tile_end == 0: all); `signal` is the address sample 0 would have.
+// Tiles of 32 periods (32*l outputs) [tile_begin, tile_end); `signal` is the address sample 0 would have.
 int launch_polyphase_ph(const LaunchCtx &c, const void *signal, int format, u64 len, const float *table_dev,
                         const unsigned short *xs_dev, const PhPlan &pp, u64 nout, u64 tile_begin, u64 tile_end, bool envelope,
                         float cosphi2, float sinphi, float *out);
@@ -295,7 +295,7 @@ int launch_polyphase_ph(const LaunchCtx &c, const void *signal, int format, u64 
 // Uniform-tap resampler (+ envelope): taps travel as a kernel parameter.  Returns false from make_ut_plan when
 // (l, m, taps) does not fit (L other than 13/14, tap stream too long, rows too long for shared memory).
 bool make_ut_plan(u32 l, u32 m, const std::vector<float> &taps, UtPlan &up, std::vector<float> &stream);
-// Blocks [blk_begin, blk_end) (blk_end == 0: all); `signal` is the 16-byte-aligned address sample 0 would have;
+// Blocks [blk_begin, blk_end); `signal` is the 16-byte-aligned address sample 0 would have;
 // `h` the filter taps in device memory (for the one halo output per block).
 int launch_polyphase_ut(const LaunchCtx &c, const float *signal, u64 len, const float *h, const UtPlan &up,
                         const std::vector<float> &stream, u64 nout, u64 blk_begin, u64 blk_end, bool envelope,

@@ -1,6 +1,5 @@
 // Geometry and phase table of the phase-major resampler (kernels_ph.cuh): host logic only.
 #include <algorithm>
-#include <cstdlib>
 
 #include "launch.hpp"
 
@@ -9,7 +8,6 @@ namespace aptb200 {
 bool make_ph_plan(u32 l, u32 m, const std::vector<float> &taps, PhPlan &pp, std::vector<float> &table,
                   std::vector<unsigned short> &xs) {
     pp = PhPlan{};
-    if (getenv("APTB200_NO_PH_RESAMPLER")) return false;
     if (l < 32 || m == 0 || m > 4096 || taps.empty()) return false;       // small L: the uniform-tap / tiled kernels
     const u64 n = taps.size();
     const u64 off2 = 2 * ((n - 1) / 2);                                   // highest tap index fast_resampling touches

@@ -28,7 +28,6 @@ inline uint64_t floor16(uint64_t x) { return x & ~static_cast<uint64_t>(15); }
 
 // Everything the buffers depend on: (plan, sync, max_push).
 struct Geom {
-    FrontUnits fu;
     uint64_t G = 0, D = 0, row = 0;
     uint64_t cap_in = 0, cap_e = 0, cap_c = 0, root_cap = 0, gather_cap = 0;
     uint64_t latency = 0, bytes = 0;
@@ -52,19 +51,15 @@ int check_stream_args(uint32_t input_rate, const apt_settings *s, int sync, uint
 }
 
 Geom make_geom(const Plan &p, int sync, uint64_t max_push) {
+    const FrontPlan &f = p.front;
     Geom g;
-    g.fu = front_units(p);
     g.G = p.guard.size();
     g.D = p.dist;
     g.row = p.row;
-    const uint64_t l = p.first.l, m = p.first.m;
     // input tail: from the next unit's first sample to the end of what was pushed (less than one unit span)
-    uint64_t t_in;
-    if (!p.first_polyphase) t_in = p.h.size() + 2 * m + 32;
-    else if (g.fu.tiled) t_in = g.fu.before + g.fu.after + g.fu.unit_in + 32;
-    else t_in = (2 * p.off2 + 2 * m) / l + 32;
+    const uint64_t t_in = f.tail();
     // envelope outputs one step can finalise (finish: the units the input tail still held)
-    const uint64_t w_new = (max_push + t_in) * l / m + 2 * g.fu.unit_out + 64;
+    const uint64_t w_new = (max_push + t_in) * f.r.l / f.r.m + 2 * f.unit_out + 64;
     // envelope tail: a pending row (< row + 1 before work_final) or a pending peak (>= decided >= c_end - D), plus the
     // low-pass halo and the 16-sample alignment of the window start
     const uint64_t t_e = g.row + g.D + g.G + kHalo + 64;
@@ -76,7 +71,7 @@ Geom make_geom(const Plan &p, int sync, uint64_t max_push) {
     g.gather_cap = w_new / g.row + 4;
     g.latency = sync ? g.D + 1 : 0;
     const uint64_t rows_floats = (g.gather_cap + 1) * kPxPerRow;
-    g.bytes = plan_table_bytes(p) + g.cap_in * 4 + max_push * (2 + 4) + g.cap_e * 4 * (p.first_polyphase ? 1 : 2) +
+    g.bytes = plan_table_bytes(p) + g.cap_in * 4 + max_push * (2 + 4) + g.cap_e * 4 * (f.needs_scratch() ? 2 : 1) +
               (sync ? g.cap_c * 4 + g.root_cap * 4 + kRunRing * 8 + sizeof(StreamCarry) : sizeof(StreamCarry)) +
               g.gather_cap * 4 + rows_floats * 4;
     return g;
@@ -156,9 +151,8 @@ uint64_t envelope_keep(const apt_stream *st) {
 }
 
 int compact_all(apt_stream *st) {
-    const Plan &p = st->dec.plan;
     uint64_t xa, xb;
-    front_span(p, st->g.fu, st->units_done, st->units_done + 1, ~0ull, xa, xb);
+    st->dec.plan.front.span(st->units_done, st->units_done + 1, ~0ull, xa, xb);
     APT_TRY(compact(st, st->d_in, st->in_base, xa, st->samples_in));
     const uint64_t ek = envelope_keep(st);
     const uint64_t ekeep = ek > kHalo ? ek - kHalo : 0;
@@ -207,36 +201,19 @@ int step(apt_stream *st, const void *host, int format, uint64_t n, bool finish, 
         st->samples_in += n;
     }
     const uint64_t N = st->samples_in;
-    const uint64_t nw = plan_work_len(p, N);
+    const uint64_t nw = p.front.work_len(N);
     if (finish && nw < 10ull * p.row) {    // decode.rs:79-83
         status = fail(APT_ERR_TOO_SHORT, "Got less than 10 rows of samples, audio file is too short");
         return APT_OK;
     }
     // ---- first stage: the units whose input span is complete (all of them at the end) ----
-    const uint64_t l = p.first.l, m = p.first.m;
-    uint64_t u_hi;
-    if (!p.first_polyphase) u_hi = nw;                                       // output k needs samples [.., (k+1)m)
-    else if (g.fu.tiled) {
-        const uint64_t total = (nw + g.fu.unit_out - 1) / g.fu.unit_out;
-        u_hi = finish ? total : std::min(N >= g.fu.after ? (N - g.fu.after) / g.fu.unit_in + 1 : 0, nw / g.fu.unit_out);
-    } else {
-        u_hi = finish ? nw : std::min(N * l > p.off2 ? (N * l - p.off2 - 1) / m + 1 : 0, nw);   // (k*m + off2)/l < N
-    }
+    const uint64_t u_hi = p.front.complete(N, nw, finish);
     const uint64_t work_before = st->work_final;
     if (u_hi > st->units_done) {
-        const uint64_t work_hi = finish ? nw : std::min(nw, u_hi * g.fu.unit_out);
+        const uint64_t work_hi = finish ? nw : std::min(nw, u_hi * p.front.unit_out);
         if (work_hi - st->e_base > g.cap_e) return fail(APT_ERR_BAD_ARG, "internal: envelope window overflow");
-        const float *in = st->d_in - st->in_base;
-        float *e = st->d_e - st->e_base;
-        if (p.first_polyphase) {
-            const bool t = g.fu.tiled;
-            APT_TRY(launch_front_polyphase(&d, in, APT_F32, N, nw, t ? st->units_done : 0, t ? u_hi : 0, t ? 0 : st->units_done,
-                                           t ? 0 : u_hi, nullptr, e));
-        } else {
-            float *r = st->d_r - st->e_base;
-            APT_TRY(launch_fir_decimate(c, in, APT_F32, d.d_h, static_cast<u32>(p.h.size()), p.first.m, u_hi, r, st->units_done));
-            APT_TRY(launch_envelope(c, r, u_hi, p.cosphi2, p.sinphi, e, st->units_done));
-        }
+        APT_TRY(front_launch(c, p.front, d.front, st->d_in - st->in_base, APT_F32, nullptr, N, nw, st->units_done, u_hi, true,
+                             p.cosphi2, p.sinphi, st->d_r ? st->d_r - st->e_base : nullptr, st->d_e - st->e_base, nullptr));
         st->units_done = u_hi;
         st->work_final = work_hi;
     }
@@ -320,7 +297,7 @@ int step(apt_stream *st, const void *host, int format, uint64_t n, bool finish, 
 }
 
 uint64_t rows_bound(const apt_stream *st, uint64_t n) {
-    const uint64_t nw = plan_work_len(st->dec.plan, st->samples_in + n);
+    const uint64_t nw = st->dec.plan.front.work_len(st->samples_in + n);
     const uint64_t most = nw / st->g.row + 1;
     return most > st->rows_out ? (most - st->rows_out) * kPxPerRow : 0;
 }
@@ -373,7 +350,7 @@ extern "C" int apt_stream_create(int device, uint32_t input_rate, const apt_sett
     APT_CUDA(cudaMalloc(&st->d_pcm, max_push * sizeof(int16_t)));
     APT_CUDA(cudaMalloc(&st->d_conv, max_push * sizeof(float)));
     APT_CUDA(cudaMalloc(&st->d_e, g.cap_e * sizeof(float)));
-    if (!p.first_polyphase) APT_CUDA(cudaMalloc(&st->d_r, g.cap_e * sizeof(float)));
+    if (p.front.needs_scratch()) APT_CUDA(cudaMalloc(&st->d_r, g.cap_e * sizeof(float)));
     const size_t carry_bytes = sizeof(StreamCarry) + (st->sync ? 2 * kRunRing * sizeof(u32) : 0);
     APT_CUDA(cudaMalloc(&st->d_carry, carry_bytes));
     if (st->sync) {
@@ -409,7 +386,7 @@ extern "C" int apt_stream_push(apt_stream *st, const void *samples, int format, 
     if (format != APT_F32 && format != APT_PCM16) return fail(APT_ERR_BAD_ARG, "unknown sample format %d", format);
     if (n == 0) return APT_OK;
     if (!samples) return fail(APT_ERR_BAD_ARG, "null samples");
-    if (plan_work_len(st->dec.plan, st->samples_in + n) >= (1ull << 32))
+    if (st->dec.plan.front.work_len(st->samples_in + n) >= (1ull << 32))
         return fail(APT_ERR_BAD_ARG, "recording too long: the work-rate index would pass 2^32-1");
     const uint64_t need = rows_bound(st, n);
     if (need && (!rows || cap < need)) return fail(APT_ERR_CAPACITY, "rows needs room for %llu floats", (unsigned long long)need);

@@ -12,7 +12,7 @@ constexpr u32 kInflightBytes = 40 * 1024;   // keep about this much of the signa
 }  // namespace
 
 bool make_ut_plan(u32 l, u32 m, const std::vector<float> &taps, UtPlan &up, std::vector<float> &stream) {
-    if (l < 2 || m == 0 || taps.empty() || getenv("APTB200_NO_UNIFORM_TAPS")) return false;
+    if (l < 2 || m == 0 || taps.empty()) return false;
     const u32 np = (l + 1) / 2;
     if (l != kUtL) return false;                            // the kernel is instantiated for L = 13
     const u64 off2 = 2 * ((static_cast<u64>(taps.size()) - 1) / 2);
