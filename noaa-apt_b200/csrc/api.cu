@@ -23,10 +23,6 @@ using namespace aptb200;
 namespace aptb200 {
 int decoder_enqueue(apt_decoder *d, const void *in, int format, uint64_t n, int sync, float *rows_out,
                     const void *host_chunked);
-int run_find_sync(apt_decoder *d, uint64_t nwork);
-int ensure_legacy_sync(apt_decoder *d);
-int redo_sync_legacy(apt_decoder *d);
-int materialise_stages(apt_decoder *d);
 extern std::atomic<int> g_jobs_in_flight[64];
 }  // namespace aptb200
 
@@ -73,9 +69,8 @@ int aptb200::free_decoder_buffers(apt_decoder *d) {
     cudaSetDevice(d->device);
     if (d->stream) cudaStreamSynchronize(d->stream);
     d->front.release();
-    for (void *p : {(void *)d->d_lp, (void *)d->d_one, (void *)d->d_guard, d->d_in, (void *)d->d_r,
-                    (void *)d->d_e, (void *)d->d_f, (void *)d->d_corr, (void *)d->d_aligned, (void *)d->d_root_list,
-                    (void *)d->d_root_count, (void *)d->d_pos, (void *)d->d_res, (void *)d->d_out, d->d_pick, (void *)d->d_conv, (void *)d->d_ctl, (void *)d->d_desc, (void *)d->d_pool, (void *)d->d_roots2, (void *)d->d_tile_base, (void *)d->d_by_id})
+    d->back.release();
+    for (void *p : {(void *)d->d_lp, (void *)d->d_one, d->d_in, (void *)d->d_r, (void *)d->d_e, (void *)d->d_out, (void *)d->d_conv})
         if (p) cudaFree(p);
     if (d->h_res) cudaFreeHost(d->h_res);
     if (d->h_out) cudaFreeHost(d->h_out);
@@ -93,68 +88,6 @@ int aptb200::free_decoder_buffers(apt_decoder *d) {
     if (d->stream) cudaStreamDestroy(d->stream);
     return APT_OK;
 }
-
-namespace {
-
-// Allocates what find_sync needs for up to max_work work-rate samples: the picker's buffers always, the fused stage's
-// record pool when the plan has one (the legacy f / corr / per-block root lists come on first use: ensure_legacy_sync).
-int alloc_sync_buffers(apt_decoder *d) {
-    const Plan &p = d->plan;
-    if (getenv("APTB200_SEQUENTIAL_PICK")) d->use_parallel_pick = false;
-    if (getenv("APTB200_GENERIC_LOWPASS")) d->use_fused_lowpass = false;
-    if (!p.work_multiple || d->max_work <= p.guard.size()) return APT_OK;
-    if (p.dist > 16384) return APT_OK;   // k_roots holds two blocks of min_distance floats in shared memory (work_rate <=
-                                         // 9 * 4160): decoding with sync is refused at submit, --no-sync still works
-    d->max_corr = d->max_work - p.guard.size();
-    d->max_blocks = static_cast<uint32_t>((d->max_corr + p.dist - 1) / p.dist);
-    d->max_positions = static_cast<uint32_t>(d->max_work / p.row + 4);
-    d->use_records = d->use_fused_lowpass && !getenv("APTB200_LEGACY_SYNC") &&
-                     lowpass_corr_supported(static_cast<u32>(p.lp.size()), p.dec);
-    if (d->use_records) {
-        d->tile_w = records_tile(p.dec);
-        d->max_tiles = static_cast<uint32_t>((d->max_corr + d->tile_w - 1) / d->tile_w);
-        // Record pool: every tile owns a region of kRegion records (a noisy recording has ~200 per tile of 1920 positions: a
-        // third), tiles with more take theirs from a shared overflow area behind the regions (one atomic, rare).  A
-        // recording that does not fit even that (silence, ramps: every position a record) is decoded by the exact-order legacy
-        // kernels (kSyncRedo).  APTB200_RECORD_POOL=<records> shrinks the pool (tests of that path): no regions then.
-        constexpr uint64_t kRegion = 640;
-        uint64_t region = kRegion;
-        if (const char *e = getenv("APTB200_RECORD_REGION")) region = strtoull(e, nullptr, 10);
-        uint64_t cap = static_cast<uint64_t>(d->max_tiles) * region + std::max<uint64_t>(d->max_corr / 8, 1u << 16);
-        if (const char *e = getenv("APTB200_RECORD_POOL")) {
-            cap = std::max<uint64_t>(strtoull(e, nullptr, 10), 64);
-            if (static_cast<uint64_t>(d->max_tiles) * region > cap / 2) region = 0;
-        }
-        if (cap > (1u << 30)) {                  // hours at once: cap the pool, give the regions what is left of it
-            cap = 1u << 30;
-            region = std::min<uint64_t>(region, cap / 2 / std::max<uint32_t>(d->max_tiles, 1));
-        }
-        d->pool_cap = static_cast<uint32_t>(cap);
-        d->pool_region = static_cast<uint32_t>(region);
-        APT_CUDA(cudaMalloc(&d->d_ctl, sizeof(SyncCtl)));
-        APT_CUDA(cudaMemset(d->d_ctl, 0, sizeof(SyncCtl)));
-        APT_CUDA(cudaMalloc(&d->d_desc, static_cast<size_t>(d->max_tiles) * sizeof(TileDesc)));
-        APT_CUDA(cudaMalloc(&d->d_pool, static_cast<size_t>(d->pool_cap) * sizeof(Rec)));
-        APT_CUDA(cudaMalloc(&d->d_roots2, static_cast<size_t>(d->pool_cap) * sizeof(u32)));
-        APT_CUDA(cudaMalloc(&d->d_by_id, static_cast<size_t>(d->pool_cap) * sizeof(u32)));
-        APT_CUDA(cudaMalloc(&d->d_tile_base, static_cast<size_t>(d->max_tiles) * sizeof(u32)));
-    }
-    const uint32_t count_blocks = std::max(d->max_blocks, d->max_tiles);
-    APT_CUDA(cudaMalloc(&d->d_guard, p.guard.size()));
-    APT_CUDA(cudaMemcpy(d->d_guard, p.guard.data(), p.guard.size(), cudaMemcpyHostToDevice));
-    APT_CUDA(cudaMalloc(&d->d_root_count, static_cast<size_t>(count_blocks) * sizeof(u32)));
-    APT_CUDA(cudaMalloc(&d->d_pos, static_cast<size_t>(d->max_positions) * sizeof(u32)));
-    // parallel picker: room for every row-aligned start plus ~63 roots per row (noisy recordings have ~35);
-    // beyond that the kernel falls back to the sequential walk by itself.
-    const u32 cap = static_cast<u32>(std::min<uint64_t>(static_cast<uint64_t>(d->max_positions) * 64 + 65536, 1u << 28));
-    APT_CUDA(cudaMalloc(&d->d_pick, pick_scratch_bytes(count_blocks, d->max_positions, cap)));
-    d->pick = pick_scratch_carve(d->d_pick, count_blocks, d->max_positions, cap);
-    APT_CUDA(cudaMemset(d->pick.ticket, 0, 8));
-    if (d->d_ctl) d->pick.ticket = &d->d_ctl->pad[0];   // zeroed with the control block at the start of every job
-    return APT_OK;
-}
-
-}  // namespace
 
 // ============================================================================ misc / status
 
@@ -354,49 +287,51 @@ extern "C" int apt_filter_signal(const float *signal, uint64_t n, const apt_filt
 extern "C" int apt_find_sync(const float *signal, uint64_t n, uint32_t work_rate, uint64_t *positions, size_t cap,
                              size_t *npositions, float *corr) {
     if (!signal || !npositions) return fail(APT_ERR_BAD_ARG, "null argument");
-    apt_decoder d;   // a decoder shell that only owns the sync workspaces
-    d.plan.st.work_rate = work_rate;
-    int st = sync_frame(work_rate, d.plan.guard);
+    Plan p;
+    p.st.work_rate = work_rate;
+    int st = sync_frame(work_rate, p.guard);
     if (st != APT_OK) return fail(st, "work_rate is not multiple of FINAL_RATE");
     if (work_rate > UINT32_MAX / kPxPerRow) return fail(APT_ERR_BAD_ARG, "work_rate too large");
-    d.plan.work_multiple = true;
-    d.plan.row = kPxPerRow * work_rate / kFinalRate;
-    d.plan.dist = static_cast<uint32_t>(static_cast<uint64_t>(d.plan.row) * 8 / 10);
-    if (n < d.plan.guard.size()) return fail(APT_ERR_BAD_ARG, "signal shorter than the sync frame");   // decode.rs:225 underflow
+    p.work_multiple = true;
+    p.row = kPxPerRow * work_rate / kFinalRate;
+    p.dist = static_cast<uint32_t>(static_cast<uint64_t>(p.row) * 8 / 10);
+    if (n < p.guard.size()) return fail(APT_ERR_BAD_ARG, "signal shorter than the sync frame");   // decode.rs:225 underflow
     if (n >= (1ull << 32)) return fail(APT_ERR_BAD_ARG, "signal too long");
     APT_TRY(require_device());
-    struct Guard {
-        apt_decoder *d;
-        ~Guard() { free_decoder_buffers(d); }
-    } guard{&d};
-    APT_CUDA(cudaGetDevice(&d.device));
-    APT_CUDA(cudaStreamCreateWithFlags(&d.stream, cudaStreamNonBlocking));
-    d.max_work = n;
-    size_t got = 0;
-    if (n == d.plan.guard.size()) {
+    if (n == p.guard.size()) {
         // empty correlation: the peak list is just the seed (0, 0.0) (decode.rs:208-209)
         if (positions && cap > 0) positions[0] = 0;
         *npositions = 1;
         return APT_OK;
     }
-    d.use_fused_lowpass = false;            // the stage entry point takes an already filtered signal: exact-order kernels
-    APT_TRY(alloc_sync_buffers(&d));
-    APT_TRY(ensure_legacy_sync(&d));
-    APT_CUDA(cudaMalloc(&d.d_res, sizeof(SyncResult)));
-    APT_CUDA(cudaMemsetAsync(d.d_res, 0, sizeof(SyncResult), d.stream));
-    APT_CUDA(cudaMemcpyAsync(d.d_f, signal, n * sizeof(float), cudaMemcpyHostToDevice, d.stream));
-    APT_TRY(run_find_sync(&d, n));
+    // the stage takes an already filtered signal: the plan has no low-pass, so the kind is Generic (exact-order kernels)
+    const BackPlan bp = make_back(p, n);
+    if (!bp.can_sync) return fail(APT_ERR_BAD_ARG, "work_rate %u is too high for the sync picker (min_distance %u > 16384)",
+                                  work_rate, p.dist);
+    BackBuffers b;
+    struct Stream {                          // drains before b is freed
+        cudaStream_t s = nullptr;
+        ~Stream() {
+            if (s) cudaStreamSynchronize(s), cudaStreamDestroy(s);
+        }
+    } stream;
+    APT_TRY(b.alloc(p, bp));
+    APT_CUDA(cudaStreamCreateWithFlags(&stream.s, cudaStreamNonBlocking));
+    LaunchCtx c = stage_ctx();
+    c.stream = stream.s;
+    APT_CUDA(cudaMemcpyAsync(b.f, signal, n * sizeof(float), cudaMemcpyHostToDevice, c.stream));
+    APT_TRY(back_find_sync(c, p, bp, b, n));
     SyncResult res;
-    APT_CUDA(cudaMemcpyAsync(&res, d.d_res, sizeof(res), cudaMemcpyDeviceToHost, d.stream));
-    APT_CUDA(cudaStreamSynchronize(d.stream));
-    got = res.n_peaks;
+    APT_CUDA(cudaMemcpyAsync(&res, b.res, sizeof(res), cudaMemcpyDeviceToHost, c.stream));
+    APT_CUDA(cudaStreamSynchronize(c.stream));
+    const size_t got = res.n_peaks;
     *npositions = got;
     if (positions) {
         std::vector<u32> tmp(got);
-        APT_CUDA(cudaMemcpy(tmp.data(), d.d_pos, got * sizeof(u32), cudaMemcpyDeviceToHost));
+        APT_CUDA(cudaMemcpy(tmp.data(), b.pos, got * sizeof(u32), cudaMemcpyDeviceToHost));
         for (size_t i = 0; i < std::min(got, cap); ++i) positions[i] = tmp[i];
     }
-    if (corr) APT_CUDA(cudaMemcpy(corr, d.d_corr, (n - d.plan.guard.size()) * sizeof(float), cudaMemcpyDeviceToHost));
+    if (corr) APT_CUDA(cudaMemcpy(corr, b.corr, (n - p.guard.size()) * sizeof(float), cudaMemcpyDeviceToHost));
     if (positions && got > cap) return fail(APT_ERR_CAPACITY, "positions needs %zu entries", got);
     return APT_OK;
 }
@@ -471,10 +406,8 @@ extern "C" int apt_decoder_create(int device, uint32_t input_rate, const apt_set
     const size_t work_bytes = std::max<uint64_t>(d->max_work, 1) * sizeof(float);
     if (p.front.needs_scratch()) APT_CUDA(cudaMalloc(&d->d_r, work_bytes));
     APT_CUDA(cudaMalloc(&d->d_e, work_bytes));
-    APT_TRY(alloc_sync_buffers(d.get()));
-    if (!d->use_records) APT_TRY(ensure_legacy_sync(d.get()));
-    APT_CUDA(cudaMalloc(&d->d_res, sizeof(SyncResult)));
-    APT_CUDA(cudaMemset(d->d_res, 0, sizeof(SyncResult)));
+    d->back_plan = make_back(p, d->max_work);
+    APT_TRY(d->back.alloc(p, d->back_plan));
     APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&d->h_res), sizeof(SyncResult), cudaHostAllocDefault));
     memset(d->h_res, 0, sizeof(SyncResult));
     rollback.armed = false;
@@ -499,7 +432,7 @@ int enqueue_image_stage(apt_decoder *d, unsigned char *out8) {
         DecoderHook hook(d);
         ProcessLaunch a{};
         a.rows = d->d_out;
-        a.result = d->job_sync ? d->d_res : nullptr;
+        a.result = d->job_sync ? d->back.res : nullptr;
         a.fixed_rows = fixed;
         a.max_rows = max_rows;
         a.contrast = d->proc.contrast;
@@ -519,7 +452,7 @@ int enqueue_image_stage(apt_decoder *d, unsigned char *out8) {
         APT_CUDA(cudaMemcpyAsync(d->h_post, d->d_post, offsetof(PostCtl, buckets), cudaMemcpyDeviceToHost, d->stream));
         return APT_OK;
     }
-    APT_TRY(launch_image_stage(c, d->d_out, d->job_sync ? d->d_res : nullptr, fixed, max_rows, kPxPerRow, d->image_contrast,
+    APT_TRY(launch_image_stage(c, d->d_out, d->job_sync ? d->back.res : nullptr, fixed, max_rows, kPxPerRow, d->image_contrast,
                                d->image_percent, d->d_post, d->d_tel, d->d_tel + max_rows, d->d_tel + 2 * static_cast<size_t>(max_rows),
                                nullptr, out8, false));
     d->launches += d->image_contrast == APT_CONTRAST_PERCENT ? 4 : 3;
@@ -553,7 +486,7 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
         d->job_status = fail(APT_ERR_TOO_SHORT, "Got less than 10 rows of samples, audio file is too short");
         return d->job_status;
     }
-    if (d->job_sync && p.work_multiple && !d->d_pos)
+    if (d->job_sync && p.work_multiple && !d->back_plan.can_sync)
         return fail(APT_ERR_BAD_ARG, "work_rate %u is too high for the sync picker (min_distance %u > 16384); decode without "
                                      "sync or use a work_rate <= 37440", p.st.work_rate, p.dist);
     const uint64_t need = d->job_sync ? (nwork / p.row) * kPxPerRow : plan_out_bound(p, n);
@@ -641,7 +574,7 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
         d->job_status = st;
         return st;
     }
-    if (d->job_sync) APT_CUDA(cudaMemcpyAsync(d->h_res, d->d_res, sizeof(SyncResult), cudaMemcpyDeviceToHost, d->stream));
+    if (d->job_sync) APT_CUDA(cudaMemcpyAsync(d->h_res, d->back.res, sizeof(SyncResult), cudaMemcpyDeviceToHost, d->stream));
     d->job_d2h_floats = 0;
     if (host) {
         // the rows come back with the job: when syncing n_rows is only known on the device, so the copy covers the bound
@@ -683,21 +616,21 @@ extern "C" int apt_decoder_wait(apt_decoder *d, uint64_t *nout) {
     uint64_t produced = d->job_fixed_out;
     d->last_work = d->job_work;
     d->last_peaks = 0;
-    d->last_fused = d->job_fused;
     if (d->job_sync) {
         if (d->h_res->status == kSyncRedo) {
-            // the record pool of the fused stage overflowed (silence, ramps: every index a record): the sync stage runs
-            // again with the legacy kernels on the envelope that is still in d_e
-            APT_TRY(redo_sync_legacy(d));
+            // the record pool overflowed (silence, ramps: every index a record): the sync decode runs again with the Hbm
+            // kernels on the envelope that is still in d_e
+            DecoderHook hook(d);
+            APT_TRY(back_redo(LaunchCtx{d->stream, d->sm_count}, d->plan, d->back_plan, d->back, d->d_e, d->job_work,
+                              const_cast<float *>(d->job_rows_src), &hook, d->last_back));
             if (d->job_image)
                 APT_TRY(enqueue_image_stage(d, d->job_host ? d->d_out8 : reinterpret_cast<unsigned char *>(d->job_out)));
-            APT_CUDA(cudaMemcpyAsync(d->h_res, d->d_res, sizeof(SyncResult), cudaMemcpyDeviceToHost, d->stream));
+            APT_CUDA(cudaMemcpyAsync(d->h_res, d->back.res, sizeof(SyncResult), cudaMemcpyDeviceToHost, d->stream));
             if (d->job_host && d->job_d2h_floats)
                 APT_CUDA(cudaMemcpyAsync(d->job_out_pageable ? static_cast<void *>(d->h_out) : static_cast<void *>(d->job_out),
                                          d->job_image ? static_cast<const void *>(d->d_out8) : static_cast<const void *>(d->d_out),
                                          d->job_d2h_floats * (d->job_image ? d->job_bpp : sizeof(float)), cudaMemcpyDeviceToHost, d->stream));
             APT_CUDA(cudaStreamSynchronize(d->stream));
-            d->last_fused = false;
         }
         const SyncResult res = *d->h_res;
         d->last_peaks = res.n_peaks;
@@ -816,7 +749,7 @@ extern "C" int apt_decoder_last_sync(apt_decoder *d, uint64_t *positions, size_t
     *npositions = got;
     if (positions && got) {
         std::vector<u32> tmp(got);
-        APT_CUDA(cudaMemcpy(tmp.data(), d->d_pos, got * sizeof(u32), cudaMemcpyDeviceToHost));
+        APT_CUDA(cudaMemcpy(tmp.data(), d->back.pos, got * sizeof(u32), cudaMemcpyDeviceToHost));
         for (size_t i = 0; i < std::min(got, cap); ++i) positions[i] = tmp[i];
     }
     return APT_OK;
@@ -838,34 +771,8 @@ extern "C" int apt_decoder_last_root_count(apt_decoder *d, uint64_t *n_roots) {
 
 extern "C" int apt_decoder_last_roots(apt_decoder *d, uint64_t *roots, size_t cap, size_t *nroots) {
     if (!d || !nroots) return fail(APT_ERR_BAD_ARG, "null argument");
-    *nroots = 0;
-    if (!d->d_root_count || d->last_work <= d->plan.guard.size()) return APT_OK;
     APT_CUDA(cudaSetDevice(d->device));
-    const uint64_t ncorr = d->last_work - d->plan.guard.size();
-    const bool fused = d->last_fused && d->d_desc;
-    const uint32_t block = fused ? d->tile_w : d->plan.dist;
-    const uint32_t nb = static_cast<uint32_t>((ncorr + block - 1) / block);
-    std::vector<u32> counts(nb);
-    APT_CUDA(cudaMemcpy(counts.data(), d->d_root_count, nb * sizeof(u32), cudaMemcpyDeviceToHost));
-    std::vector<TileDesc> desc;
-    if (fused) {
-        desc.resize(nb);
-        APT_CUDA(cudaMemcpy(desc.data(), d->d_desc, nb * sizeof(TileDesc), cudaMemcpyDeviceToHost));
-    }
-    size_t total = 0;
-    std::vector<u32> tmp;
-    for (uint32_t b = 0; b < nb; ++b) {
-        if (roots && counts[b]) {
-            tmp.resize(counts[b]);
-            const u32 *src = fused ? d->d_roots2 + desc[b].off : d->d_root_list + static_cast<size_t>(b) * block;
-            APT_CUDA(cudaMemcpy(tmp.data(), src, counts[b] * sizeof(u32), cudaMemcpyDeviceToHost));
-            for (u32 i = 0; i < counts[b]; ++i)
-                if (total + i < cap) roots[total + i] = tmp[i];
-        }
-        total += counts[b];
-    }
-    *nroots = total;
-    return APT_OK;
+    return back_roots(d->plan, d->back_plan, d->back, d->last_back, d->last_work, roots, cap, nroots);
 }
 
 extern "C" int apt_decoder_read_stage(apt_decoder *d, int which, float *out, uint64_t cap, uint64_t *n) {
@@ -873,12 +780,15 @@ extern "C" int apt_decoder_read_stage(apt_decoder *d, int which, float *out, uin
     APT_CUDA(cudaSetDevice(d->device));
     const float *src = nullptr;
     uint64_t len = d->last_work;
-    if (which != 0 && d->last_fused && len) APT_TRY(materialise_stages(d));   // f / corr were never written: compute them now
+    if (which != 0 && d->last_back == BackKind::Records && len) {   // f / corr were never written: compute them now
+        APT_TRY(back_materialise(LaunchCtx{d->stream, d->sm_count}, d->plan, d->back_plan, d->back, d->d_e, len));
+        d->last_back = BackKind::Hbm;
+    }
     switch (which) {
     case 0: src = d->d_e; break;
-    case 1: src = d->d_f; break;
+    case 1: src = d->back.f; break;
     case 2:
-        src = d->d_corr;
+        src = d->back.corr;
         len = d->last_work > d->plan.guard.size() ? d->last_work - d->plan.guard.size() : 0;
         break;
     default: return fail(APT_ERR_BAD_ARG, "unknown stage %d", which);

@@ -110,6 +110,8 @@ void prof_end(apt_decoder *d, int slot) {
     if (slot >= 0) cudaEventRecord(d->ev_end[slot], d->stream);
 }
 
+void DecoderHook::extra(int kernels) { d->launches += static_cast<uint64_t>(kernels); }
+
 namespace {
 
 struct Prof : DecoderHook {   // a slot around a scope
@@ -118,90 +120,6 @@ struct Prof : DecoderHook {   // a slot around a scope
 };
 
 }  // namespace
-
-// Cross-correlation + roots + orbit walk: decode::find_sync (decode.rs:204-263) on d_f[0..nwork).
-int run_find_sync(apt_decoder *d, uint64_t nwork) {
-    const Plan &p = d->plan;
-    const LaunchCtx c{d->stream, d->sm_count};
-    const uint32_t glen = static_cast<uint32_t>(p.guard.size());
-    const uint64_t ncorr = nwork - glen;
-    const uint32_t nblocks = static_cast<uint32_t>((ncorr + p.dist - 1) / p.dist);
-    if (!d->job_corr_done) {
-        Prof pr(d, "sync_correlation");
-        APT_TRY(launch_corr(c, d->d_f, ncorr, d->d_guard, glen, d->d_corr));
-    }
-    {
-        Prof pr(d, "sync_roots");
-        APT_TRY(launch_roots(c, d->d_corr, ncorr, p.dist, d->d_root_list, d->d_root_count, d->d_res,
-                             d->use_parallel_pick && d->d_pick ? &d->pick : nullptr));
-    }
-    {
-        Prof pr(d, "sync_pick");
-        const u32 *boff = d->d_pick ? d->pick.block_off : nullptr;
-        const RootIndex ri{d->d_root_list, d->d_root_count, boff, nullptr, nullptr, boff ? boff + nblocks : nullptr, p.dist, nblocks};
-        APT_TRY(launch_pick(c, ncorr, nwork, p.row, p.dist, ri, d->d_pos, d->max_positions, d->d_res,
-                            d->use_parallel_pick && d->d_pick ? &d->pick : nullptr));
-    }
-    return APT_OK;
-}
-
-// Legacy / debug buffers (f, corr, per-block root lists): generic shapes, read_stage, and the redo after a record-pool
-// overflow.  Allocated on first use.
-int ensure_legacy_sync(apt_decoder *d) {
-    const Plan &p = d->plan;
-    APT_CUDA(cudaSetDevice(d->device));
-    const size_t work_bytes = std::max<uint64_t>(d->max_work, 1) * sizeof(float);
-    if (!d->d_f) APT_CUDA(cudaMalloc(&d->d_f, work_bytes));
-    if (p.work_multiple && d->max_corr) {
-        if (!d->d_corr) APT_CUDA(cudaMalloc(&d->d_corr, d->max_corr * sizeof(float)));
-        if (!d->d_root_list) APT_CUDA(cudaMalloc(&d->d_root_list, static_cast<size_t>(d->max_blocks) * p.dist * sizeof(u32)));
-    }
-    return APT_OK;
-}
-
-// The back half with f and corr materialised in HBM: low-pass (+ correlation), roots, orbit walk, row gather.
-static int enqueue_back_legacy(apt_decoder *d, uint64_t nwork, int sync, float *rows_out) {
-    const Plan &p = d->plan;
-    const LaunchCtx c{d->stream, d->sm_count};
-    APT_TRY(ensure_legacy_sync(d));
-    d->job_corr_done = false;
-    const bool want_corr = sync && p.work_multiple && d->d_corr != nullptr;
-    const u32 ntaps = static_cast<u32>(p.lp.size());
-    if (d->use_fused_lowpass && lowpass_corr_supported(ntaps, p.dec) && p.work_multiple) {
-        // low-pass and (when syncing) the sync cross-correlation in one pass over the envelope
-        Prof pr(d, want_corr ? "lowpass_correlation" : "lowpass");
-        APT_TRY(launch_lowpass_corr(c, d->d_e, nwork, p.lp.data(), ntaps, p.dec, d->d_f, want_corr ? d->d_corr : nullptr));
-        d->job_corr_done = want_corr;
-    } else {
-        Prof pr(d, "lowpass");
-        APT_TRY(launch_fir_decimate(c, d->d_e, APT_F32, d->d_lp, ntaps, 1, nwork, d->d_f));
-    }
-    if (sync) {
-        APT_TRY(run_find_sync(d, nwork));
-        Prof pr(d, "gather_rows");
-        const u32 max_rows = static_cast<u32>(std::min<uint64_t>(nwork / p.row + 1, 1u << 30));
-        APT_TRY(launch_gather(c, d->d_f, d->d_pos, d->d_res, 0, max_rows, p.row, kPxPerRow, p.dec, rows_out));
-    }
-    return APT_OK;
-}
-
-// Re-runs the sync stage of the job that just drained with the legacy kernels (record pool overflow); d_e is intact.
-int redo_sync_legacy(apt_decoder *d) {
-    APT_CUDA(cudaMemsetAsync(d->d_res, 0, sizeof(SyncResult), d->stream));
-    return enqueue_back_legacy(d, d->job_work, 1, const_cast<float *>(d->job_rows_src));
-}
-
-// On-demand f / corr of the last job for read_stage after a fused run.
-int materialise_stages(apt_decoder *d) {
-    const Plan &p = d->plan;
-    const LaunchCtx c{d->stream, d->sm_count};
-    APT_TRY(ensure_legacy_sync(d));
-    const u32 ntaps = static_cast<u32>(p.lp.size());
-    APT_TRY(launch_lowpass_corr(c, d->d_e, d->last_work, p.lp.data(), ntaps, p.dec, d->d_f, d->d_corr));
-    APT_CUDA(cudaStreamSynchronize(d->stream));
-    d->last_fused = false;
-    return APT_OK;
-}
 
 int ensure_conv(apt_decoder *d, uint64_t need, uint64_t alloc) {
     if (d->conv_cap >= need) return APT_OK;
@@ -343,85 +261,18 @@ int decoder_enqueue(apt_decoder *d, const void *in, int format, uint64_t n, int 
     d->ev_used = 0;
     set_envelope_l2_window(d, nwork, c.busy == 0);
 
-    if (sync && d->use_records && d->d_ctl) APT_CUDA(cudaMemsetAsync(d->d_ctl, 0, sizeof(SyncCtl), d->stream));
     APT_TRY(enqueue_front(d, in, format, n, nwork, host_chunked));
-    d->job_fused = false;
-    const u32 ntaps = static_cast<u32>(p.lp.size());
-
     if (sync) {
-        if (!p.work_multiple) {
-            if (d->cb) d->cb(0.5f, "Syncing", d->cb_user);                  // decode.rs:107
-            return fail(APT_ERR_WORK_RATE, "work_rate is not multiple of FINAL_RATE");   // decode.rs:172-176
-        }
-        d->job_fixed_out = 0;
-        if (d->use_records && d->d_pool) {
-            // fused stage: f and corr stay on chip; records -> roots -> orbit -> rows straight from the envelope
-            const u64 ncorr = nwork - p.guard.size();
-            const u32 ntiles = static_cast<u32>((ncorr + d->tile_w - 1) / d->tile_w);
-            d->job_fused = true;
-            {
-                Prof pr(d, "lowpass_records");
-                APT_TRY(launch_lowpass_records(c, d->d_e, nwork, ncorr, p.lp.data(), ntaps, p.dec, d->d_ctl, d->d_desc, d->d_pool,
-                                               d->pool_cap, d->pool_region, ntiles));
-            }
-            if (d->cb) d->cb(0.5f, "Syncing", d->cb_user);
-            {
-                Prof pr(d, "resolve_roots");
-                APT_TRY(launch_resolve_roots(c, d->d_desc, d->d_pool, ntiles, d->tile_w, p.dist, ncorr, d->d_roots2, d->d_root_count,
-                                             d->d_tile_base, d->d_by_id, d->d_ctl, d->d_res));
-            }
-            {
-                Prof pr(d, "sync_pick");
-                const RootIndex ri{d->d_roots2, d->d_root_count, d->d_tile_base, d->d_desc, d->d_by_id, &d->d_ctl->root_cursor,
-                                   d->tile_w, ntiles};
-                int nk = 1;
-                APT_TRY(launch_pick(c, ncorr, nwork, p.row, p.dist, ri, d->d_pos, d->max_positions, d->d_res,
-                                    d->use_parallel_pick && d->d_pick ? &d->pick : nullptr, &nk));
-                d->launches += static_cast<uint64_t>(nk - 1);               // Prof counted one
-            }
-            if (d->cb) d->cb(0.9f, "Resampling to 4160", d->cb_user);       // decode.rs:154
-            Prof pr(d, "gather_rows");
-            const u32 max_rows = static_cast<u32>(std::min<uint64_t>(nwork / p.row + 1, 1u << 30));
-            APT_TRY(launch_gather_lp(c, d->d_e, nwork, d->d_pos, d->d_res, 0, max_rows, p.row, kPxPerRow, p.dec, p.lp.data(), ntaps,
-                                     rows_out));
-            return APT_OK;
-        }
-        if (d->cb) d->cb(0.5f, "Syncing", d->cb_user);
-        APT_TRY(enqueue_back_legacy(d, nwork, 1, rows_out));
-        if (d->cb) d->cb(0.9f, "Resampling to 4160", d->cb_user);
-        return APT_OK;
+        if (d->cb) d->cb(0.5f, "Syncing", d->cb_user);                      // decode.rs:107
+        if (!p.work_multiple) return fail(APT_ERR_WORK_RATE, "work_rate is not multiple of FINAL_RATE");   // decode.rs:172-176
+    } else {
+        if (d->cb) d->cb(0.5f, "Skipping Syncing", d->cb_user);             // decode.rs:136
+        if (d->cb) d->cb(0.9f, "Resampling to 4160", d->cb_user);           // decode.rs:154
     }
-
-    if (d->cb) d->cb(0.5f, "Skipping Syncing", d->cb_user);                 // decode.rs:136
-    const uint64_t rows = nwork / p.row;                                    // decode.rs:141-147
-    if (d->cb) d->cb(0.9f, "Resampling to 4160", d->cb_user);
-    if (p.work_multiple) {
-        if (d->use_records) {
-            d->job_fused = true;
-            Prof pr(d, "gather_rows");
-            APT_TRY(launch_gather_lp(c, d->d_e, nwork, nullptr, d->d_res, static_cast<u32>(rows), static_cast<u32>(rows), p.row,
-                                     kPxPerRow, p.dec, p.lp.data(), ntaps, rows_out));
-        } else {
-            APT_TRY(enqueue_back_legacy(d, nwork, 0, rows_out));
-            Prof pr(d, "gather_rows");
-            APT_TRY(launch_gather(c, d->d_f, nullptr, d->d_res, static_cast<u32>(rows), static_cast<u32>(rows), p.row,
-                                  kPxPerRow, p.dec, rows_out));
-        }
-        d->job_fixed_out = rows * kPxPerRow;
-        return APT_OK;
-    }
-    APT_TRY(enqueue_back_legacy(d, nwork, 0, rows_out));
-    // work_rate is not a multiple of 4160: the final stage is a real L/M resample with the one-tap
-    // NoFilter (dsp.rs:79-98), i.e. zero-stuffing then keeping every M-th sample.
-    if (p.last.l == 0) return fail(APT_ERR_RESAMPLE_TO_ZERO, "Can't resample to 0Hz");
-    if (static_cast<uint64_t>(p.st.work_rate) * p.last.l > UINT32_MAX)
-        return fail(APT_ERR_RATE_OVERFLOW, "Can't resample, looks like the sample rates do not have a big divisor "
-                                           "in common. input_rate: %u, output_rate: %u", p.st.work_rate, kFinalRate);
-    const uint64_t alen = rows * p.row;
-    const uint64_t nout = polyphase_len(alen, p.last.l, p.last.m, 1);
-    Prof pr(d, "final_resample");
-    APT_TRY(launch_polyphase(c, d->d_f, APT_F32, alen, d->d_one, p.last.l, p.last.m, 0, 0, nout, false, 0.f, 1.f, rows_out));
-    d->job_fixed_out = nout;
+    DecoderHook hook(d);
+    APT_TRY(back_launch(c, p, d->back_plan, d->back, d->d_lp, d->d_one, d->d_e, nwork, sync != 0, rows_out, &hook, d->last_back));
+    if (sync && d->cb) d->cb(0.9f, "Resampling to 4160", d->cb_user);
+    d->job_fixed_out = sync ? 0 : plan_out_bound(p, n);
     return APT_OK;
 }
 

@@ -11,6 +11,7 @@
 #include "aptb200.h"
 #include <memory>
 
+#include "back.hpp"
 #include "filters_host.hpp"
 #include "front.hpp"
 #include "hostpool.hpp"
@@ -61,6 +62,7 @@ struct DecoderHook : KernelHook {
     explicit DecoderHook(apt_decoder *dec) : d(dec) {}
     void begin(const char *name) override { slot = prof_begin(d, name); }
     void end() override { prof_end(d, slot); }
+    void extra(int kernels) override;
 };
 
 }  // namespace aptb200
@@ -71,8 +73,7 @@ struct apt_decoder {
     cudaStream_t stream = nullptr;
     aptb200::Plan plan;
 
-    uint64_t max_samples = 0, max_work = 0, max_corr = 0, max_out = 0;
-    uint32_t max_blocks = 0, max_positions = 0;
+    uint64_t max_samples = 0, max_work = 0, max_out = 0;
 
     aptb200::FrontTables front;    // the first stage's taps and tables
     float *d_lp = nullptr, *d_one = nullptr;
@@ -89,27 +90,10 @@ struct apt_decoder {
     float *d_r = nullptr;          // resampled signal, only for a first stage that needs the scratch
     float *d_e = nullptr;          // envelope           ("demodulation_result")
     uint64_t l2_window_bytes = 0;  // bytes of d_e covered by a persisting L2 access-policy window on `stream` (0: none)
-    // fused sync stage (kernels_sync2.cuh): f and corr never reach HBM; per-tile records -> roots
-    bool use_records = false;      // the fused stage serves this plan (standard / fast / slow profiles)
-    aptb200::u32 tile_w = 0, max_tiles = 0, pool_cap = 0, pool_region = 0;   // pool_region: records of a tile's own pool region
-    aptb200::SyncCtl *d_ctl = nullptr;
-    aptb200::TileDesc *d_desc = nullptr;
-    aptb200::Rec *d_pool = nullptr;
-    aptb200::u32 *d_roots2 = nullptr;   // roots of tile t at d_roots2 + d_desc[t].off
-    aptb200::u32 *d_tile_base = nullptr, *d_by_id = nullptr;   // dense root ids: first id of tile t, position by id
-    bool job_fused = false;        // the current job ran the fused stage (f / corr were not materialised)
-    bool last_fused = false;
-    // legacy / debug buffers, allocated on first use (generic shapes, read_stage, pool overflow)
-    float *d_f = nullptr;          // low-passed         ("filter_result")
-    float *d_corr = nullptr;       // sync correlation   ("sync_correlation")
-    float *d_aligned = nullptr;    // only when work_rate is not a multiple of 4160 (no-sync)
-    aptb200::u32 *d_root_list = nullptr, *d_root_count = nullptr, *d_pos = nullptr;
-    aptb200::SyncResult *d_res = nullptr;
-    void *d_pick = nullptr;        // scratch of the parallel picker
-    aptb200::PickScratch pick{};
-    bool use_parallel_pick = true;
-    bool use_fused_lowpass = true;
-    bool job_corr_done = false;    // the correlation of the current job was produced by the fused low-pass kernel
+    aptb200::BackPlan back_plan;   // the back half's kind and buffer sizes
+    aptb200::BackBuffers back;     // its buffers
+    aptb200::BackKind last_back = aptb200::BackKind::Generic;   // the kind that ran the last job: where its roots are, and
+                                                                  // whether its f / corr exist
     float *d_out = nullptr;        // rows for submit_host
     // pageable host buffers (what the reference-facing apt_decode receives) go through a pinned ring + copy threads
     aptb200::HostStager *stager = nullptr;                 // the one in use (own_stager, or the batch feeder's)
@@ -141,8 +125,7 @@ struct apt_decoder {
     bool in_flight = false;
     bool job_host = false, job_sync = false;
     int job_status = APT_OK;
-    uint64_t job_n = 0, job_work = 0, job_corr = 0, job_fixed_out = 0;
-    const void *job_dev_in = nullptr;   // device address sample 0 would have (for a redo of the sync stage)
+    uint64_t job_n = 0, job_work = 0, job_fixed_out = 0;
     float *job_out = nullptr;      // caller's buffer (host or device)
     uint64_t job_cap = 0;
     const float *job_rows_src = nullptr;

@@ -17,12 +17,6 @@ int upload_vec(P *&dst, const std::vector<T> &src) {   // dst is set before the 
     return APT_OK;
 }
 
-struct Slot {   // one kernel's profiling slot
-    KernelHook *hook;
-    Slot(KernelHook *h, const char *name) : hook(h) { if (hook) hook->begin(name); }
-    ~Slot() { if (hook) hook->end(); }
-};
-
 }  // namespace
 
 FrontPlan make_front(Ratio r, std::vector<float> taps) {
@@ -122,14 +116,14 @@ int front_launch(const LaunchCtx &c, const FrontPlan &f, const FrontTables &t, c
                  float *scratch, float *out, KernelHook *hook) {
     if (f.kind == FrontKind::Decimate) {
         {
-            Slot s(hook, "filter_decimate");
+            KernelSlot s(hook, "filter_decimate");
             APT_TRY(launch_fir_decimate(c, in, format, t.h, static_cast<u32>(f.h.size()), f.r.m, u1, envelope ? scratch : out, u0));
         }
         if (!envelope) return APT_OK;
-        Slot s(hook, "envelope");
+        KernelSlot s(hook, "envelope");
         return launch_envelope(c, scratch, u1, cosphi2, sinphi, out, u0);
     }
-    Slot s(hook, kFrontSlot);
+    KernelSlot s(hook, kFrontSlot);
     const float *fin = format == APT_F32 ? static_cast<const float *>(in) : conv;
     if (f.kind == FrontKind::Tiled && fin)
         return launch_polyphase_tiled(c, fin, n, t.table, static_cast<const u32 *>(t.xs), f.tile, nwork, u0, u1, envelope,

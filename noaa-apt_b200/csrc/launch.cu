@@ -6,7 +6,6 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <type_traits>
 
 #include "aptb200.h"
 #include "common.hpp"
@@ -319,39 +318,13 @@ static bool smem_attr_once(std::atomic<signed char> *flags, K kern, size_t smem)
 }
 
 int launch_pick(const LaunchCtx &c, u64 ncorr, u64 nwork, u32 row, u32 dist, const RootIndex &ri_in, u32 *positions,
-                u32 max_positions, SyncResult *result, const PickScratch *scratch, int *kernels_launched) {
+                u32 max_positions, SyncResult *result, Walk walk, const PickScratch &scratch, int *kernels_launched) {
     RootIndex ri = ri_in;
     int dummy = 0;
     int &nk = kernels_launched ? *kernels_launched : dummy;
     nk = 1;
-    // Which parallel orbit walk: APTB200_PICK = compress | cluster | grid forces one; by default the whole-GPU cooperative
-    // walk (faster, but it needs every SM) when the device is otherwise idle, the 8-CTA cluster walk (8 SMs) when
-    // other recordings are in flight on other streams (the batch workload runs faster with it).
-    static const int forced = [] {
-        const char *e = getenv("APTB200_PICK");
-        if (getenv("APTB200_GRID_PICK")) return 2;
-        if (!e) return -1;
-        return !strcmp(e, "compress") ? 0 : !strcmp(e, "cluster") ? 1 : !strcmp(e, "grid") ? 2 : -1;
-    }();
-    const int mode = forced >= 0 ? forced : (c.busy ? 1 : 2);
     const u64 nr = (ncorr + row - 1) / row;
-    if (scratch && mode == 0 && nr + 1 <= static_cast<u64>(kPickEMax - 2) * kPickR) {
-        // compressed walk: J0 and E = J0^8 over the whole GPU, then one CTA (see kernels_sync.cuh)
-        const size_t smem = (3ull * kPickKMax + kPickEMax) * sizeof(u32);
-        // the attribute belongs to the (function, device) pair: one flag per device, not one per process
-        static std::atomic<signed char> attr_final[kMaxDevices];
-        if (smem_attr_once(attr_final, k_pick_final, smem)) {
-            PickScratch sc = *scratch;
-            const unsigned grid = (sc.cap + 1 + 255) / 256;       // one thread per possible node; the kernels know how many exist
-            k_pick_j0<<<grid, 256, 0, c.stream>>>(ncorr, row, dist, ri, positions, max_positions, result, sc);
-            k_pick_e8<<<grid, 256, 0, c.stream>>>(ncorr, row, ri, max_positions, result, sc);
-            k_pick_final<<<1, 1024, smem, c.stream>>>(ncorr, nwork, row, dist, ri, positions, max_positions, result, sc);
-            APT_CUDA(cudaGetLastError());
-            nk = 3;
-            return APT_OK;
-        }
-    }
-    if (scratch && mode <= 1 && nr <= 20000) {
+    if (walk == Walk::Cluster && nr <= 20000) {
         // one 8-CTA cluster, jump tables in distributed shared memory (larger recordings: the whole-GPU cooperative grid)
         const size_t smem = 2ull * kPickClusterPer * sizeof(u32);
         static std::atomic<signed char> attr_cluster[kMaxDevices];
@@ -368,7 +341,7 @@ int launch_pick(const LaunchCtx &c, u64 ncorr, u64 nwork, u32 row, u32 dist, con
             at[0].val.clusterDim.z = 1;
             cfg.attrs = at;
             cfg.numAttrs = 1;
-            PickScratch sc = *scratch;
+            PickScratch sc = scratch;
             const unsigned j0_grid = (sc.cap + 1 + 255) / 256;      // one thread per possible node; the kernel knows how many exist
             k_pick_j0<<<j0_grid, 256, 0, c.stream>>>(ncorr, row, dist, ri, positions, max_positions, result, sc);
             APT_CUDA(cudaGetLastError());
@@ -377,13 +350,13 @@ int launch_pick(const LaunchCtx &c, u64 ncorr, u64 nwork, u32 row, u32 dist, con
             return APT_OK;
         }
     }
-    if (scratch) {
+    if (walk != Walk::Sequential) {
         // cooperative launch: the kernel's grid barriers need every CTA resident (1024 threads, no dynamic smem)
         int per_sm = 0;
         APT_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_pick_links, 1024, 0));
-        const unsigned want = (scratch->cap + 1 + 1023) / 1024;
+        const unsigned want = (scratch.cap + 1 + 1023) / 1024;
         const unsigned grid = std::max(1u, std::min(want, static_cast<unsigned>(std::max(per_sm, 1) * c.sm_count)));
-        PickScratch sc = *scratch;
+        PickScratch sc = scratch;
         void *args[] = {&ncorr, &nwork, &row, &dist, &ri, &positions, &max_positions, &result, &sc};
         APT_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void *>(k_pick_links), dim3(grid), dim3(1024), args, 0,
                                              c.stream));
@@ -406,60 +379,26 @@ static LpTaps make_lp_taps(const float *taps_host, u32 ntaps, int dec = 0) {
     return t;
 }
 
-// Rows of 32 low-passed samples per tile of the record kernel (64, or 32 with APTB200_REC_TB=32); fixed per process.
-static int records_tb() {
-    static const int tb = [] {
-        const char *e = getenv("APTB200_REC_TB");
-        return e && atoi(e) == 32 ? 32 : 64;
-    }();
-    return tb;
-}
-
-u32 records_tile(u32 pw) { return static_cast<u32>(rec_tile_outputs(static_cast<int>(pw), records_tb())); }
+u32 records_tile(u32 pw) { return static_cast<u32>(rec_tile_outputs(static_cast<int>(pw))); }
 
 int launch_lowpass_records(const LaunchCtx &c, const float *e, u64 n, u64 ncorr, const float *taps_host, u32 ntaps, u32 pw,
                            SyncCtl *ctl, TileDesc *desc, Rec *pool, u32 pool_cap, u32 region, u32 ntiles) {
     if (ntiles == 0) return APT_OK;
     const LpTaps t = make_lp_taps(taps_host, ntaps);
-    const int tb = records_tb();
-    static const int nbuf = [] {
-        const char *e = getenv("APTB200_REC_NBUF");
-        return e && atoi(e) == 2 ? 2 : 1;
-    }();
-    auto launch = [&](auto kern, auto nwc) {
-        constexpr int NWc = decltype(nwc)::value;
-        const size_t smem = static_cast<size_t>(nbuf) * NWc * rec_smem_floats(tb) * sizeof(float);
-        if (smem > (48u << 10))      // the attribute is per device: set on every launch, not cached
-            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    auto launch = [&](auto kern) {
+        constexpr size_t smem = kRecSmemFloats * sizeof(float);   // under the 48 KB that need no attribute
         static const int per_sm = [&] {
             int v = 0;
-            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, kern, 32 * NWc, smem) != cudaSuccess || v < 1) v = 1;
+            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, kern, 32, smem) != cudaSuccess || v < 1) v = 1;
             return v;
         }();
-        const unsigned want = (ntiles + NWc - 1) / NWc;
-        unsigned ctas = static_cast<unsigned>(per_sm);
-        static const int forced_w = [] { const char *e = getenv("APTB200_REC_WARPS"); return e ? atoi(e) : 0; }();
-        if (forced_w > 0) ctas = std::max(1u, std::min<unsigned>(static_cast<unsigned>(forced_w) / NWc, ctas));
-        const unsigned grid = std::min<unsigned>(want, static_cast<unsigned>(c.sm_count) * ctas);
-        kern<<<grid, 32 * NWc, smem, c.stream>>>(e, n, ncorr, t, ctl, desc, pool, pool_cap, region, ntiles);
+        const unsigned grid = std::min<unsigned>(ntiles, static_cast<unsigned>(c.sm_count) * per_sm);
+        kern<<<grid, 32, smem, c.stream>>>(e, n, ncorr, t, ctl, desc, pool, pool_cap, region, ntiles);
     };
-    using I1 = std::integral_constant<int, 1>;
-    using I2 = std::integral_constant<int, 2>;
-    auto pick = [&](auto tbc, auto nbc) -> int {
-        constexpr int TBc = decltype(tbc)::value, NBc = decltype(nbc)::value;
-        if (ntaps == 37 && pw == 3) {
-            launch(k_lowpass_records<37, 3, TBc, NBc>, I1{});
-        } else if (ntaps == 43 && pw == 4) launch(k_lowpass_records<43, 4, TBc, NBc>, I1{});
-        else if (ntaps == 61 && pw == 5) launch(k_lowpass_records<61, 5, TBc, NBc>, I1{});
-        else return fail(APT_ERR_BAD_ARG, "no fused low-pass/record kernel for %u taps, pixel width %u", ntaps, pw);
-        return APT_OK;
-    };
-    using T32 = std::integral_constant<int, 32>;
-    using T64 = std::integral_constant<int, 64>;
-    int rc;
-    if (tb == 64) rc = nbuf == 2 ? pick(T64{}, I2{}) : pick(T64{}, I1{});
-    else rc = nbuf == 2 ? pick(T32{}, I2{}) : pick(T32{}, I1{});
-    if (rc != APT_OK) return rc;
+    if (ntaps == 37 && pw == 3) launch(k_lowpass_records<37, 3>);
+    else if (ntaps == 43 && pw == 4) launch(k_lowpass_records<43, 4>);
+    else if (ntaps == 61 && pw == 5) launch(k_lowpass_records<61, 5>);
+    else return fail(APT_ERR_BAD_ARG, "no fused low-pass/record kernel for %u taps, pixel width %u", ntaps, pw);
     APT_CUDA(cudaGetLastError());
     return APT_OK;
 }
@@ -537,11 +476,6 @@ int launch_process_stage(const LaunchCtx &c, const ProcessLaunch &a, KernelHook 
     if (a.max_rows == 0) return APT_OK;
     if (((reinterpret_cast<uintptr_t>(a.rows) & 15) | (reinterpret_cast<uintptr_t>(a.grey) & 15) | (reinterpret_cast<uintptr_t>(a.out) & 15)) != 0)
         return fail(APT_ERR_BAD_ARG, "process stage: buffers must be 16-byte aligned");
-    struct Scope {                 // hook->begin / end around one launch
-        KernelHook *h;
-        Scope(KernelHook *hk, const char *name) : h(hk) { if (h) h->begin(name); }
-        ~Scope() { if (h) h->end(); }
-    };
     const unsigned wide = static_cast<unsigned>(c.sm_count) * 8;
     const u32 px = 2080;
     const bool hist = a.contrast == 3;
@@ -552,33 +486,33 @@ int launch_process_stage(const LaunchCtx &c, const ProcessLaunch &a, KernelHook 
     APT_CUDA(cudaMemsetAsync(a.ctl, 0, sizeof(PostCtl), c.stream));
     if (hist) APT_CUDA(cudaMemsetAsync(a.proc->hist, 0, sizeof(a.proc->hist), c.stream));
     {
-        Scope s(hook, "post_stats");
+        KernelSlot s(hook, "post_stats");
         k_post_stats<<<std::min<unsigned>(a.max_rows, wide), 256, 0, c.stream>>>(a.rows, a.result, a.fixed_rows, px, a.ctl, a.tel_a,
                                                                                  a.tel_b, a.tel_v);
     }
     if (bounds_mode == 1) {
-        Scope s(hook, "post_histogram");
+        KernelSlot s(hook, "post_histogram");
         k_post_histogram<<<wide / 2, 256, 0, c.stream>>>(a.rows, a.result, a.fixed_rows, px, a.ctl);
     }
     {
-        Scope s(hook, "post_bounds");
+        KernelSlot s(hook, "post_bounds");
         k_post_bounds<<<1, 1024, 0, c.stream>>>(bounds_mode, a.percent, a.result, a.fixed_rows, px, a.ctl, a.tel_a, a.tel_b, a.tel_v);
     }
     if (hist) {
         {
             // two CTAs per SM: every CTA adds its 512 counts to the same 512 global words at the end
-            Scope s(hook, "post_map_u8_hist");
+            KernelSlot s(hook, "post_map_u8_hist");
             k_post_map_u8_hist<<<static_cast<unsigned>(c.sm_count) * 2, 256, 0, c.stream>>>(a.rows, a.result, a.fixed_rows, a.ctl,
                                                                                               grey, a.proc);
         }
-        Scope s(hook, "post_eq_lut");
+        KernelSlot s(hook, "post_eq_lut");
         k_post_eq_lut<<<1, 512, 0, c.stream>>>(a.proc);
     } else {
-        Scope s(hook, "post_map_u8");
+        KernelSlot s(hook, "post_map_u8");
         k_post_map_u8<<<wide, 256, 0, c.stream>>>(a.rows, a.result, a.fixed_rows, px, a.ctl, nullptr, grey);
     }
     if (finish) {
-        Scope s(hook, "post_finish");
+        KernelSlot s(hook, "post_finish");
         const int mode = a.palette ? 2 : (hist ? 1 : 0);
         const float4 tune = make_float4(a.tune[0], a.tune[1], a.tune[2], a.tune[3]);
         if (a.rgba) k_post_finish<true><<<wide, 256, 0, c.stream>>>(grey, a.ctl, a.proc, mode, a.rotate ? 1 : 0, a.palette, tune, a.out);
@@ -603,7 +537,7 @@ int launch_quantize_i16(const LaunchCtx &c, const float *x, u64 n, PostCtl *ctl,
 static size_t align_up(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
 
 size_t pick_scratch_bytes(u32 max_blocks, u32 max_positions, u32 cap) {
-    return align_up((static_cast<size_t>(max_blocks) + 1) * 4) + 5 * align_up((static_cast<size_t>(cap) + 1) * 4) +
+    return align_up((static_cast<size_t>(max_blocks) + 1) * 4) + 4 * align_up((static_cast<size_t>(cap) + 1) * 4) +
            align_up((static_cast<size_t>(max_positions) + 1) * 4) + align_up(8);
 }
 
@@ -620,7 +554,6 @@ PickScratch pick_scratch_carve(void *base, u32 max_blocks, u32 max_positions, u3
     s.cand_peak = take(static_cast<size_t>(cap) + 1);
     s.ja = take(static_cast<size_t>(cap) + 1);
     s.jb = take(static_cast<size_t>(cap) + 1);
-    s.idx = take(static_cast<size_t>(cap) + 1);
     s.orbit = take(static_cast<size_t>(max_positions) + 1);
     s.ticket = take(2);
     s.cap = cap;

@@ -29,7 +29,7 @@ constexpr u32 kSyncRedo = 100;
 
 // Control block of the fused sync stage (kernels_sync2.cuh); zeroed at the start of every job.
 struct SyncCtl {
-    u32 tile_ticket;   // (unused since the tiles of k_lowpass_records are dealt out statically)
+    u32 pad0;          // keeps the layout of the fields below
     u32 pool_cursor;   // record-pool entries handed out
     u32 overflow;      // the pool was exhausted
     u32 root_cursor;   // dense root ids handed out by k_resolve_roots (= number of roots when it is done)
@@ -77,8 +77,7 @@ struct PickScratch {
     u32 *block_off;    // [nblocks + 1] exclusive scan of root_count (dense root numbering)
     u32 *cand_s;       // [cap + 1] start position of each candidate
     u32 *cand_peak;    // [cap + 1] firstroot(start)
-    u32 *ja, *jb;      // [cap + 1] jump tables (J0, and the global ping-pong pair when smem is too small / E = J0^8)
-    u32 *idx;          // [cap + 1] compressed walk: image flag, then compact id of a node
+    u32 *ja, *jb;      // [cap + 1] jump tables (J0, and the global ping-pong pair when smem is too small)
     u32 *orbit;        // [max_positions + 1]
     u32 *ticket;       // [2] last-CTA tickets of k_roots / k_pick_links (zero between launches)
     u32 cap;           // candidate capacity
@@ -182,10 +181,12 @@ int launch_lowpass_corr(const LaunchCtx &c, const float *e, u64 n, const float *
 // roots of the correlation (see kernels_sync.cuh).
 int launch_roots(const LaunchCtx &c, const float *corr, u64 ncorr, u32 dist, u32 *root_list, u32 *root_count,
                  SyncResult *result, const PickScratch *scratch /* nullptr: no dense numbering */);
-// orbit walk -> sync positions (decode.rs:241-253).
+// The orbit walks: one thread; k_pick_j0 + k_pick_cluster (one 8-CTA cluster); k_pick_links (cooperative, whole GPU).
+enum class Walk { Sequential, Cluster, Grid };
+// orbit walk -> sync positions (decode.rs:241-253).  The cluster walk becomes the grid walk for recordings of more than
+// 20000 rows or when the device refuses its shared memory; scratch is unused by the sequential walk.
 int launch_pick(const LaunchCtx &c, u64 ncorr, u64 nwork, u32 row, u32 dist, const RootIndex &ri, u32 *positions,
-                u32 max_positions, SyncResult *result, const PickScratch *scratch /* nullptr: sequential walk */,
-                int *kernels_launched = nullptr);
+                u32 max_positions, SyncResult *result, Walk walk, const PickScratch &scratch, int *kernels_launched = nullptr);
 // Fused sync stage (kernels_sync2.cuh): low-pass + correlation + per-tile records, then the roots; f and corr never reach HBM.
 u32 records_tile(u32 pixel_width);   // correlation positions per tile
 int launch_lowpass_records(const LaunchCtx &c, const float *e, u64 n, u64 ncorr, const float *taps_host, u32 ntaps,
@@ -248,6 +249,13 @@ int launch_image_stage(const LaunchCtx &c, const float *rows, const SyncResult *
 struct KernelHook {
     virtual void begin(const char *name) = 0;
     virtual void end() = 0;
+    virtual void extra(int kernels) {}   // launches inside the current slot beyond the one begin() counts
+};
+// hook->begin / end around one scope (hook may be nullptr).
+struct KernelSlot {
+    KernelHook *hook;
+    KernelSlot(KernelHook *h, const char *name) : hook(h) { if (hook) hook->begin(name); }
+    ~KernelSlot() { if (hook) hook->end(); }
 };
 
 // The rest of noaa_apt::process (kernels_post.cuh, aptb200.h apt_process_settings) on rows of 2080 pixels.  All pointers are

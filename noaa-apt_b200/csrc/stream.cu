@@ -42,7 +42,7 @@ int check_stream_args(uint32_t input_rate, const apt_settings *s, int sync, uint
         return fail(APT_ERR_BAD_ARG, "the stream needs a work rate that is a multiple of 4160 (the final NoFilter resample is "
                                      "not streamed)");
     }
-    if (!lowpass_corr_supported(static_cast<u32>(p.lp.size()), p.dec))
+    if (!back_fused(p))
         return fail(APT_ERR_BAD_ARG, "the stream supports the standard, fast and slow demodulation low-pass (37/43/61 taps), "
                                      "not %zu taps at %u samples per pixel", p.lp.size(), p.dec);
     if (sync && p.dist > 16384)
