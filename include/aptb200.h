@@ -254,7 +254,15 @@ int apt_decode_image(const void *signal, int format, uint64_t n, uint32_t input_
 
 typedef struct apt_decoder apt_decoder;
 
-typedef enum apt_sample_format { APT_F32 = 0, APT_PCM16 = 1 } apt_sample_format;
+/* APT_F32 / APT_PCM16: audio samples.  APT_CU8 / APT_CF32 / APT_CS16: complex I/Q samples, interleaved I, Q (only the I/Q
+ * entry points below take them; every other entry point that takes a format rejects them like an unknown format). */
+typedef enum apt_sample_format {
+    APT_F32 = 0,
+    APT_PCM16 = 1,
+    APT_CU8 = 2,                  /* unsigned 8-bit I/Q: rtl_sdr / librtlsdr */
+    APT_CF32 = 3,                 /* complex float: GQRX I/Q recordings, the GNU Radio file sink */
+    APT_CS16 = 4                  /* signed 16-bit I/Q: baseband WAVs of SDR# and SDR++ */
+} apt_sample_format;
 
 /* Creates a decoder bound to CUDA device `device` for recordings of `input_rate` Hz of up to
  * `max_samples` samples.  Designs both filters, uploads the taps and allocates every workspace
@@ -429,6 +437,50 @@ int apt_stream_sync_positions(apt_stream *st, uint64_t *positions, size_t cap, s
 int apt_stream_get_info(apt_stream *st, apt_stream_info *info);
 /* Host only, no device: the geometry a stream of these parameters would have (latency_work, max_push, device_bytes). */
 int apt_stream_geometry(uint32_t input_rate, const apt_settings *s, int sync, uint64_t max_push, apt_stream_info *info);
+
+/* ------------------------------------------------------------------ I/Q input: FM demodulation on the device */
+
+/* Decoding straight from SDR I/Q (DESIGN.md §10; the reference has no I/Q path, so this stage is the project's own
+ * definition).  One fused kernel loads the I/Q (APT_CU8 (u - 127.5), APT_CS16, APT_CF32), mixes the channel at offset_hz
+ * to 0 Hz, runs the channel Lowpass (filters::Lowpass designed at iq_rate) decimated by D = iq_rate / audio_rate, and
+ * discriminates: a[0] = 0, a[m] = atan2f(Im(z[m] conj z[m-1]), Re(..)) * audio_rate / 2pi, the instantaneous frequency
+ * in Hz.  Output m reads inputs <= m*D only; its arithmetic depends on m and the input values alone, never on how the
+ * input is split into chunks.  n counts complex samples. */
+typedef struct apt_iq_settings {
+    uint32_t iq_rate;             /* complex samples per second */
+    uint32_t audio_rate;          /* discriminator output rate; must divide iq_rate */
+    int32_t offset_hz;            /* signal centre minus tuned centre */
+    float cutout, delta_freq, atten;   /* channel Lowpass: Hz, Hz, dB */
+} apt_iq_settings;
+
+/* cutout 22 kHz, delta_freq 8 kHz, atten 40 dB; audio_rate the smallest iq_rate / D that is >= 48 kHz.  APT_ERR_BAD_ARG
+ * when no D >= 1 gives that or the settings fail the checks of apt_fm_demod_len. */
+int apt_iq_default_settings(uint32_t iq_rate, int32_t offset_hz, apt_iq_settings *s);
+/* Audio samples of n I/Q samples: ceil(n / D).  Host only.  APT_ERR_BAD_ARG unless iq_rate % audio_rate == 0,
+ * cutout > 0, delta_freq > 0, atten > 8, cutout < audio_rate / 2, |offset_hz| + cutout < iq_rate / 2 and the channel
+ * filter has at most 8191 taps. */
+int apt_fm_demod_len(uint64_t n, const apt_iq_settings *s, uint64_t *nout);
+/* The stage alone: host I/Q in, host audio (f32, Hz) out; cap in floats. */
+int apt_fm_demod(const void *iq, int format, uint64_t n, const apt_iq_settings *s, float *out, uint64_t cap,
+                 uint64_t *nout);
+/* apt_decode at s->audio_rate of the audio apt_fm_demod would return, produced on the device: the I/Q is uploaded in
+ * chunks and the audio never leaves the GPU.  Rows, status and sync positions equal apt_decode(apt_fm_demod(iq)).
+ * cap in floats >= apt_decode_len_bound(ceil(n / D), audio_rate). */
+int apt_decode_iq(const void *iq, int format, uint64_t n, const apt_iq_settings *s, const apt_settings *settings, int sync,
+                  float *out, uint64_t cap, uint64_t *nout, apt_status_cb cb, void *user);
+/* Live decoding from a radio: a stream (apt_stream_push / finish / reset / ... as above) whose pushes are I/Q samples of
+ * APT_CU8, APT_CS16 or APT_CF32, mixed freely; audio pushes are APT_ERR_BAD_ARG, as are I/Q pushes to an audio stream.
+ * max_push and apt_stream_push_bound's n count I/Q samples.  Every push is converted into a cf32 window on the device that
+ * keeps the N - 1 + D samples the next audio output reads; the FM kernel writes each audio sample as soon as its input is
+ * complete.  The rows, positions and status equal apt_decode_iq on the whole input.  samples_in counts I/Q samples,
+ * device_bytes includes the I/Q window; work_final, latency_work and the emission rule are the audio stream's. */
+int apt_stream_create_iq(int device, const apt_iq_settings *iq, const apt_settings *s, int sync, uint64_t max_push,
+                         apt_stream **st);
+int apt_stream_geometry_iq(const apt_iq_settings *iq, const apt_settings *s, int sync, uint64_t max_push,
+                           apt_stream_info *info);
+/* A 2-channel 16-bit PCM WAV (SDR# / SDR++ baseband) as interleaved APT_CS16: out receives 2 * *n int16, *n the frames
+ * (complex samples), cap in int16.  Any other layout is APT_ERR_IO. */
+int apt_wav_load_iq16(const char *path, int16_t *out, uint64_t cap, uint64_t *n, uint32_t *sample_rate);
 
 #ifdef __cplusplus
 }

@@ -208,6 +208,12 @@ class Stream {
         const apt_settings s = settings.to_c();
         err::check(apt_stream_create(device, input_rate.get_hz(), &s, sync ? 1 : 0, max_push, &st_));
     }
+    // I/Q stream (apt_stream_create_iq): push_iq() takes APT_CU8 / APT_CS16 / APT_CF32 samples, max_push counts them.
+    Stream(const apt_iq_settings &iq, const config::Settings &settings, bool sync = true, uint64_t max_push = 1200000,
+           int device = 0) {
+        const apt_settings s = settings.to_c();
+        err::check(apt_stream_create_iq(device, &iq, &s, sync ? 1 : 0, max_push, &st_));
+    }
     ~Stream() { apt_stream_destroy(st_); }
     Stream(const Stream &) = delete;
     Stream &operator=(const Stream &) = delete;
@@ -217,6 +223,9 @@ class Stream {
     Signal push(const int16_t *samples, size_t n) { return rows(n, [&](float *o, uint64_t c, uint64_t *k) {
         return apt_stream_push(st_, samples, APT_PCM16, n, o, c, k); }); }
     Signal push(const Signal &samples) { return push(samples.data(), samples.size()); }
+    // n complex samples, interleaved I, Q
+    Signal push_iq(const void *samples, int format, size_t n) { return rows(n, [&](float *o, uint64_t c, uint64_t *k) {
+        return apt_stream_push(st_, samples, format, n, o, c, k); }); }
     Signal finish() { return rows(0, [&](float *o, uint64_t c, uint64_t *k) { return apt_stream_finish(st_, o, c, k); }); }
     void reset() { err::check(apt_stream_reset(st_)); }
     std::vector<uint64_t> positions() const {
@@ -244,5 +253,33 @@ class Stream {
     }
     apt_stream *st_ = nullptr;
 };
+
+// Decoding straight from SDR I/Q (DESIGN.md §10).  format: APT_CU8 / APT_CS16 / APT_CF32, n complex samples.
+namespace iq {
+inline apt_iq_settings default_settings(uint32_t iq_rate, int32_t offset_hz = 0) {
+    apt_iq_settings s{};
+    err::check(apt_iq_default_settings(iq_rate, offset_hz, &s));
+    return s;
+}
+inline Signal fm_demod(const void *samples, int format, uint64_t n, const apt_iq_settings &s) {
+    uint64_t len = 0, got = 0;
+    err::check(apt_fm_demod_len(n, &s, &len));
+    Signal out(len ? len : 1);
+    err::check(apt_fm_demod(samples, format, n, &s, out.data(), out.size(), &got));
+    out.resize(got);
+    return out;
+}
+inline Signal decode_iq(Context &ctx, const config::Settings &settings, const void *samples, int format, uint64_t n,
+                        const apt_iq_settings &s, bool sync) {
+    const apt_settings st = settings.to_c();
+    uint64_t len = 0, bound = 0, got = 0;
+    err::check(apt_fm_demod_len(n, &s, &len));
+    err::check(apt_decode_len_bound(len, s.audio_rate, &st, &bound));
+    Signal out(bound ? bound : 1);
+    err::check(apt_decode_iq(samples, format, n, &s, &st, sync ? 1 : 0, out.data(), out.size(), &got, &Context::trampoline, &ctx));
+    out.resize(got);
+    return out;
+}
+}  // namespace iq
 
 }  // namespace noaa_apt

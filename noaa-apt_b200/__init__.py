@@ -10,17 +10,17 @@ Mirrors the module layout of martinber/noaa-apt's hot path:
 Every compute call goes through the C ABI of libaptb200.so (include/aptb200.h) into hand-written
 sm_90a CUDA kernels.  There is no CPU path: importing works anywhere, computing needs a GPU.
 """
-from . import _lib, config, context, dsp, err, filters, frequency, image, wav  # noqa: F401
+from . import _lib, config, context, dsp, err, filters, frequency, image, iq, wav  # noqa: F401
 from . import decode as _decode_mod
 from .config import Settings
 from .context import Context
 from .decode import (CARRIER_FREQ, FINAL_RATE, PX_PER_ROW, Decoder, Stream, decode, decode_batch, decode_len_bound,
-                     find_sync, generate_sync_frame, stream_geometry)
+                     find_sync, generate_sync_frame, stream_geometry, stream_geometry_iq)
 from .frequency import Freq, Rate
 
 __all__ = ["decode", "decode_batch", "decode_len_bound", "find_sync", "generate_sync_frame", "Decoder", "Stream",
-           "stream_geometry",
-           "Settings", "Context", "Freq", "Rate", "dsp", "filters", "err", "config", "frequency", "image", "wav",
+           "stream_geometry", "stream_geometry_iq",
+           "Settings", "Context", "Freq", "Rate", "dsp", "filters", "err", "config", "frequency", "image", "iq", "wav",
            "FINAL_RATE", "PX_PER_ROW", "CARRIER_FREQ"]
 
 

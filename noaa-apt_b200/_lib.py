@@ -24,6 +24,7 @@ ERR_IO = 11
 
 FILTER_NONE, FILTER_LOWPASS, FILTER_LOWPASS_DC = 0, 1, 2
 F32, PCM16 = 0, 1
+CU8, CF32, CS16 = 2, 3, 4   # I/Q formats (apt_fm_demod / apt_decode_iq only)
 
 
 class CSettings(C.Structure):
@@ -82,6 +83,11 @@ class CPhInfo(C.Structure):
 class CStreamInfo(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("samples_in", "work_final", "rows_out", "peaks", "latency_work", "max_push",
                                           "device_bytes")]
+
+
+class CIqSettings(C.Structure):
+    _fields_ = [("iq_rate", C.c_uint32), ("audio_rate", C.c_uint32), ("offset_hz", C.c_int32), ("cutout", C.c_float),
+                ("delta_freq", C.c_float), ("atten", C.c_float)]
 
 
 STATUS_CB = C.CFUNCTYPE(None, C.c_float, C.c_char_p, C.c_void_p)
@@ -176,6 +182,16 @@ SIGNATURES = {
     "apt_stream_sync_positions": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, _szp]),
     "apt_stream_get_info": (C.c_int, [C.c_void_p, C.POINTER(CStreamInfo)]),
     "apt_stream_geometry": (C.c_int, [C.c_uint32, C.POINTER(CSettings), C.c_int, C.c_uint64, C.POINTER(CStreamInfo)]),
+    "apt_iq_default_settings": (C.c_int, [C.c_uint32, C.c_int32, C.POINTER(CIqSettings)]),
+    "apt_fm_demod_len": (C.c_int, [C.c_uint64, C.POINTER(CIqSettings), _u64p]),
+    "apt_fm_demod": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64, C.POINTER(CIqSettings), C.c_void_p, C.c_uint64, _u64p]),
+    "apt_decode_iq": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64, C.POINTER(CIqSettings), C.POINTER(CSettings), C.c_int,
+                                C.c_void_p, C.c_uint64, _u64p, STATUS_CB, C.c_void_p]),
+    "apt_stream_create_iq": (C.c_int, [C.c_int, C.POINTER(CIqSettings), C.POINTER(CSettings), C.c_int, C.c_uint64,
+                                       C.POINTER(C.c_void_p)]),
+    "apt_stream_geometry_iq": (C.c_int, [C.POINTER(CIqSettings), C.POINTER(CSettings), C.c_int, C.c_uint64,
+                                         C.POINTER(CStreamInfo)]),
+    "apt_wav_load_iq16":(C.c_int, [C.c_char_p, C.c_void_p, C.c_uint64, _u64p, C.POINTER(C.c_uint32)]),
 }
 
 _lib = None

@@ -77,6 +77,9 @@ int aptb200::free_decoder_buffers(apt_decoder *d) {
     if (d->h_post) cudaFreeHost(d->h_post);
     for (void *p : {(void *)d->d_post, (void *)d->d_tel, (void *)d->d_out8, (void *)d->d_palette, (void *)d->d_proc, (void *)d->d_grey})
         if (p) cudaFree(p);
+    d->iq_tables.release();
+    d->iq_win.release();
+    if (d->d_audio) cudaFree(d->d_audio);
     d->own_stager.reset();
     for (auto e : d->ev_begin) cudaEventDestroy(e);
     for (auto e : d->ev_end) cudaEventDestroy(e);
@@ -1005,6 +1008,80 @@ extern "C" int apt_decode(const float *signal, uint64_t n, uint32_t input_rate, 
 extern "C" int apt_decode_pcm16(const int16_t *pcm, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
                                 float *out, uint64_t cap, uint64_t *nout, apt_status_cb cb, void *user) {
     return decode_oneshot(pcm, APT_PCM16, n, input_rate, s, sync, out, cap, nout, cb, user);
+}
+
+// apt_decode at audio_rate of the audio the FM kernel writes into the parked decoder's device input.
+extern "C" int apt_decode_iq(const void *iq, int format, uint64_t n, const apt_iq_settings *is, const apt_settings *s, int sync,
+                             float *out, uint64_t cap, uint64_t *nout, apt_status_cb cb, void *user) {
+    if (!is || !s || !nout) return fail(APT_ERR_BAD_ARG, "null argument");
+    *nout = 0;
+    if (n == 0 || !iq) return fail(APT_ERR_BAD_ARG, "empty signal");
+    if (!iq_sample_bytes(format)) return fail(APT_ERR_BAD_ARG, "unknown I/Q sample format %d", format);
+    IqPlan ip;
+    APT_TRY(make_iq(*is, ip));
+    const uint64_t na = ip.out_len(n);
+    const uint32_t rate = is->audio_rate;
+    uint64_t need = 0;
+    {
+        // errors that do not need a device come first, in decode_oneshot's order
+        Plan p;
+        APT_TRY(make_plan(rate, *s, p));
+        const uint64_t nwork = p.front.work_len(na);
+        if (nwork < 10ull * p.row) return fail(APT_ERR_TOO_SHORT, "Got less than 10 rows of samples, audio file is too short");
+        if (sync && !p.work_multiple) return fail(APT_ERR_WORK_RATE, "work_rate is not multiple of FINAL_RATE");
+        need = sync ? (nwork / p.row) * kPxPerRow : plan_out_bound(p, na);
+    }
+    if (!out || cap < need) return fail(APT_ERR_CAPACITY, "output needs room for %llu floats", (unsigned long long)need);
+    APT_TRY(require_device());
+    int device = 0;
+    if (cudaGetDevice(&device) != cudaSuccess) device = 0;
+    static const bool use_cache = getenv("APTB200_NO_CACHE") == nullptr;
+    apt_decoder *d = use_cache ? cache_take(device, rate, *s, na) : nullptr;
+    if (!d) {
+        const uint64_t room = use_cache ? ((na + na / 8 + (1u << 20)) & ~((1ull << 20) - 1)) : na;
+        APT_TRY(apt_decoder_create(device, rate, s, room, &d));
+    }
+    auto run = [&]() -> int {
+        APT_CUDA(cudaSetDevice(d->device));
+        if (!d->iq_tables_valid || memcmp(&d->iq_settings, is, sizeof(*is)) != 0) {
+            d->iq_tables_valid = false;
+            APT_TRY(d->iq_tables.upload(ip));
+            d->iq_settings = *is;
+            d->iq_tables_valid = true;
+        }
+        if (d->audio_cap < d->max_samples) {
+            if (d->d_audio) APT_CUDA(cudaFree(d->d_audio));
+            d->d_audio = nullptr;
+            d->audio_cap = 0;
+            APT_CUDA(cudaMalloc(&d->d_audio, std::max<uint64_t>(d->max_samples, 1) * sizeof(float)));
+            d->audio_cap = d->max_samples;
+        }
+        if (!d->d_out) APT_CUDA(cudaMalloc(&d->d_out, std::max<uint64_t>(d->max_out, 1) * sizeof(float)));
+        if (is_pageable(iq) && !d->stager && !getenv("APTB200_NO_STAGER")) {
+            int threads = 8;
+            if (const char *e = getenv("APTB200_COPY_THREADS")) threads = std::max(1, atoi(e));
+            d->own_stager.reset(new (std::nothrow) HostStager(d->device, 16u << 20, 3, threads));
+            if (d->own_stager && !d->own_stager->ok()) d->own_stager.reset();
+            d->stager = d->own_stager.get();
+        }
+        APT_TRY(iq_demod_host(LaunchCtx{d->stream, d->sm_count}, ip, d->iq_tables, iq, format, n, d->iq_win,
+                              is_pageable(iq) ? d->stager : nullptr, d->d_audio, nullptr));
+        APT_TRY(apt_decoder_submit_device(d, d->d_audio, APT_F32, na, sync, d->d_out, d->max_out));
+        uint64_t produced = 0;
+        APT_TRY(apt_decoder_wait(d, &produced));
+        APT_CUDA(cudaMemcpy(out, d->d_out, produced * sizeof(float), cudaMemcpyDeviceToHost));
+        *nout = produced;
+        return APT_OK;
+    };
+    d->cb = cb;
+    d->cb_user = user;
+    const int st = run();
+    if (st != APT_OK) cudaStreamSynchronize(d->stream);
+    d->cb = nullptr;
+    d->cb_user = nullptr;
+    if (use_cache) cache_put(device, rate, *s, d);
+    else apt_decoder_destroy(d);
+    return st;
 }
 
 // ============================================================================== image stage

@@ -15,6 +15,7 @@
 #include "filters_host.hpp"
 #include "front.hpp"
 #include "hostpool.hpp"
+#include "iq.hpp"
 #include "launch.hpp"
 
 namespace aptb200 {
@@ -120,6 +121,15 @@ struct apt_decoder {
     aptb200::ProcCtl *d_proc = nullptr;
     unsigned char *d_grey = nullptr;        // max_out B intermediate grey plane
     uint64_t job_bpp = 1;          // output bytes per pixel of the image job in flight
+
+    // apt_decode_iq (allocated on first use): the I/Q stage's tables for iq_settings, one chunk's I/Q window and the
+    // audio the FM kernel writes, which is the input of the decode job
+    apt_iq_settings iq_settings{};
+    bool iq_tables_valid = false;
+    aptb200::IqTables iq_tables;
+    aptb200::IqWindow iq_win;
+    float *d_audio = nullptr;
+    uint64_t audio_cap = 0;        // floats d_audio holds
 
     // job in flight
     bool in_flight = false;

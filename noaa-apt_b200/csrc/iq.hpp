@@ -1,0 +1,77 @@
+// The I/Q stage (DESIGN.md §10): FM demodulation of complex samples to audio at audio_rate.  This module alone reads
+// apt_iq_settings: it validates them, designs the channel filter, lays out the polyphase taps and the phasor table, owns
+// their device copies and launches k_fm_demod.
+#pragma once
+
+#include <cstdint>
+#include <vector>
+
+#include "aptb200.h"
+#include "launch.hpp"
+
+namespace aptb200 {
+
+struct IqPlan {
+    apt_iq_settings s{};
+    u32 D = 1;                    // iq_rate / audio_rate
+    std::vector<float> h;         // channel Lowpass, N taps
+    u32 qpad = 0;                 // taps per polyphase plane, rounded up to 16
+    std::vector<float> hp;        // D x qpad: hp[r][q] = h[q*D + r], 0 past N
+    std::vector<float> W;         // kIqBlock interleaved phasors W[t] = exp(-2 pi j ((t f) mod fs) / fs)
+    uint64_t f = 0;               // offset_hz mod iq_rate, in [0, iq_rate)
+    float scale = 0.f;            // (float)(audio_rate / 2pi)
+    u32 tz = 0, lp16 = 0, ps = 0; // tile geometry of k_fm_demod
+    size_t smem = 0;              // its dynamic shared memory
+
+    uint64_t out_len(uint64_t n) const { return (n + D - 1) / D; }
+    // I/Q samples [xa, xb) that audio outputs [m0, m1) read (z[m0 - 1] included), clipped to a recording of n samples.
+    void span(uint64_t m0, uint64_t m1, uint64_t n, uint64_t &xa, uint64_t &xb) const;
+};
+
+// Validation (host only, APT_ERR_BAD_ARG on failure), D, the taps, W and the tile geometry.
+int make_iq(const apt_iq_settings &s, IqPlan &plan);
+int iq_default_settings(uint32_t iq_rate, int32_t offset_hz, apt_iq_settings &s);
+// bytes per complex sample of an I/Q format, 0 for any other format
+size_t iq_sample_bytes(int format);
+
+// Device copies of the taps and the phasor table.
+struct IqTables {
+    float *hp = nullptr;
+    float *W = nullptr;
+    IqTables() = default;
+    IqTables(const IqTables &) = delete;
+    ~IqTables() { release(); }
+    int upload(const IqPlan &p);
+    void release();
+};
+
+// Audio outputs [m0, m1) of a recording of n I/Q samples.  `window` holds the absolute samples [w_lo, w_hi), which must
+// cover plan.span(m0, m1, n); in and out are the addresses sample / output 0 would have.
+int iq_launch(const LaunchCtx &c, const IqPlan &plan, const IqTables &t, const void *in, uint64_t w_lo, uint64_t w_hi,
+              int format, uint64_t m0, uint64_t m1, float *out);
+
+// n samples of an I/Q format, converted exactly to interleaved f32 at out (the streaming decoder's cf32 window).
+int iq_to_cf32(const LaunchCtx &c, const void *in, int format, uint64_t n, float *out);
+
+// I/Q samples per upload chunk: 32 Mi, or APTB200_IQ_CHUNK (diagnostic: puts chunk boundaries inside short inputs).
+uint64_t iq_chunk_samples();
+
+// Device buffer of one chunk's I/Q window (grows, never shrinks).
+struct IqWindow {
+    void *p = nullptr;
+    uint64_t cap = 0;   // bytes
+    IqWindow() = default;
+    IqWindow(const IqWindow &) = delete;
+    ~IqWindow() { release(); }
+    int reserve(uint64_t bytes);
+    void release();
+};
+
+// All ceil(n / D) audio samples of the host I/Q `iq` into device d_audio, on c.stream: chunk by chunk, each chunk's window
+// (its samples and the halo its first output reads) uploaded through `stager` (pageable input) or cudaMemcpyAsync
+// (stager == nullptr), then one launch for the outputs the chunk completes.  The audio is the same for every chunk size.
+class HostStager;
+int iq_demod_host(const LaunchCtx &c, const IqPlan &p, const IqTables &t, const void *iq, int format, uint64_t n,
+                  IqWindow &win, HostStager *stager, float *d_audio, KernelHook *hook);
+
+}  // namespace aptb200

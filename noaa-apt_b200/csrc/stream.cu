@@ -100,6 +100,16 @@ struct apt_stream {
     const StreamCarry &carry() const { return *reinterpret_cast<const StreamCarry *>(h_carry); }
     const u32 *run_pos() const { return reinterpret_cast<const u32 *>(h_carry + sizeof(StreamCarry)); }
     const u32 *run_cnt() const { return run_pos() + kRunRing; }
+
+    // I/Q stream (apt_stream_create_iq): every push is converted into the cf32 window d_iq, which keeps the halo the next
+    // audio output reads, and k_fm_demod writes the new audio into d_in; the audio counters above then count audio samples
+    bool iq = false;
+    uint64_t iq_max_push = 0;       // I/Q samples one step takes
+    IqPlan iqp;
+    IqTables iqt;
+    float *d_iq = nullptr;          // interleaved cf32, iq_cap complex samples from absolute sample iq_base
+    void *d_iqraw = nullptr;        // one step's pushed samples as they came
+    uint64_t iq_cap = 0, iq_in = 0, iq_base = 0;
 };
 
 namespace {
@@ -112,12 +122,16 @@ void free_stream(apt_stream *st) {
         if (p) cudaFree(p);
     if (st->h_carry) cudaFreeHost(st->h_carry);
     if (st->h_rows) cudaFreeHost(st->h_rows);
+    if (st->d_iq) cudaFree(st->d_iq);
+    if (st->d_iqraw) cudaFree(st->d_iqraw);
+    st->iqt.release();
     free_decoder_buffers(&st->dec);
 }
 
 int reset_state(apt_stream *st) {
     st->samples_in = st->in_base = st->units_done = st->work_final = st->e_base = st->c_base = st->c_end = 0;
     st->rows_out = st->gathered = st->held_slot = st->runs_seen = 0;
+    st->iq_in = st->iq_base = 0;
     st->finished = false;
     st->positions.clear();
     APT_CUDA(cudaSetDevice(st->dec.device));
@@ -180,17 +194,15 @@ void take_rows(apt_stream *st, uint64_t rel_hi, float *rows, uint64_t &nout) {
     st->rows_out = rel_hi;
 }
 
-// One step: `n` new samples (maybe none) and, when `finish`, the end of the recording.
-int step(apt_stream *st, const void *host, int format, uint64_t n, bool finish, float *rows, uint64_t &nout, int &status) {
+// The new audio of one step into the input window, from either source: audio pushes are uploaded as they are (PCM16 cast
+// into the f32 window, so pushes may mix formats); I/Q pushes are converted into the cf32 window and every audio sample
+// they complete is demodulated into the input window.  `added` receives the number of new audio samples.
+int upload(apt_stream *st, const void *host, int format, uint64_t n, uint64_t &added) {
     apt_decoder &d = st->dec;
-    const Plan &p = d.plan;
-    const Geom &g = st->g;
     const LaunchCtx c{d.stream, d.sm_count};
-    APT_TRY(compact_all(st));
-    // ---- upload (PCM16 is cast into the f32 window: pushes may mix formats) ----
-    if (n) {
-        const uint64_t off = st->samples_in - st->in_base;
-        if (off + n > g.cap_in) return fail(APT_ERR_BAD_ARG, "internal: input window overflow");
+    const uint64_t off = st->samples_in - st->in_base;
+    if (!st->iq) {
+        if (off + n > st->g.cap_in) return fail(APT_ERR_BAD_ARG, "internal: input window overflow");
         if (format == APT_PCM16) {
             APT_CUDA(cudaMemcpyAsync(st->d_pcm, host, n * 2, cudaMemcpyHostToDevice, d.stream));
             APT_TRY(launch_pcm16_to_f32(c, st->d_pcm, n, st->d_conv));
@@ -198,7 +210,41 @@ int step(apt_stream *st, const void *host, int format, uint64_t n, bool finish, 
         } else {
             APT_CUDA(cudaMemcpyAsync(st->d_in + off, host, n * 4, cudaMemcpyHostToDevice, d.stream));
         }
-        st->samples_in += n;
+        added = n;
+        return APT_OK;
+    }
+    const IqPlan &q = st->iqp;
+    // the cf32 window keeps what the next audio output reads; its tail moves to the front when that does not overlap
+    uint64_t xa, xb;
+    q.span(st->samples_in, st->samples_in + 1, ~0ull, xa, xb);
+    if (xa > st->iq_base && st->iq_in - xa <= xa - st->iq_base) {
+        if (st->iq_in > xa)
+            APT_CUDA(cudaMemcpyAsync(st->d_iq, st->d_iq + 2 * (xa - st->iq_base), (st->iq_in - xa) * 2 * sizeof(float),
+                                     cudaMemcpyDeviceToDevice, d.stream));
+        st->iq_base = xa;
+    }
+    if (st->iq_in - st->iq_base + n > st->iq_cap) return fail(APT_ERR_BAD_ARG, "internal: I/Q window overflow");
+    APT_CUDA(cudaMemcpyAsync(st->d_iqraw, host, n * iq_sample_bytes(format), cudaMemcpyHostToDevice, d.stream));
+    APT_TRY(iq_to_cf32(c, st->d_iqraw, format, n, st->d_iq + 2 * (st->iq_in - st->iq_base)));
+    st->iq_in += n;
+    const uint64_t m1 = q.out_len(st->iq_in);
+    added = m1 - st->samples_in;
+    if (off + added > st->g.cap_in) return fail(APT_ERR_BAD_ARG, "internal: input window overflow");
+    return iq_launch(c, q, st->iqt, st->d_iq - 2 * st->iq_base, st->iq_base, st->iq_in, APT_CF32, st->samples_in, m1,
+                     st->d_in - st->in_base);
+}
+
+// One step: `n` new samples (maybe none) and, when `finish`, the end of the recording.
+int step(apt_stream *st, const void *host, int format, uint64_t n, bool finish, float *rows, uint64_t &nout, int &status) {
+    apt_decoder &d = st->dec;
+    const Plan &p = d.plan;
+    const Geom &g = st->g;
+    const LaunchCtx c{d.stream, d.sm_count};
+    APT_TRY(compact_all(st));
+    if (n) {
+        uint64_t added = 0;
+        APT_TRY(upload(st, host, format, n, added));
+        st->samples_in += added;
     }
     const uint64_t N = st->samples_in;
     const uint64_t nw = p.front.work_len(N);
@@ -296,8 +342,11 @@ int step(apt_stream *st, const void *host, int format, uint64_t n, bool finish, 
     return APT_OK;
 }
 
+// audio samples a push of n samples adds
+uint64_t audio_of(const apt_stream *st, uint64_t n) { return st->iq ? st->iqp.out_len(st->iq_in + n) - st->samples_in : n; }
+
 uint64_t rows_bound(const apt_stream *st, uint64_t n) {
-    const uint64_t nw = st->dec.plan.front.work_len(st->samples_in + n);
+    const uint64_t nw = st->dec.plan.front.work_len(st->samples_in + audio_of(st, n));
     const uint64_t most = nw / st->g.row + 1;
     return most > st->rows_out ? (most - st->rows_out) * kPxPerRow : 0;
 }
@@ -316,12 +365,88 @@ extern "C" int apt_stream_geometry(uint32_t input_rate, const apt_settings *s, i
     return APT_OK;
 }
 
+namespace {
+
+// The I/Q stream's geometry: its audio stream takes at most max_push / D + 1 audio samples per step; the cf32 window holds
+// one step, the halo of the next output (N - 1 + D samples) and the same again so that compaction never overlaps.
+int check_iq_stream_args(const apt_iq_settings *is, const apt_settings *s, int sync, uint64_t max_push, IqPlan &q, Plan &p,
+                         uint64_t &audio_push) {
+    if (!is) return fail(APT_ERR_BAD_ARG, "null I/Q settings");
+    if (max_push == 0 || max_push > (1ull << 28)) return fail(APT_ERR_BAD_ARG, "max_push %llu outside [1, 2^28]", (unsigned long long)max_push);
+    APT_TRY(make_iq(*is, q));
+    audio_push = max_push / q.D + 1;
+    return check_stream_args(is->audio_rate, s, sync, audio_push, p);
+}
+
+uint64_t iq_window(const IqPlan &q, uint64_t max_push) { return 2 * (q.h.size() + 2ull * q.D) + max_push + 64; }
+
+uint64_t iq_bytes(const IqPlan &q, uint64_t max_push) {
+    return iq_window(q, max_push) * 8 + max_push * 8 + (q.hp.size() + q.W.size()) * sizeof(float);
+}
+
+int create(int device, uint32_t input_rate, int sync, uint64_t max_push, std::unique_ptr<apt_stream> &st);
+
+}  // namespace
+
+extern "C" int apt_stream_geometry_iq(const apt_iq_settings *is, const apt_settings *s, int sync, uint64_t max_push,
+                                      apt_stream_info *info) {
+    if (!info) return fail(APT_ERR_BAD_ARG, "null argument");
+    IqPlan q;
+    Plan p;
+    uint64_t audio_push = 0;
+    APT_TRY(check_iq_stream_args(is, s, sync, max_push, q, p, audio_push));
+    const Geom g = make_geom(p, sync, audio_push);
+    *info = apt_stream_info{};
+    info->latency_work = g.latency;
+    info->max_push = max_push;
+    info->device_bytes = g.bytes + iq_bytes(q, max_push);
+    return APT_OK;
+}
+
 extern "C" int apt_stream_create(int device, uint32_t input_rate, const apt_settings *s, int sync, uint64_t max_push, apt_stream **out) {
     if (!out) return fail(APT_ERR_BAD_ARG, "null argument");
     *out = nullptr;
     std::unique_ptr<apt_stream> st(new (std::nothrow) apt_stream);
     if (!st) return fail(APT_ERR_NOMEM, "out of host memory");
     APT_TRY(check_stream_args(input_rate, s, sync, max_push, st->dec.plan));
+    APT_TRY(create(device, input_rate, sync, max_push, st));
+    *out = st.release();
+    return APT_OK;
+}
+
+extern "C" int apt_stream_create_iq(int device, const apt_iq_settings *is, const apt_settings *s, int sync, uint64_t max_push,
+                                    apt_stream **out) {
+    if (!out) return fail(APT_ERR_BAD_ARG, "null argument");
+    *out = nullptr;
+    std::unique_ptr<apt_stream> st(new (std::nothrow) apt_stream);
+    if (!st) return fail(APT_ERR_NOMEM, "out of host memory");
+    uint64_t audio_push = 0;
+    APT_TRY(check_iq_stream_args(is, s, sync, max_push, st->iqp, st->dec.plan, audio_push));
+    st->iq = true;
+    st->iq_max_push = max_push;
+    st->iq_cap = iq_window(st->iqp, max_push);
+    APT_TRY(create(device, is->audio_rate, sync, audio_push, st));
+    apt_stream *raw = st.get();
+    struct Rollback {
+        apt_stream *st;
+        bool armed = true;
+        ~Rollback() {
+            if (armed) free_stream(st);
+        }
+    } rollback{raw};
+    APT_TRY(raw->iqt.upload(raw->iqp));
+    APT_CUDA(cudaMalloc(&raw->d_iq, raw->iq_cap * 2 * sizeof(float)));
+    APT_CUDA(cudaMalloc(&raw->d_iqraw, max_push * 8));
+    raw->g.bytes += iq_bytes(raw->iqp, max_push);
+    rollback.armed = false;
+    *out = st.release();
+    return APT_OK;
+}
+
+namespace {
+
+// Device side of apt_stream_create once the plan is checked: `max_push` counts audio samples.
+int create(int device, uint32_t input_rate, int sync, uint64_t max_push, std::unique_ptr<apt_stream> &st) {
     int count = 0;
     if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0) {
         cudaGetLastError();
@@ -363,9 +488,10 @@ extern "C" int apt_stream_create(int device, uint32_t input_rate, const apt_sett
     APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&st->h_rows), rows_floats * sizeof(float), cudaHostAllocDefault));
     APT_TRY(reset_state(st.get()));
     rollback.armed = false;
-    *out = st.release();
     return APT_OK;
 }
+
+}  // namespace
 
 extern "C" void apt_stream_destroy(apt_stream *st) {
     if (!st) return;
@@ -383,19 +509,22 @@ extern "C" int apt_stream_push(apt_stream *st, const void *samples, int format, 
     if (nout) *nout = 0;
     if (!st) return fail(APT_ERR_BAD_ARG, "null stream");
     if (st->finished) return fail(APT_ERR_BAD_ARG, "push after finish: call apt_stream_reset to start a new recording");
-    if (format != APT_F32 && format != APT_PCM16) return fail(APT_ERR_BAD_ARG, "unknown sample format %d", format);
+    if (st->iq ? !iq_sample_bytes(format) : format != APT_F32 && format != APT_PCM16)
+        return fail(APT_ERR_BAD_ARG, "sample format %d is not one this stream takes (%s)", format,
+                    st->iq ? "APT_CU8, APT_CS16 or APT_CF32" : "APT_F32 or APT_PCM16");
     if (n == 0) return APT_OK;
     if (!samples) return fail(APT_ERR_BAD_ARG, "null samples");
-    if (st->dec.plan.front.work_len(st->samples_in + n) >= (1ull << 32))
+    if (st->dec.plan.front.work_len(st->samples_in + audio_of(st, n)) >= (1ull << 32))
         return fail(APT_ERR_BAD_ARG, "recording too long: the work-rate index would pass 2^32-1");
     const uint64_t need = rows_bound(st, n);
     if (need && (!rows || cap < need)) return fail(APT_ERR_CAPACITY, "rows needs room for %llu floats", (unsigned long long)need);
     APT_CUDA(cudaSetDevice(st->dec.device));
     uint64_t got = 0;
-    const size_t sb = format == APT_PCM16 ? 2 : 4;
+    const size_t sb = st->iq ? iq_sample_bytes(format) : format == APT_PCM16 ? 2 : 4;
+    const uint64_t per_step = st->iq ? st->iq_max_push : st->max_push;
     int status = APT_OK;
     for (uint64_t done = 0; done < n;) {
-        const uint64_t k = std::min(st->max_push, n - done);
+        const uint64_t k = std::min(per_step, n - done);
         APT_TRY(step(st, static_cast<const char *>(samples) + done * sb, format, k, false, rows, got, status));
         done += k;
     }
@@ -435,12 +564,12 @@ extern "C" int apt_stream_sync_positions(apt_stream *st, uint64_t *positions, si
 
 extern "C" int apt_stream_get_info(apt_stream *st, apt_stream_info *info) {
     if (!st || !info) return fail(APT_ERR_BAD_ARG, "null argument");
-    info->samples_in = st->samples_in;
+    info->samples_in = st->iq ? st->iq_in : st->samples_in;
     info->work_final = st->work_final;
     info->rows_out = st->rows_out;
     info->peaks = st->positions.size();
     info->latency_work = st->g.latency;
-    info->max_push = st->max_push;
+    info->max_push = st->iq ? st->iq_max_push : st->max_push;
     info->device_bytes = st->g.bytes;
     return APT_OK;
 }

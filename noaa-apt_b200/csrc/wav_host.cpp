@@ -136,6 +136,27 @@ extern "C" int apt_wav_load_pcm16(const char *path, int16_t *out, uint64_t cap, 
     return read_channel0(w, out, cap, n, [](const unsigned char *p) { return static_cast<int16_t>(rd16(p)); });
 }
 
+extern "C" int apt_wav_load_iq16(const char *path, int16_t *out, uint64_t cap, uint64_t *n, uint32_t *sample_rate) {
+    if (!n) return fail(APT_ERR_BAD_ARG, "null argument");
+    WavFile w;
+    APT_TRY(open_wav(path, w));
+    if (w.info.is_float || w.info.bits_per_sample != 16 || w.info.channels != 2)
+        return fail(APT_ERR_IO, "'%s' is not a 2-channel 16-bit PCM WAV (I/Q baseband)", path);
+    if (sample_rate) *sample_rate = w.info.sample_rate;
+    const uint64_t frames = w.info.frames;
+    *n = frames;
+    if (2 * frames > cap || (!out && frames)) return fail(APT_ERR_CAPACITY, "output needs room for %llu int16", (unsigned long long)(2 * frames));
+    fseek(w.f, w.data_pos, SEEK_SET);
+    std::vector<unsigned char> buf(4 * 65536);
+    for (uint64_t done = 0; done < frames;) {
+        const size_t want = static_cast<size_t>(frames - done < 65536 ? frames - done : 65536);
+        if (fread(buf.data(), 4, want, w.f) != want) return fail(APT_ERR_IO, "WavOpen: truncated data chunk");
+        for (size_t i = 0; i < 2 * want; ++i) out[2 * done + i] = static_cast<int16_t>(rd16(buf.data() + 2 * i));
+        done += want;
+    }
+    return APT_OK;
+}
+
 extern "C" int apt_wav_write_i16(const char *path, const int16_t *samples, uint64_t n, uint32_t sample_rate) {
     if (!path || (!samples && n)) return fail(APT_ERR_BAD_ARG, "null argument");
     if (n * 2 > 0xFFFFFFFFull - 36) return fail(APT_ERR_BAD_ARG, "too many samples for a RIFF file");

@@ -236,17 +236,37 @@ def stream_geometry(input_rate, settings=None, sync=True, max_push=48000):
     return _stream_info(ci)
 
 
+def stream_geometry_iq(iq_settings, settings=None, sync=True, max_push=1_200_000):
+    """apt_stream_geometry_iq: the same for an I/Q stream (max_push in I/Q samples)."""
+    s = (settings or Settings()).to_c()
+    ci = _lib.CStreamInfo()
+    raise_for(_lib.load().apt_stream_geometry_iq(C.byref(iq_settings.to_c()), C.byref(s), int(bool(sync)), int(max_push),
+                                                 C.byref(ci)))
+    return _stream_info(ci)
+
+
 class Stream:
     """apt_stream: live decoding.  push() audio as it arrives and get back the image rows that became final; the rows
-    of all pushes plus finish() are bit-identical to decode() on the whole recording."""
+    of all pushes plus finish() are bit-identical to decode() on the whole recording.  Stream.for_iq(...) takes I/Q
+    instead (uint8 / int16 interleaved, complex64 or interleaved float32, as iq.decode_iq), bit-identical to iq.decode_iq."""
 
-    def __init__(self, input_rate, settings=None, sync=True, max_push=48000, device=0):
+    def __init__(self, input_rate, settings=None, sync=True, max_push=48000, device=0, _iq=None):
         self._lib = _lib.load()
+        self._iq = _iq is not None
         s = (settings or Settings()).to_c()
         h = C.c_void_p(None)
-        raise_for(self._lib.apt_stream_create(int(device), _rate_hz(input_rate), C.byref(s), int(bool(sync)), int(max_push),
-                                              C.byref(h)))
+        if self._iq:
+            raise_for(self._lib.apt_stream_create_iq(int(device), C.byref(_iq.to_c()), C.byref(s), int(bool(sync)), int(max_push),
+                                                     C.byref(h)))
+        else:
+            raise_for(self._lib.apt_stream_create(int(device), _rate_hz(input_rate), C.byref(s), int(bool(sync)), int(max_push),
+                                                  C.byref(h)))
         self._h = h
+
+    @classmethod
+    def for_iq(cls, iq_settings, settings=None, sync=True, max_push=1_200_000, device=0):
+        """apt_stream_create_iq: pushes are I/Q samples (max_push counts them)."""
+        return cls(iq_settings.audio_rate, settings, sync, max_push, device, _iq=iq_settings)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -272,9 +292,13 @@ class Stream:
     def push(self, samples):
         """float32 or int16 samples -> (k, 2080) float32 rows that became final."""
         x = np.ascontiguousarray(samples).ravel()
-        fmt = _fmt_of(x)
-        return self._rows(x.size, lambda out, got: self._lib.apt_stream_push(self._h, x.ctypes.data, fmt, x.size, out.ctypes.data,
-                                                                             out.size, C.byref(got)))
+        if self._iq:
+            from .iq import iq_format
+            x, fmt, n = iq_format(x)
+        else:
+            fmt, n = _fmt_of(x), x.size
+        return self._rows(n, lambda out, got: self._lib.apt_stream_push(self._h, x.ctypes.data, fmt, n, out.ctypes.data,
+                                                                        out.size, C.byref(got)))
 
     def finish(self):
         """The remaining rows; raises the error decode() would raise (too short, too few sync frames)."""

@@ -108,3 +108,37 @@ def apt_pcm16(rate_hz, seconds=None, seed=0, n_samples=None, start=0, amplitude=
 def apt_signal(rate_hz, seconds=None, seed=0, **kw):
     """The same recording as the f32 `Signal` wav::load_wav would return (wav.rs:37)."""
     return apt_pcm16(rate_hz, seconds, seed, **kw).astype(np.float32)
+
+
+_IQ_SCALE = {"cu8": 100.0, "cs16": 20000.0, "cf32": 1.0}
+
+
+def apt_iq(iq_rate, seconds=None, seed=0, offset_hz=0, deviation_hz=17000.0, fmt="cu8", n_samples=None,
+           noise_rel=0.03, audio_amplitude=20000.0, chunk=1 << 22):
+    """The synthetic APT audio of `seed` (apt_pcm16 at iq_rate, no audio noise) FM-modulated onto a carrier at offset_hz:
+    instantaneous frequency offset_hz + deviation_hz * audio / audio_amplitude, phase accumulated in float64 and carried
+    across generation chunks, complex Gaussian noise of noise_rel times the carrier amplitude (counter-based, keyed by the
+    seed), quantised to `fmt`: "cu8" (interleaved uint8 around 127.5), "cs16" (interleaved int16) or "cf32" (complex64)."""
+    if n_samples is None:
+        n_samples = int(round(iq_rate * seconds))
+    scale = _IQ_SCALE[fmt]
+    out = np.empty(n_samples, dtype=np.complex128)
+    phase = 0.3 + 0.1 * (seed % 17)
+    done = 0
+    while done < n_samples:
+        m = min(chunk, n_samples - done)
+        audio = apt_pcm16(iq_rate, seed=seed, n_samples=m, start=done, noise_sigma=0.0, chunk=chunk).astype(np.float64)
+        inc = 2.0 * np.pi * (offset_hz + deviation_hz * audio / audio_amplitude) / iq_rate
+        ph = phase + np.cumsum(inc) - inc        # phase of sample k: sum of the increments before it
+        phase = ph[-1] + inc[-1]
+        rng = np.random.Generator(np.random.Philox(key=[0x1B5 + seed, done // chunk]))
+        noise = rng.standard_normal((2, m)) * noise_rel if noise_rel > 0 else np.zeros((2, m))
+        out[done:done + m] = np.exp(1j * ph) + (noise[0] + 1j * noise[1])
+        done += m
+    if fmt == "cf32":
+        return out.astype(np.complex64)
+    inter = np.empty(2 * n_samples, dtype=np.float64)
+    inter[0::2], inter[1::2] = out.real * scale, out.imag * scale
+    if fmt == "cu8":
+        return np.clip(np.rint(inter + 127.5), 0, 255).astype(np.uint8)
+    return np.clip(np.rint(inter), -32768, 32767).astype(np.int16)

@@ -33,6 +33,15 @@ def load_wav_pcm16(path):
     return out[: n.value], rate.value
 
 
+def load_iq(path):
+    """A 2-channel 16-bit PCM WAV (SDR# / SDR++ baseband) -> (interleaved int16 I/Q, sample rate); input of iq.decode_iq."""
+    i = info(path)
+    out = np.empty(max(2 * i["frames"], 2), dtype=np.int16)
+    n, rate = C.c_uint64(0), C.c_uint32(0)
+    raise_for(_lib.load().apt_wav_load_iq16(os.fsencode(path), out.ctypes.data, out.size, C.byref(n), C.byref(rate)))
+    return out[: 2 * n.value], rate.value
+
+
 def write_wav_i16(path, samples, rate):
     x = np.ascontiguousarray(samples, dtype=np.int16)
     raise_for(_lib.load().apt_wav_write_i16(os.fsencode(path), x.ctypes.data, x.size, int(rate)))

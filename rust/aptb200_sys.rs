@@ -100,6 +100,32 @@ extern "C" {
     pub fn apt_stream_sync_positions(st: *mut apt_stream, pos: *mut u64, cap: usize, n: *mut usize) -> c_int;
     pub fn apt_stream_get_info(st: *mut apt_stream, info: *mut apt_stream_info) -> c_int;
     pub fn apt_stream_geometry(input_rate: u32, s: *const apt_settings, sync: c_int, max_push: u64, info: *mut apt_stream_info) -> c_int;
+    pub fn apt_iq_default_settings(iq_rate: u32, offset_hz: i32, s: *mut apt_iq_settings) -> c_int;
+    pub fn apt_fm_demod_len(n: u64, s: *const apt_iq_settings, nout: *mut u64) -> c_int;
+    pub fn apt_fm_demod(iq: *const c_void, format: c_int, n: u64, s: *const apt_iq_settings, out: *mut c_float, cap: u64,
+                        nout: *mut u64) -> c_int;
+    pub fn apt_decode_iq(iq: *const c_void, format: c_int, n: u64, s: *const apt_iq_settings, settings: *const apt_settings,
+                         sync: c_int, out: *mut c_float, cap: u64, nout: *mut u64, cb: apt_status_cb, user: *mut c_void) -> c_int;
+    pub fn apt_stream_create_iq(device: c_int, iq: *const apt_iq_settings, s: *const apt_settings, sync: c_int, max_push: u64,
+                                st: *mut *mut apt_stream) -> c_int;
+    pub fn apt_stream_geometry_iq(iq: *const apt_iq_settings, s: *const apt_settings, sync: c_int, max_push: u64,
+                                  info: *mut apt_stream_info) -> c_int;
+    pub fn apt_wav_load_iq16(path: *const c_char, out: *mut i16, cap: u64, n: *mut u64, sample_rate: *mut u32) -> c_int;
+}
+
+pub const APT_CU8: c_int = 2;
+pub const APT_CF32: c_int = 3;
+pub const APT_CS16: c_int = 4;
+
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct apt_iq_settings {
+    pub iq_rate: u32,
+    pub audio_rate: u32,
+    pub offset_hz: i32,
+    pub cutout: c_float,
+    pub delta_freq: c_float,
+    pub atten: c_float,
 }
 
 #[repr(C)]

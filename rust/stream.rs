@@ -68,6 +68,31 @@ impl Stream {
         })
     }
 
+    /// A stream fed with I/Q (apt_stream_create_iq): push_iq() only; max_push counts I/Q samples.
+    pub fn new_iq(iq: &sys::apt_iq_settings, settings: &config::Settings, sync: bool, max_push: u64, device: i32)
+                  -> err::Result<Stream> {
+        let s = sys::apt_settings {
+            work_rate: settings.work_rate,
+            resample_atten: settings.resample_atten,
+            resample_delta_freq: settings.resample_delta_freq,
+            resample_cutout: settings.resample_cutout,
+            demodulation_atten: settings.demodulation_atten,
+        };
+        let mut st: *mut sys::apt_stream = ptr::null_mut();
+        let rc = unsafe { sys::apt_stream_create_iq(device, iq, &s, sync as i32, max_push, &mut st) };
+        if rc != sys::APT_OK {
+            return Err(to_error(rc));
+        }
+        Ok(Stream { st })
+    }
+
+    /// I/Q samples of an I/Q stream (cu8 / cs16 / cf32 pushes may be mixed).
+    pub fn push_iq(&mut self, samples: &crate::iq::Iq) -> err::Result<Signal> {
+        let st = self.st;
+        let (p, fmt, n) = samples.raw();
+        self.rows(n, |o, c, k| unsafe { sys::apt_stream_push(st, p, fmt, n, o, c, k) })
+    }
+
     /// The remaining rows; the error `decode` would return (too short, too few sync frames) means the rows returned
     /// so far are not an image and are discarded.
     pub fn finish(&mut self) -> err::Result<Signal> {
