@@ -151,7 +151,8 @@ int apt_decode(const float *signal, uint64_t n, uint32_t input_rate, const apt_s
                float *out, uint64_t cap, uint64_t *nout, apt_status_cb cb, void *user);
 
 /* apt_decode / apt_decode_pcm16 keep the decoder they used (plan, device workspaces, pinned staging) parked per
- * (device, rate, settings) for the next call; this frees the parked ones.  Thread-safe. */
+ * (device, rate, settings) for the next call; this frees the parked ones, and the workspaces apt_png_encode keeps per
+ * device.  Thread-safe. */
 void apt_cache_clear(void);
 
 /* Same, taking the PCM16 samples of the WAV directly: half the host->device bytes; the `as f32` cast of
@@ -481,6 +482,51 @@ int apt_stream_geometry_iq(const apt_iq_settings *iq, const apt_settings *s, int
 /* A 2-channel 16-bit PCM WAV (SDR# / SDR++ baseband) as interleaved APT_CS16: out receives 2 * *n int16, *n the frames
  * (complex samples), cap in int16.  Any other layout is APT_ERR_IO. */
 int apt_wav_load_iq16(const char *path, int16_t *out, uint64_t cap, uint64_t *n, uint32_t *sample_rate);
+
+/* ------------------------------------------------------------------ PNG output: encoding on the device */
+
+/* A deterministic PNG encoder (DESIGN.md §11; the reference's `img.save` pins no encoder, so the bytes are this project's
+ * definition): per-row adaptive filter (minimum sum of absolute residuals, ties to the lower type), greedy LZ77 with zlib's
+ * 15-bit hash, a 32 KiB window and matches of 4..258 bytes, one dynamic-Huffman deflate block per block_bytes of the
+ * filtered stream with package-merge code lengths, zlib framing, and a PNG of IHDR, one IDAT and IEND.  The output bytes
+ * are a pure function of the pixels and the settings.  8-bit grey (1 channel), RGB (3) or RGBA (4); no interlace.
+ *   filter         -1: adaptive per row; 0..4: that PNG filter on every row
+ *   matches        0: literals only (Huffman-only deflate); else LZ77 matches
+ *   block_bytes    filtered bytes per deflate block: a power of two in [4096, 65536]
+ *   rgb_from_rgba  1: RGBA input is written as RGB (colour type 2); every alpha must be 255, else APT_ERR_BAD_ARG */
+typedef struct apt_png_settings {
+    int filter;
+    int matches;
+    uint32_t block_bytes;
+    int rgb_from_rgba;
+} apt_png_settings;
+
+/* filter -1, matches 1, block_bytes 65536, rgb_from_rgba 0. */
+void apt_png_default_settings(apt_png_settings *ps);
+/* Upper bound of the PNG size in bytes (host only): 63 + ceil(sum over blocks of (9 * len + 2409) / 8). */
+int apt_png_bound(uint32_t width, uint32_t height, int channels, const apt_png_settings *ps, uint64_t *bytes);
+/* PNG of host pixels (height rows of width * channels bytes).  out receives the file's bytes, *nout their count; a cap
+ * below that count is APT_ERR_CAPACITY with the required count in *nout (cap >= apt_png_bound always suffices).  Argument
+ * errors (NULL pointers, channels not 1 / 3 / 4, width or height 0, bad settings, alpha != 255 with rgb_from_rgba, an
+ * IDAT that could exceed 2^31 - 1 bytes) come back before any device is touched.  The device workspace (about 5 bytes per
+ * filtered byte plus the bound) is kept per device for the next call, one encode per device at a time; apt_cache_clear
+ * frees it. */
+int apt_png_encode(const uint8_t *pixels, uint32_t width, uint32_t height, int channels, const apt_png_settings *ps,
+                   uint8_t *out, uint64_t cap, uint64_t *nout);
+/* apt_decode_image + apt_png_encode in one call: the image is encoded on the device and only the PNG bytes cross PCIe.
+ * Errors as apt_decode_image, plus the settings checks of apt_png_encode and APT_ERR_CAPACITY as there. */
+int apt_decode_png(const void *signal, int format, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
+                   const apt_process_settings *ps, const apt_png_settings *png, uint8_t *out, uint64_t cap, uint64_t *nout,
+                   apt_image_info *info, apt_status_cb cb, void *user);
+/* PNG mode of a decoder in process or image mode: every following job ends in the PNG of its image; `out` / `cap` / *nout
+ * of submit and wait then count PNG bytes (cap >= apt_png_bound of the largest image suffices; a smaller one that the
+ * PNG does not fit is APT_ERR_CAPACITY at wait, *nout the required count).  NULL switches PNG mode off.  Leaving image and
+ * process mode also leaves PNG mode. */
+int apt_decoder_set_png_mode(apt_decoder *dec, const apt_png_settings *ps);
+/* The reference CLI's main job (main.rs): load a WAV (as apt_wav_load / apt_wav_load_pcm16), decode, process and write the
+ * PNG to output_path.  info may be NULL. */
+int apt_decode_wav_png(const char *input_path, const char *output_path, const apt_settings *s, int sync,
+                       const apt_process_settings *ps, const apt_png_settings *png, apt_image_info *info);
 
 #ifdef __cplusplus
 }

@@ -282,4 +282,44 @@ inline Signal decode_iq(Context &ctx, const config::Settings &settings, const vo
 }
 }  // namespace iq
 
+// PNG output encoded on the device (DESIGN.md §11): the file's bytes, ready to write.
+namespace png {
+inline apt_png_settings default_settings() {
+    apt_png_settings s{};
+    apt_png_default_settings(&s);
+    return s;
+}
+// pixels: height rows of width * channels bytes (channels 1 grey, 3 RGB, 4 RGBA)
+inline std::vector<uint8_t> encode(const uint8_t *pixels, uint32_t width, uint32_t height, int channels,
+                                   const apt_png_settings &ps = default_settings()) {
+    uint64_t cap = 0, got = 0;
+    err::check(apt_png_bound(width, height, channels, &ps, &cap));
+    std::vector<uint8_t> out(cap);
+    err::check(apt_png_encode(pixels, width, height, channels, &ps, out.data(), out.size(), &got));
+    out.resize(got);
+    return out;
+}
+// decode() + process() (no map overlay) + PNG in one call; only the PNG bytes leave the GPU
+inline std::vector<uint8_t> decode_png(Context &ctx, const config::Settings &settings, const Signal &signal, Rate input_rate,
+                                       bool sync, const apt_process_settings &ps,
+                                       const apt_png_settings &png = default_settings(), apt_image_info *info = nullptr) {
+    const apt_settings s = settings.to_c();
+    uint64_t bound = 0, cap = 0, got = 0;
+    err::check(apt_decode_len_bound(signal.size(), input_rate.get_hz(), &s, &bound));
+    const uint64_t rows = bound / 2080 ? bound / 2080 : 1;
+    err::check(apt_png_bound(2080, static_cast<uint32_t>(rows), ps.rgba ? 4 : 1, &png, &cap));
+    std::vector<uint8_t> out(cap);
+    err::check(apt_decode_png(signal.data(), APT_F32, signal.size(), input_rate.get_hz(), &s, sync ? 1 : 0, &ps, &png,
+                              out.data(), out.size(), &got, info, &Context::trampoline, &ctx));
+    out.resize(got);
+    return out;
+}
+// The reference CLI's job: WAV in, PNG file out
+inline void decode_wav_png(const std::string &input, const std::string &output, const config::Settings &settings, bool sync,
+                           const apt_process_settings &ps, const apt_png_settings &png = default_settings()) {
+    const apt_settings s = settings.to_c();
+    err::check(apt_decode_wav_png(input.c_str(), output.c_str(), &s, sync ? 1 : 0, &ps, &png, nullptr));
+}
+}  // namespace png
+
 }  // namespace noaa_apt

@@ -90,6 +90,10 @@ class CIqSettings(C.Structure):
                 ("delta_freq", C.c_float), ("atten", C.c_float)]
 
 
+class CPngSettings(C.Structure):
+    _fields_ = [("filter", C.c_int), ("matches", C.c_int), ("block_bytes", C.c_uint32), ("rgb_from_rgba", C.c_int)]
+
+
 STATUS_CB = C.CFUNCTYPE(None, C.c_float, C.c_char_p, C.c_void_p)
 
 # name -> (restype, argtypes); every symbol include/aptb200.h declares.
@@ -192,6 +196,16 @@ SIGNATURES = {
     "apt_stream_geometry_iq": (C.c_int, [C.POINTER(CIqSettings), C.POINTER(CSettings), C.c_int, C.c_uint64,
                                          C.POINTER(CStreamInfo)]),
     "apt_wav_load_iq16":(C.c_int, [C.c_char_p, C.c_void_p, C.c_uint64, _u64p, C.POINTER(C.c_uint32)]),
+    "apt_png_default_settings": (None, [C.POINTER(CPngSettings)]),
+    "apt_png_bound": (C.c_int, [C.c_uint32, C.c_uint32, C.c_int, C.POINTER(CPngSettings), _u64p]),
+    "apt_png_encode": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_int, C.POINTER(CPngSettings), C.c_void_p,
+                                 C.c_uint64, _u64p]),
+    "apt_decode_png": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64, C.c_uint32, C.POINTER(CSettings), C.c_int,
+                                 C.POINTER(CProcessSettings), C.POINTER(CPngSettings), C.c_void_p, C.c_uint64, _u64p,
+                                 C.POINTER(CImageInfo), STATUS_CB, C.c_void_p]),
+    "apt_decoder_set_png_mode": (C.c_int, [C.c_void_p, C.POINTER(CPngSettings)]),
+    "apt_decode_wav_png": (C.c_int, [C.c_char_p, C.c_char_p, C.POINTER(CSettings), C.c_int, C.POINTER(CProcessSettings),
+                                     C.POINTER(CPngSettings), C.POINTER(CImageInfo)]),
 }
 
 _lib = None

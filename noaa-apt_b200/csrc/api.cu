@@ -79,6 +79,8 @@ int aptb200::free_decoder_buffers(apt_decoder *d) {
         if (p) cudaFree(p);
     d->iq_tables.release();
     d->iq_win.release();
+    d->png_work.release();
+    if (d->h_png) cudaFreeHost(d->h_png);
     if (d->d_audio) cudaFree(d->d_audio);
     d->own_stager.reset();
     for (auto e : d->ev_begin) cudaEventDestroy(e);
@@ -495,8 +497,14 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
     const uint64_t need = d->job_sync ? (nwork / p.row) * kPxPerRow : plan_out_bound(p, n);
     // bytes per output pixel of an image job: RGBA in process mode, else grey
     const uint64_t bpp = d->image_contrast >= 0 && d->proc_active && d->proc.rgba ? 4 : 1;
-    if (!out || cap < need * bpp) return fail(APT_ERR_CAPACITY, "output needs room for %llu %s", (unsigned long long)(need * bpp),
-                                              d->image_contrast >= 0 ? "bytes" : "floats");
+    // PNG mode: cap counts PNG bytes, checked at wait() once the file's length is known
+    const bool png = d->image_contrast >= 0 && d->png_active;
+    if (png && d->png.rgb_from_rgba && bpp != 4) return fail(APT_ERR_BAD_ARG, "rgb_from_rgba needs RGBA process output");
+    if (png && !out) return fail(APT_ERR_BAD_ARG, "null output");
+    if (!png && (!out || cap < need * bpp))
+        return fail(APT_ERR_CAPACITY, "output needs room for %llu %s", (unsigned long long)(need * bpp),
+                    d->image_contrast >= 0 ? "bytes" : "floats");
+    d->job_png = png;
     d->job_image = d->image_contrast >= 0;
     d->job_bpp = bpp;
     if (d->job_image) {
@@ -509,7 +517,7 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
         }
         if (!d->d_out) APT_CUDA(cudaMalloc(&d->d_out, std::max<uint64_t>(d->max_out, 1) * sizeof(float)));
         const uint64_t out8_need = std::max<uint64_t>(d->max_out, 1) * bpp;
-        if (host && d->out8_bytes < out8_need) {
+        if ((host || png) && d->out8_bytes < out8_need) {
             if (d->d_out8) APT_CUDA(cudaFree(d->d_out8));
             d->d_out8 = nullptr;
             d->out8_bytes = 0;
@@ -529,7 +537,7 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
     d->job_in_pageable = d->job_out_pageable = false;
     if (host) {
         d->job_in_pageable = is_pageable(signal);
-        d->job_out_pageable = is_pageable(out);
+        d->job_out_pageable = !png && is_pageable(out);   // PNG mode copies the file straight into `out` at wait()
         if ((d->job_in_pageable || d->job_out_pageable) && !d->stager && !getenv("APTB200_NO_STAGER")) {
             int threads = 8;
             if (const char *e = getenv("APTB200_COPY_THREADS")) threads = std::max(1, atoi(e));
@@ -571,7 +579,8 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
     if (d->job_image) rows_dst = d->d_out;      // the f32 rows are an intermediate of the image job
     d->job_rows_src = rows_dst;
     int st = decoder_enqueue(d, dev_in, format, n, sync, rows_dst, host_chunked);
-    if (st == APT_OK && d->job_image) st = enqueue_image_stage(d, host ? d->d_out8 : reinterpret_cast<unsigned char *>(out));
+    if (st == APT_OK && d->job_image)
+        st = enqueue_image_stage(d, host || png ? d->d_out8 : reinterpret_cast<unsigned char *>(out));
     if (st != APT_OK) {
         cudaStreamSynchronize(d->stream);
         d->job_status = st;
@@ -582,7 +591,7 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
     if (host) {
         // the rows come back with the job: when syncing n_rows is only known on the device, so the copy covers the bound
         // (at most one row more than is produced)
-        d->job_d2h_floats = d->job_sync ? need : d->job_fixed_out;
+        d->job_d2h_floats = png ? 0 : d->job_sync ? need : d->job_fixed_out;
         if (d->job_d2h_floats)
             APT_CUDA(cudaMemcpyAsync(d->job_out_pageable ? static_cast<void *>(d->h_out) : static_cast<void *>(out),
                                      d->job_image ? static_cast<const void *>(d->d_out8) : static_cast<const void *>(d->d_out),
@@ -604,6 +613,29 @@ extern "C" int apt_decoder_submit_host(apt_decoder *dec, const void *signal, int
                                        float *out, uint64_t cap) {
     return submit_common(dec, signal, format, n, sync, out, cap, true);
 }
+
+namespace {
+
+// PNG mode, at wait(): encode the job's image (in d_out8) on the decoder's stream, read the file's length from the pinned
+// control block, then copy exactly that many bytes to the caller's buffer.  Two stream synchronisations.
+int png_job(apt_decoder *d, uint64_t rows, uint64_t *bytes) {
+    PngPlan p;
+    APT_TRY(make_png(kPxPerRow, static_cast<uint32_t>(rows), static_cast<int>(d->job_bpp), &d->png, p));
+    if (!d->h_png) APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&d->h_png), sizeof(PngCtl), cudaHostAllocDefault));
+    DecoderHook hook(d);
+    APT_TRY(png_encode_device(LaunchCtx{d->stream, d->sm_count}, p, d->png_work, d->d_out8, &hook));
+    APT_CUDA(cudaMemcpyAsync(d->h_png, d->png_work.ctl, sizeof(PngCtl), cudaMemcpyDeviceToHost, d->stream));
+    APT_CUDA(cudaStreamSynchronize(d->stream));
+    const uint64_t total = d->h_png->total;
+    *bytes = total;
+    if (total > d->job_cap) return fail(APT_ERR_CAPACITY, "output needs room for %llu PNG bytes", (unsigned long long)total);
+    APT_CUDA(cudaMemcpyAsync(d->job_out, d->png_work.out, total, d->job_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice,
+                             d->stream));
+    APT_CUDA(cudaStreamSynchronize(d->stream));
+    return APT_OK;
+}
+
+}  // namespace
 
 extern "C" int apt_decoder_wait(apt_decoder *d, uint64_t *nout) {
     if (!d) return fail(APT_ERR_BAD_ARG, "null decoder");
@@ -627,7 +659,7 @@ extern "C" int apt_decoder_wait(apt_decoder *d, uint64_t *nout) {
             APT_TRY(back_redo(LaunchCtx{d->stream, d->sm_count}, d->plan, d->back_plan, d->back, d->d_e, d->job_work,
                               const_cast<float *>(d->job_rows_src), &hook, d->last_back));
             if (d->job_image)
-                APT_TRY(enqueue_image_stage(d, d->job_host ? d->d_out8 : reinterpret_cast<unsigned char *>(d->job_out)));
+                APT_TRY(enqueue_image_stage(d, d->job_host || d->job_png ? d->d_out8 : reinterpret_cast<unsigned char *>(d->job_out)));
             APT_CUDA(cudaMemcpyAsync(d->h_res, d->back.res, sizeof(SyncResult), cudaMemcpyDeviceToHost, d->stream));
             if (d->job_host && d->job_d2h_floats)
                 APT_CUDA(cudaMemcpyAsync(d->job_out_pageable ? static_cast<void *>(d->h_out) : static_cast<void *>(d->job_out),
@@ -645,7 +677,7 @@ extern "C" int apt_decoder_wait(apt_decoder *d, uint64_t *nout) {
         produced = static_cast<uint64_t>(res.n_rows) * kPxPerRow;
     }
     const size_t elem = d->job_image ? d->job_bpp : sizeof(float);
-    if (d->job_host && d->job_out_pageable && produced) {
+    if (d->job_host && d->job_out_pageable && produced && !d->job_png) {
         if (d->stager) d->stager->scatter(d->job_out, d->h_out, produced * elem);
         else memcpy(d->job_out, d->h_out, produced * elem);
     }
@@ -670,11 +702,20 @@ extern "C" int apt_decoder_wait(apt_decoder *d, uint64_t *nout) {
     }
     d->last_rows = d->plan.work_multiple ? produced / kPxPerRow : 0;
     d->last_out = produced;
+    uint64_t png_bytes = 0;
+    if (d->job_png) {
+        const int st = png_job(d, produced / kPxPerRow, &png_bytes);
+        if (st != APT_OK) {
+            if (st == APT_ERR_CAPACITY && nout) *nout = png_bytes;
+            d->job_status = st;
+            return st;
+        }
+    }
     if (d->profiling) {
         d->kernel_ms.assign(d->ev_used, 0.f);
         for (int i = 0; i < d->ev_used; ++i) cudaEventElapsedTime(&d->kernel_ms[i], d->ev_begin[i], d->ev_end[i]);
     }
-    if (nout) *nout = d->job_image ? produced * d->job_bpp : produced;
+    if (nout) *nout = d->job_png ? png_bytes : d->job_image ? produced * d->job_bpp : produced;
     return APT_OK;
 }
 
@@ -687,6 +728,7 @@ extern "C" int apt_decoder_set_image_mode(apt_decoder *d, int contrast, float pe
     d->image_contrast = contrast;
     d->image_percent = percent;
     d->proc_active = false;
+    if (contrast < 0) d->png_active = false;
     return APT_OK;
 }
 
@@ -720,6 +762,7 @@ extern "C" int apt_decoder_set_process_mode(apt_decoder *d, const apt_process_se
     if (!ps) {
         d->proc_active = false;
         d->image_contrast = -1;
+        d->png_active = false;
         return APT_OK;
     }
     APT_TRY(check_process_settings(ps));
@@ -736,6 +779,26 @@ extern "C" int apt_decoder_set_process_mode(apt_decoder *d, const apt_process_se
     d->proc_active = true;
     d->image_contrast = ps->contrast;
     d->image_percent = ps->percent;
+    return APT_OK;
+}
+
+// The settings rules of PNG output for an image of `channels` channels (no device, no pixels).
+static int check_png_settings(const apt_png_settings *png, int channels) {
+    PngPlan p;
+    return make_png(kPxPerRow, 1, channels, png, p);
+}
+
+extern "C" int apt_decoder_set_png_mode(apt_decoder *d, const apt_png_settings *ps) {
+    if (!d) return fail(APT_ERR_BAD_ARG, "null decoder");
+    if (d->in_flight) return fail(APT_ERR_BAD_ARG, "decoder has a job in flight");
+    if (!ps) {
+        d->png_active = false;
+        return APT_OK;
+    }
+    if (d->image_contrast < 0) return fail(APT_ERR_BAD_ARG, "PNG mode needs image or process mode");
+    APT_TRY(check_png_settings(ps, d->proc_active && d->proc.rgba ? 4 : 1));
+    d->png = *ps;
+    d->png_active = true;
     return APT_OK;
 }
 
@@ -945,7 +1008,8 @@ void cache_put_multi(int device, uint32_t rate, const apt_settings &st, apt_deco
 
 int decode_oneshot(const void *signal, int format, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
                    float *out, uint64_t cap, uint64_t *nout, apt_status_cb cb, void *user, int contrast = -1,
-                   float percent = 0.f, apt_image_info *info = nullptr, const apt_process_settings *ps = nullptr) {
+                   float percent = 0.f, apt_image_info *info = nullptr, const apt_process_settings *ps = nullptr,
+                   const apt_png_settings *png = nullptr) {
     if (!s || !nout) return fail(APT_ERR_BAD_ARG, "null argument");
     *nout = 0;
     if (n == 0 || !signal) return fail(APT_ERR_BAD_ARG, "empty signal");
@@ -972,11 +1036,13 @@ int decode_oneshot(const void *signal, int format, uint64_t n, uint32_t input_ra
     d->image_contrast = contrast;
     d->image_percent = percent;
     int st = ps ? apt_decoder_set_process_mode(d, ps) : APT_OK;
+    if (st == APT_OK && png) st = apt_decoder_set_png_mode(d, png);
     if (st == APT_OK) st = apt_decoder_submit_host(d, signal, format, n, sync, out, cap);
     if (st == APT_OK) st = apt_decoder_wait(d, nout);
     if (st == APT_OK && info) *info = d->last_image;
     d->image_contrast = -1;
     d->proc_active = false;
+    d->png_active = false;
     d->cb = nullptr;
     d->cb_user = nullptr;
     if (use_cache) cache_put(device, input_rate, *s, d);
@@ -998,6 +1064,7 @@ extern "C" void apt_cache_clear(void) {
         drop.swap(g_cache);
     }
     for (auto &e : drop) apt_decoder_destroy(e.dec);
+    png_stage_cache_clear();
 }
 
 extern "C" int apt_decode(const float *signal, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
@@ -1102,6 +1169,52 @@ extern "C" int apt_decode_image(const void *signal, int format, uint64_t n, uint
     APT_TRY(check_process_settings(ps));
     return decode_oneshot(signal, format, n, input_rate, s, sync, reinterpret_cast<float *>(out), cap, nout, cb, user,
                           ps->contrast, ps->percent, info, ps);
+}
+
+extern "C" int apt_decode_png(const void *signal, int format, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
+                              const apt_process_settings *ps, const apt_png_settings *png, uint8_t *out, uint64_t cap,
+                              uint64_t *nout, apt_image_info *info, apt_status_cb cb, void *user) {
+    APT_TRY(check_process_settings(ps));
+    APT_TRY(check_png_settings(png, ps->rgba ? 4 : 1));
+    if (!out) return fail(APT_ERR_BAD_ARG, "null output");
+    return decode_oneshot(signal, format, n, input_rate, s, sync, reinterpret_cast<float *>(out), cap, nout, cb, user,
+                          ps->contrast, ps->percent, info, ps, png);
+}
+
+extern "C" int apt_decode_wav_png(const char *input_path, const char *output_path, const apt_settings *s, int sync,
+                                  const apt_process_settings *ps, const apt_png_settings *png, apt_image_info *info) {
+    if (!input_path || !output_path || !s) return fail(APT_ERR_BAD_ARG, "null argument");
+    APT_TRY(check_process_settings(ps));
+    APT_TRY(check_png_settings(png, ps->rgba ? 4 : 1));
+    apt_wav_info wi;
+    APT_TRY(apt_wav_info_read(input_path, &wi));
+    uint32_t rate = 0;
+    uint64_t n = 0;
+    std::vector<int16_t> pcm;
+    std::vector<float> x;
+    const bool pcm16 = !wi.is_float && wi.bits_per_sample == 16;
+    if (pcm16) {
+        pcm.resize(std::max<uint64_t>(wi.frames, 1));
+        APT_TRY(apt_wav_load_pcm16(input_path, pcm.data(), pcm.size(), &n, &rate));
+    } else {
+        x.resize(std::max<uint64_t>(wi.frames, 1));
+        APT_TRY(apt_wav_load(input_path, x.data(), x.size(), &n, &rate));
+    }
+    uint64_t rows_bound = 0, cap = 0;
+    APT_TRY(apt_decode_len_bound(n, rate, s, &rows_bound));
+    rows_bound = std::max<uint64_t>(rows_bound / kPxPerRow, 1);
+    if (rows_bound > 0xFFFFFFFFull) return fail(APT_ERR_BAD_ARG, "recording too long");
+    APT_TRY(apt_png_bound(kPxPerRow, static_cast<uint32_t>(rows_bound), ps->rgba ? 4 : 1, png, &cap));
+    std::vector<uint8_t> bytes(cap);
+    uint64_t nout = 0;
+    APT_TRY(apt_decode_png(pcm16 ? static_cast<const void *>(pcm.data()) : static_cast<const void *>(x.data()),
+                           pcm16 ? APT_PCM16 : APT_F32, n, rate, s, sync, ps, png, bytes.data(), cap, &nout, info, nullptr,
+                           nullptr));
+    FILE *fp = fopen(output_path, "wb");
+    if (!fp) return fail(APT_ERR_IO, "cannot open %s for writing", output_path);
+    const bool ok = fwrite(bytes.data(), 1, nout, fp) == nout;
+    if (fclose(fp) != 0 || !ok) return fail(APT_ERR_IO, "cannot write %s", output_path);
+    return APT_OK;
 }
 
 namespace {

@@ -17,6 +17,7 @@
 #include "hostpool.hpp"
 #include "iq.hpp"
 #include "launch.hpp"
+#include "png.hpp"
 
 namespace aptb200 {
 
@@ -121,6 +122,13 @@ struct apt_decoder {
     aptb200::ProcCtl *d_proc = nullptr;
     unsigned char *d_grey = nullptr;        // max_out B intermediate grey plane
     uint64_t job_bpp = 1;          // output bytes per pixel of the image job in flight
+    // PNG mode (apt_decoder_set_png_mode): the image of an image / process job is encoded on the device at wait(); only the
+    // PNG bytes are copied out.  The workspaces are sized at first use from the image size.
+    bool png_active = false;
+    apt_png_settings png{};
+    aptb200::PngWork png_work;
+    aptb200::PngCtl *h_png = nullptr;   // pinned copy of the encoder's control block
+    bool job_png = false;
 
     // apt_decode_iq (allocated on first use): the I/Q stage's tables for iq_settings, one chunk's I/Q window and the
     // audio the FM kernel writes, which is the input of the decode job

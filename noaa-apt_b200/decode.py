@@ -98,6 +98,7 @@ class Decoder:
         self._h = h
         self._keep = None
         self._bpp = None       # bytes per pixel of the process mode's image; None: f32 rows
+        self._png = None       # PNG mode: (filter, matches, block_bytes, rgb_from_rgba)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -130,10 +131,23 @@ class Decoder:
         if contrast is None:
             raise_for(self._lib.apt_decoder_set_process_mode(self._h, None))
             self._bpp = None
+            self._png = None
             return
         ps, bpp, _pal = image.process_settings(contrast, percent, rotate, palette, tune, rgba)
         raise_for(self._lib.apt_decoder_set_process_mode(self._h, C.byref(ps)))   # the palette is copied here
         self._bpp = bpp
+
+    def set_png_mode(self, enabled=True, filter=-1, matches=True, block_bytes=65536, rgb_from_rgba=False):
+        """In process mode: every job ends in the PNG of its image; submit()/wait()/decode() then return the file's
+        bytes.  enabled=False goes back to the image arrays."""
+        from . import image
+        if not enabled:
+            raise_for(self._lib.apt_decoder_set_png_mode(self._h, None))
+            self._png = None
+            return
+        ps = image.png_settings(filter, matches, block_bytes, rgb_from_rgba)
+        raise_for(self._lib.apt_decoder_set_png_mode(self._h, C.byref(ps)))
+        self._png = (filter, matches, block_bytes, rgb_from_rgba)
 
     def image_info(self):
         from . import image
@@ -147,7 +161,11 @@ class Decoder:
         fmt = _fmt_of(x)
         bpp = self._bpp
         if out is None:
-            if bpp:
+            if bpp and self._png:
+                from . import image
+                rows = max(self.out_bound(x.size) // PX_PER_ROW, 1)
+                out = np.empty(image.png_bound(PX_PER_ROW, rows, bpp, *self._png), dtype=np.uint8)
+            elif bpp:
                 out = np.empty(max(self.out_bound(x.size) * bpp, 1), dtype=np.uint8)
             else:
                 out = np.empty(max(self.out_bound(x.size), 1), dtype=np.float32)
@@ -162,6 +180,8 @@ class Decoder:
         raise_for(st)
         if keep is not None:
             bpp = self._bpp
+            if bpp and self._png:
+                return keep[1][: n.value].tobytes()
             if bpp:
                 flat = keep[1][: n.value]
                 return flat.reshape(-1, PX_PER_ROW, 4) if bpp == 4 else flat.reshape(-1, PX_PER_ROW)
@@ -170,7 +190,8 @@ class Decoder:
 
     def decode(self, signal, sync=True):
         self.submit(signal, sync)
-        return self.wait().copy()
+        r = self.wait()
+        return r if isinstance(r, bytes) else r.copy()
 
     # --- introspection ---
     def last_sync(self):

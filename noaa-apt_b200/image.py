@@ -87,6 +87,93 @@ def decode_image(context, settings, signal, input_rate, sync=True, contrast=MINM
     return _shape(out[: n.value].copy(), bpp), _info(ci)
 
 
+def png_settings(filter=-1, matches=True, block_bytes=65536, rgb_from_rgba=False):
+    """apt_png_settings (DESIGN.md §11): filter -1 adaptive or 0..4 fixed; matches False gives Huffman-only deflate;
+    block_bytes a power of two in [4096, 65536]; rgb_from_rgba writes RGBA pixels (alpha all 255) as RGB."""
+    ps = _lib.CPngSettings()
+    ps.filter = int(filter)
+    ps.matches = int(bool(matches))
+    ps.block_bytes = int(block_bytes)
+    ps.rgb_from_rgba = int(bool(rgb_from_rgba))
+    return ps
+
+
+def _channels(shape):
+    if len(shape) == 2:
+        return 1
+    if len(shape) == 3 and shape[2] in (1, 3, 4):
+        return shape[2]
+    raise InvalidInput(_lib.ERR_BAD_ARG, f"pixels must be (h, w) or (h, w, 1 / 3 / 4), got {shape}")
+
+
+def png_bound(width, height, channels, filter=-1, matches=True, block_bytes=65536, rgb_from_rgba=False):
+    """Upper bound of encode_png's output size in bytes (host arithmetic, no device)."""
+    ps = png_settings(filter, matches, block_bytes, rgb_from_rgba)
+    b = C.c_uint64(0)
+    raise_for(_lib.load().apt_png_bound(int(width), int(height), int(channels), C.byref(ps), C.byref(b)))
+    return b.value
+
+
+def encode_png(pixels, filter=-1, matches=True, block_bytes=65536, rgb_from_rgba=False):
+    """PNG file bytes of u8 pixels (h, w) grey, (h, w, 3) RGB or (h, w, 4) RGBA, encoded on the device."""
+    x = np.ascontiguousarray(pixels, dtype=np.uint8)
+    ch = _channels(x.shape)
+    if x.ndim != 2 and x.ndim != 3:
+        raise InvalidInput(_lib.ERR_BAD_ARG, "pixels must be 2-D or 3-D")
+    h, w = x.shape[0], x.shape[1]
+    ps = png_settings(filter, matches, block_bytes, rgb_from_rgba)
+    lib = _lib.load()
+    b = C.c_uint64(0)
+    raise_for(lib.apt_png_bound(w, h, ch, C.byref(ps), C.byref(b)))
+    out = np.empty(max(b.value, 1), dtype=np.uint8)
+    n = C.c_uint64(0)
+    raise_for(lib.apt_png_encode(x.ctypes.data, w, h, ch, C.byref(ps), out.ctypes.data, out.size, C.byref(n)))
+    return out[: n.value].tobytes()
+
+
+def decode_png(context, settings, signal, input_rate, sync=True, contrast=MINMAX, percent=0.98, rotate=False, palette=None,
+               tune=(0, 0, 0, 0), rgba=None, filter=-1, matches=True, block_bytes=65536, rgb_from_rgba=False):
+    """decode() + process() + PNG encoding in one call; only the PNG bytes leave the GPU -> (bytes, info)."""
+    lib = _lib.load()
+    x = np.ascontiguousarray(signal)
+    fmt = _lib.PCM16 if x.dtype == np.int16 else _lib.F32
+    if fmt == _lib.F32:
+        x = np.ascontiguousarray(x, dtype=np.float32)
+    ps, bpp, _pal = process_settings(contrast, percent, rotate, palette, tune, rgba)
+    png = png_settings(filter, matches, block_bytes, rgb_from_rgba)
+    s = (settings or Settings()).to_c()
+    rate = _rate_hz(input_rate)
+    bound = C.c_uint64(0)
+    raise_for(lib.apt_decode_len_bound(x.size, rate, C.byref(s), C.byref(bound)))
+    cap = C.c_uint64(0)
+    raise_for(lib.apt_png_bound(2080, max(bound.value // 2080, 1), bpp, C.byref(png), C.byref(cap)))
+    out = np.empty(cap.value, dtype=np.uint8)
+    n = C.c_uint64(0)
+    ci = _lib.CImageInfo()
+
+    def _cb(progress, desc, _user):
+        if context is not None:
+            context.status(progress, desc.decode())
+
+    cb = _lib.STATUS_CB(_cb)
+    raise_for(lib.apt_decode_png(x.ctypes.data, fmt, x.size, rate, C.byref(s), int(bool(sync)), C.byref(ps), C.byref(png),
+                                 out.ctypes.data, out.size, C.byref(n), C.byref(ci), cb, None))
+    return out[: n.value].tobytes(), _info(ci)
+
+
+def decode_wav_png(input_path, output_path, settings=None, sync=True, contrast=MINMAX, percent=0.98, rotate=False,
+                   palette=None, tune=(0, 0, 0, 0), rgba=None, filter=-1, matches=True, block_bytes=65536,
+                   rgb_from_rgba=False):
+    """The reference CLI's job: WAV file in, PNG file out (decode, process and encode on the device) -> info."""
+    ps, _bpp, _pal = process_settings(contrast, percent, rotate, palette, tune, rgba)
+    png = png_settings(filter, matches, block_bytes, rgb_from_rgba)
+    s = (settings or Settings()).to_c()
+    ci = _lib.CImageInfo()
+    raise_for(_lib.load().apt_decode_wav_png(str(input_path).encode(), str(output_path).encode(), C.byref(s),
+                                             int(bool(sync)), C.byref(ps), C.byref(png), C.byref(ci)))
+    return _info(ci)
+
+
 def _info(ci):
     return {"low": ci.low, "high": ci.high, "rows": int(ci.rows), "telemetry_row": int(ci.telemetry_row),
             "wedges_a": np.array(ci.wedges_a[:], dtype=np.float32), "wedges_b": np.array(ci.wedges_b[:], dtype=np.float32)}

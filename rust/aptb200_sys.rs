@@ -111,6 +111,17 @@ extern "C" {
     pub fn apt_stream_geometry_iq(iq: *const apt_iq_settings, s: *const apt_settings, sync: c_int, max_push: u64,
                                   info: *mut apt_stream_info) -> c_int;
     pub fn apt_wav_load_iq16(path: *const c_char, out: *mut i16, cap: u64, n: *mut u64, sample_rate: *mut u32) -> c_int;
+    // PNG output: the file's bytes encoded on the device (DESIGN.md §11)
+    pub fn apt_png_default_settings(ps: *mut apt_png_settings);
+    pub fn apt_png_bound(width: u32, height: u32, channels: c_int, ps: *const apt_png_settings, bytes: *mut u64) -> c_int;
+    pub fn apt_png_encode(pixels: *const u8, width: u32, height: u32, channels: c_int, ps: *const apt_png_settings,
+                          out: *mut u8, cap: u64, nout: *mut u64) -> c_int;
+    pub fn apt_decode_png(signal: *const c_void, format: c_int, n: u64, input_rate: u32, s: *const apt_settings, sync: c_int,
+                          ps: *const apt_process_settings, png: *const apt_png_settings, out: *mut u8, cap: u64,
+                          nout: *mut u64, info: *mut apt_image_info, cb: apt_status_cb, user: *mut c_void) -> c_int;
+    pub fn apt_decoder_set_png_mode(dec: *mut apt_decoder, ps: *const apt_png_settings) -> c_int;
+    pub fn apt_decode_wav_png(input_path: *const c_char, output_path: *const c_char, s: *const apt_settings, sync: c_int,
+                              ps: *const apt_process_settings, png: *const apt_png_settings, info: *mut apt_image_info) -> c_int;
 }
 
 pub const APT_CU8: c_int = 2;
@@ -157,3 +168,15 @@ pub struct apt_image_info { pub low: f32, pub high: f32, pub rows: u64, pub tele
 #[derive(Clone, Copy)]
 pub struct apt_process_settings { pub contrast: c_int, pub percent: c_float, pub rotate: c_int,
                                   pub palette: *const u8 /* 256*256*3 RGB or null */, pub tune: [c_float; 4], pub rgba: c_int }
+
+#[repr(C)]
+pub struct apt_decoder { _private: [u8; 0] }
+
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct apt_png_settings { pub filter: c_int /* -1 adaptive, 0..4 fixed */, pub matches: c_int, pub block_bytes: u32,
+                              pub rgb_from_rgba: c_int }
+
+impl Default for apt_png_settings {
+    fn default() -> Self { apt_png_settings { filter: -1, matches: 1, block_bytes: 65536, rgb_from_rgba: 0 } }
+}

@@ -1,5 +1,5 @@
 #!/bin/bash
-# compute-sanitizer memcheck + racecheck over small decodes of every resampler path; logs under $OUT (default tool_out/).
+# compute-sanitizer memcheck + racecheck over small decodes of every resampler path and a small PNG encode; logs under $OUT (default tool_out/).
 OUT=${OUT:-tool_out}
 mkdir -p "$OUT"
 CS=/usr/local/cuda/bin/compute-sanitizer

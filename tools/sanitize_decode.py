@@ -1,4 +1,4 @@
-"""Small decodes through every resampler path, for compute-sanitizer (tools/sanitize.sh)."""
+"""Small decodes through every resampler path and a small PNG encode, for compute-sanitizer (tools/sanitize.sh)."""
 import os
 import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -23,3 +23,24 @@ for rate, profile, seconds in cases:
     ref, st = oracle.decode_steps(x, rate, os_)
     ok = np.array_equal(pos, st["sync_pos"]) and got.size == ref.size and got16.size == ref.size
     print(rate, profile, "rows", got.size // 2080, "sync equal" if ok else "MISMATCH", flush=True)
+
+# The PNG encoder (DESIGN.md §11): one small RGBA encode of several 4 KiB blocks with matches (look-back across block
+# boundaries, words shared by blocks and warps), checked against the CPU restatement, and one decoder job in PNG mode.
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+import _png_oracle as po                                            # noqa: E402
+from noaa_apt_b200 import image                                     # noqa: E402
+
+g = np.load(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden",
+                         "argentina_excerpt.npz"))["grey"][:6, :700]
+rgba = np.empty(g.shape + (4,), dtype=np.uint8)
+rgba[..., :3] = g[..., None]
+rgba[..., 3] = 255
+png = image.encode_png(rgba, block_bytes=4096)
+print("png encode", len(png), "bytes", "equal" if png == po.encode(rgba, block_bytes=4096) else "MISMATCH", flush=True)
+x = synth.apt_signal(11025, 14, seed=3)
+with na.Decoder(11025, na.Settings(), max_samples=x.size) as dec:
+    dec.set_process_mode(image.MINMAX, rgba=True)
+    img = dec.decode(x)
+    dec.set_png_mode(block_bytes=4096)
+    png = dec.decode(x)
+print("png mode", len(png), "bytes", "equal" if png == image.encode_png(img, block_bytes=4096) else "MISMATCH", flush=True)
