@@ -74,9 +74,8 @@ int aptb200::free_decoder_buffers(apt_decoder *d) {
         if (p) cudaFree(p);
     if (d->h_res) cudaFreeHost(d->h_res);
     if (d->h_out) cudaFreeHost(d->h_out);
-    if (d->h_post) cudaFreeHost(d->h_post);
-    for (void *p : {(void *)d->d_post, (void *)d->d_tel, (void *)d->d_out8, (void *)d->d_palette, (void *)d->d_proc, (void *)d->d_grey})
-        if (p) cudaFree(p);
+    if (d->d_out8) cudaFree(d->d_out8);
+    d->post.release();
     d->iq_tables.release();
     d->iq_win.release();
     d->png_work.release();
@@ -428,40 +427,25 @@ extern "C" void apt_decoder_destroy(apt_decoder *dec) {
 
 namespace {
 
-// contrast bounds + u8 map of the rows the job leaves in d_out; the head of the control block follows the job to the host
-int enqueue_image_stage(apt_decoder *d, unsigned char *out8) {
-    const LaunchCtx c{d->stream, d->sm_count};
-    const u32 max_rows = static_cast<u32>(std::max<uint64_t>(d->max_out / kPxPerRow, 1));
-    const u32 fixed = d->job_sync ? 0u : static_cast<u32>(d->job_fixed_out / kPxPerRow);
-    if (d->proc_active) {
+// Bytes of one output pixel of the job: the plan's, or an f32 row value.
+size_t out_elem(const apt_decoder *d) { return d->post_plan ? static_cast<size_t>(d->post_plan->bpp) : sizeof(float); }
+
+// The job after the rows, at submit and again after a sync redo: the image stage on the rows in d_out (its head follows
+// to the pinned copy), the SyncResult and, for host jobs, the rows or the image to the caller.
+int enqueue_job_tail(apt_decoder *d) {
+    if (d->post_plan) {
+        const u32 max_rows = static_cast<u32>(std::max<uint64_t>(d->max_out / kPxPerRow, 1));
+        const u32 fixed = d->job_sync ? 0u : static_cast<u32>(d->job_fixed_out / kPxPerRow);
+        unsigned char *image = d->job_host || d->job_png ? d->d_out8 : reinterpret_cast<unsigned char *>(d->job_out);
         DecoderHook hook(d);
-        ProcessLaunch a{};
-        a.rows = d->d_out;
-        a.result = d->job_sync ? d->back.res : nullptr;
-        a.fixed_rows = fixed;
-        a.max_rows = max_rows;
-        a.contrast = d->proc.contrast;
-        a.percent = d->proc.percent;
-        a.rotate = d->proc.rotate != 0;
-        a.rgba = d->proc.rgba != 0;
-        a.palette = d->proc_palette ? d->d_palette : nullptr;
-        memcpy(a.tune, d->proc.tune, sizeof(a.tune));
-        a.ctl = d->d_post;
-        a.tel_a = d->d_tel;
-        a.tel_b = d->d_tel + max_rows;
-        a.tel_v = d->d_tel + 2 * static_cast<size_t>(max_rows);
-        a.proc = d->d_proc;
-        a.grey = d->d_grey;
-        a.out = out8;
-        APT_TRY(launch_process_stage(c, a, &hook));
-        APT_CUDA(cudaMemcpyAsync(d->h_post, d->d_post, offsetof(PostCtl, buckets), cudaMemcpyDeviceToHost, d->stream));
-        return APT_OK;
+        APT_TRY(post_launch(LaunchCtx{d->stream, d->sm_count}, *d->post_plan, d->post, d->d_out, d->job_sync ? d->back.res : nullptr,
+                            fixed, max_rows, kPxPerRow, nullptr, image, &hook));
     }
-    APT_TRY(launch_image_stage(c, d->d_out, d->job_sync ? d->back.res : nullptr, fixed, max_rows, kPxPerRow, d->image_contrast,
-                               d->image_percent, d->d_post, d->d_tel, d->d_tel + max_rows, d->d_tel + 2 * static_cast<size_t>(max_rows),
-                               nullptr, out8, false));
-    d->launches += d->image_contrast == APT_CONTRAST_PERCENT ? 4 : 3;
-    APT_CUDA(cudaMemcpyAsync(d->h_post, d->d_post, offsetof(PostCtl, buckets), cudaMemcpyDeviceToHost, d->stream));
+    if (d->job_sync) APT_CUDA(cudaMemcpyAsync(d->h_res, d->back.res, sizeof(SyncResult), cudaMemcpyDeviceToHost, d->stream));
+    if (d->job_host && d->job_d2h_floats)
+        APT_CUDA(cudaMemcpyAsync(d->job_out_pageable ? static_cast<void *>(d->h_out) : static_cast<void *>(d->job_out),
+                                 d->post_plan ? static_cast<const void *>(d->d_out8) : static_cast<const void *>(d->d_out),
+                                 d->job_d2h_floats * out_elem(d), cudaMemcpyDeviceToHost, d->stream));
     return APT_OK;
 }
 
@@ -495,28 +479,21 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
         return fail(APT_ERR_BAD_ARG, "work_rate %u is too high for the sync picker (min_distance %u > 16384); decode without "
                                      "sync or use a work_rate <= 37440", p.st.work_rate, p.dist);
     const uint64_t need = d->job_sync ? (nwork / p.row) * kPxPerRow : plan_out_bound(p, n);
-    // bytes per output pixel of an image job: RGBA in process mode, else grey
-    const uint64_t bpp = d->image_contrast >= 0 && d->proc_active && d->proc.rgba ? 4 : 1;
-    // PNG mode: cap counts PNG bytes, checked at wait() once the file's length is known
-    const bool png = d->image_contrast >= 0 && d->png_active;
-    if (png && d->png.rgb_from_rgba && bpp != 4) return fail(APT_ERR_BAD_ARG, "rgb_from_rgba needs RGBA process output");
+    const PostPlan *post = d->post_plan ? &*d->post_plan : nullptr;
+    // cap counts bytes of an image job, floats of an f32 one; in PNG mode PNG bytes, checked at wait() once the file's
+    // length is known
+    const uint64_t per_px = post ? post->bpp : 1;
+    const bool png = post && d->png_active;
+    if (png && d->png.rgb_from_rgba && per_px != 4) return fail(APT_ERR_BAD_ARG, "rgb_from_rgba needs RGBA process output");
     if (png && !out) return fail(APT_ERR_BAD_ARG, "null output");
-    if (!png && (!out || cap < need * bpp))
-        return fail(APT_ERR_CAPACITY, "output needs room for %llu %s", (unsigned long long)(need * bpp),
-                    d->image_contrast >= 0 ? "bytes" : "floats");
+    if (!png && (!out || cap < need * per_px))
+        return fail(APT_ERR_CAPACITY, "output needs room for %llu %s", (unsigned long long)(need * per_px), post ? "bytes" : "floats");
     d->job_png = png;
-    d->job_image = d->image_contrast >= 0;
-    d->job_bpp = bpp;
-    if (d->job_image) {
+    if (post) {
         if (!p.work_multiple) return fail(APT_ERR_BAD_ARG, "the image stage needs rows of 2080 pixels (work_rate multiple of 4160)");
-        const uint64_t max_rows = std::max<uint64_t>(d->max_out / kPxPerRow, 1);
-        if (!d->d_post) {
-            APT_CUDA(cudaMalloc(&d->d_post, sizeof(PostCtl)));
-            APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&d->h_post), sizeof(PostCtl), cudaHostAllocDefault));
-            APT_CUDA(cudaMalloc(&d->d_tel, 3 * max_rows * sizeof(float)));
-        }
+        APT_TRY(d->post.alloc(*post, static_cast<u32>(std::max<uint64_t>(d->max_out / kPxPerRow, 1))));
         if (!d->d_out) APT_CUDA(cudaMalloc(&d->d_out, std::max<uint64_t>(d->max_out, 1) * sizeof(float)));
-        const uint64_t out8_need = std::max<uint64_t>(d->max_out, 1) * bpp;
+        const uint64_t out8_need = std::max<uint64_t>(d->max_out, 1) * per_px;
         if ((host || png) && d->out8_bytes < out8_need) {
             if (d->d_out8) APT_CUDA(cudaFree(d->d_out8));
             d->d_out8 = nullptr;
@@ -524,12 +501,7 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
             APT_CUDA(cudaMalloc(&d->d_out8, out8_need));
             d->out8_bytes = out8_need;
         }
-        if (d->proc_active) {
-            if (!d->d_proc) APT_CUDA(cudaMalloc(&d->d_proc, sizeof(ProcCtl)));
-            if (!d->d_grey) APT_CUDA(cudaMalloc(&d->d_grey, std::max<uint64_t>(d->max_out, 1)));
-        }
     }
-    const size_t elem = d->job_image ? bpp : sizeof(float);
 
     const void *dev_in = signal;
     float *rows_dst = out;
@@ -576,26 +548,17 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
         }
         rows_dst = d->d_out;
     }
-    if (d->job_image) rows_dst = d->d_out;      // the f32 rows are an intermediate of the image job
+    if (post) rows_dst = d->d_out;      // the f32 rows are an intermediate of the image job
     d->job_rows_src = rows_dst;
     int st = decoder_enqueue(d, dev_in, format, n, sync, rows_dst, host_chunked);
-    if (st == APT_OK && d->job_image)
-        st = enqueue_image_stage(d, host || png ? d->d_out8 : reinterpret_cast<unsigned char *>(out));
+    // the rows come back with the job: when syncing n_rows is only known on the device, so the copy covers the bound
+    // (at most one row more than is produced)
+    d->job_d2h_floats = !host || png ? 0 : d->job_sync ? need : d->job_fixed_out;
+    if (st == APT_OK) st = enqueue_job_tail(d);
     if (st != APT_OK) {
         cudaStreamSynchronize(d->stream);
         d->job_status = st;
         return st;
-    }
-    if (d->job_sync) APT_CUDA(cudaMemcpyAsync(d->h_res, d->back.res, sizeof(SyncResult), cudaMemcpyDeviceToHost, d->stream));
-    d->job_d2h_floats = 0;
-    if (host) {
-        // the rows come back with the job: when syncing n_rows is only known on the device, so the copy covers the bound
-        // (at most one row more than is produced)
-        d->job_d2h_floats = png ? 0 : d->job_sync ? need : d->job_fixed_out;
-        if (d->job_d2h_floats)
-            APT_CUDA(cudaMemcpyAsync(d->job_out_pageable ? static_cast<void *>(d->h_out) : static_cast<void *>(out),
-                                     d->job_image ? static_cast<const void *>(d->d_out8) : static_cast<const void *>(d->d_out),
-                                     d->job_d2h_floats * elem, cudaMemcpyDeviceToHost, d->stream));
     }
     d->in_flight = true;
     if (d->device >= 0 && d->device < 64) g_jobs_in_flight[d->device].fetch_add(1, std::memory_order_relaxed);
@@ -620,7 +583,7 @@ namespace {
 // control block, then copy exactly that many bytes to the caller's buffer.  Two stream synchronisations.
 int png_job(apt_decoder *d, uint64_t rows, uint64_t *bytes) {
     PngPlan p;
-    APT_TRY(make_png(kPxPerRow, static_cast<uint32_t>(rows), static_cast<int>(d->job_bpp), &d->png, p));
+    APT_TRY(make_png(kPxPerRow, static_cast<uint32_t>(rows), d->post_plan->bpp, &d->png, p));
     if (!d->h_png) APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&d->h_png), sizeof(PngCtl), cudaHostAllocDefault));
     DecoderHook hook(d);
     APT_TRY(png_encode_device(LaunchCtx{d->stream, d->sm_count}, p, d->png_work, d->d_out8, &hook));
@@ -658,13 +621,7 @@ extern "C" int apt_decoder_wait(apt_decoder *d, uint64_t *nout) {
             DecoderHook hook(d);
             APT_TRY(back_redo(LaunchCtx{d->stream, d->sm_count}, d->plan, d->back_plan, d->back, d->d_e, d->job_work,
                               const_cast<float *>(d->job_rows_src), &hook, d->last_back));
-            if (d->job_image)
-                APT_TRY(enqueue_image_stage(d, d->job_host || d->job_png ? d->d_out8 : reinterpret_cast<unsigned char *>(d->job_out)));
-            APT_CUDA(cudaMemcpyAsync(d->h_res, d->back.res, sizeof(SyncResult), cudaMemcpyDeviceToHost, d->stream));
-            if (d->job_host && d->job_d2h_floats)
-                APT_CUDA(cudaMemcpyAsync(d->job_out_pageable ? static_cast<void *>(d->h_out) : static_cast<void *>(d->job_out),
-                                         d->job_image ? static_cast<const void *>(d->d_out8) : static_cast<const void *>(d->d_out),
-                                         d->job_d2h_floats * (d->job_image ? d->job_bpp : sizeof(float)), cudaMemcpyDeviceToHost, d->stream));
+            APT_TRY(enqueue_job_tail(d));
             APT_CUDA(cudaStreamSynchronize(d->stream));
         }
         const SyncResult res = *d->h_res;
@@ -676,7 +633,7 @@ extern "C" int apt_decoder_wait(apt_decoder *d, uint64_t *nout) {
         }
         produced = static_cast<uint64_t>(res.n_rows) * kPxPerRow;
     }
-    const size_t elem = d->job_image ? d->job_bpp : sizeof(float);
+    const size_t elem = out_elem(d);
     if (d->job_host && d->job_out_pageable && produced && !d->job_png) {
         if (d->stager) d->stager->scatter(d->job_out, d->h_out, produced * elem);
         else memcpy(d->job_out, d->h_out, produced * elem);
@@ -686,18 +643,8 @@ extern "C" int apt_decoder_wait(apt_decoder *d, uint64_t *nout) {
                 std::chrono::duration<double>(t_synced - t_begin).count() * 1e3,
                 std::chrono::duration<double>(std::chrono::steady_clock::now() - t_synced).count() * 1e3,
                 d->job_out_pageable ? "pageable" : "direct");
-    if (d->job_image) {
-        const PostCtl &pc = *d->h_post;
-        apt_image_info &ii = d->last_image;
-        ii.low = pc.low;
-        ii.high = pc.high;
-        ii.rows = pc.rows;
-        ii.telemetry_row = pc.telemetry_row;
-        memcpy(ii.wedges_a, pc.wedges_a, sizeof(ii.wedges_a));
-        memcpy(ii.wedges_b, pc.wedges_b, sizeof(ii.wedges_b));
-        if (pc.status == 3) d->job_status = fail(APT_ERR_TOO_SHORT, "Recording too short for telemetry decoding");
-        else if (pc.status != 0) d->job_status = fail(APT_ERR_BAD_ARG, "image stage: %s", pc.status == 1 ? "empty image" :
-                                                      pc.status == 2 ? "no contrast bucket found" : "telemetry frame runs off the image");
+    if (d->post_plan) {
+        d->job_status = post_result(*d->post.head, &d->last_image);
         if (d->job_status != APT_OK) return d->job_status;
     }
     d->last_rows = d->plan.work_multiple ? produced / kPxPerRow : 0;
@@ -715,43 +662,31 @@ extern "C" int apt_decoder_wait(apt_decoder *d, uint64_t *nout) {
         d->kernel_ms.assign(d->ev_used, 0.f);
         for (int i = 0; i < d->ev_used; ++i) cudaEventElapsedTime(&d->kernel_ms[i], d->ev_begin[i], d->ev_end[i]);
     }
-    if (nout) *nout = d->job_png ? png_bytes : d->job_image ? produced * d->job_bpp : produced;
+    if (nout) *nout = d->job_png ? png_bytes : d->post_plan ? produced * d->post_plan->bpp : produced;
     return APT_OK;
 }
 
 extern "C" int apt_decoder_set_image_mode(apt_decoder *d, int contrast, float percent) {
     if (!d) return fail(APT_ERR_BAD_ARG, "null decoder");
     if (d->in_flight) return fail(APT_ERR_BAD_ARG, "decoder has a job in flight");
-    if (contrast > APT_CONTRAST_TELEMETRY) return fail(APT_ERR_BAD_ARG, "unknown contrast mode %d", contrast);
-    if (contrast == APT_CONTRAST_PERCENT && !(percent >= 0.f && percent <= 1.f))
-        return fail(APT_ERR_BAD_ARG, "Percent given should be between 0 and 1");      // misc.rs:120-124
-    d->image_contrast = contrast;
-    d->image_percent = percent;
-    d->proc_active = false;
-    if (contrast < 0) d->png_active = false;
+    if (contrast < 0) {
+        d->post_plan.reset();
+        d->png_active = false;
+        return APT_OK;
+    }
+    if (contrast == APT_CONTRAST_HISTOGRAM) return fail(APT_ERR_BAD_ARG, "unknown contrast mode %d", contrast);
+    PostPlan plan;
+    APT_TRY(make_post(image_settings(contrast, percent), plan));
+    d->post_plan = plan;
     return APT_OK;
 }
 
 namespace {
 
-// The argument rules of the process entry points; no device needed.
-int check_process_settings(const apt_process_settings *ps) {
+// make_post for the entry points that take the settings by pointer.
+int process_plan(const apt_process_settings *ps, PostPlan &plan) {
     if (!ps) return fail(APT_ERR_BAD_ARG, "null process settings");
-    if (ps->contrast < 0 || ps->contrast > APT_CONTRAST_HISTOGRAM) return fail(APT_ERR_BAD_ARG, "unknown contrast mode %d", ps->contrast);
-    if (ps->contrast == APT_CONTRAST_PERCENT && !(ps->percent >= 0.f && ps->percent <= 1.f))
-        return fail(APT_ERR_BAD_ARG, "Percent given should be between 0 and 1");      // misc.rs:120-124
-    if (ps->palette && !ps->rgba) return fail(APT_ERR_BAD_ARG, "false colour needs RGBA output");
-    if (ps->palette && ps->contrast == APT_CONTRAST_HISTOGRAM)
-        return fail(APT_ERR_BAD_ARG, "colour histogram equalisation is not available");
-    return APT_OK;
-}
-
-// 256*256*3 RGB -> 256*256 u32 with R in the low byte and alpha 255 (Rgb::to_rgba), one 4-byte load per coloured pixel
-std::vector<u32> pack_palette(const uint8_t *rgb) {
-    std::vector<u32> p(256 * 256);
-    for (size_t i = 0; i < p.size(); ++i)
-        p[i] = static_cast<u32>(rgb[3 * i]) | (static_cast<u32>(rgb[3 * i + 1]) << 8) | (static_cast<u32>(rgb[3 * i + 2]) << 16) | 0xFF000000u;
-    return p;
+    return make_post(*ps, plan);
 }
 
 }  // namespace
@@ -760,25 +695,17 @@ extern "C" int apt_decoder_set_process_mode(apt_decoder *d, const apt_process_se
     if (!d) return fail(APT_ERR_BAD_ARG, "null decoder");
     if (d->in_flight) return fail(APT_ERR_BAD_ARG, "decoder has a job in flight");
     if (!ps) {
-        d->proc_active = false;
-        d->image_contrast = -1;
+        d->post_plan.reset();
         d->png_active = false;
         return APT_OK;
     }
-    APT_TRY(check_process_settings(ps));
-    if (ps->palette) {
+    PostPlan plan;
+    APT_TRY(make_post(*ps, plan));
+    if (plan.palette) {
         APT_CUDA(cudaSetDevice(d->device));
-        if (!d->d_palette) APT_CUDA(cudaMalloc(&d->d_palette, 256 * 256 * sizeof(u32)));
-        const std::vector<u32> packed = pack_palette(ps->palette);
-        APT_CUDA(cudaMemcpyAsync(d->d_palette, packed.data(), packed.size() * sizeof(u32), cudaMemcpyHostToDevice, d->stream));
-        APT_CUDA(cudaStreamSynchronize(d->stream));
+        APT_TRY(d->post.upload_palette(ps->palette, d->stream));
     }
-    d->proc = *ps;
-    d->proc.palette = nullptr;
-    d->proc_palette = ps->palette != nullptr;
-    d->proc_active = true;
-    d->image_contrast = ps->contrast;
-    d->image_percent = ps->percent;
+    d->post_plan = plan;
     return APT_OK;
 }
 
@@ -795,8 +722,8 @@ extern "C" int apt_decoder_set_png_mode(apt_decoder *d, const apt_png_settings *
         d->png_active = false;
         return APT_OK;
     }
-    if (d->image_contrast < 0) return fail(APT_ERR_BAD_ARG, "PNG mode needs image or process mode");
-    APT_TRY(check_png_settings(ps, d->proc_active && d->proc.rgba ? 4 : 1));
+    if (!d->post_plan) return fail(APT_ERR_BAD_ARG, "PNG mode needs image or process mode");
+    APT_TRY(check_png_settings(ps, d->post_plan->bpp));
     d->png = *ps;
     d->png_active = true;
     return APT_OK;
@@ -1006,9 +933,10 @@ void cache_put_multi(int device, uint32_t rate, const apt_settings &st, apt_deco
     if (victim) apt_decoder_destroy(victim);
 }
 
+// ps: the image of process(), else (nullptr) f32 rows; png: that image as a PNG file.
 int decode_oneshot(const void *signal, int format, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
-                   float *out, uint64_t cap, uint64_t *nout, apt_status_cb cb, void *user, int contrast = -1,
-                   float percent = 0.f, apt_image_info *info = nullptr, const apt_process_settings *ps = nullptr,
+                   float *out, uint64_t cap, uint64_t *nout, apt_status_cb cb, void *user,
+                   const apt_process_settings *ps = nullptr, apt_image_info *info = nullptr,
                    const apt_png_settings *png = nullptr) {
     if (!s || !nout) return fail(APT_ERR_BAD_ARG, "null argument");
     *nout = 0;
@@ -1033,15 +961,12 @@ int decode_oneshot(const void *signal, int format, uint64_t n, uint32_t input_ra
     }
     d->cb = cb;
     d->cb_user = user;
-    d->image_contrast = contrast;
-    d->image_percent = percent;
     int st = ps ? apt_decoder_set_process_mode(d, ps) : APT_OK;
     if (st == APT_OK && png) st = apt_decoder_set_png_mode(d, png);
     if (st == APT_OK) st = apt_decoder_submit_host(d, signal, format, n, sync, out, cap);
     if (st == APT_OK) st = apt_decoder_wait(d, nout);
     if (st == APT_OK && info) *info = d->last_image;
-    d->image_contrast = -1;
-    d->proc_active = false;
+    d->post_plan.reset();
     d->png_active = false;
     d->cb = nullptr;
     d->cb_user = nullptr;
@@ -1156,36 +1081,37 @@ extern "C" int apt_decode_iq(const void *iq, int format, uint64_t n, const apt_i
 extern "C" int apt_decode_image_u8(const void *signal, int format, uint64_t n, uint32_t input_rate, const apt_settings *s,
                                    int sync, int contrast, float percent, uint8_t *out, uint64_t cap, uint64_t *nout,
                                    apt_image_info *info, apt_status_cb cb, void *user) {
-    if (contrast < 0 || contrast > APT_CONTRAST_TELEMETRY) return fail(APT_ERR_BAD_ARG, "unknown contrast mode %d", contrast);
-    if (contrast == APT_CONTRAST_PERCENT && !(percent >= 0.f && percent <= 1.f))
-        return fail(APT_ERR_BAD_ARG, "Percent given should be between 0 and 1");
-    return decode_oneshot(signal, format, n, input_rate, s, sync, reinterpret_cast<float *>(out), cap, nout, cb, user, contrast,
-                          percent, info);
+    if (contrast == APT_CONTRAST_HISTOGRAM) return fail(APT_ERR_BAD_ARG, "unknown contrast mode %d", contrast);
+    const apt_process_settings ps = image_settings(contrast, percent);
+    PostPlan plan;
+    APT_TRY(make_post(ps, plan));
+    return decode_oneshot(signal, format, n, input_rate, s, sync, reinterpret_cast<float *>(out), cap, nout, cb, user, &ps, info);
 }
 
 extern "C" int apt_decode_image(const void *signal, int format, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
                                 const apt_process_settings *ps, uint8_t *out, uint64_t cap, uint64_t *nout, apt_image_info *info,
                                 apt_status_cb cb, void *user) {
-    APT_TRY(check_process_settings(ps));
-    return decode_oneshot(signal, format, n, input_rate, s, sync, reinterpret_cast<float *>(out), cap, nout, cb, user,
-                          ps->contrast, ps->percent, info, ps);
+    PostPlan plan;
+    APT_TRY(process_plan(ps, plan));
+    return decode_oneshot(signal, format, n, input_rate, s, sync, reinterpret_cast<float *>(out), cap, nout, cb, user, ps, info);
 }
 
 extern "C" int apt_decode_png(const void *signal, int format, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
                               const apt_process_settings *ps, const apt_png_settings *png, uint8_t *out, uint64_t cap,
                               uint64_t *nout, apt_image_info *info, apt_status_cb cb, void *user) {
-    APT_TRY(check_process_settings(ps));
-    APT_TRY(check_png_settings(png, ps->rgba ? 4 : 1));
+    PostPlan plan;
+    APT_TRY(process_plan(ps, plan));
+    APT_TRY(check_png_settings(png, plan.bpp));
     if (!out) return fail(APT_ERR_BAD_ARG, "null output");
-    return decode_oneshot(signal, format, n, input_rate, s, sync, reinterpret_cast<float *>(out), cap, nout, cb, user,
-                          ps->contrast, ps->percent, info, ps, png);
+    return decode_oneshot(signal, format, n, input_rate, s, sync, reinterpret_cast<float *>(out), cap, nout, cb, user, ps, info, png);
 }
 
 extern "C" int apt_decode_wav_png(const char *input_path, const char *output_path, const apt_settings *s, int sync,
                                   const apt_process_settings *ps, const apt_png_settings *png, apt_image_info *info) {
     if (!input_path || !output_path || !s) return fail(APT_ERR_BAD_ARG, "null argument");
-    APT_TRY(check_process_settings(ps));
-    APT_TRY(check_png_settings(png, ps->rgba ? 4 : 1));
+    PostPlan plan;
+    APT_TRY(process_plan(ps, plan));
+    APT_TRY(check_png_settings(png, plan.bpp));
     apt_wav_info wi;
     APT_TRY(apt_wav_info_read(input_path, &wi));
     uint32_t rate = 0;
@@ -1204,7 +1130,7 @@ extern "C" int apt_decode_wav_png(const char *input_path, const char *output_pat
     APT_TRY(apt_decode_len_bound(n, rate, s, &rows_bound));
     rows_bound = std::max<uint64_t>(rows_bound / kPxPerRow, 1);
     if (rows_bound > 0xFFFFFFFFull) return fail(APT_ERR_BAD_ARG, "recording too long");
-    APT_TRY(apt_png_bound(kPxPerRow, static_cast<uint32_t>(rows_bound), ps->rgba ? 4 : 1, png, &cap));
+    APT_TRY(apt_png_bound(kPxPerRow, static_cast<uint32_t>(rows_bound), plan.bpp, png, &cap));
     std::vector<uint8_t> bytes(cap);
     uint64_t nout = 0;
     APT_TRY(apt_decode_png(pcm16 ? static_cast<const void *>(pcm.data()) : static_cast<const void *>(x.data()),
@@ -1219,7 +1145,8 @@ extern "C" int apt_decode_wav_png(const char *input_path, const char *output_pat
 
 namespace {
 
-// rows on the host -> device, image-stage kernels, results back (stage entry points; one call, no retained state)
+// rows on the host -> device, image-mode stage, results back (stage entry points; one call, no retained state).  bounds:
+// map with these; out == nullptr: statistics and bounds only.  A signal that is not whole rows is one row of n pixels.
 int image_stage_host(const float *signal, uint64_t n, int contrast, float percent, const float *bounds, apt_image_info *info,
                      uint8_t *out, float *mean_a, float *mean_b, float *variance) {
     if (!signal || n == 0) return fail(APT_ERR_BAD_ARG, "empty signal");   // get_min of an empty vector is an error, dsp.rs:21-25
@@ -1227,44 +1154,34 @@ int image_stage_host(const float *signal, uint64_t n, int contrast, float percen
     const uint64_t rows = n / kPxPerRow;
     const bool whole = rows * kPxPerRow == n && rows > 0;
     if (!whole && (contrast == APT_CONTRAST_TELEMETRY || mean_a)) return fail(APT_ERR_BAD_ARG, "not a whole number of 2080-px rows");
-    DevBuf dx, dctl, dtel, dout, dbounds;
+    if (!whole && n >= (1ull << 32)) return fail(APT_ERR_BAD_ARG, "signal too long");
+    PostPlan plan;
+    APT_TRY(make_post(image_settings(contrast, percent), plan));
+    // a partial last row cannot occur in an image; min/max, percent and the map treat the signal as one row of n pixels then
+    const u32 nrows = whole ? static_cast<u32>(rows) : 1u;
+    const u32 px = whole ? kPxPerRow : static_cast<u32>(n);
+    DevBuf dx, dout, dbounds;
+    PostBuffers b;
     APT_TRY(dx.alloc(n * sizeof(float)));
-    APT_TRY(dctl.alloc(sizeof(PostCtl)));
-    APT_TRY(dtel.alloc(3 * std::max<uint64_t>(rows, 1) * sizeof(float)));
+    APT_TRY(b.alloc(plan, nrows));
     if (out) APT_TRY(dout.alloc(n));
     APT_CUDA(cudaMemcpy(dx.p, signal, n * sizeof(float), cudaMemcpyHostToDevice));
     if (bounds) {
         APT_TRY(dbounds.alloc(2 * sizeof(float)));
         APT_CUDA(cudaMemcpy(dbounds.p, bounds, 2 * sizeof(float), cudaMemcpyHostToDevice));
     }
-    const LaunchCtx c = stage_ctx();
-    // a partial last row cannot occur in an image; min/max, percent and the map treat the signal as one row of n pixels then
-    const u32 nrows = whole ? static_cast<u32>(rows) : 1u;
-    const u32 px = whole ? kPxPerRow : static_cast<u32>(n);
-    if (!whole && n >= (1ull << 32)) return fail(APT_ERR_BAD_ARG, "signal too long");
-    float *tel = dtel.as<float>();
-    APT_TRY(launch_image_stage(c, dx.as<float>(), nullptr, nrows, nrows, px, contrast, percent, dctl.as<PostCtl>(), tel,
-                               tel + std::max<uint64_t>(rows, 1), tel + 2 * std::max<uint64_t>(rows, 1), bounds ? dbounds.as<float>() : nullptr,
-                               out ? dout.as<unsigned char>() : nullptr, out == nullptr));
+    APT_TRY(post_launch(stage_ctx(), plan, b, dx.as<float>(), nullptr, nrows, nrows, px, dbounds.as<float>(), dout.p, nullptr));
     APT_CUDA(cudaDeviceSynchronize());
     if (!bounds) {
-        PostCtl pc;
-        APT_CUDA(cudaMemcpy(&pc, dctl.p, offsetof(PostCtl, buckets), cudaMemcpyDeviceToHost));
-        if (pc.status == 3) return fail(APT_ERR_TOO_SHORT, "Recording too short for telemetry decoding");
-        if (pc.status != 0) return fail(APT_ERR_BAD_ARG, "image stage failed (status %u)", pc.status);
-        if (info) {
-            info->low = pc.low;
-            info->high = pc.high;
-            info->rows = whole ? rows : 0;
-            info->telemetry_row = pc.telemetry_row;
-            memcpy(info->wedges_a, pc.wedges_a, sizeof(info->wedges_a));
-            memcpy(info->wedges_b, pc.wedges_b, sizeof(info->wedges_b));
-        }
+        apt_image_info ii{};
+        APT_TRY(post_result(*b.head, &ii));
+        if (info) *info = ii;
+        if (info && !whole) info->rows = 0;
     }
     if (out) APT_CUDA(cudaMemcpy(out, dout.p, n, cudaMemcpyDeviceToHost));
-    if (mean_a) APT_CUDA(cudaMemcpy(mean_a, tel, rows * sizeof(float), cudaMemcpyDeviceToHost));
-    if (mean_b) APT_CUDA(cudaMemcpy(mean_b, tel + rows, rows * sizeof(float), cudaMemcpyDeviceToHost));
-    if (variance) APT_CUDA(cudaMemcpy(variance, tel + 2 * rows, rows * sizeof(float), cudaMemcpyDeviceToHost));
+    if (mean_a) APT_CUDA(cudaMemcpy(mean_a, b.tel, rows * sizeof(float), cudaMemcpyDeviceToHost));
+    if (mean_b) APT_CUDA(cudaMemcpy(mean_b, b.tel + rows, rows * sizeof(float), cudaMemcpyDeviceToHost));
+    if (variance) APT_CUDA(cudaMemcpy(variance, b.tel + 2 * rows, rows * sizeof(float), cudaMemcpyDeviceToHost));
     return APT_OK;
 }
 
@@ -1279,9 +1196,9 @@ extern "C" int apt_map_signal_u8(const float *signal, uint64_t n, float low, flo
 
 extern "C" int apt_contrast_bounds(const float *signal, uint64_t n, int contrast, float percent, apt_image_info *info) {
     if (!info) return fail(APT_ERR_BAD_ARG, "null argument");
-    if (contrast < 0 || contrast > APT_CONTRAST_TELEMETRY) return fail(APT_ERR_BAD_ARG, "unknown contrast mode %d", contrast);
-    if (contrast == APT_CONTRAST_PERCENT && !(percent >= 0.f && percent <= 1.f))
-        return fail(APT_ERR_BAD_ARG, "Percent given should be between 0 and 1");
+    if (contrast == APT_CONTRAST_HISTOGRAM) return fail(APT_ERR_BAD_ARG, "unknown contrast mode %d", contrast);
+    PostPlan plan;
+    APT_TRY(make_post(image_settings(contrast, percent), plan));
     memset(info, 0, sizeof(*info));
     return image_stage_host(signal, n, contrast, percent, nullptr, info, nullptr, nullptr, nullptr, nullptr);
 }
@@ -1293,61 +1210,31 @@ extern "C" int apt_telemetry_rows(const float *signal, uint64_t n, float *mean_a
 
 extern "C" int apt_process(const float *rows, uint64_t n, const apt_process_settings *ps, uint8_t *out, uint64_t cap,
                            uint64_t *nout, apt_image_info *info) {
-    APT_TRY(check_process_settings(ps));
+    PostPlan plan;
+    APT_TRY(process_plan(ps, plan));
     if (!nout) return fail(APT_ERR_BAD_ARG, "null argument");
     *nout = 0;
     if (!rows || n == 0) return fail(APT_ERR_BAD_ARG, "empty signal");   // get_min of an empty vector is an error, dsp.rs:21-25
     const uint64_t nrows = n / kPxPerRow;
     if (nrows * kPxPerRow != n) return fail(APT_ERR_BAD_ARG, "not a whole number of 2080-px rows");
     if (nrows >= (1ull << 32) / kPxPerRow) return fail(APT_ERR_BAD_ARG, "image too large");
-    const uint64_t bytes = n * (ps->rgba ? 4 : 1);
+    const uint64_t bytes = n * plan.bpp;
     if (!out || cap < bytes) return fail(APT_ERR_CAPACITY, "output needs room for %llu bytes", (unsigned long long)bytes);
     APT_TRY(require_device());
-    DevBuf dx, dctl, dtel, dproc, dgrey, dout, dpal;
+    DevBuf dx, dout;
+    PostBuffers b;
     APT_TRY(dx.alloc(n * sizeof(float)));
-    APT_TRY(dctl.alloc(sizeof(PostCtl)));
-    APT_TRY(dtel.alloc(3 * nrows * sizeof(float)));
-    APT_TRY(dproc.alloc(sizeof(ProcCtl)));
-    APT_TRY(dgrey.alloc(n));
+    APT_TRY(b.alloc(plan, static_cast<u32>(nrows)));
     APT_TRY(dout.alloc(bytes));
     APT_CUDA(cudaMemcpy(dx.p, rows, n * sizeof(float), cudaMemcpyHostToDevice));
-    if (ps->palette) {
-        APT_TRY(dpal.alloc(256 * 256 * sizeof(u32)));
-        const std::vector<u32> packed = pack_palette(ps->palette);
-        APT_CUDA(cudaMemcpy(dpal.p, packed.data(), packed.size() * sizeof(u32), cudaMemcpyHostToDevice));
-    }
-    ProcessLaunch a{};
-    a.rows = dx.as<float>();
-    a.result = nullptr;
-    a.fixed_rows = a.max_rows = static_cast<u32>(nrows);
-    a.contrast = ps->contrast;
-    a.percent = ps->percent;
-    a.rotate = ps->rotate != 0;
-    a.rgba = ps->rgba != 0;
-    a.palette = ps->palette ? dpal.as<u32>() : nullptr;
-    memcpy(a.tune, ps->tune, sizeof(a.tune));
-    a.ctl = dctl.as<PostCtl>();
-    a.tel_a = dtel.as<float>();
-    a.tel_b = a.tel_a + nrows;
-    a.tel_v = a.tel_a + 2 * nrows;
-    a.proc = dproc.as<ProcCtl>();
-    a.grey = dgrey.as<unsigned char>();
-    a.out = dout.p;
-    APT_TRY(launch_process_stage(stage_ctx(), a, nullptr));
+    if (plan.palette) APT_TRY(b.upload_palette(ps->palette, nullptr));
+    APT_TRY(post_launch(stage_ctx(), plan, b, dx.as<float>(), nullptr, static_cast<u32>(nrows), static_cast<u32>(nrows), kPxPerRow,
+                        nullptr, dout.p, nullptr));
     APT_CUDA(cudaDeviceSynchronize());
-    PostCtl pc;
-    APT_CUDA(cudaMemcpy(&pc, dctl.p, offsetof(PostCtl, buckets), cudaMemcpyDeviceToHost));
-    if (pc.status == 3) return fail(APT_ERR_TOO_SHORT, "Recording too short for telemetry decoding");
-    if (pc.status != 0) return fail(APT_ERR_BAD_ARG, "image stage failed (status %u)", pc.status);
+    apt_image_info ii{};
+    APT_TRY(post_result(*b.head, &ii));
     APT_CUDA(cudaMemcpy(out, dout.p, bytes, cudaMemcpyDeviceToHost));
-    if (info) {
-        info->low = pc.low;
-        info->high = pc.high;
-        info->rows = nrows;
-        info->telemetry_row = pc.telemetry_row;
-        memcpy(info->wedges_a, pc.wedges_a, sizeof(info->wedges_a));
-        memcpy(info->wedges_b, pc.wedges_b, sizeof(info->wedges_b));
-    }
+    if (info) *info = ii;
     *nout = bytes;
     return APT_OK;
 }
@@ -1531,8 +1418,7 @@ extern "C" int apt_decode_batch(const void *const *signals, int format, const ui
                     } else {
                         d->stager = decs[0]->stager;
                     }
-                    d->image_contrast = -1;
-                    d->proc_active = false;
+                    d->post_plan.reset();
                     decs.push_back(d);
                     job_of.push_back(-1);
                 }

@@ -10,6 +10,7 @@
 
 #include "aptb200.h"
 #include <memory>
+#include <optional>
 
 #include "back.hpp"
 #include "filters_host.hpp"
@@ -18,6 +19,7 @@
 #include "iq.hpp"
 #include "launch.hpp"
 #include "png.hpp"
+#include "post.hpp"
 
 namespace aptb200 {
 
@@ -105,23 +107,12 @@ struct apt_decoder {
     uint64_t job_d2h_floats = 0;   // rows copied back by the job (an upper bound when syncing: n_rows is not known yet)
     aptb200::SyncResult *h_res = nullptr;   // pinned
 
-    // image mode (kernels_post.cuh): the job's output is the u8 image
-    int image_contrast = -1;       // < 0: f32 rows
-    float image_percent = 0.98f;
-    aptb200::PostCtl *d_post = nullptr, *h_post = nullptr;   // device block; pinned copy of its head for the host
-    float *d_tel = nullptr;        // 3 * max_rows floats: telemetry band means and variance per row
+    // image / process mode (post.hpp): the job's output is the image of the plan; no plan: f32 rows
+    std::optional<aptb200::PostPlan> post_plan;
+    aptb200::PostBuffers post;
     unsigned char *d_out8 = nullptr;
     uint64_t out8_bytes = 0;       // size of d_out8 (max_out, or 4 * max_out once an RGBA process job ran)
-    bool job_image = false;
     apt_image_info last_image{};
-    // process mode (apt_decoder_set_process_mode): the image stage is the whole of process() but the map overlay
-    bool proc_active = false;
-    apt_process_settings proc{};   // palette field unused: the palette lives in d_palette
-    bool proc_palette = false;
-    aptb200::u32 *d_palette = nullptr;      // 256*256 packed RGBA
-    aptb200::ProcCtl *d_proc = nullptr;
-    unsigned char *d_grey = nullptr;        // max_out B intermediate grey plane
-    uint64_t job_bpp = 1;          // output bytes per pixel of the image job in flight
     // PNG mode (apt_decoder_set_png_mode): the image of an image / process job is encoded on the device at wait(); only the
     // PNG bytes are copied out.  The workspaces are sized at first use from the image size.
     bool png_active = false;

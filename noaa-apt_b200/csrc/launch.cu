@@ -16,7 +16,6 @@
 #include "kernels_sync.cuh"
 #include "kernels_sync2.cuh"
 #include "kernels_stream.cuh"
-#include "kernels_post.cuh"
 #include "kernels_ut.cuh"
 
 namespace aptb200 {
@@ -452,84 +451,6 @@ int launch_stream_sync(const LaunchCtx &c, const StreamSyncArgs &a) {
     auto kern = k_stream_sync<kStreamChunk>;
     APT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     kern<<<1, kStreamThreads, smem, c.stream>>>(a);
-    APT_CUDA(cudaGetLastError());
-    return APT_OK;
-}
-
-int launch_image_stage(const LaunchCtx &c, const float *rows, const SyncResult *result, u32 fixed_rows, u32 max_rows, u32 px,
-                       int contrast, float percent, PostCtl *ctl, float *tel_a, float *tel_b, float *tel_v,
-                       const float *bounds_dev, unsigned char *out, bool stats_only) {
-    if (max_rows == 0) return APT_OK;
-    const unsigned wide = static_cast<unsigned>(c.sm_count) * 8;
-    if (!bounds_dev) {
-        APT_CUDA(cudaMemsetAsync(ctl, 0, sizeof(PostCtl), c.stream));
-        k_post_stats<<<std::min<unsigned>(max_rows, wide), 256, 0, c.stream>>>(rows, result, fixed_rows, px, ctl, tel_a, tel_b, tel_v);
-        if (contrast == 1) k_post_histogram<<<wide / 2, 256, 0, c.stream>>>(rows, result, fixed_rows, px, ctl);
-        k_post_bounds<<<1, 1024, 0, c.stream>>>(contrast, percent, result, fixed_rows, px, ctl, tel_a, tel_b, tel_v);
-    }
-    if (!stats_only) k_post_map_u8<<<wide, 256, 0, c.stream>>>(rows, result, fixed_rows, px, ctl, bounds_dev, out);
-    APT_CUDA(cudaGetLastError());
-    return APT_OK;
-}
-
-int launch_process_stage(const LaunchCtx &c, const ProcessLaunch &a, KernelHook *hook) {
-    if (a.max_rows == 0) return APT_OK;
-    if (((reinterpret_cast<uintptr_t>(a.rows) & 15) | (reinterpret_cast<uintptr_t>(a.grey) & 15) | (reinterpret_cast<uintptr_t>(a.out) & 15)) != 0)
-        return fail(APT_ERR_BAD_ARG, "process stage: buffers must be 16-byte aligned");
-    const unsigned wide = static_cast<unsigned>(c.sm_count) * 8;
-    const u32 px = 2080;
-    const bool hist = a.contrast == 3;
-    const int bounds_mode = hist ? 0 : a.contrast;          // Contrast::Histogram takes the MinMax bounds, noaa_apt.rs:158-163
-    // the grey image is the output when nothing follows the map
-    const bool finish = hist || a.rotate || a.rgba || a.palette;
-    unsigned char *grey = finish ? a.grey : static_cast<unsigned char *>(a.out);
-    APT_CUDA(cudaMemsetAsync(a.ctl, 0, sizeof(PostCtl), c.stream));
-    if (hist) APT_CUDA(cudaMemsetAsync(a.proc->hist, 0, sizeof(a.proc->hist), c.stream));
-    {
-        KernelSlot s(hook, "post_stats");
-        k_post_stats<<<std::min<unsigned>(a.max_rows, wide), 256, 0, c.stream>>>(a.rows, a.result, a.fixed_rows, px, a.ctl, a.tel_a,
-                                                                                 a.tel_b, a.tel_v);
-    }
-    if (bounds_mode == 1) {
-        KernelSlot s(hook, "post_histogram");
-        k_post_histogram<<<wide / 2, 256, 0, c.stream>>>(a.rows, a.result, a.fixed_rows, px, a.ctl);
-    }
-    {
-        KernelSlot s(hook, "post_bounds");
-        k_post_bounds<<<1, 1024, 0, c.stream>>>(bounds_mode, a.percent, a.result, a.fixed_rows, px, a.ctl, a.tel_a, a.tel_b, a.tel_v);
-    }
-    if (hist) {
-        {
-            // two CTAs per SM: every CTA adds its 512 counts to the same 512 global words at the end
-            KernelSlot s(hook, "post_map_u8_hist");
-            k_post_map_u8_hist<<<static_cast<unsigned>(c.sm_count) * 2, 256, 0, c.stream>>>(a.rows, a.result, a.fixed_rows, a.ctl,
-                                                                                              grey, a.proc);
-        }
-        KernelSlot s(hook, "post_eq_lut");
-        k_post_eq_lut<<<1, 512, 0, c.stream>>>(a.proc);
-    } else {
-        KernelSlot s(hook, "post_map_u8");
-        k_post_map_u8<<<wide, 256, 0, c.stream>>>(a.rows, a.result, a.fixed_rows, px, a.ctl, nullptr, grey);
-    }
-    if (finish) {
-        KernelSlot s(hook, "post_finish");
-        const int mode = a.palette ? 2 : (hist ? 1 : 0);
-        const float4 tune = make_float4(a.tune[0], a.tune[1], a.tune[2], a.tune[3]);
-        if (a.rgba) k_post_finish<true><<<wide, 256, 0, c.stream>>>(grey, a.ctl, a.proc, mode, a.rotate ? 1 : 0, a.palette, tune, a.out);
-        else k_post_finish<false><<<wide, 256, 0, c.stream>>>(grey, a.ctl, a.proc, mode, a.rotate ? 1 : 0, nullptr, tune, a.out);
-    }
-    APT_CUDA(cudaGetLastError());
-    return APT_OK;
-}
-
-int launch_quantize_i16(const LaunchCtx &c, const float *x, u64 n, PostCtl *ctl, short *out) {
-    if (n == 0) return APT_OK;
-    if (n >= (1ull << 32)) return fail(APT_ERR_BAD_ARG, "signal too long");
-    APT_CUDA(cudaMemsetAsync(ctl, 0, sizeof(PostCtl), c.stream));
-    const unsigned wide = static_cast<unsigned>(c.sm_count) * 8;
-    // the signal as one "row" of n pixels: only the maximum is used
-    k_post_stats<<<1, 256, 0, c.stream>>>(x, nullptr, 1, static_cast<u32>(n), ctl, nullptr, nullptr, nullptr);
-    k_quantize_i16<<<wide, 256, 0, c.stream>>>(x, n, ctl, out);
     APT_CUDA(cudaGetLastError());
     return APT_OK;
 }

@@ -238,13 +238,6 @@ PickScratch pick_scratch_carve(void *base, u32 max_blocks, u32 max_positions, u3
 int launch_gather(const LaunchCtx &c, const float *f, const u32 *positions, const SyncResult *result,
                   u32 fixed_rows, u32 max_rows, u32 row, u32 px, u32 dec, float *out);
 
-// Image stage (SURVEY.md §8 f3): contrast bounds + telemetry statistics + u8 map of `rows` (f32, device), rows counted by
-// `result` (sync decode) or fixed_rows.  contrast: 0 min/max, 1 percent, 2 telemetry (aptb200.h apt_contrast); bounds_dev !=
-// nullptr: map with the two floats there instead (stage entry point).  tel_* are per-row scratch (max_rows floats each).
-int launch_image_stage(const LaunchCtx &c, const float *rows, const SyncResult *result, u32 fixed_rows, u32 max_rows, u32 px,
-                       int contrast, float percent, PostCtl *ctl, float *tel_a, float *tel_b, float *tel_v,
-                       const float *bounds_dev, unsigned char *out, bool stats_only);
-
 // Called around every kernel of a stage (profiling events and launch counting of a decoder).
 struct KernelHook {
     virtual void begin(const char *name) = 0;
@@ -257,28 +250,6 @@ struct KernelSlot {
     KernelSlot(KernelHook *h, const char *name) : hook(h) { if (hook) hook->begin(name); }
     ~KernelSlot() { if (hook) hook->end(); }
 };
-
-// The rest of noaa_apt::process (kernels_post.cuh, aptb200.h apt_process_settings) on rows of 2080 pixels.  All pointers are
-// device pointers; rows counted by `result` (sync decode) or fixed_rows, as in launch_image_stage.
-struct ProcessLaunch {
-    const float *rows;
-    const SyncResult *result;
-    u32 fixed_rows, max_rows;
-    int contrast;                  // apt_contrast, APT_CONTRAST_HISTOGRAM included
-    float percent;
-    bool rotate, rgba;
-    const u32 *palette;            // 256*256 packed RGBA (R in the low byte, alpha 255), row = channel B value; nullptr: none
-    float tune[4];
-    PostCtl *ctl;
-    float *tel_a, *tel_b, *tel_v;  // per-row scratch, max_rows floats each
-    ProcCtl *proc;                 // histograms + equalisation table (histogram mode)
-    unsigned char *grey;           // max_rows * 2080 B intermediate grey plane (unused when the output is that plane)
-    void *out;                     // max_rows * 2080 * (rgba ? 4 : 1) B
-};
-int launch_process_stage(const LaunchCtx &c, const ProcessLaunch &a, KernelHook *hook);
-
-// wav.rs:71-85: normalise by the maximum and quantise to i16 (x, out: device; ctl: scratch control block).
-int launch_quantize_i16(const LaunchCtx &c, const float *x, u64 n, PostCtl *ctl, short *out);
 
 // Builds the geometry and the zero-padded per-group tap table of the tiled polyphase kernel for
 // (l, m, taps).  Returns false when the shape does not fit the kernel (the generic kernel is used then).

@@ -50,7 +50,7 @@ for name, kw in MODES.items():
     dec.set_profiling(False)
     res["decode_48k"][name] = {"rows": int(img.shape[0]), "us": {k: med(v) for k, v in acc.items()}}
     print("48k", name, img.shape[0], {k: round(med(v), 1) for k, v in acc.items()})
-# (the existing image mode launches the minmax_grey kernels above; it records no profiling events of its own)
+# (image mode is process mode with default settings: it launches the minmax_grey kernels above, under the same slot names)
 dec.close()
 
 # ---- end to end: apt_decode_image (RGBA, palette, rotation, telemetry) vs apt_decode_image_u8, same recording
