@@ -404,8 +404,9 @@ int apt_decode_batch(const void *const *signals, int format, const uint64_t *len
  * every row k with max(p_k + row, p_{k+1} + G) + latency_work <= work_final has been returned (p_k: sync position k,
  * row: samples per row, G: template length); without sync, every row r with (r+1)*row + latency_work <= work_final.
  *
- * All device memory is allocated by apt_stream_create and depends only on (input_rate, settings, max_push); push and
- * finish allocate nothing.  Pushes are synchronous (the rows are in `rows` on return) and take pageable host pointers;
+ * Device memory is allocated by apt_stream_create, where it depends only on (input_rate, settings, max_push), and by
+ * apt_stream_set_process_mode / apt_stream_set_png_mode (image output, below); push and finish allocate nothing.  Pushes
+ * are synchronous (the rows are in `rows` on return) and take pageable host pointers;
  * pushes larger than max_push are split into steps of max_push samples.  Supported: the standard, fast and slow
  * profiles (any settings whose demodulation low-pass has 37, 43 or 61 taps) at every input rate apt_decode accepts,
  * with a work rate that is a multiple of 4160.  sync with another work rate fails with APT_ERR_WORK_RATE, sync = 0
@@ -418,7 +419,7 @@ typedef struct apt_stream_info {
     uint64_t peaks;           /* sync positions decided so far */
     uint64_t latency_work;    /* slack of the emission rule, in work-rate samples (constant per stream) */
     uint64_t max_push;        /* samples one internal step takes; larger pushes are split */
-    uint64_t device_bytes;    /* device memory the stream owns (constant from create to destroy) */
+    uint64_t device_bytes;    /* device memory the stream owns (image output included; changes only when a mode is set) */
 } apt_stream_info;
 
 int apt_stream_create(int device, uint32_t input_rate, const apt_settings *s, int sync, uint64_t max_push, apt_stream **st);
@@ -438,6 +439,7 @@ int apt_stream_sync_positions(apt_stream *st, uint64_t *positions, size_t cap, s
 int apt_stream_get_info(apt_stream *st, apt_stream_info *info);
 /* Host only, no device: the geometry a stream of these parameters would have (latency_work, max_push, device_bytes). */
 int apt_stream_geometry(uint32_t input_rate, const apt_settings *s, int sync, uint64_t max_push, apt_stream_info *info);
+
 
 /* ------------------------------------------------------------------ I/Q input: FM demodulation on the device */
 
@@ -527,6 +529,36 @@ int apt_decoder_set_png_mode(apt_decoder *dec, const apt_png_settings *ps);
  * PNG to output_path.  info may be NULL. */
 int apt_decode_wav_png(const char *input_path, const char *output_path, const apt_settings *s, int sync,
                        const apt_process_settings *ps, const apt_png_settings *png, apt_image_info *info);
+
+/* ------------------------------------------------------------------ streaming decoder: image and PNG output */
+
+/* Image output of a stream (DESIGN.md §9): the rows of the pass are kept on the device (f32, up to max_rows rows) and
+ * apt_stream_finish_image ends the pass in the image apt_process describes.  Allowed only when nothing has been pushed
+ * since create / reset.  ps == NULL switches image output (and PNG output) off and frees its buffers; setting a process
+ * mode also switches PNG output off.  All device memory of the image output is allocated here; push and finish still
+ * allocate nothing.  apt_stream_reset keeps both modes for the next pass; plain apt_stream_finish still works and makes
+ * no image.  APT_ERR_BAD_ARG before the device is touched: a push since create / reset, max_rows == 0 (or 2^32 / 2080 or
+ * more), and the settings apt_process rejects. */
+int apt_stream_set_process_mode(apt_stream *st, const apt_process_settings *ps, uint64_t max_rows);
+/* PNG output (needs process mode): apt_stream_finish_image writes the PNG file instead of the pixels.  The encoder
+ * workspace for a max_rows image is reserved here.  NULL switches PNG output off.  APT_ERR_BAD_ARG before the device is
+ * touched: a push since create / reset, no process mode, the settings apt_png_encode rejects for the process mode's
+ * channels (rgb_from_rgba on grey output, a bad block_bytes, ...), and an IDAT for max_rows rows that could pass
+ * 2^31 - 1 bytes. */
+int apt_stream_set_png_mode(apt_stream *st, const apt_png_settings *png);
+/* apt_stream_finish, plus the image: `image` receives rows*2080*bpp pixel bytes, or the PNG file in PNG mode; *image_n
+ * its byte count; info as apt_decode_image.  The pixels, info and status equal apt_decode_image (the PNG bytes
+ * apt_decode_png) on the whole recording with the same settings, sync and modes, for any split into pushes; for an I/Q
+ * stream they equal apt_process (apt_png_encode) of apt_decode_iq's rows.  The rows are those apt_stream_finish returns.
+ * Status, the first that applies:
+ *   1. the decode's own (APT_ERR_TOO_SHORT, APT_ERR_FEW_SYNC_FRAMES): no image;
+ *   2. the pass has more than max_rows rows: APT_ERR_CAPACITY, info->rows the pass's row count (the pushes still returned
+ *      every row; only the image is refused);
+ *   3. the image stage's errors, as apt_decode_image returns them (e.g. telemetry on a pass too short for a frame);
+ *   4. image_cap below the image's size: APT_ERR_CAPACITY, *image_n the required byte count.
+ * In cases 2 to 4 the pass is finished.  A stream without image output is APT_ERR_BAD_ARG. */
+int apt_stream_finish_image(apt_stream *st, float *rows, uint64_t cap, uint64_t *nout, uint8_t *image, uint64_t image_cap,
+                            uint64_t *image_n, apt_image_info *info);
 
 #ifdef __cplusplus
 }

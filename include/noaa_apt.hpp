@@ -228,6 +228,36 @@ class Stream {
         return apt_stream_push(st_, samples, format, n, o, c, k); }); }
     Signal finish() { return rows(0, [&](float *o, uint64_t c, uint64_t *k) { return apt_stream_finish(st_, o, c, k); }); }
     void reset() { err::check(apt_stream_reset(st_)); }
+
+    // Image output (before the first push of a pass): finish_image() also returns the image of process() (ps) for up to
+    // max_rows rows, or with set_png_mode its PNG file.  set_process_mode(nullptr) switches both off.
+    void set_process_mode(const apt_process_settings *ps, uint64_t max_rows = 2400) {
+        err::check(apt_stream_set_process_mode(st_, ps, max_rows));
+        max_rows_ = ps ? max_rows : 0;
+        bpp_ = ps && ps->rgba ? 4 : 1;
+        png_ = false;
+    }
+    void set_png_mode(const apt_png_settings *png) {
+        err::check(apt_stream_set_png_mode(st_, png));
+        png_ = png != nullptr;
+        if (png) png_settings_ = *png;
+    }
+    struct Image {
+        Signal rows;                  // the rows finish() would return
+        std::vector<uint8_t> bytes;   // rows * 2080 * (1 grey | 4 RGBA) pixel bytes, or the PNG file
+        apt_image_info info{};
+    };
+    Image finish_image() {
+        Image im;
+        uint64_t cap = max_rows_ * 2080 * bpp_, n = 0;
+        if (png_) err::check(apt_png_bound(2080, static_cast<uint32_t>(max_rows_ ? max_rows_ : 1), bpp_, &png_settings_, &cap));
+        im.bytes.resize(cap ? cap : 1);
+        im.rows = rows(0, [&](float *o, uint64_t c, uint64_t *k) {
+            return apt_stream_finish_image(st_, o, c, k, im.bytes.data(), im.bytes.size(), &n, &im.info);
+        });
+        im.bytes.resize(n);
+        return im;
+    }
     std::vector<uint64_t> positions() const {
         size_t n = 0;
         err::check(apt_stream_sync_positions(st_, nullptr, 0, &n));
@@ -252,6 +282,10 @@ class Stream {
         return out;
     }
     apt_stream *st_ = nullptr;
+    uint64_t max_rows_ = 0;
+    int bpp_ = 1;
+    bool png_ = false;
+    apt_png_settings png_settings_{};
 };
 
 // Decoding straight from SDR I/Q (DESIGN.md §10).  format: APT_CU8 / APT_CS16 / APT_CF32, n complex samples.

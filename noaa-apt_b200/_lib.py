@@ -206,6 +206,10 @@ SIGNATURES = {
     "apt_decoder_set_png_mode": (C.c_int, [C.c_void_p, C.POINTER(CPngSettings)]),
     "apt_decode_wav_png": (C.c_int, [C.c_char_p, C.c_char_p, C.POINTER(CSettings), C.c_int, C.POINTER(CProcessSettings),
                                      C.POINTER(CPngSettings), C.POINTER(CImageInfo)]),
+    "apt_stream_set_process_mode": (C.c_int, [C.c_void_p, C.POINTER(CProcessSettings), C.c_uint64]),
+    "apt_stream_set_png_mode": (C.c_int, [C.c_void_p, C.POINTER(CPngSettings)]),
+    "apt_stream_finish_image": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, _u64p, C.c_void_p, C.c_uint64, _u64p,
+                                          C.POINTER(CImageInfo)]),
 }
 
 _lib = None

@@ -5,6 +5,8 @@
 //   final range -> k_stream_sync (roots, seed, orbit walk, rows to gather) -> k_gather_rows_lp -> one copy back.
 // The input, envelope and correlation live in windows that keep only what a later step can still read; a window is
 // compacted by moving its tail to the front when the tail is shorter than the part dropped (so the move never overlaps).
+// With image output (apt_stream_set_process_mode) every round's new rows are also copied into an image buffer on the device,
+// and apt_stream_finish_image runs the image stage (post.hpp) and the PNG encoder (png.hpp) on it.
 #include <algorithm>
 #include <cstring>
 #include <memory>
@@ -77,6 +79,43 @@ Geom make_geom(const Plan &p, int sync, uint64_t max_push) {
     return g;
 }
 
+// Image output of a stream: the rows of the pass (f32, up to max_rows) and everything the image stage and the encoder need,
+// allocated when the mode is set so that push and finish allocate nothing.
+struct ImageOut {
+    PostPlan plan;
+    uint64_t max_rows = 0;
+    PostBuffers post;
+    float *d_rows = nullptr;          // max_rows * 2080 f32: row r of the pass at r * 2080
+    unsigned char *d_px = nullptr;    // max_rows * 2080 * bpp: the image
+    PngCtl *h_png = nullptr;          // pinned copy of the encoder's control block
+    uint64_t bytes = 0;               // device bytes of the above
+    bool png = false;                 // PNG output (apt_stream_set_png_mode)
+    apt_png_settings png_settings{};
+    PngWork png_work;                 // reserved for a max_rows image
+
+    // The stage's and the image's device memory (PostBuffers::alloc and upload_palette for max_rows rows).
+    uint64_t post_bytes() const {
+        return sizeof(PostCtl) + 3 * max_rows * sizeof(float) + (plan.hist ? sizeof(ProcCtl) : 0) +
+               (plan.finish ? max_rows * kPxPerRow : 0) + (plan.palette ? 256 * 256 * sizeof(u32) : 0) +
+               max_rows * kPxPerRow * (sizeof(float) + plan.bpp);
+    }
+    void release_png() {
+        png_work.release();
+        png = false;
+    }
+    void release() {
+        release_png();
+        post.release();
+        if (d_rows) cudaFree(d_rows);
+        if (d_px) cudaFree(d_px);
+        if (h_png) cudaFreeHost(h_png);
+        d_rows = nullptr;
+        d_px = nullptr;
+        h_png = nullptr;
+        max_rows = bytes = 0;
+    }
+};
+
 }  // namespace
 
 struct apt_stream {
@@ -110,6 +149,8 @@ struct apt_stream {
     float *d_iq = nullptr;          // interleaved cf32, iq_cap complex samples from absolute sample iq_base
     void *d_iqraw = nullptr;        // one step's pushed samples as they came
     uint64_t iq_cap = 0, iq_in = 0, iq_base = 0;
+
+    ImageOut img;                   // image output: on when img.d_rows is set
 };
 
 namespace {
@@ -125,6 +166,7 @@ void free_stream(apt_stream *st) {
     if (st->d_iq) cudaFree(st->d_iq);
     if (st->d_iqraw) cudaFree(st->d_iqraw);
     st->iqt.release();
+    st->img.release();
     free_decoder_buffers(&st->dec);
 }
 
@@ -192,6 +234,16 @@ void take_rows(apt_stream *st, uint64_t rel_hi, float *rows, uint64_t &nout) {
     nout += n * kPxPerRow;
     st->held_slot = st->gathered > rel_hi ? st->gathered - 1 - st->rows_out : 0;
     st->rows_out = rel_hi;
+}
+
+// Image output: rows [first, end) of the pass, at `src` on the device, into the image buffer.  Rows past max_rows are left
+// out; finish_image then refuses the image (the pass has more rows than the buffer).
+int keep_rows(apt_stream *st, uint64_t first, uint64_t end, const float *src) {
+    end = std::min(end, st->img.max_rows);
+    if (first >= end) return APT_OK;
+    APT_CUDA(cudaMemcpyAsync(st->img.d_rows + first * kPxPerRow, src, (end - first) * kPxPerRow * sizeof(float),
+                             cudaMemcpyDeviceToDevice, st->dec.stream));
+    return APT_OK;
 }
 
 // The new audio of one step into the input window, from either source: audio pushes are uploaded as they are (PCM16 cast
@@ -271,6 +323,7 @@ int step(apt_stream *st, const void *host, int format, uint64_t n, bool finish, 
             const uint64_t cnt = std::min<uint64_t>(r_hi - st->rows_out, g.gather_cap);
             APT_TRY(launch_gather_lp(c, e, st->work_final, nullptr, nullptr, static_cast<u32>(cnt), static_cast<u32>(cnt), p.row, kPxPerRow,
                                      p.dec, p.lp.data(), ntaps, st->d_rows, static_cast<u32>(st->rows_out)));
+            if (st->img.d_rows) APT_TRY(keep_rows(st, st->rows_out, st->rows_out + cnt, st->d_rows));
             APT_CUDA(cudaMemcpyAsync(st->h_rows, st->d_rows, cnt * kPxPerRow * sizeof(float), cudaMemcpyDeviceToHost, d.stream));
             APT_CUDA(cudaStreamSynchronize(d.stream));
             st->gathered = st->rows_out + cnt;
@@ -328,6 +381,8 @@ int step(apt_stream *st, const void *host, int format, uint64_t n, bool finish, 
         for (; st->runs_seen < cy.run_tail; ++st->runs_seen)
             st->positions.insert(st->positions.end(), st->run_cnt()[st->runs_seen % kRunRing], st->run_pos()[st->runs_seen % kRunRing]);
         if (st->positions.size() != cy.len) return fail(APT_ERR_BAD_ARG, "internal: peak runs and peak count disagree");
+        // the round's new rows sit behind the held ones; the copy runs on the stream ahead of the next round's gather
+        if (st->img.d_rows) APT_TRY(keep_rows(st, st->gathered, cy.gathered, st->d_rows + held * kPxPerRow));
         st->gathered = cy.gathered;
         // released: rows whose next peak exists; a failed decode (fewer than 5 peaks at the end) releases nothing more
         const bool failed = finish && cy.len < 5;
@@ -548,6 +603,117 @@ extern "C" int apt_stream_finish(apt_stream *st, float *rows, uint64_t cap, uint
     return status;
 }
 
+namespace {
+
+bool pushed(const apt_stream *st) { return st->samples_in || st->iq_in || st->finished; }
+
+// The image of a finished pass from the rows kept on the device: the image stage, in PNG mode the encoder, then the pixels or
+// the file to the caller.  One stream synchronisation for pixels, two for a PNG file (its length is read first).
+int finish_image(apt_stream *st, uint8_t *image, uint64_t cap, uint64_t *image_n, apt_image_info *info) {
+    ImageOut &o = st->img;
+    const uint64_t rows = st->rows_out;
+    if (rows > o.max_rows) {
+        if (info) {
+            *info = apt_image_info{};
+            info->rows = rows;
+        }
+        return fail(APT_ERR_CAPACITY, "the pass has %llu rows, more than the image output's max_rows %llu", (unsigned long long)rows,
+                    (unsigned long long)o.max_rows);
+    }
+    apt_decoder &d = st->dec;
+    const LaunchCtx c{d.stream, d.sm_count};
+    APT_TRY(post_launch(c, o.plan, o.post, o.d_rows, nullptr, static_cast<u32>(rows), static_cast<u32>(o.max_rows), kPxPerRow,
+                        nullptr, o.d_px, nullptr));
+    const uint64_t px_bytes = rows * kPxPerRow * o.plan.bpp;
+    if (o.png) {
+        PngPlan pp;
+        APT_TRY(make_png(kPxPerRow, static_cast<uint32_t>(rows), o.plan.bpp, &o.png_settings, pp));
+        APT_TRY(png_encode_device(c, pp, o.png_work, o.d_px, nullptr));
+        APT_CUDA(cudaMemcpyAsync(o.h_png, o.png_work.ctl, sizeof(PngCtl), cudaMemcpyDeviceToHost, d.stream));
+    } else if (image && cap >= px_bytes) {
+        APT_CUDA(cudaMemcpyAsync(image, o.d_px, px_bytes, cudaMemcpyDeviceToHost, d.stream));
+    }
+    APT_CUDA(cudaStreamSynchronize(d.stream));
+    APT_TRY(post_result(*o.post.head, info));
+    const uint64_t bytes = o.png ? o.h_png->total : px_bytes;
+    *image_n = bytes;
+    if (!image || cap < bytes)
+        return fail(APT_ERR_CAPACITY, "image needs room for %llu %s bytes", (unsigned long long)bytes, o.png ? "PNG" : "pixel");
+    if (o.png) {
+        APT_CUDA(cudaMemcpyAsync(image, o.png_work.out, bytes, cudaMemcpyDeviceToHost, d.stream));
+        APT_CUDA(cudaStreamSynchronize(d.stream));
+    }
+    return APT_OK;
+}
+
+}  // namespace
+
+extern "C" int apt_stream_set_process_mode(apt_stream *st, const apt_process_settings *ps, uint64_t max_rows) {
+    if (!st) return fail(APT_ERR_BAD_ARG, "null stream");
+    if (pushed(st)) return fail(APT_ERR_BAD_ARG, "image output is set before the first push (after create or reset)");
+    PostPlan plan;
+    if (ps) {
+        APT_TRY(make_post(*ps, plan));
+        if (max_rows == 0) return fail(APT_ERR_BAD_ARG, "max_rows must be at least 1");
+        if (max_rows >= (1ull << 32) / kPxPerRow) return fail(APT_ERR_BAD_ARG, "max_rows %llu: image too large", (unsigned long long)max_rows);
+    }
+    APT_CUDA(cudaSetDevice(st->dec.device));
+    APT_CUDA(cudaStreamSynchronize(st->dec.stream));
+    ImageOut &o = st->img;
+    o.release();   // a new process mode also leaves PNG mode
+    if (!ps) return APT_OK;
+    struct Rollback {
+        ImageOut &o;
+        bool armed = true;
+        ~Rollback() {
+            if (armed) o.release();
+        }
+    } rollback{o};
+    o.plan = plan;
+    o.max_rows = max_rows;
+    APT_TRY(o.post.alloc(plan, static_cast<u32>(max_rows)));
+    if (plan.palette) APT_TRY(o.post.upload_palette(ps->palette, st->dec.stream));
+    APT_CUDA(cudaMalloc(&o.d_rows, max_rows * kPxPerRow * sizeof(float)));
+    APT_CUDA(cudaMalloc(&o.d_px, max_rows * kPxPerRow * plan.bpp));
+    APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&o.h_png), sizeof(PngCtl), cudaHostAllocDefault));
+    o.bytes = o.post_bytes();
+    rollback.armed = false;
+    return APT_OK;
+}
+
+extern "C" int apt_stream_set_png_mode(apt_stream *st, const apt_png_settings *png) {
+    if (!st) return fail(APT_ERR_BAD_ARG, "null stream");
+    if (pushed(st)) return fail(APT_ERR_BAD_ARG, "PNG output is set before the first push (after create or reset)");
+    ImageOut &o = st->img;
+    PngPlan pp;
+    if (png) {
+        if (!o.d_rows) return fail(APT_ERR_BAD_ARG, "PNG output needs process mode (apt_stream_set_process_mode)");
+        APT_TRY(make_png(kPxPerRow, static_cast<uint32_t>(o.max_rows), o.plan.bpp, png, pp));
+    }
+    APT_CUDA(cudaSetDevice(st->dec.device));
+    APT_CUDA(cudaStreamSynchronize(st->dec.stream));
+    o.release_png();
+    if (!png) return APT_OK;
+    const int rc = o.png_work.reserve(pp);
+    if (rc != APT_OK) {
+        o.release_png();
+        return rc;
+    }
+    o.png_settings = *png;
+    o.png = true;
+    return APT_OK;
+}
+
+extern "C" int apt_stream_finish_image(apt_stream *st, float *rows, uint64_t cap, uint64_t *nout, uint8_t *image,
+                                       uint64_t image_cap, uint64_t *image_n, apt_image_info *info) {
+    if (nout) *nout = 0;
+    if (image_n) *image_n = 0;
+    if (!st || !image_n) return fail(APT_ERR_BAD_ARG, "null argument");
+    if (!st->img.d_rows) return fail(APT_ERR_BAD_ARG, "the stream has no image output (apt_stream_set_process_mode)");
+    APT_TRY(apt_stream_finish(st, rows, cap, nout));
+    return finish_image(st, image, image_cap, image_n, info);
+}
+
 extern "C" int apt_stream_reset(apt_stream *st) {
     if (!st) return fail(APT_ERR_BAD_ARG, "null stream");
     return reset_state(st);
@@ -570,6 +736,6 @@ extern "C" int apt_stream_get_info(apt_stream *st, apt_stream_info *info) {
     info->peaks = st->positions.size();
     info->latency_work = st->g.latency;
     info->max_push = st->iq ? st->iq_max_push : st->max_push;
-    info->device_bytes = st->g.bytes;
+    info->device_bytes = st->g.bytes + st->img.bytes + st->img.png_work.device_bytes();
     return APT_OK;
 }

@@ -7,7 +7,7 @@ import numpy as np
 from . import _lib
 from .config import Settings
 from .context import Context
-from .err import raise_for
+from .err import InvalidInput, raise_for
 from .frequency import _rate_hz
 
 FINAL_RATE = 4160        # decode.rs:14
@@ -283,6 +283,9 @@ class Stream:
             raise_for(self._lib.apt_stream_create(int(device), _rate_hz(input_rate), C.byref(s), int(bool(sync)), int(max_push),
                                                   C.byref(h)))
         self._h = h
+        self._bpp = None       # image output: bytes per pixel of the process mode's image; None: off
+        self._max_rows = 0
+        self._png = None       # PNG output: (filter, matches, block_bytes, rgb_from_rgba)
 
     @classmethod
     def for_iq(cls, iq_settings, settings=None, sync=True, max_push=1_200_000, device=0):
@@ -326,7 +329,58 @@ class Stream:
         return self._rows(0, lambda out, got: self._lib.apt_stream_finish(self._h, out.ctypes.data, out.size, C.byref(got)))
 
     def reset(self):
+        """A new pass with the same plan, buffers and image / PNG output."""
         raise_for(self._lib.apt_stream_reset(self._h))
+
+    # --- image output (apt_stream_set_process_mode / set_png_mode / finish_image) ---
+    def set_process_mode(self, contrast=None, percent=0.98, rotate=False, palette=None, tune=(0, 0, 0, 0), rgba=None,
+                         max_rows=2400):
+        """Before the first push of a pass: keep the pass's rows (up to max_rows) on the device so that finish_image()
+        returns the image of image.process, as image.decode_image would for the whole recording.  contrast=None switches
+        image output (and PNG output) off and frees its device memory.  Setting a process mode switches PNG output off."""
+        from . import image
+        if contrast is None:
+            raise_for(self._lib.apt_stream_set_process_mode(self._h, None, 0))
+            self._bpp = None
+            self._png = None
+            return
+        ps, bpp, _pal = image.process_settings(contrast, percent, rotate, palette, tune, rgba)
+        raise_for(self._lib.apt_stream_set_process_mode(self._h, C.byref(ps), int(max_rows)))   # the palette is copied here
+        self._bpp = bpp
+        self._max_rows = int(max_rows)
+        self._png = None
+
+    def set_png_mode(self, enabled=True, filter=-1, matches=True, block_bytes=65536, rgb_from_rgba=False):
+        """In process mode, before the first push: finish_image() returns the PNG file's bytes (as image.decode_png)
+        instead of the pixels.  The encoder workspace for max_rows rows is reserved here.  enabled=False: pixels again."""
+        from . import image
+        if not enabled:
+            raise_for(self._lib.apt_stream_set_png_mode(self._h, None))
+            self._png = None
+            return
+        ps = image.png_settings(filter, matches, block_bytes, rgb_from_rgba)
+        raise_for(self._lib.apt_stream_set_png_mode(self._h, C.byref(ps)))
+        self._png = (filter, matches, block_bytes, rgb_from_rgba)
+
+    def finish_image(self):
+        """finish() plus the image -> (rows, image, info): the remaining (k, 2080) float32 rows, the (h, 2080) / (h, 2080, 4)
+        u8 image or the PNG bytes, and the contrast info.  Raises as finish() does, and when the pass has more rows than
+        max_rows."""
+        from . import image
+        if self._bpp is None:
+            raise InvalidInput(_lib.ERR_BAD_ARG, "the stream has no image output: call set_process_mode first")
+        if self._png:
+            cap = image.png_bound(PX_PER_ROW, self._max_rows, self._bpp, *self._png)
+        else:
+            cap = self._max_rows * PX_PER_ROW * self._bpp
+        out = np.empty(max(cap, 1), dtype=np.uint8)
+        n = C.c_uint64(0)
+        ci = _lib.CImageInfo()
+        rows = self._rows(0, lambda o, got: self._lib.apt_stream_finish_image(self._h, o.ctypes.data, o.size, C.byref(got),
+                                                                             out.ctypes.data, out.size, C.byref(n), C.byref(ci)))
+        if self._png:
+            return rows, out[: n.value].tobytes(), image._info(ci)
+        return rows, image._shape(out[: n.value].copy(), self._bpp), image._info(ci)
 
     def positions(self):
         n = C.c_size_t(0)

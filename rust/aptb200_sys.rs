@@ -122,6 +122,11 @@ extern "C" {
     pub fn apt_decoder_set_png_mode(dec: *mut apt_decoder, ps: *const apt_png_settings) -> c_int;
     pub fn apt_decode_wav_png(input_path: *const c_char, output_path: *const c_char, s: *const apt_settings, sync: c_int,
                               ps: *const apt_process_settings, png: *const apt_png_settings, info: *mut apt_image_info) -> c_int;
+    // image output of a stream: the pass ends in its processed image or PNG file (DESIGN.md §9)
+    pub fn apt_stream_set_process_mode(st: *mut apt_stream, ps: *const apt_process_settings, max_rows: u64) -> c_int;
+    pub fn apt_stream_set_png_mode(st: *mut apt_stream, png: *const apt_png_settings) -> c_int;
+    pub fn apt_stream_finish_image(st: *mut apt_stream, rows: *mut c_float, cap: u64, nout: *mut u64, image: *mut u8,
+                                   image_cap: u64, image_n: *mut u64, info: *mut apt_image_info) -> c_int;
 }
 
 pub const APT_CU8: c_int = 2;

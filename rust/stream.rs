@@ -13,6 +13,16 @@ use crate::err;
 
 pub struct Stream {
     st: *mut sys::apt_stream,
+    image: Option<(u64, i32)>,                 // image output: (max_rows, bytes per pixel)
+    png: Option<sys::apt_png_settings>,        // PNG output
+}
+
+/// What `finish_image` returns: the rows `finish` would return, the image (rows * 2080 pixels of 1 grey or 4 RGBA bytes,
+/// or the PNG file) and the contrast info.
+pub struct PassImage {
+    pub rows: Signal,
+    pub image: Vec<u8>,
+    pub info: sys::apt_image_info,
 }
 
 // The stream is used from one thread at a time; moving it to another thread is fine.
@@ -33,7 +43,7 @@ impl Stream {
         if rc != sys::APT_OK {
             return Err(to_error(rc));
         }
-        Ok(Stream { st })
+        Ok(Stream { st, image: None, png: None })
     }
 
     fn rows(&mut self, n: u64, call: impl FnOnce(*mut f32, u64, *mut u64) -> i32) -> err::Result<Signal> {
@@ -83,7 +93,7 @@ impl Stream {
         if rc != sys::APT_OK {
             return Err(to_error(rc));
         }
-        Ok(Stream { st })
+        Ok(Stream { st, image: None, png: None })
     }
 
     /// I/Q samples of an I/Q stream (cu8 / cs16 / cf32 pushes may be mixed).
@@ -119,6 +129,51 @@ impl Stream {
             return Err(to_error(rc));
         }
         Ok(pos)
+    }
+
+    /// Image output, before the first push of a pass: `finish_image` also returns the image of `process` (`ps`) for a pass
+    /// of up to `max_rows` rows.  `None` switches image and PNG output off and frees their device memory.
+    pub fn set_process_mode(&mut self, ps: Option<&sys::apt_process_settings>, max_rows: u64) -> err::Result<()> {
+        let p = ps.map_or(ptr::null(), |p| p as *const _);
+        let rc = unsafe { sys::apt_stream_set_process_mode(self.st, p, max_rows) };
+        if rc != sys::APT_OK {
+            return Err(to_error(rc));
+        }
+        self.image = ps.map(|p| (max_rows, if p.rgba != 0 { 4 } else { 1 }));
+        self.png = None;
+        Ok(())
+    }
+
+    /// PNG output (needs process mode): `finish_image` returns the PNG file's bytes, ready to write.
+    pub fn set_png_mode(&mut self, png: Option<&sys::apt_png_settings>) -> err::Result<()> {
+        let p = png.map_or(ptr::null(), |p| p as *const _);
+        let rc = unsafe { sys::apt_stream_set_png_mode(self.st, p) };
+        if rc != sys::APT_OK {
+            return Err(to_error(rc));
+        }
+        self.png = png.copied();
+        Ok(())
+    }
+
+    /// `finish` plus the image of the pass (equal to `decode_image` / `decode_to_png` on the whole recording).
+    pub fn finish_image(&mut self) -> err::Result<PassImage> {
+        let (max_rows, bpp) = self.image.unwrap_or((0, 1));
+        let mut cap: u64 = max_rows * 2080 * bpp as u64;
+        if let Some(png) = self.png {
+            let rc = unsafe { sys::apt_png_bound(2080, max_rows.max(1) as u32, bpp, &png, &mut cap) };
+            if rc != sys::APT_OK {
+                return Err(to_error(rc));
+            }
+        }
+        let mut image = vec![0_u8; cap.max(1) as usize];
+        let mut info = sys::apt_image_info::default();
+        let mut n: u64 = 0;
+        let st = self.st;
+        let rows = self.rows(0, |o, c, k| unsafe {
+            sys::apt_stream_finish_image(st, o, c, k, image.as_mut_ptr(), image.len() as u64, &mut n, &mut info)
+        })?;
+        image.truncate(n as usize);
+        Ok(PassImage { rows, image, info })
     }
 
     pub fn info(&self) -> err::Result<sys::apt_stream_info> {

@@ -44,3 +44,14 @@ with na.Decoder(11025, na.Settings(), max_samples=x.size) as dec:
     dec.set_png_mode(block_bytes=4096)
     png = dec.decode(x)
 print("png mode", len(png), "bytes", "equal" if png == image.encode_png(img, block_bytes=4096) else "MISMATCH", flush=True)
+
+# The stream's image output (DESIGN.md §9): a small pass pushed in pieces with PNG output, the rows kept on the device,
+# the image stage and the encoder at finish, against apt_decode_png of the whole recording.
+with na.Stream(11025, na.Settings(), max_push=20000) as st:
+    st.set_process_mode(image.PERCENT, rotate=True, rgba=True, max_rows=64)
+    st.set_png_mode(block_bytes=4096)
+    for at in range(0, x.size, 30011):
+        st.push(x[at:at + 30011])
+    _rows, spng, _info = st.finish_image()
+want, _ = image.decode_png(None, na.Settings(), x, 11025, contrast=image.PERCENT, rotate=True, rgba=True, block_bytes=4096)
+print("stream png", len(spng), "bytes", "equal" if spng == want else "MISMATCH", flush=True)
