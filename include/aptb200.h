@@ -515,6 +515,13 @@ int apt_png_bound(uint32_t width, uint32_t height, int channels, const apt_png_s
  * frees it. */
 int apt_png_encode(const uint8_t *pixels, uint32_t width, uint32_t height, int channels, const apt_png_settings *ps,
                    uint8_t *out, uint64_t cap, uint64_t *nout);
+/* apt_png_encode of `count` host images of one width, channel count and settings, heights[k] rows each, in one batched
+ * encode (one launch sequence for the group): outs[k] receives exactly the bytes apt_png_encode gives for image k alone.
+ * A file larger than caps[k] is APT_ERR_CAPACITY with the required count in nouts[k]; the others are still written.
+ * Returns the first failing status.  apt_png_encode is this call with count 1 and shares its per-device workspace. */
+int apt_png_encode_batch(const uint8_t *const *pixels, const uint32_t *heights, uint32_t count, uint32_t width,
+                         int channels, const apt_png_settings *ps, uint8_t *const *outs, const uint64_t *caps,
+                         uint64_t *nouts);
 /* apt_decode_image + apt_png_encode in one call: the image is encoded on the device and only the PNG bytes cross PCIe.
  * Errors as apt_decode_image, plus the settings checks of apt_png_encode and APT_ERR_CAPACITY as there. */
 int apt_decode_png(const void *signal, int format, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
@@ -529,6 +536,39 @@ int apt_decoder_set_png_mode(apt_decoder *dec, const apt_png_settings *ps);
  * PNG to output_path.  info may be NULL. */
 int apt_decode_wav_png(const char *input_path, const char *output_path, const apt_settings *s, int sync,
                        const apt_process_settings *ps, const apt_png_settings *png, apt_image_info *info);
+
+/* apt_decode_batch, ending each recording in the image apt_process describes (png == NULL) or its PNG file.
+ * outs[i] / caps[i] / nouts[i] count bytes; infos (may be NULL) receives each recording's apt_image_info.
+ * Sharding, feeders and the out-of-memory fallback are those of apt_decode_batch.  Per recording, the status, info and
+ * bytes equal apt_decode_image (png == NULL) or apt_decode_png of that recording alone with the same arguments; a
+ * recording that fails (decode, image stage, or a file larger than caps[i]: APT_ERR_CAPACITY with the required count in
+ * nouts[i]) leaves the others unaffected.  With PNG output each device's decoders hand their images to a fixed pool and
+ * the images that are ready are encoded together, one launch sequence per group, on a stream of their own.  Argument
+ * errors (NULL pointers, the settings checks of apt_process and apt_png_encode, rgb_from_rgba on grey output) come back
+ * before any device is touched.  Returns the first failing status; statuses are never left "ok" by default. */
+int apt_decode_batch_image(const void *const *signals, int format, const uint64_t *lens, int count,
+                           uint32_t input_rate, const apt_settings *s, int sync,
+                           const apt_process_settings *ps, const apt_png_settings *png,
+                           uint8_t *const *outs, const uint64_t *caps, uint64_t *nouts, apt_image_info *infos,
+                           int *statuses, const int *devices, int ndevices, int streams_per_device);
+
+/* The layout of one batched PNG encode (host arithmetic, no device; DESIGN.md §11, "Batched encode"): `count` images of
+ * width x heights[k] pixels with `channels` channels share a filtered-stream buffer (also the per-position arrays), the
+ * per-block arrays and one output buffer.  images (may be NULL, else `cap` entries) receives each image's regions. */
+typedef struct apt_png_group_image {
+    uint64_t stream_offset;   /* of the filtered stream and the per-position arrays */
+    uint64_t stream_bytes;    /* filtered bytes (the region has 16 bytes of padding after them) */
+    uint64_t out_offset;      /* of the file in the output buffer */
+    uint64_t out_bytes;       /* bytes reserved for the file (apt_png_bound rounded up to words) */
+    uint64_t bound;           /* apt_png_bound of the image */
+    uint32_t first_row, first_span, first_block, blocks, first_chunk, pad;
+} apt_png_group_image;
+typedef struct apt_png_group_info {
+    uint64_t stream_bytes, out_bytes;          /* sizes of the shared buffers */
+    uint32_t rows, spans, blocks, chunks;      /* grid sizes: filter warps, match CTAs, block CTAs, CRC threads */
+} apt_png_group_info;
+int apt_png_group_plan(uint32_t width, int channels, const apt_png_settings *ps, const uint32_t *heights, uint32_t count,
+                       apt_png_group_info *info, apt_png_group_image *images, size_t cap);
 
 /* ------------------------------------------------------------------ streaming decoder: image and PNG output */
 

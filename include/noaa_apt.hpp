@@ -348,6 +348,43 @@ inline std::vector<uint8_t> decode_png(Context &ctx, const config::Settings &set
     out.resize(got);
     return out;
 }
+// A batch of recordings, each ending in its PNG file (png != nullptr) or its processed image (png == nullptr), sharded
+// over `devices` as apt_decode_batch does.  files[i] is empty where statuses[i] is not APT_OK; infos[i] is that
+// recording's apt_image_info.  Returns the first failing status (0 when every recording succeeded).
+struct BatchImages {
+    std::vector<std::vector<uint8_t>> files;
+    std::vector<apt_image_info> infos;
+    std::vector<int> statuses;
+};
+inline int decode_batch_png(const std::vector<Signal> &signals, Rate input_rate, const config::Settings &settings, bool sync,
+                            const apt_process_settings &ps, const apt_png_settings *png, BatchImages &res,
+                            const std::vector<int> &devices = {}, int streams_per_device = 4) {
+    const apt_settings s = settings.to_c();
+    const size_t count = signals.size();
+    std::vector<const void *> sigs(count);
+    std::vector<uint64_t> lens(count), caps(count), nouts(count);
+    std::vector<uint8_t *> outs(count);
+    res.files.assign(count, {});
+    res.infos.assign(count, apt_image_info{});
+    res.statuses.assign(count, APT_ERR_CUDA);
+    for (size_t i = 0; i < count; ++i) {
+        uint64_t bound = 0;
+        err::check(apt_decode_len_bound(signals[i].size(), input_rate.get_hz(), &s, &bound));
+        const uint64_t rows = bound / 2080 ? bound / 2080 : 1;
+        if (png) err::check(apt_png_bound(2080, static_cast<uint32_t>(rows), ps.rgba ? 4 : 1, png, &caps[i]));
+        else caps[i] = (bound ? bound : 1) * (ps.rgba ? 4 : 1);
+        res.files[i].resize(caps[i]);
+        sigs[i] = signals[i].data();
+        lens[i] = signals[i].size();
+        outs[i] = res.files[i].data();
+    }
+    const int rc = apt_decode_batch_image(sigs.data(), APT_F32, lens.data(), static_cast<int>(count), input_rate.get_hz(), &s,
+                                          sync ? 1 : 0, &ps, png, outs.data(), caps.data(), nouts.data(), res.infos.data(),
+                                          res.statuses.data(), devices.empty() ? nullptr : devices.data(),
+                                          static_cast<int>(devices.size()), streams_per_device);
+    for (size_t i = 0; i < count; ++i) res.files[i].resize(res.statuses[i] == APT_OK ? nouts[i] : 0);
+    return rc;
+}
 // The reference CLI's job: WAV in, PNG file out
 inline void decode_wav_png(const std::string &input, const std::string &output, const config::Settings &settings, bool sync,
                            const apt_process_settings &ps, const apt_png_settings &png = default_settings()) {

@@ -94,6 +94,16 @@ class CPngSettings(C.Structure):
     _fields_ = [("filter", C.c_int), ("matches", C.c_int), ("block_bytes", C.c_uint32), ("rgb_from_rgba", C.c_int)]
 
 
+class CPngGroupImage(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("stream_offset", "stream_bytes", "out_offset", "out_bytes", "bound")] + \
+               [(n, C.c_uint32) for n in ("first_row", "first_span", "first_block", "blocks", "first_chunk", "pad")]
+
+
+class CPngGroupInfo(C.Structure):
+    _fields_ = [("stream_bytes", C.c_uint64), ("out_bytes", C.c_uint64)] + \
+               [(n, C.c_uint32) for n in ("rows", "spans", "blocks", "chunks")]
+
+
 STATUS_CB = C.CFUNCTYPE(None, C.c_float, C.c_char_p, C.c_void_p)
 
 # name -> (restype, argtypes); every symbol include/aptb200.h declares.
@@ -206,6 +216,14 @@ SIGNATURES = {
     "apt_decoder_set_png_mode": (C.c_int, [C.c_void_p, C.POINTER(CPngSettings)]),
     "apt_decode_wav_png": (C.c_int, [C.c_char_p, C.c_char_p, C.POINTER(CSettings), C.c_int, C.POINTER(CProcessSettings),
                                      C.POINTER(CPngSettings), C.POINTER(CImageInfo)]),
+    "apt_decode_batch_image": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, _u64p, C.c_int, C.c_uint32, C.POINTER(CSettings),
+                                         C.c_int, C.POINTER(CProcessSettings), C.POINTER(CPngSettings),
+                                         C.POINTER(C.c_void_p), _u64p, _u64p, C.POINTER(CImageInfo), C.POINTER(C.c_int),
+                                         C.POINTER(C.c_int), C.c_int, C.c_int]),
+    "apt_png_encode_batch": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_uint32), C.c_uint32, C.c_uint32, C.c_int,
+                                       C.POINTER(CPngSettings), C.POINTER(C.c_void_p), _u64p, _u64p]),
+    "apt_png_group_plan": (C.c_int, [C.c_uint32, C.c_int, C.POINTER(CPngSettings), C.POINTER(C.c_uint32), C.c_uint32,
+                                     C.POINTER(CPngGroupInfo), C.POINTER(CPngGroupImage), C.c_size_t]),
     "apt_stream_set_process_mode": (C.c_int, [C.c_void_p, C.POINTER(CProcessSettings), C.c_uint64]),
     "apt_stream_set_png_mode": (C.c_int, [C.c_void_p, C.POINTER(CPngSettings)]),
     "apt_stream_finish_image": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, _u64p, C.c_void_p, C.c_uint64, _u64p,

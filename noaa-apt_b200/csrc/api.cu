@@ -484,9 +484,10 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
     // length is known
     const uint64_t per_px = post ? post->bpp : 1;
     const bool png = post && d->png_active;
+    const bool keep = post && d->keep_image && host;
     if (png && d->png.rgb_from_rgba && per_px != 4) return fail(APT_ERR_BAD_ARG, "rgb_from_rgba needs RGBA process output");
     if (png && !out) return fail(APT_ERR_BAD_ARG, "null output");
-    if (!png && (!out || cap < need * per_px))
+    if (!png && !keep && (!out || cap < need * per_px))
         return fail(APT_ERR_CAPACITY, "output needs room for %llu %s", (unsigned long long)(need * per_px), post ? "bytes" : "floats");
     d->job_png = png;
     if (post) {
@@ -509,7 +510,7 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
     d->job_in_pageable = d->job_out_pageable = false;
     if (host) {
         d->job_in_pageable = is_pageable(signal);
-        d->job_out_pageable = !png && is_pageable(out);   // PNG mode copies the file straight into `out` at wait()
+        d->job_out_pageable = !png && !keep && is_pageable(out);   // PNG mode copies the file straight into `out` at wait()
         if ((d->job_in_pageable || d->job_out_pageable) && !d->stager && !getenv("APTB200_NO_STAGER")) {
             int threads = 8;
             if (const char *e = getenv("APTB200_COPY_THREADS")) threads = std::max(1, atoi(e));
@@ -553,7 +554,7 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
     int st = decoder_enqueue(d, dev_in, format, n, sync, rows_dst, host_chunked);
     // the rows come back with the job: when syncing n_rows is only known on the device, so the copy covers the bound
     // (at most one row more than is produced)
-    d->job_d2h_floats = !host || png ? 0 : d->job_sync ? need : d->job_fixed_out;
+    d->job_d2h_floats = !host || png || keep ? 0 : d->job_sync ? need : d->job_fixed_out;
     if (st == APT_OK) st = enqueue_job_tail(d);
     if (st != APT_OK) {
         cudaStreamSynchronize(d->stream);
@@ -586,7 +587,8 @@ int png_job(apt_decoder *d, uint64_t rows, uint64_t *bytes) {
     APT_TRY(make_png(kPxPerRow, static_cast<uint32_t>(rows), d->post_plan->bpp, &d->png, p));
     if (!d->h_png) APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&d->h_png), sizeof(PngCtl), cudaHostAllocDefault));
     DecoderHook hook(d);
-    APT_TRY(png_encode_device(LaunchCtx{d->stream, d->sm_count}, p, d->png_work, d->d_out8, &hook));
+    const unsigned char *px = d->d_out8;
+    APT_TRY(png_encode_device(LaunchCtx{d->stream, d->sm_count}, &p, &px, 1, d->png_work, &hook));
     APT_CUDA(cudaMemcpyAsync(d->h_png, d->png_work.ctl, sizeof(PngCtl), cudaMemcpyDeviceToHost, d->stream));
     APT_CUDA(cudaStreamSynchronize(d->stream));
     const uint64_t total = d->h_png->total;
@@ -1342,15 +1344,200 @@ extern "C" int apt_decoder_poll(apt_decoder *d) {
     return 1;   // finished (or failed: wait() reports it)
 }
 
+namespace {
+
+// The image side of apt_decode_batch_image: every decoder runs in process mode; with PNG output each feeder also has a
+// PngFeed.
+struct BatchImage {
+    const apt_process_settings *ps;
+    int bpp;
+    const apt_png_settings *png;   // nullptr: the images go to the caller
+    std::vector<apt_image_info> *infos;
+};
+
+// One feeder's PNG side.  The decoders keep their images on the device (keep_image); at reap the image is copied into a
+// free slot of a fixed pool, so the decoder takes its next recording at once.  When the encoder is idle, every ready
+// slot forms one group, encoded on the feeder's own stream after the events of the copies; the feeder reads the
+// lengths back once the encode's event has fired and copies each file to its caller.
+struct PngFeed {
+    int bpp = 1;
+    apt_png_settings png{};
+    u64 slot_bytes = 0;
+    unsigned char *pool = nullptr;
+    std::vector<int> job;            // per slot: the recording, -1 free
+    std::vector<u32> rows;
+    std::vector<char> encoding;      // per slot: part of the encode in flight
+    std::vector<cudaEvent_t> ready;  // per slot: the copy into it has finished
+    std::vector<int> group;          // slots of the encode in flight, in the order of its images
+    cudaStream_t stream = nullptr;
+    cudaEvent_t done = nullptr;
+    int sms = 1;
+    PngWork w;
+    PngCtl *h_ctl = nullptr;
+    size_t h_ctl_cap = 0;
+    size_t max_group = SIZE_MAX;     // the largest group whose workspace could be allocated
+
+    // `slots` slots of `bytes` each; fewer when the device is short of memory, at least one
+    int init(int device, int slots, u64 bytes) {
+        APT_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+        APT_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+        APT_CUDA(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
+        slot_bytes = (bytes + 255) & ~255ull;
+        for (;; slots /= 2) {
+            if (cudaMalloc(&pool, slots * slot_bytes) == cudaSuccess) break;
+            cudaGetLastError();
+            pool = nullptr;
+            if (slots == 1) return fail(APT_ERR_CUDA, "out of device memory for the PNG image pool");
+        }
+        job.assign(slots, -1);
+        rows.assign(slots, 0);
+        encoding.assign(slots, 0);
+        ready.assign(slots, nullptr);
+        for (auto &e : ready) APT_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        return APT_OK;
+    }
+    ~PngFeed() {
+        if (stream) cudaStreamSynchronize(stream);
+        w.release();
+        if (pool) cudaFree(pool);
+        for (auto e : ready)
+            if (e) cudaEventDestroy(e);
+        if (done) cudaEventDestroy(done);
+        if (h_ctl) cudaFreeHost(h_ctl);
+        if (stream) cudaStreamDestroy(stream);
+    }
+    int free_slot() const {
+        for (size_t k = 0; k < job.size(); ++k)
+            if (job[k] < 0) return static_cast<int>(k);
+        return -1;
+    }
+    bool busy() const { return !group.empty(); }
+    bool pending() const { return std::any_of(job.begin(), job.end(), [](int j) { return j >= 0; }); }
+    bool any_ready() const {
+        for (size_t k = 0; k < job.size(); ++k)
+            if (job[k] >= 0 && !encoding[k]) return true;
+        return false;
+    }
+    // the image of decoder d's finished job (in d_out8) into a free slot, on the decoder's stream
+    int put(apt_decoder *d, int jb, u64 bytes) {
+        const int k = free_slot();
+        if (k < 0) return fail(APT_ERR_CUDA, "no free slot in the PNG image pool");
+        if (bytes > slot_bytes) return fail(APT_ERR_CUDA, "image of %llu bytes exceeds the pool's slots", (unsigned long long)bytes);
+        APT_CUDA(cudaMemcpyAsync(pool + k * slot_bytes, d->d_out8, bytes, cudaMemcpyDeviceToDevice, d->stream));
+        APT_CUDA(cudaEventRecord(ready[k], d->stream));
+        job[k] = jb;
+        rows[k] = static_cast<u32>(bytes / (static_cast<u64>(kPxPerRow) * bpp));
+        return APT_OK;
+    }
+    // one encode over every ready slot, at most max_group of them
+    void launch(std::vector<int> &status) {
+        std::vector<int> slots;
+        std::vector<PngPlan> plans;
+        for (size_t k = 0; k < job.size(); ++k) {
+            if (job[k] < 0 || encoding[k]) continue;
+            PngPlan p;
+            const int st = make_png(kPxPerRow, rows[k], bpp, &png, p);
+            if (st != APT_OK) {
+                status[job[k]] = st;
+                job[k] = -1;
+                continue;
+            }
+            slots.push_back(static_cast<int>(k));
+            plans.push_back(p);
+        }
+        std::vector<const unsigned char *> px;
+        for (int k : slots) {
+            px.push_back(pool + k * slot_bytes);
+            if (cudaStreamWaitEvent(stream, ready[k], 0) != cudaSuccess) {
+                for (int j : slots) {
+                    status[job[j]] = fail(APT_ERR_CUDA, "CUDA error: %s", cudaGetErrorString(cudaGetLastError()));
+                    job[j] = -1;
+                }
+                return;
+            }
+        }
+        // the workspace first: while it cannot be allocated the group is halved, and the largest group that fitted is
+        // remembered so that later launches do not try a larger one again
+        size_t g = std::min(slots.size(), max_group);
+        for (;;) {
+            PngLayout lay;
+            int st = png_layout(plans.data(), px.data(), static_cast<u32>(g), lay);
+            if (st == APT_OK) st = w.reserve(lay);
+            if (st == APT_OK) break;
+            cudaGetLastError();
+            w.release();
+            if (g == 1) {   // not even one image fits: that recording fails, the rest wait for the next launch
+                status[job[slots[0]]] = st;
+                job[slots[0]] = -1;
+                return;
+            }
+            g /= 2;         // a smaller group: the rest stay ready for the next launch
+            max_group = g;
+        }
+        int st = png_encode_device(LaunchCtx{stream, sms}, plans.data(), px.data(), static_cast<u32>(g), w, nullptr);
+        if (st == APT_OK && h_ctl_cap < g) {
+            if (h_ctl) cudaFreeHost(h_ctl);
+            h_ctl = nullptr;
+            h_ctl_cap = 0;
+            st = cudaHostAlloc(reinterpret_cast<void **>(&h_ctl), g * sizeof(PngCtl), cudaHostAllocDefault) == cudaSuccess
+                     ? APT_OK : fail(APT_ERR_CUDA, "out of pinned host memory");
+            if (st == APT_OK) h_ctl_cap = g;
+        }
+        if (st == APT_OK)
+            st = cudaMemcpyAsync(h_ctl, w.ctl, g * sizeof(PngCtl), cudaMemcpyDeviceToHost, stream) == cudaSuccess &&
+                         cudaEventRecord(done, stream) == cudaSuccess
+                     ? APT_OK : fail(APT_ERR_CUDA, "CUDA error: %s", cudaGetErrorString(cudaGetLastError()));
+        if (st != APT_OK) {   // the encode itself failed: its recordings have that status
+            cudaStreamSynchronize(stream);
+            for (size_t i = 0; i < g; ++i) {
+                status[job[slots[i]]] = st;
+                job[slots[i]] = -1;
+            }
+            return;
+        }
+        group.assign(slots.begin(), slots.begin() + g);
+        for (int k : group) encoding[k] = 1;
+    }
+    // waits for the encode in flight and copies each file to its caller (or reports the capacity it needs)
+    void finish(uint8_t *const *outs, const uint64_t *caps, uint64_t *nouts, std::vector<int> &status) {
+        cudaError_t e = cudaEventSynchronize(done);
+        for (size_t i = 0; i < group.size(); ++i) {
+            const int k = group[i], jb = job[k];
+            if (e != cudaSuccess) {
+                status[jb] = fail(APT_ERR_CUDA, "CUDA error: %s", cudaGetErrorString(e));
+                continue;
+            }
+            const uint64_t total = h_ctl[i].total;
+            nouts[jb] = total;
+            if (total > caps[jb]) {
+                status[jb] = fail(APT_ERR_CAPACITY, "output needs room for %llu PNG bytes", (unsigned long long)total);
+                continue;
+            }
+            e = cudaMemcpyAsync(outs[jb], w.out + w.lay.img[i].out, total, cudaMemcpyDeviceToHost, stream);
+            status[jb] = e == cudaSuccess ? APT_OK : fail(APT_ERR_CUDA, "CUDA error: %s", cudaGetErrorString(e));
+        }
+        const cudaError_t es = cudaStreamSynchronize(stream);
+        for (size_t i = 0; i < group.size(); ++i) {
+            const int k = group[i];
+            if (es != cudaSuccess && status[job[k]] == APT_OK)
+                status[job[k]] = fail(APT_ERR_CUDA, "CUDA error: %s", cudaGetErrorString(es));
+            job[k] = -1;
+            encoding[k] = 0;
+        }
+        group.clear();
+    }
+};
+
+// Pool slots per feeder with PNG output: enough to group the images of several rounds of decoders, bounded so that the
+// pool's memory does not grow with the batch.
+constexpr int kPngPoolSlots = 16;
+
 // One feeder thread per device: binds itself to the device's NUMA node, owns `streams_per_device` decoders and one copy
 // stager, keeps every decoder busy and reaps the jobs in the order they complete.  Nothing is shared between devices.
-extern "C" int apt_decode_batch(const void *const *signals, int format, const uint64_t *lens, int count,
-                                uint32_t input_rate, const apt_settings *s, int sync, float *const *outs,
-                                const uint64_t *caps, uint64_t *nouts, int *statuses, const int *devices, int ndevices,
-                                int streams_per_device) {
-    if (!signals || !lens || !s || !outs || !caps || !nouts || count < 0)
-        return fail(APT_ERR_BAD_ARG, "null argument");
-    if (count == 0) return APT_OK;
+// img == nullptr: f32 rows (apt_decode_batch); else process mode, and with img->png the feeder's PngFeed.
+int run_batch(const void *const *signals, int format, const uint64_t *lens, int count, uint32_t input_rate, const apt_settings *s,
+              int sync, const BatchImage *img, void *const *outs, const uint64_t *caps, uint64_t *nouts, int *statuses,
+              const int *devices, int ndevices, int streams_per_device) {
     APT_TRY(require_device());
     int default_device = 0;
     if (!devices || ndevices <= 0) {
@@ -1378,10 +1565,17 @@ extern "C" int apt_decode_batch(const void *const *signals, int format, const ui
         std::vector<int> job_of;
         int next = g;                                  // recording i -> device i % G   (SURVEY.md §8e)
         int in_flight = 0;
+        std::unique_ptr<PngFeed> feed;
         auto reap = [&](size_t k) {
             uint64_t got = 0;
-            const int st = apt_decoder_wait(decs[k], &got);
+            int st = apt_decoder_wait(decs[k], &got);
             const int job = job_of[k];
+            if (img && st == APT_OK) (*img->infos)[job] = decs[k]->last_image;
+            if (feed && st == APT_OK) {
+                st = feed->put(decs[k], job, got);
+                got = 0;                               // the file's length comes with its encode
+                if (st == APT_OK) st = APT_ERR_CUDA;   // until the encode reports
+            }
             nouts[job] = got;
             local_status[job] = st;
             job_of[k] = -1;
@@ -1392,7 +1586,32 @@ extern "C" int apt_decode_batch(const void *const *signals, int format, const ui
             messages[g] = apt_last_error();
             for (; next < count; next += ndevices) local_status[next] = st;
         };
-        while (next < count || in_flight > 0) {
+        if (img && img->png && next < count) {
+            Plan p;
+            uint64_t bound = 0;
+            int st = make_plan(input_rate, *s, p);
+            if (st == APT_OK) st = cudaSetDevice(device) == cudaSuccess ? APT_OK : fail(APT_ERR_CUDA, "cannot select device %d", device);
+            if (st == APT_OK) {
+                bound = std::max<uint64_t>(plan_out_bound(p, max_len), kPxPerRow) * img->bpp;
+                feed.reset(new PngFeed());
+                feed->bpp = img->bpp;
+                feed->png = *img->png;
+                st = feed->init(device, std::min(kPngPoolSlots, (count - g + ndevices - 1) / ndevices), bound);
+            }
+            if (st != APT_OK) {
+                feed.reset();
+                fail_rest(st);
+            }
+        }
+        while (next < count || in_flight > 0 || (feed && feed->pending())) {
+            if (feed && feed->busy() && cudaEventQuery(feed->done) != cudaErrorNotReady) {
+                feed->finish(reinterpret_cast<uint8_t *const *>(outs), caps, nouts, local_status);
+                continue;
+            }
+            if (feed && !feed->busy() && feed->any_ready()) {
+                feed->launch(local_status);
+                continue;
+            }
             // a free decoder takes the next recording of this device
             size_t free_k = decs.size();
             for (size_t k = 0; k < decs.size(); ++k)
@@ -1400,7 +1619,14 @@ extern "C" int apt_decode_batch(const void *const *signals, int format, const ui
             if (next < count && (free_k < decs.size() || static_cast<int>(decs.size()) < streams_per_device)) {
                 if (free_k == decs.size()) {
                     apt_decoder *d = cache_take(device, input_rate, *s, max_len);     // parked by an earlier call
-                    const int st = d ? APT_OK : apt_decoder_create(device, input_rate, s, max_len, &d);
+                    int st = d ? APT_OK : apt_decoder_create(device, input_rate, s, max_len, &d);
+                    if (st == APT_OK && img) {
+                        st = apt_decoder_set_process_mode(d, img->ps);
+                        if (st != APT_OK) {
+                            if (use_cache) cache_put_multi(device, input_rate, *s, d);
+                            else apt_decoder_destroy(d);
+                        }
+                    }
                     if (st != APT_OK) {
                         if (decs.empty()) { fail_rest(st); continue; }
                         streams_per_device = static_cast<int>(decs.size());   // out of memory: make do with what exists
@@ -1418,13 +1644,15 @@ extern "C" int apt_decode_batch(const void *const *signals, int format, const ui
                     } else {
                         d->stager = decs[0]->stager;
                     }
-                    d->post_plan.reset();
+                    if (!img) d->post_plan.reset();
+                    d->keep_image = feed != nullptr;
                     decs.push_back(d);
                     job_of.push_back(-1);
                 }
                 const int job = next;
                 next += ndevices;
-                const int st = apt_decoder_submit_host(decs[free_k], signals[job], format, lens[job], sync, outs[job], caps[job]);
+                const int st = apt_decoder_submit_host(decs[free_k], signals[job], format, lens[job], sync,
+                                                       static_cast<float *>(outs[job]), caps[job]);
                 if (st == APT_OK) {
                     job_of[free_k] = job;
                     ++in_flight;
@@ -1433,22 +1661,32 @@ extern "C" int apt_decode_batch(const void *const *signals, int format, const ui
                 }
                 continue;
             }
-            // every decoder is busy (or nothing is left to submit): take whichever job has finished, else the oldest
-            bool reaped = false;
-            for (size_t k = 0; k < decs.size() && !reaped; ++k)
-                if (job_of[k] >= 0 && apt_decoder_poll(decs[k])) { reap(k); reaped = true; }
-            if (!reaped) {
-                size_t oldest = decs.size();
-                for (size_t k = 0; k < decs.size(); ++k)
-                    if (job_of[k] >= 0 && (oldest == decs.size() || job_of[k] < job_of[oldest])) oldest = k;
-                if (oldest < decs.size()) reap(oldest);
+            if (in_flight > 0 && (!feed || feed->free_slot() >= 0)) {
+                // every decoder is busy (or nothing is left to submit): take whichever job has finished, else the oldest
+                bool reaped = false;
+                for (size_t k = 0; k < decs.size() && !reaped; ++k)
+                    if (job_of[k] >= 0 && apt_decoder_poll(decs[k])) { reap(k); reaped = true; }
+                if (!reaped) {
+                    size_t oldest = decs.size();
+                    for (size_t k = 0; k < decs.size(); ++k)
+                        if (job_of[k] >= 0 && (oldest == decs.size() || job_of[k] < job_of[oldest])) oldest = k;
+                    if (oldest < decs.size()) reap(oldest);
+                }
+                continue;
             }
+            if (feed && feed->busy()) feed->finish(reinterpret_cast<uint8_t *const *>(outs), caps, nouts, local_status);   // the pool is full
         }
         for (auto *d : decs) {
             d->stager = d->own_stager.get();           // nullptr unless it owns one: never keep a pointer into another decoder
+            if (img) {
+                cudaStreamSynchronize(d->stream);      // the last copy into the pool has left d_out8
+                d->post_plan.reset();
+                d->keep_image = false;
+            }
             if (use_cache) cache_put_multi(device, input_rate, *s, d);
             else apt_decoder_destroy(d);
         }
+        feed.reset();
     };
 
     if (ndevices == 1) {
@@ -1466,4 +1704,50 @@ extern "C" int apt_decode_batch(const void *const *signals, int format, const ui
     for (int g = 0; g < ndevices; ++g)
         if (fatal[g] != APT_OK) return fail(fatal[g], "device %d: %s", devices[g], messages[g].c_str());
     return first_error;
+}
+
+}  // namespace
+
+extern "C" int apt_decode_batch(const void *const *signals, int format, const uint64_t *lens, int count,
+                                uint32_t input_rate, const apt_settings *s, int sync, float *const *outs,
+                                const uint64_t *caps, uint64_t *nouts, int *statuses, const int *devices, int ndevices,
+                                int streams_per_device) {
+    if (!signals || !lens || !s || !outs || !caps || !nouts || count < 0)
+        return fail(APT_ERR_BAD_ARG, "null argument");
+    if (count == 0) return APT_OK;
+    return run_batch(signals, format, lens, count, input_rate, s, sync, nullptr, reinterpret_cast<void *const *>(outs), caps, nouts,
+                     statuses, devices, ndevices, streams_per_device);
+}
+
+extern "C" int apt_decode_batch_image(const void *const *signals, int format, const uint64_t *lens, int count,
+                                      uint32_t input_rate, const apt_settings *s, int sync, const apt_process_settings *ps,
+                                      const apt_png_settings *png, uint8_t *const *outs, const uint64_t *caps, uint64_t *nouts,
+                                      apt_image_info *infos, int *statuses, const int *devices, int ndevices,
+                                      int streams_per_device) {
+    if (!signals || !lens || !s || !outs || !caps || !nouts || count < 0) return fail(APT_ERR_BAD_ARG, "null argument");
+    PostPlan plan;
+    APT_TRY(process_plan(ps, plan));
+    if (png) APT_TRY(check_png_settings(png, plan.bpp));
+    {
+        Plan p;
+        APT_TRY(make_plan(input_rate, *s, p));
+        if (!p.work_multiple) {
+            if (sync) return fail(APT_ERR_WORK_RATE, "work_rate is not multiple of FINAL_RATE");
+            return fail(APT_ERR_BAD_ARG, "the image stage needs rows of 2080 pixels (work_rate multiple of 4160)");
+        }
+    }
+    if (format != APT_F32 && format != APT_PCM16) return fail(APT_ERR_BAD_ARG, "unknown sample format %d", format);
+    for (int i = 0; i < count; ++i)
+        if (!outs[i]) return fail(APT_ERR_BAD_ARG, "null output of recording %d", i);
+    if (count == 0) return APT_OK;
+    std::vector<apt_image_info> got(count);
+    std::vector<int> st(count, APT_ERR_CUDA);
+    const BatchImage bi{ps, plan.bpp, png, &got};
+    const int rc = run_batch(signals, format, lens, count, input_rate, s, sync, &bi, reinterpret_cast<void *const *>(outs), caps,
+                             nouts, st.data(), devices, ndevices, streams_per_device);
+    for (int i = 0; i < count; ++i) {
+        if (statuses) statuses[i] = st[i];
+        if (infos) infos[i] = st[i] == APT_OK ? got[i] : apt_image_info{};   // as the one-shot calls: info of a success only
+    }
+    return rc;
 }

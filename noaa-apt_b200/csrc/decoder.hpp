@@ -120,6 +120,9 @@ struct apt_decoder {
     aptb200::PngWork png_work;
     aptb200::PngCtl *h_png = nullptr;   // pinned copy of the encoder's control block
     bool job_png = false;
+    // image left on the device: a host job of image / process mode keeps its image in d_out8 and copies nothing back
+    // (the batch's PNG feeder takes it from there); out and cap are not used
+    bool keep_image = false;
 
     // apt_decode_iq (allocated on first use): the I/Q stage's tables for iq_settings, one chunk's I/Q window and the
     // audio the FM kernel writes, which is the input of the decode job

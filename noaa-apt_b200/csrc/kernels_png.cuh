@@ -29,18 +29,11 @@ __constant__ u32 c_png_crc_table[256];
 __constant__ u32 c_png_x2n[32];                               // x^(2^k) mod P, reflected (zlib's x2n_table)
 
 // Bounds-checking build (-DAPTB200_PNG_CHECK, tools/png_bounds_check.sh): every global and shared index of the encoder is
-// checked against its buffer's size; a violation sets a bit of g_png_violation (no fault) and the encode then fails with
-// APT_ERR_CUDA.  Ordinary builds compile the checks away.
-struct PngLimits {
-    u64 f_bytes;     // filtered stream incl. padding
-    u64 n;           // positions (lcode, dist, flag)
-    u64 px_bytes;    // input pixels
-    u64 out_bytes;   // output buffer
-    u32 nblocks;
-};
+// checked against its image's region of the buffer (PngImage: n + 16 bytes of f, n positions, height * width * in_ch
+// pixels, out_bytes of out, nblocks blocks); a violation sets a bit of g_png_violation (no fault) and the encode then
+// fails with APT_ERR_CUDA.  Ordinary builds compile the checks away.
 #ifdef APTB200_PNG_CHECK
 __device__ u32 g_png_violation;
-__constant__ PngLimits c_png_lim;
 #define PNG_CHECK(cond, bit)                                                  \
     do {                                                                      \
         if (!(cond)) atomicOr(&::aptb200::g_png_violation, 1u << (bit));      \
@@ -50,6 +43,18 @@ __constant__ PngLimits c_png_lim;
     do {                     \
     } while (0)
 #endif
+
+// The image of a global index (row, span, block or CRC chunk): the last image whose first index is <= key.
+template <u32 PngImage::*First>
+__device__ __forceinline__ u32 png_image_of(const PngImage *__restrict__ im, u32 g, u32 key) {
+    u32 lo = 0, hi = g;
+    while (hi - lo > 1) {
+        const u32 mid = (lo + hi) / 2;
+        if (im[mid].*First <= key) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}
 
 __device__ __forceinline__ u32 png_dist_sym(u32 d) {   // d >= 1
     const u32 dd = d - 1;
@@ -66,19 +71,25 @@ __device__ __forceinline__ int png_paeth(int a, int b, int c) {
     return (pa <= pb && pa <= pc) ? a : (pb <= pc ? b : c);
 }
 
-// One warp per row: the five residual sums, the winner (ties to the lower type) and the row of F it gives.
+// One warp per row of any image of the group: the five residual sums, the winner (ties to the lower type) and the row of
+// F it gives; the warp of an image's last row also zeroes the 16 bytes of padding after its stream.
 // CIN: channels of the input, C: channels written (C = 3, CIN = 4 drops alpha).
 template <int CIN, int C>
-__global__ void __launch_bounds__(256) k_png_filter(const unsigned char *__restrict__ px, u32 width, u32 height, int fixed,
-                                                    unsigned char *__restrict__ f) {
+__global__ void __launch_bounds__(256) k_png_filter(const PngImage *__restrict__ im, u32 g, u32 rows, u32 width, int fixed,
+                                                    unsigned char *__restrict__ f_all) {
     const u32 lane = threadIdx.x & 31;
-    const u32 r = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
-    if (r >= height) return;
+    const u32 gr = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
+    if (gr >= rows) return;
+    const PngImage I = im[png_image_of<&PngImage::row0>(im, g, gr)];
+    const u32 r = gr - I.row0;
+    const unsigned char *__restrict__ px = I.px;
+    unsigned char *__restrict__ f = f_all + I.pos;
     const u64 R = static_cast<u64>(width) * C;
     const u64 rin = static_cast<u64>(width) * CIN;
+    if (r + 1 == I.height && lane < 16) f[I.n + lane] = 0;
     auto get = [&](u32 rr, u64 x) -> int {
         const u64 k = CIN == C ? rr * rin + x : rr * rin + (x / 3) * 4 + x % 3;
-        PNG_CHECK(k < c_png_lim.px_bytes, 0);
+        PNG_CHECK(k < static_cast<u64>(I.height) * rin, 0);
         return px[k];
     };
     auto res = [&](int t, u64 x) -> u32 {
@@ -120,28 +131,34 @@ __global__ void __launch_bounds__(256) k_png_filter(const unsigned char *__restr
             if (s[t] < s[type]) type = t;
     }
     unsigned char *row = f + static_cast<u64>(r) * (R + 1);
-    PNG_CHECK(static_cast<u64>(r + 1) * (R + 1) <= c_png_lim.n, 1);
+    PNG_CHECK(static_cast<u64>(r + 1) * (R + 1) <= I.n, 1);
     if (lane == 0) row[0] = static_cast<unsigned char>(type);
     for (u64 x = lane; x < R; x += 32) row[1 + x] = static_cast<unsigned char>(res(type, x));
 }
 
 // ------------------------------------------------------------------------------------------------------ 3. matches
 
-__device__ __forceinline__ u32 png_ld32(const unsigned char *f, u32 pos) {   // 4 bytes at any offset (F is padded)
+__device__ __forceinline__ u32 png_ld32(const unsigned char *f, u32 pos, u32 n) {   // 4 bytes at any offset (F is padded)
     const u32 *w = reinterpret_cast<const u32 *>(f + (pos & ~3u));
-    PNG_CHECK((pos & ~3u) + 8ull <= c_png_lim.f_bytes, 2);
+    PNG_CHECK((pos & ~3u) + 8ull <= n + 16ull, 2);
     return __funnelshift_r(w[0], w[1], (pos & 3u) * 8);
 }
 
-// One warp per span of kPngSpan positions.  It walks the window before the span and the span itself 32 positions at a
+// One warp per span of kPngSpan positions of one image (each image's positions are cut into spans of its own).  It walks the window before the span and the span itself 32 positions at a
 // time with a head table (last position of each hash, as a u16 offset from the walk's start) in shared memory; lanes
 // with the same hash in one step resolve among themselves with __match_any_sync.  Every position with a hash updates the
 // head, so m(i) is the same whatever the parse does.  Positions of the span get lcode (0 or l - 3) and dist (d - 1).
-__global__ void __launch_bounds__(32) k_png_match(const unsigned char *__restrict__ f, u32 n, u32 block_bytes,
-                                                  unsigned char *__restrict__ lcode, uint16_t *__restrict__ dist) {
+__global__ void __launch_bounds__(32) k_png_match(const PngImage *__restrict__ im, u32 g, const unsigned char *__restrict__ f_all,
+                                                  u32 block_bytes, unsigned char *__restrict__ lcode_all,
+                                                  uint16_t *__restrict__ dist_all) {
     extern __shared__ uint16_t head[];   // 32768 entries
+    const PngImage &I = im[png_image_of<&PngImage::span0>(im, g, blockIdx.x)];
+    const u32 n = I.n;
+    const unsigned char *__restrict__ f = f_all + I.pos;
+    unsigned char *__restrict__ lcode = lcode_all + I.pos;
+    uint16_t *__restrict__ dist = dist_all + I.pos;
     const u32 lane = threadIdx.x;
-    const u32 s = blockIdx.x * kPngSpan;
+    const u32 s = (blockIdx.x - I.span0) * kPngSpan;
     const u32 e = min(n, s + kPngSpan);
     const u32 b = s > kPngWindow ? s - kPngWindow : 0;
     for (u32 k = lane; k < 32768; k += 32) head[k] = 0xFFFFu;
@@ -169,7 +186,7 @@ __global__ void __launch_bounds__(32) k_png_match(const unsigned char *__restric
             const u32 cap = min(kPngMaxMatch, bend - i);
             const u32 j = static_cast<u32>(cand);
             while (len < cap) {
-                const u32 x = png_ld32(f, j + len) ^ png_ld32(f, i + len);
+                const u32 x = png_ld32(f, j + len, n) ^ png_ld32(f, i + len, n);
                 if (x) {
                     len += (__ffs(x) - 1) >> 3;
                     break;
@@ -178,7 +195,7 @@ __global__ void __launch_bounds__(32) k_png_match(const unsigned char *__restric
             }
             len = min(len, cap);
         }
-        PNG_CHECK(i < c_png_lim.n && (len < kPngMinMatch || i + len <= c_png_lim.n), 3);
+        PNG_CHECK(i < n && (len < kPngMinMatch || i + len <= n), 3);
         if (len >= kPngMinMatch) {
             lcode[i] = static_cast<unsigned char>(len - 3);
             dist[i] = static_cast<uint16_t>(i - static_cast<u32>(cand) - 1);
@@ -190,19 +207,25 @@ __global__ void __launch_bounds__(32) k_png_match(const unsigned char *__restric
 
 // ------------------------------------------------------------------------------------------------------ 4. parse
 
-// One CTA per deflate block: thread 0 walks the greedy jump chain over the block's lcode in shared memory and marks the
+// One CTA per deflate block of the group: thread 0 walks the greedy jump chain over the block's lcode in shared memory and marks the
 // token positions; then the block's literal/length and distance histograms (end of block counted).
-__global__ void __launch_bounds__(256) k_png_parse(const unsigned char *__restrict__ f, const unsigned char *__restrict__ lcode,
-                                                   const uint16_t *__restrict__ dist, u32 n, u32 block_bytes,
-                                                   unsigned char *__restrict__ flag, u32 *__restrict__ hist) {
+__global__ void __launch_bounds__(256) k_png_parse(const PngImage *__restrict__ im, u32 g, const unsigned char *__restrict__ f_all,
+                                                   const unsigned char *__restrict__ lcode_all, const uint16_t *__restrict__ dist_all,
+                                                   u32 block_bytes, unsigned char *__restrict__ flag_all, u32 *__restrict__ hist) {
     extern __shared__ unsigned char sl[];   // block_bytes
     __shared__ u32 h[kPngLit + kPngDist];
-    const u32 start = blockIdx.x * block_bytes;
+    const PngImage &I = im[png_image_of<&PngImage::blk0>(im, g, blockIdx.x)];
+    const u32 n = I.n;
+    const unsigned char *__restrict__ f = f_all + I.pos;
+    const unsigned char *__restrict__ lcode = lcode_all + I.pos;
+    const uint16_t *__restrict__ dist = dist_all + I.pos;
+    unsigned char *__restrict__ flag = flag_all + I.pos;
+    const u32 start = (blockIdx.x - I.blk0) * block_bytes;
     const u32 len = min(block_bytes, n - start);
-    PNG_CHECK(start + len <= c_png_lim.n && blockIdx.x < c_png_lim.nblocks && start + len + 16 <= c_png_lim.f_bytes, 13);
+    PNG_CHECK(start + len <= n && blockIdx.x - I.blk0 < I.nblocks, 13);
     for (u32 k = threadIdx.x; k < kPngLit + kPngDist; k += blockDim.x) h[k] = 0;
     const u32 nw = len / 4;
-    const u32 *src = reinterpret_cast<const u32 *>(lcode + start);   // start is a multiple of block_bytes: aligned
+    const u32 *src = reinterpret_cast<const u32 *>(lcode + start);   // pos and start are multiples of 4: aligned
     for (u32 k = threadIdx.x; k < nw; k += blockDim.x) reinterpret_cast<u32 *>(sl)[k] = src[k];
     for (u32 k = 4 * nw + threadIdx.x; k < len; k += blockDim.x) sl[k] = lcode[start + k];
     __syncthreads();
@@ -210,7 +233,7 @@ __global__ void __launch_bounds__(256) k_png_parse(const unsigned char *__restri
         unsigned char *fl = flag + start;
         u32 p = 0;
         while (p < len) {
-            PNG_CHECK(start + p < c_png_lim.n && p < block_bytes, 4);
+            PNG_CHECK(start + p < n && p < block_bytes, 4);
             fl[p] = 1;
             const u32 c = sl[p];
             p += c ? c + 3 : 1;
@@ -356,9 +379,10 @@ struct PngBits {   // plain (non-atomic) LSB-first writer into zeroed words
     }
 };
 
-// One warp per block: the three trees, the header bits and the block's bit count.
-__global__ void __launch_bounds__(32) k_png_huffman(const u32 *__restrict__ hist, u32 nblocks, u32 *__restrict__ codes,
-                                                    u32 *__restrict__ hdr, u32 *__restrict__ hdr_bits, u64 *__restrict__ bits) {
+// One warp per block of the group: the three trees, the header bits and the block's bit count.
+__global__ void __launch_bounds__(32) k_png_huffman(const PngImage *__restrict__ im, u32 g, const u32 *__restrict__ hist,
+                                                    u32 *__restrict__ codes, u32 *__restrict__ hdr, u32 *__restrict__ hdr_bits,
+                                                    u64 *__restrict__ bits) {
     __shared__ PngPmShared sh;
     __shared__ u32 fr[kPngLit + kPngDist];
     __shared__ unsigned char len[kPngLit + kPngDist];
@@ -430,7 +454,8 @@ __global__ void __launch_bounds__(32) k_png_huffman(const u32 *__restrict__ hist
         u32 hclen = kPngCl;
         while (hclen > 4 && cll[c_png_cl_order[hclen - 1]] == 0) --hclen;
         PngBits wr{hw, 0};
-        wr.put(blk + 1 == nblocks ? 1u : 0u, 1);
+        const PngImage &I = im[png_image_of<&PngImage::blk0>(im, g, blk)];
+        wr.put(blk + 1 == I.blk0 + I.nblocks ? 1u : 0u, 1);   // BFINAL on the image's last block
         wr.put(2u, 2);
         wr.put(hlit - 257, 5);
         wr.put(hdist - 1, 5);
@@ -458,10 +483,15 @@ __global__ void __launch_bounds__(32) k_png_huffman(const u32 *__restrict__ hist
     for (u32 k = lane; k < kPngHdrWords; k += 32) hdr[static_cast<u64>(blk) * kPngHdrWords + k] = hw[k];
 }
 
-// Exclusive scan of the block bit counts (one CTA of 1024 threads) and the stream's total.
-__global__ void __launch_bounds__(1024) k_png_scan(const u64 *__restrict__ bits, u32 nblocks, u64 *__restrict__ off,
-                                                   PngCtl *__restrict__ ctl) {
+// Segmented exclusive scan of the block bit counts, one CTA of 1024 threads per image, and each stream's total.
+__global__ void __launch_bounds__(1024) k_png_scan(const PngImage *__restrict__ im, const u64 *__restrict__ bits_all,
+                                                   u64 *__restrict__ off_all, PngCtl *__restrict__ ctl_all) {
     __shared__ u64 part[1024];
+    const PngImage &I = im[blockIdx.x];
+    const u32 nblocks = I.nblocks;
+    const u64 *__restrict__ bits = bits_all + I.blk0;
+    u64 *__restrict__ off = off_all + I.blk0;
+    PngCtl *__restrict__ ctl = ctl_all + blockIdx.x;
     const u32 t = threadIdx.x;
     const u32 per = (nblocks + 1023) / 1024;
     const u32 b0 = min(nblocks, t * per), b1 = min(nblocks, b0 + per);
@@ -493,12 +523,13 @@ struct PngOut {   // LSB-first writer into zeroed words shared with other thread
     u64 pos;      // bit position of acc's bit 0
     u64 acc;
     u32 nacc;
+    u64 lim;      // bytes of w (bounds-checking build)
     __device__ void flush_word(u32 v, u32 nb) {
         const u64 k = pos >> 5;
         const u32 sh = static_cast<u32>(pos & 31);
         if (nb < 32) v &= (1u << nb) - 1u;
         if (v) {
-            PNG_CHECK(4 * (k + (sh && (v >> (32 - sh)) ? 2 : 1)) <= c_png_lim.out_bytes, 7);
+            PNG_CHECK(4 * (k + (sh && (v >> (32 - sh)) ? 2 : 1)) <= lim, 7);
             atomicOr(&w[k], v << sh);
             if (sh && (v >> (32 - sh))) atomicOr(&w[k + 1], v >> (32 - sh));
         }
@@ -520,27 +551,37 @@ struct PngOut {   // LSB-first writer into zeroed words shared with other thread
     }
 };
 
-// One CTA per block, kPngEmitThreads / 32 warps, each owning a contiguous segment of the block's positions.  A warp reads
+// One CTA per block of the group, kPngEmitThreads / 32 warps, each owning a contiguous segment of the block's positions.  A warp reads
 // its segment 32 consecutive positions at a time (coalesced); a warp scan of the token bit counts places each lane's
 // token, the lanes OR their bits into a per-warp staging buffer in shared memory, and the warp ORs the covered words into
 // the output.  Pass 1 counts the bits of each segment so that a CTA scan gives the segments' offsets; thread 0 writes the
 // header and the end-of-block code.  The Adler-32 partial sums of the block ride along.
 constexpr u32 kPngStageWords = 50;   // 32 tokens of at most 48 bits plus an offset of < 32 bits
-__global__ void __launch_bounds__(kPngEmitThreads) k_png_emit(const unsigned char *__restrict__ f, const unsigned char *__restrict__ lcode,
-                                                              const uint16_t *__restrict__ dist, const unsigned char *__restrict__ flag,
-                                                              u32 n, u32 block_bytes, const u32 *__restrict__ codes,
-                                                              const u32 *__restrict__ hdr, const u32 *__restrict__ hdr_bits,
-                                                              const u64 *__restrict__ off, u32 *__restrict__ out_words,
-                                                              u64 *__restrict__ sums) {
+__global__ void __launch_bounds__(kPngEmitThreads) k_png_emit(const PngImage *__restrict__ im, u32 g,
+                                                              const unsigned char *__restrict__ f_all,
+                                                              const unsigned char *__restrict__ lcode_all,
+                                                              const uint16_t *__restrict__ dist_all,
+                                                              const unsigned char *__restrict__ flag_all, u32 block_bytes,
+                                                              const u32 *__restrict__ codes, const u32 *__restrict__ hdr,
+                                                              const u32 *__restrict__ hdr_bits, const u64 *__restrict__ off,
+                                                              unsigned char *__restrict__ out_all, u64 *__restrict__ sums) {
     constexpr u32 kWarps = kPngEmitThreads / 32;
     __shared__ u32 tab[kPngLit + kPngDist];
     __shared__ u64 wsum[kWarps];
     __shared__ u64 red[2][kWarps];
     __shared__ u32 stage[kWarps][kPngStageWords];
     const u32 blk = blockIdx.x, t = threadIdx.x, lane = t & 31, wid = t >> 5;
-    const u32 start = blk * block_bytes;
+    const PngImage &I = im[png_image_of<&PngImage::blk0>(im, g, blk)];
+    const u32 n = I.n;
+    const unsigned char *__restrict__ f = f_all + I.pos;
+    const unsigned char *__restrict__ lcode = lcode_all + I.pos;
+    const uint16_t *__restrict__ dist = dist_all + I.pos;
+    const unsigned char *__restrict__ flag = flag_all + I.pos;
+    u32 *__restrict__ out_words = reinterpret_cast<u32 *>(out_all + I.out);
+    const u64 out_lim = I.out_bytes;
+    const u32 start = (blk - I.blk0) * block_bytes;
     const u32 len = min(block_bytes, n - start);
-    PNG_CHECK(start + len <= c_png_lim.n && blockIdx.x < c_png_lim.nblocks && start + len + 16 <= c_png_lim.f_bytes, 13);
+    PNG_CHECK(start + len <= n && blk - I.blk0 < I.nblocks, 13);
     for (u32 k = t; k < kPngLit + kPngDist; k += blockDim.x) tab[k] = codes[static_cast<u64>(blk) * (kPngLit + kPngDist) + k];
     for (u32 k = lane; k < kPngStageWords; k += 32) stage[wid][k] = 0;
     __syncthreads();
@@ -624,7 +665,7 @@ __global__ void __launch_bounds__(kPngEmitThreads) k_png_emit(const unsigned cha
         const u64 w0 = pos >> 5;
         for (u32 k = lane; k < nw; k += 32) {
             const u32 v = st[k];
-            PNG_CHECK(4 * (w0 + k + 1) <= c_png_lim.out_bytes, 9);
+            PNG_CHECK(4 * (w0 + k + 1) <= out_lim, 9);
             if (v) atomicOr(&out_words[w0 + k], v);
             st[k] = 0;
         }
@@ -632,11 +673,11 @@ __global__ void __launch_bounds__(kPngEmitThreads) k_png_emit(const unsigned cha
         pos += total;
     }
     if (t == 0) {
-        PngOut h{out_words, base, 0, 0};
+        PngOut h{out_words, base, 0, 0, out_lim};
         const u32 *hw = hdr + static_cast<u64>(blk) * kPngHdrWords;
         for (u32 k = 0; k * 32 < hb; ++k) h.put(hw[k], min(32u, hb - k * 32));
         h.done();
-        PngOut eob{out_words, base + hb + toks, 0, 0};
+        PngOut eob{out_words, base + hb + toks, 0, 0, out_lim};
         eob.put(tab[256] & 0xFFFFu, tab[256] >> 16);
         eob.done();
         u64 x1 = 0, x2 = 0;
@@ -682,13 +723,17 @@ __device__ __forceinline__ void png_be32(unsigned char *p, u32 v) {
     p[3] = static_cast<unsigned char>(v);
 }
 
-struct PngIhdr {
-    unsigned char b[25];
-};
-
-// One thread: Adler-32 from the block sums, the signature, IHDR, the IDAT length and type, the zlib header and trailer.
-__global__ void k_png_frame(const u64 *__restrict__ sums, u32 nblocks, u32 n, u32 block_bytes, PngIhdr ihdr,
-                            unsigned char *__restrict__ out, PngCtl *__restrict__ ctl) {
+// One thread per image: Adler-32 from the block sums, the signature, IHDR, the IDAT length and type, the zlib header and
+// trailer.
+__global__ void k_png_frame(const PngImage *__restrict__ im, u32 g, const u64 *__restrict__ sums_all, u32 block_bytes,
+                            unsigned char *__restrict__ out_all, PngCtl *__restrict__ ctl_all) {
+    const u32 k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= g) return;
+    const PngImage &I = im[k];
+    const u32 n = I.n, nblocks = I.nblocks;
+    const u64 *__restrict__ sums = sums_all + 2 * static_cast<u64>(I.blk0);
+    unsigned char *__restrict__ out = out_all + I.out;
+    PngCtl *__restrict__ ctl = ctl_all + k;
     const u64 M = 65521;
     u64 s1 = 1, s2 = n % M;
     for (u32 b = 0; b < nblocks; ++b) {
@@ -701,8 +746,8 @@ __global__ void k_png_frame(const u64 *__restrict__ sums, u32 nblocks, u32 n, u3
     ctl->adler = adler;
     const u64 dbytes = (ctl->deflate_bits + 7) / 8;
     const unsigned char sig[8] = {0x89, 'P', 'N', 'G', '\r', '\n', 0x1A, '\n'};
-    for (int k = 0; k < 8; ++k) out[k] = sig[k];
-    for (int k = 0; k < 25; ++k) out[8 + k] = ihdr.b[k];
+    for (int j = 0; j < 8; ++j) out[j] = sig[j];
+    for (int j = 0; j < 25; ++j) out[8 + j] = I.ihdr[j];
     png_be32(out + 33, static_cast<u32>(2 + dbytes + 4));
     out[37] = 'I';
     out[38] = 'D';
@@ -710,24 +755,31 @@ __global__ void k_png_frame(const u64 *__restrict__ sums, u32 nblocks, u32 n, u3
     out[40] = 'T';
     out[41] = 0x78;
     out[42] = 0x9C;
-    PNG_CHECK(kPngDeflateBase + dbytes + 20 <= c_png_lim.out_bytes, 10);
+    PNG_CHECK(kPngDeflateBase + dbytes + 20 <= I.out_bytes, 10);
     png_be32(out + kPngDeflateBase + dbytes, adler);
     ctl->total = kPngDeflateBase + dbytes + 4 + 4 + 12;
 }
 
-// CRC-32 contributions: each thread takes kPngCrcChunk bytes of "IDAT" + zlib stream, computes their CRC from a zero
-// register and shifts it by the bytes that follow (x^(8 k) mod P); the contributions XOR together (CRC linearity).
-__global__ void __launch_bounds__(256) k_png_crc(const unsigned char *__restrict__ out, PngCtl *__restrict__ ctl) {
+// CRC-32 contributions: each thread takes kPngCrcChunk bytes of one image's "IDAT" + zlib stream, computes their CRC
+// from a zero register and shifts it by the bytes that follow (x^(8 k) mod P); the contributions XOR together (CRC
+// linearity).  Each image's chunks start at a multiple of 32, so a warp's contributions belong to one image.
+__global__ void __launch_bounds__(256) k_png_crc(const PngImage *__restrict__ im, u32 g, u32 chunks,
+                                                 const unsigned char *__restrict__ out_all, PngCtl *__restrict__ ctl_all) {
     __shared__ u32 tab[256];
     for (u32 k = threadIdx.x; k < 256; k += blockDim.x) tab[k] = c_png_crc_table[k];
     __syncthreads();
+    const u32 gc = blockIdx.x * blockDim.x + threadIdx.x;
+    const u32 k = png_image_of<&PngImage::chunk0>(im, g, min(gc, chunks - 1));
+    const PngImage &I = im[k];
+    const unsigned char *__restrict__ out = out_all + I.out;
+    PngCtl *__restrict__ ctl = ctl_all + k;
     const u64 lo = 37, hi = ctl->total - 16;   // IDAT type .. Adler-32 inclusive
-    const u64 a = lo + (static_cast<u64>(blockIdx.x) * blockDim.x + threadIdx.x) * kPngCrcChunk;
+    const u64 a = lo + static_cast<u64>(gc - I.chunk0) * kPngCrcChunk;
     u32 contrib = 0;
-    if (a < hi) {
+    if (gc < chunks && a < hi) {
         const u64 b = min(hi, a + kPngCrcChunk);
         u32 c = 0;
-        PNG_CHECK(b <= c_png_lim.out_bytes, 11);
+        PNG_CHECK(b <= I.out_bytes, 11);
         for (u64 k = a; k < b; ++k) c = tab[(c ^ out[k]) & 0xFF] ^ (c >> 8);
         contrib = png_multmodp(png_x8n(hi - b), c);
     }
@@ -735,14 +787,20 @@ __global__ void __launch_bounds__(256) k_png_crc(const unsigned char *__restrict
     if ((threadIdx.x & 31) == 0 && contrib) atomicXor(&ctl->crc_raw, contrib);
 }
 
-// One thread: the IDAT CRC (initial register and final XOR applied) and the IEND chunk.
-__global__ void k_png_end(unsigned char *__restrict__ out, const PngCtl *__restrict__ ctl) {
+// One thread per image: the IDAT CRC (initial register and final XOR applied) and the IEND chunk.
+__global__ void k_png_end(const PngImage *__restrict__ im, u32 g, unsigned char *__restrict__ out_all,
+                          const PngCtl *__restrict__ ctl_all) {
+    const u32 k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= g) return;
+    const PngImage &I = im[k];
+    unsigned char *__restrict__ out = out_all + I.out;
+    const PngCtl *__restrict__ ctl = ctl_all + k;
     const u64 hi = ctl->total - 16;
     const u32 crc = ctl->crc_raw ^ png_multmodp(png_x8n(hi - 37), 0xFFFFFFFFu) ^ 0xFFFFFFFFu;
-    PNG_CHECK(hi + 16 <= c_png_lim.out_bytes, 12);
+    PNG_CHECK(hi + 16 <= I.out_bytes, 12);
     png_be32(out + hi, crc);
     const unsigned char iend[12] = {0, 0, 0, 0, 'I', 'E', 'N', 'D', 0xAE, 0x42, 0x60, 0x82};
-    for (int k = 0; k < 12; ++k) out[hi + 4 + k] = iend[k];
+    for (int j = 0; j < 12; ++j) out[hi + 4 + j] = iend[j];
 }
 
 }  // namespace aptb200

@@ -135,27 +135,70 @@ bool png_alpha_opaque(const uint8_t *px, uint64_t npx) {
     return true;
 }
 
-int PngWork::reserve(const PngPlan &p) {
-    APT_TRY(grow(f, cap_n, p.n + 16, 1));
-    if (cap_n_pos < p.n) {
+int png_layout(const PngPlan *plans, const unsigned char *const *pixels, u32 g, PngLayout &lay) {
+    if (g == 0) return fail(APT_ERR_BAD_ARG, "empty PNG group");
+    const PngPlan &s = plans[0];
+    lay.shape = s;
+    lay.img.assign(g, PngImage{});
+    u64 pos = 0, out = 0;
+    u64 rows = 0, spans = 0, blocks = 0, chunks = 0;
+    for (u32 k = 0; k < g; ++k) {
+        const PngPlan &p = plans[k];
+        if (p.width != s.width || p.in_ch != s.in_ch || p.ch != s.ch || p.s.filter != s.s.filter || p.s.matches != s.s.matches ||
+            p.s.block_bytes != s.s.block_bytes || p.s.rgb_from_rgba != s.s.rgb_from_rgba)
+            return fail(APT_ERR_BAD_ARG, "the images of a PNG group must share width, channels and settings");
+        PngImage &im = lay.img[k];
+        im.px = pixels ? pixels[k] : nullptr;
+        im.pos = pos;
+        im.out = out;
+        im.out_bytes = (p.bound + 8) & ~3ull;
+        im.height = p.height;
+        im.n = static_cast<u32>(p.n);
+        im.row0 = static_cast<u32>(rows);
+        im.span0 = static_cast<u32>(spans);
+        im.blk0 = static_cast<u32>(blocks);
+        im.nblocks = p.nblocks;
+        im.chunk0 = static_cast<u32>(chunks);
+        memcpy(im.ihdr, p.ihdr, sizeof(im.ihdr));
+        pos += (p.n + 16 + 63) & ~63ull;   // the stream, 16 bytes of padding png_ld32 may read, 64-byte alignment
+        out += (im.out_bytes + 7) & ~7ull;
+        rows += p.height;
+        spans += (p.n + kPngSpan - 1) / kPngSpan;
+        blocks += p.nblocks;
+        chunks += ((p.bound - 37 + kPngCrcChunk - 1) / kPngCrcChunk + 31) & ~31ull;
+        if (rows > 0xFFFFFFFFull || blocks > 0xFFFFFFFFull || chunks > 0xFFFFFFFFull)
+            return fail(APT_ERR_BAD_ARG, "PNG group too large");
+    }
+    lay.f_bytes = pos;
+    lay.out_bytes = out;
+    lay.rows = static_cast<u32>(rows);
+    lay.spans = static_cast<u32>(spans);
+    lay.blocks = static_cast<u32>(blocks);
+    lay.chunks = static_cast<u32>(chunks);
+    return APT_OK;
+}
+
+int PngWork::reserve(const PngLayout &l) {
+    APT_TRY(grow(f, cap_n, l.f_bytes, 1));
+    if (cap_n_pos < l.f_bytes) {
         for (void *q : {(void *)lcode, (void *)dist, (void *)flag})
             if (q) cudaFree(q);
         lcode = nullptr;
         dist = nullptr;
         flag = nullptr;
         cap_n_pos = 0;
-        APT_CUDA(cudaMalloc(&lcode, p.n));
-        APT_CUDA(cudaMalloc(&dist, p.n * sizeof(uint16_t)));
-        APT_CUDA(cudaMalloc(&flag, p.n));
-        cap_n_pos = p.n;
+        APT_CUDA(cudaMalloc(&lcode, l.f_bytes));
+        APT_CUDA(cudaMalloc(&dist, l.f_bytes * sizeof(uint16_t)));
+        APT_CUDA(cudaMalloc(&flag, l.f_bytes));
+        cap_n_pos = l.f_bytes;
     }
-    if (cap_blocks < p.nblocks) {
+    if (cap_blocks < l.blocks) {
         for (void *q : {(void *)hist, (void *)codes, (void *)hdr, (void *)hdr_bits, (void *)bits, (void *)off, (void *)sums})
             if (q) cudaFree(q);
         hist = codes = hdr = hdr_bits = nullptr;
         bits = off = sums = nullptr;
         cap_blocks = 0;
-        const u64 nb = p.nblocks;
+        const u64 nb = l.blocks;
         APT_CUDA(cudaMalloc(&hist, nb * (kPngLit + kPngDist) * sizeof(u32)));
         APT_CUDA(cudaMalloc(&codes, nb * (kPngLit + kPngDist) * sizeof(u32)));
         APT_CUDA(cudaMalloc(&hdr, nb * kPngHdrWords * sizeof(u32)));
@@ -165,99 +208,113 @@ int PngWork::reserve(const PngPlan &p) {
         APT_CUDA(cudaMalloc(&sums, 2 * nb * sizeof(u64)));
         cap_blocks = nb;
     }
-    APT_TRY(grow(out, cap_out, (p.bound + 8) & ~3ull, 1));
-    if (!ctl) APT_CUDA(cudaMalloc(&ctl, sizeof(PngCtl)));
+    APT_TRY(grow(out, cap_out, l.out_bytes, 1));
+    const u64 g = l.img.size();
+    if (cap_img < g) {
+        if (ctl) cudaFree(ctl);
+        if (img) cudaFree(img);
+        if (h_img) cudaFreeHost(h_img);
+        ctl = nullptr;
+        img = nullptr;
+        h_img = nullptr;
+        cap_img = 0;
+        APT_CUDA(cudaMalloc(&ctl, g * sizeof(PngCtl)));
+        APT_CUDA(cudaMalloc(&img, g * sizeof(PngImage)));
+        APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&h_img), g * sizeof(PngImage), cudaHostAllocDefault));
+        cap_img = g;
+    }
     return APT_OK;
 }
 
 void PngWork::release() {
     for (void *q : {(void *)f, (void *)lcode, (void *)dist, (void *)flag, (void *)hist, (void *)codes, (void *)hdr, (void *)hdr_bits,
-                    (void *)bits, (void *)off, (void *)sums, (void *)out, (void *)ctl})
+                    (void *)bits, (void *)off, (void *)sums, (void *)out, (void *)ctl, (void *)img})
         if (q) cudaFree(q);
+    if (h_img) cudaFreeHost(h_img);
     f = lcode = flag = out = nullptr;
     dist = nullptr;
     hist = codes = hdr = hdr_bits = nullptr;
     bits = off = sums = nullptr;
     ctl = nullptr;
-    cap_n = cap_n_pos = cap_blocks = cap_out = 0;
+    img = h_img = nullptr;
+    cap_n = cap_n_pos = cap_blocks = cap_out = cap_img = 0;
 }
 
 size_t PngWork::device_bytes() const {
     return cap_n + cap_n_pos * 4 + cap_blocks * (2 * (kPngLit + kPngDist) * 4 + kPngHdrWords * 4 + 4 + 4 * 8) + cap_out +
-           (ctl ? sizeof(PngCtl) : 0);
+           cap_img * (sizeof(PngCtl) + sizeof(PngImage));
 }
 
-int png_encode_device(const LaunchCtx &c, const PngPlan &p, PngWork &w, const unsigned char *pixels, KernelHook *hook) {
+int png_encode_device(const LaunchCtx &c, const PngPlan *plans, const unsigned char *const *pixels, u32 g, PngWork &w,
+                      KernelHook *hook) {
     APT_TRY(ensure_tables());
-    APT_TRY(w.reserve(p));
-    const u32 n = static_cast<u32>(p.n);
+    PngLayout &lay = w.lay;
+    APT_TRY(png_layout(plans, pixels, g, lay));
+    APT_TRY(w.reserve(lay));
+    const PngPlan &p = lay.shape;
     const u32 bb = p.s.block_bytes;
+    memcpy(w.h_img, lay.img.data(), g * sizeof(PngImage));   // the previous encode on w has finished (png.hpp)
+    APT_CUDA(cudaMemcpyAsync(w.img, w.h_img, g * sizeof(PngImage), cudaMemcpyHostToDevice, c.stream));
 #ifdef APTB200_PNG_CHECK
-    const PngLimits lim{p.n + 16, p.n, static_cast<u64>(p.width) * p.height * p.in_ch, (p.bound + 8) & ~3ull, p.nblocks};
     const u32 zero = 0;
-    APT_CUDA(cudaMemcpyToSymbolAsync(c_png_lim, &lim, sizeof(lim), 0, cudaMemcpyHostToDevice, c.stream));
     APT_CUDA(cudaMemcpyToSymbolAsync(g_png_violation, &zero, sizeof(zero), 0, cudaMemcpyHostToDevice, c.stream));
 #endif
-    APT_CUDA(cudaMemsetAsync(w.f + p.n, 0, 16, c.stream));   // the padding png_ld32 may read past the last position
-    APT_CUDA(cudaMemsetAsync(w.flag, 0, p.n, c.stream));
-    APT_CUDA(cudaMemsetAsync(w.out, 0, (p.bound + 8) & ~3ull, c.stream));
-    APT_CUDA(cudaMemsetAsync(w.ctl, 0, sizeof(PngCtl), c.stream));
+    APT_CUDA(cudaMemsetAsync(w.flag, 0, lay.f_bytes, c.stream));
+    APT_CUDA(cudaMemsetAsync(w.out, 0, lay.out_bytes, c.stream));
+    APT_CUDA(cudaMemsetAsync(w.ctl, 0, g * sizeof(PngCtl), c.stream));
     {
         KernelSlot ks(hook, "png_filter");
-        const u32 grid = (p.height + 7) / 8;
-        if (p.in_ch == 1) k_png_filter<1, 1><<<grid, 256, 0, c.stream>>>(pixels, p.width, p.height, p.s.filter, w.f);
-        else if (p.in_ch == 3) k_png_filter<3, 3><<<grid, 256, 0, c.stream>>>(pixels, p.width, p.height, p.s.filter, w.f);
-        else if (p.ch == 4) k_png_filter<4, 4><<<grid, 256, 0, c.stream>>>(pixels, p.width, p.height, p.s.filter, w.f);
-        else k_png_filter<4, 3><<<grid, 256, 0, c.stream>>>(pixels, p.width, p.height, p.s.filter, w.f);
+        const u32 grid = (lay.rows + 7) / 8;
+        if (p.in_ch == 1) k_png_filter<1, 1><<<grid, 256, 0, c.stream>>>(w.img, g, lay.rows, p.width, p.s.filter, w.f);
+        else if (p.in_ch == 3) k_png_filter<3, 3><<<grid, 256, 0, c.stream>>>(w.img, g, lay.rows, p.width, p.s.filter, w.f);
+        else if (p.ch == 4) k_png_filter<4, 4><<<grid, 256, 0, c.stream>>>(w.img, g, lay.rows, p.width, p.s.filter, w.f);
+        else k_png_filter<4, 3><<<grid, 256, 0, c.stream>>>(w.img, g, lay.rows, p.width, p.s.filter, w.f);
         APT_CUDA(cudaGetLastError());
     }
     if (p.s.matches) {
         KernelSlot ks(hook, "png_match");
         const size_t smem = 32768 * sizeof(uint16_t);
         APT_CUDA(cudaFuncSetAttribute(k_png_match, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-        k_png_match<<<(n + kPngSpan - 1) / kPngSpan, 32, smem, c.stream>>>(w.f, n, bb, w.lcode, w.dist);
+        k_png_match<<<lay.spans, 32, smem, c.stream>>>(w.img, g, w.f, bb, w.lcode, w.dist);
         APT_CUDA(cudaGetLastError());
     } else {
-        APT_CUDA(cudaMemsetAsync(w.lcode, 0, p.n, c.stream));   // literals only
+        APT_CUDA(cudaMemsetAsync(w.lcode, 0, lay.f_bytes, c.stream));   // literals only
     }
     {
         KernelSlot ks(hook, "png_parse");
         APT_CUDA(cudaFuncSetAttribute(k_png_parse, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bb)));
-        k_png_parse<<<p.nblocks, 256, bb, c.stream>>>(w.f, w.lcode, w.dist, n, bb, w.flag, w.hist);
+        k_png_parse<<<lay.blocks, 256, bb, c.stream>>>(w.img, g, w.f, w.lcode, w.dist, bb, w.flag, w.hist);
         APT_CUDA(cudaGetLastError());
     }
     {
         KernelSlot ks(hook, "png_huffman");
-        k_png_huffman<<<p.nblocks, 32, 0, c.stream>>>(w.hist, p.nblocks, w.codes, w.hdr, w.hdr_bits, w.bits);
+        k_png_huffman<<<lay.blocks, 32, 0, c.stream>>>(w.img, g, w.hist, w.codes, w.hdr, w.hdr_bits, w.bits);
         APT_CUDA(cudaGetLastError());
     }
     {
         KernelSlot ks(hook, "png_scan");
-        k_png_scan<<<1, 1024, 0, c.stream>>>(w.bits, p.nblocks, w.off, w.ctl);
+        k_png_scan<<<g, 1024, 0, c.stream>>>(w.img, w.bits, w.off, w.ctl);
         APT_CUDA(cudaGetLastError());
     }
     {
         KernelSlot ks(hook, "png_emit");
-        k_png_emit<<<p.nblocks, kPngEmitThreads, 0, c.stream>>>(w.f, w.lcode, w.dist, w.flag, n, bb, w.codes, w.hdr, w.hdr_bits,
-                                                                  w.off, reinterpret_cast<u32 *>(w.out), w.sums);
+        k_png_emit<<<lay.blocks, kPngEmitThreads, 0, c.stream>>>(w.img, g, w.f, w.lcode, w.dist, w.flag, bb, w.codes, w.hdr,
+                                                                   w.hdr_bits, w.off, w.out, w.sums);
         APT_CUDA(cudaGetLastError());
     }
     {
         KernelSlot ks(hook, "png_frame");
-        PngIhdr ih;
-        memcpy(ih.b, p.ihdr, sizeof(ih.b));
-        k_png_frame<<<1, 1, 0, c.stream>>>(w.sums, p.nblocks, n, bb, ih, w.out, w.ctl);
+        k_png_frame<<<(g + 63) / 64, 64, 0, c.stream>>>(w.img, g, w.sums, bb, w.out, w.ctl);
         APT_CUDA(cudaGetLastError());
     }
     {
         KernelSlot ks(hook, "png_crc");
-        const u64 chunks = (p.bound - 37 + kPngCrcChunk - 1) / kPngCrcChunk;
-        k_png_crc<<<static_cast<u32>((chunks + 255) / 256), 256, 0, c.stream>>>(w.out, w.ctl);
+        k_png_crc<<<(lay.chunks + 255) / 256, 256, 0, c.stream>>>(w.img, g, lay.chunks, w.out, w.ctl);
         APT_CUDA(cudaGetLastError());
     }
     {
         KernelSlot ks(hook, "png_end");
-        k_png_end<<<1, 1, 0, c.stream>>>(w.out, w.ctl);
+        k_png_end<<<(g + 63) / 64, 64, 0, c.stream>>>(w.img, g, w.out, w.ctl);
         APT_CUDA(cudaGetLastError());
     }
 #ifdef APTB200_PNG_CHECK
@@ -285,6 +342,7 @@ struct PngStage {
     u64 px_cap = 0;
     cudaStream_t stream = nullptr;
     PngCtl *h_ctl = nullptr;
+    u64 h_ctl_cap = 0;
     void release() {
         if (stream) cudaStreamSynchronize(stream);
         w.release();
@@ -293,6 +351,7 @@ struct PngStage {
         px_cap = 0;
         if (h_ctl) cudaFreeHost(h_ctl);
         h_ctl = nullptr;
+        h_ctl_cap = 0;
         if (stream) cudaStreamDestroy(stream);
         stream = nullptr;
     }
@@ -332,18 +391,47 @@ extern "C" int apt_png_bound(uint32_t width, uint32_t height, int channels, cons
     return APT_OK;
 }
 
+extern "C" int apt_png_group_plan(uint32_t width, int channels, const apt_png_settings *ps, const uint32_t *heights, uint32_t count,
+                                  apt_png_group_info *info, apt_png_group_image *images, size_t cap) {
+    if (!heights || !info) return fail(APT_ERR_BAD_ARG, "null argument");
+    memset(info, 0, sizeof(*info));
+    std::vector<PngPlan> plans(count);
+    for (uint32_t k = 0; k < count; ++k) APT_TRY(make_png(width, heights[k], channels, ps, plans[k]));
+    PngLayout lay;
+    APT_TRY(png_layout(plans.data(), nullptr, count, lay));
+    *info = apt_png_group_info{lay.f_bytes, lay.out_bytes, lay.rows, lay.spans, lay.blocks, lay.chunks};
+    for (uint32_t k = 0; images && k < count && k < cap; ++k) {
+        const PngImage &im = lay.img[k];
+        images[k] = apt_png_group_image{im.pos, im.n, im.out, im.out_bytes, plans[k].bound, im.row0, im.span0, im.blk0,
+                                        im.nblocks, im.chunk0, 0};
+    }
+    return APT_OK;
+}
+
 extern "C" int apt_png_encode(const uint8_t *pixels, uint32_t width, uint32_t height, int channels, const apt_png_settings *ps,
                               uint8_t *out, uint64_t cap, uint64_t *nout) {
-    if (!pixels || !out || !nout) return fail(APT_ERR_BAD_ARG, "null argument");
-    *nout = 0;
-    PngPlan p;
-    APT_TRY(make_png(width, height, channels, ps, p));
-    const u64 npx = static_cast<u64>(width) * height;
-    if (ps->rgb_from_rgba && !png_alpha_opaque(pixels, npx))
-        return fail(APT_ERR_BAD_ARG, "rgb_from_rgba needs every alpha to be 255");
-    int count = 0;
-    cudaError_t e = cudaGetDeviceCount(&count);
-    if (e != cudaSuccess || count <= 0) {
+    return apt_png_encode_batch(&pixels, &height, 1, width, channels, ps, &out, &cap, nout);
+}
+
+extern "C" int apt_png_encode_batch(const uint8_t *const *pixels, const uint32_t *heights, uint32_t count, uint32_t width,
+                                    int channels, const apt_png_settings *ps, uint8_t *const *outs, const uint64_t *caps,
+                                    uint64_t *nouts) {
+    if (!pixels || !heights || !outs || !caps || !nouts) return fail(APT_ERR_BAD_ARG, "null argument");
+    std::vector<PngPlan> plans(count);
+    std::vector<u64> in_off(count + 1, 0);
+    for (uint32_t k = 0; k < count; ++k) {
+        if (!pixels[k] || !outs[k]) return fail(APT_ERR_BAD_ARG, "null argument");
+        nouts[k] = 0;
+        APT_TRY(make_png(width, heights[k], channels, ps, plans[k]));
+        const u64 npx = static_cast<u64>(width) * heights[k];
+        if (ps->rgb_from_rgba && !png_alpha_opaque(pixels[k], npx))
+            return fail(APT_ERR_BAD_ARG, "rgb_from_rgba needs every alpha to be 255");
+        in_off[k + 1] = in_off[k] + ((npx * channels + 15) & ~15ull);
+    }
+    if (count == 0) return APT_OK;
+    int ndev = 0;
+    cudaError_t e = cudaGetDeviceCount(&ndev);
+    if (e != cudaSuccess || ndev <= 0) {
         cudaGetLastError();
         return fail(APT_ERR_CUDA, "no usable CUDA device (%s); this library has no CPU fallback",
                     e == cudaSuccess ? "device count is 0" : cudaGetErrorString(e));
@@ -359,21 +447,38 @@ extern "C" int apt_png_encode(const uint8_t *pixels, uint32_t width, uint32_t he
     }
     PngStage &sg = *slot;
     std::lock_guard<std::mutex> lk(sg.mu);   // one encode per device at a time: they share the workspace
-    const u64 in_bytes = npx * channels;
     auto run = [&]() -> int {
         if (!sg.stream) APT_CUDA(cudaStreamCreateWithFlags(&sg.stream, cudaStreamNonBlocking));
-        if (!sg.h_ctl) APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&sg.h_ctl), sizeof(PngCtl), cudaHostAllocDefault));
-        APT_TRY(grow(sg.px, sg.px_cap, in_bytes, 1));
-        APT_CUDA(cudaMemcpyAsync(sg.px, pixels, in_bytes, cudaMemcpyHostToDevice, sg.stream));
-        APT_TRY(png_encode_device(LaunchCtx{sg.stream, std::max(sms, 1)}, p, sg.w, sg.px, nullptr));
-        APT_CUDA(cudaMemcpyAsync(sg.h_ctl, sg.w.ctl, sizeof(PngCtl), cudaMemcpyDeviceToHost, sg.stream));
+        if (sg.h_ctl_cap < count) {
+            if (sg.h_ctl) cudaFreeHost(sg.h_ctl);
+            sg.h_ctl = nullptr;
+            sg.h_ctl_cap = 0;
+            APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&sg.h_ctl), count * sizeof(PngCtl), cudaHostAllocDefault));
+            sg.h_ctl_cap = count;
+        }
+        APT_TRY(grow(sg.px, sg.px_cap, in_off[count], 1));
+        std::vector<const unsigned char *> px(count);
+        for (uint32_t k = 0; k < count; ++k) {
+            px[k] = sg.px + in_off[k];
+            APT_CUDA(cudaMemcpyAsync(sg.px + in_off[k], pixels[k], static_cast<u64>(width) * heights[k] * channels,
+                                     cudaMemcpyHostToDevice, sg.stream));
+        }
+        APT_TRY(png_encode_device(LaunchCtx{sg.stream, std::max(sms, 1)}, plans.data(), px.data(), count, sg.w, nullptr));
+        APT_CUDA(cudaMemcpyAsync(sg.h_ctl, sg.w.ctl, count * sizeof(PngCtl), cudaMemcpyDeviceToHost, sg.stream));
         APT_CUDA(cudaStreamSynchronize(sg.stream));
-        const u64 total = sg.h_ctl->total;
-        *nout = total;
-        if (total > cap) return fail(APT_ERR_CAPACITY, "output needs room for %llu bytes", (unsigned long long)total);
-        APT_CUDA(cudaMemcpyAsync(out, sg.w.out, total, cudaMemcpyDeviceToHost, sg.stream));
+        int first = APT_OK;
+        for (uint32_t k = 0; k < count; ++k) {
+            const u64 total = sg.h_ctl[k].total;
+            nouts[k] = total;
+            if (total > caps[k]) {
+                const int st = fail(APT_ERR_CAPACITY, "output needs room for %llu bytes", (unsigned long long)total);
+                if (first == APT_OK) first = st;
+                continue;
+            }
+            APT_CUDA(cudaMemcpyAsync(outs[k], sg.w.out + sg.w.lay.img[k].out, total, cudaMemcpyDeviceToHost, sg.stream));
+        }
         APT_CUDA(cudaStreamSynchronize(sg.stream));
-        return APT_OK;
+        return first;
     };
     const int st = run();
     if (st != APT_OK && sg.stream) cudaStreamSynchronize(sg.stream);

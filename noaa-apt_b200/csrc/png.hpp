@@ -4,6 +4,7 @@
 #pragma once
 
 #include <cstdint>
+#include <vector>
 
 #include "aptb200.h"
 #include "launch.hpp"
@@ -33,7 +34,37 @@ struct PngPlan {
 // Argument rules (host only, APT_ERR_BAD_ARG) and the plan.  Alpha is not looked at here.
 int make_png(uint32_t width, uint32_t height, int channels, const apt_png_settings *ps, PngPlan &plan);
 
-// Device workspaces of the encoder; they grow to the largest image seen and are kept.
+// One image of an encode group (DESIGN.md §11, "Batched encode").  The images of a group share width, channels and
+// settings; each has its own height and pixels.  Every offset is the image's own region of a buffer shared by the
+// group, and every kernel finds its image by a binary search of the first-index fields over the table.
+struct PngImage {
+    const unsigned char *px = nullptr;   // device pixels: height * width * in_ch bytes
+    u64 pos = 0;        // offset of the filtered stream in f and of the positions in lcode / dist / flag (a multiple of 64)
+    u64 out = 0;        // byte offset of the file in out (a multiple of 8)
+    u64 out_bytes = 0;  // bytes of out reserved for the file: the bound rounded up to words
+    u32 height = 0;
+    u32 n = 0;          // filtered stream length
+    u32 row0 = 0;       // first global row (k_png_filter: one warp per row)
+    u32 span0 = 0;      // first global match span (k_png_match)
+    u32 blk0 = 0;       // first global deflate block (parse, huffman, emit; hist / codes / hdr / bits / off / sums)
+    u32 nblocks = 0;
+    u32 chunk0 = 0;     // first global CRC chunk, a multiple of 32 so that no warp of k_png_crc spans two images
+    unsigned char ihdr[25] = {};   // the IHDR chunk, CRC included
+};
+
+// The layout of a group: its table and the sizes of the shared buffers.
+struct PngLayout {
+    PngPlan shape;                  // settings, width and channels (the first image's plan)
+    std::vector<PngImage> img;
+    u64 f_bytes = 0;                // f, lcode, flag (and dist in u16): the last image's region end
+    u64 out_bytes = 0;
+    u32 rows = 0, spans = 0, blocks = 0, chunks = 0;
+};
+
+// The layout of `g` images whose plans share width, channels and settings (APT_ERR_BAD_ARG otherwise).  Host only.
+int png_layout(const PngPlan *plans, const unsigned char *const *pixels, u32 g, PngLayout &lay);
+
+// Device workspaces of the encoder; they grow to the largest group seen and are kept.
 struct PngWork {
     unsigned char *f = nullptr;      // filtered stream (+16 bytes of padding)
     unsigned char *lcode = nullptr;  // per position: 0, or match length - 3
@@ -46,20 +77,26 @@ struct PngWork {
     u64 *bits = nullptr;             // per block: header + tokens + end of block
     u64 *off = nullptr;              // per block: exclusive scan of bits
     u64 *sums = nullptr;             // per block: Adler partial sums (sum F, sum (block end - i) F[i])
-    unsigned char *out = nullptr;    // the PNG file (bound bytes, rounded up to words)
-    PngCtl *ctl = nullptr;
-    u64 cap_n = 0, cap_n_pos = 0, cap_blocks = 0, cap_out = 0;   // bytes of f; positions of lcode / dist / flag; ...
+    unsigned char *out = nullptr;    // the PNG files (PngImage::out, out_bytes)
+    PngCtl *ctl = nullptr;           // per image
+    PngImage *img = nullptr;         // the group's table (device)
+    PngImage *h_img = nullptr;       // and its pinned staging
+    u64 cap_n = 0, cap_n_pos = 0, cap_blocks = 0, cap_out = 0, cap_img = 0;   // bytes of f; positions of lcode / dist / flag; ...
+    PngLayout lay;                   // the layout of the last encode
     PngWork() = default;
     PngWork(const PngWork &) = delete;
     ~PngWork() { release(); }
-    int reserve(const PngPlan &p);
+    int reserve(const PngLayout &lay);
     void release();
     size_t device_bytes() const;
 };
 
-// Enqueues the whole encode of `pixels` (device, height * width * in_ch bytes) on c.stream.  The file is at w.out, its
-// length in w.ctl->total.
-int png_encode_device(const LaunchCtx &c, const PngPlan &p, PngWork &w, const unsigned char *pixels, KernelHook *hook);
+// Enqueues the whole encode of `g` images (plans[k] and device pixels[k], height * width * in_ch bytes, as png_layout
+// takes them) on c.stream: one launch per kernel for the group.  Image k's file is at w.out + w.lay.img[k].out, its length
+// in w.ctl[k].total.  Every file's bytes are those of the image encoded alone.  The caller waits for the encode before
+// it starts the next one on the same workspace.
+int png_encode_device(const LaunchCtx &c, const PngPlan *plans, const unsigned char *const *pixels, u32 g, PngWork &w,
+                      KernelHook *hook);
 
 // Frees the per-device workspaces apt_png_encode keeps between calls (apt_cache_clear).
 void png_stage_cache_clear();

@@ -628,7 +628,8 @@ int finish_image(apt_stream *st, uint8_t *image, uint64_t cap, uint64_t *image_n
     if (o.png) {
         PngPlan pp;
         APT_TRY(make_png(kPxPerRow, static_cast<uint32_t>(rows), o.plan.bpp, &o.png_settings, pp));
-        APT_TRY(png_encode_device(c, pp, o.png_work, o.d_px, nullptr));
+        const unsigned char *px = o.d_px;
+        APT_TRY(png_encode_device(c, &pp, &px, 1, o.png_work, nullptr));
         APT_CUDA(cudaMemcpyAsync(o.h_png, o.png_work.ctl, sizeof(PngCtl), cudaMemcpyDeviceToHost, d.stream));
     } else if (image && cap >= px_bytes) {
         APT_CUDA(cudaMemcpyAsync(image, o.d_px, px_bytes, cudaMemcpyDeviceToHost, d.stream));
@@ -694,7 +695,9 @@ extern "C" int apt_stream_set_png_mode(apt_stream *st, const apt_png_settings *p
     APT_CUDA(cudaStreamSynchronize(st->dec.stream));
     o.release_png();
     if (!png) return APT_OK;
-    const int rc = o.png_work.reserve(pp);
+    PngLayout lay;
+    int rc = png_layout(&pp, nullptr, 1, lay);
+    if (rc == APT_OK) rc = o.png_work.reserve(lay);
     if (rc != APT_OK) {
         o.release_png();
         return rc;

@@ -131,6 +131,28 @@ def encode_png(pixels, filter=-1, matches=True, block_bytes=65536, rgb_from_rgba
     return out[: n.value].tobytes()
 
 
+def encode_png_batch(images, filter=-1, matches=True, block_bytes=65536, rgb_from_rgba=False):
+    """encode_png of several images of one width and channel count (heights may differ) in one batched encode on the
+    device -> list of PNG bytes, each equal to encode_png of that image alone."""
+    xs = [np.ascontiguousarray(x, dtype=np.uint8) for x in images]
+    if not xs:
+        return []
+    ch = _channels(xs[0].shape)
+    w = xs[0].shape[1]
+    if any(x.ndim != xs[0].ndim or _channels(x.shape) != ch or x.shape[1] != w for x in xs):
+        raise InvalidInput(_lib.ERR_BAD_ARG, "the images of a batch must share width and channels")
+    ps = png_settings(filter, matches, block_bytes, rgb_from_rgba)
+    lib = _lib.load()
+    n = len(xs)
+    outs = [np.empty(max(png_bound(w, x.shape[0], ch, filter, matches, block_bytes, rgb_from_rgba), 1), dtype=np.uint8)
+            for x in xs]
+    nouts = (C.c_uint64 * n)()
+    raise_for(lib.apt_png_encode_batch((C.c_void_p * n)(*[x.ctypes.data for x in xs]), (C.c_uint32 * n)(*[x.shape[0] for x in xs]),
+                                       n, w, ch, C.byref(ps), (C.c_void_p * n)(*[o.ctypes.data for o in outs]),
+                                       (C.c_uint64 * n)(*[o.size for o in outs]), nouts))
+    return [o[: nouts[k]].tobytes() for k, o in enumerate(outs)]
+
+
 def decode_png(context, settings, signal, input_rate, sync=True, contrast=MINMAX, percent=0.98, rotate=False, palette=None,
                tune=(0, 0, 0, 0), rgba=None, filter=-1, matches=True, block_bytes=65536, rgb_from_rgba=False):
     """decode() + process() + PNG encoding in one call; only the PNG bytes leave the GPU -> (bytes, info)."""
@@ -159,6 +181,73 @@ def decode_png(context, settings, signal, input_rate, sync=True, contrast=MINMAX
     raise_for(lib.apt_decode_png(x.ctypes.data, fmt, x.size, rate, C.byref(s), int(bool(sync)), C.byref(ps), C.byref(png),
                                  out.ctypes.data, out.size, C.byref(n), C.byref(ci), cb, None))
     return out[: n.value].tobytes(), _info(ci)
+
+
+def decode_batch_png(signals, input_rate, settings=None, sync=True, contrast=MINMAX, percent=0.98, rotate=False,
+                     palette=None, tune=(0, 0, 0, 0), rgba=None, png=True, filter=-1, matches=True, block_bytes=65536,
+                     rgb_from_rgba=False, devices=None, streams_per_device=4):
+    """decode_batch ending each recording in its PNG file (png=True) or its processed image (png=False), sharded as
+    decode_batch.  With PNG output the images of each device are encoded in groups, one launch sequence per group.
+    Returns (list of bytes or pixel arrays or None, list of infos or None, list of status codes); raises when nothing
+    decoded at all."""
+    from .decode import _fmt_of, decode_len_bound
+    lib = _lib.load()
+    s = (settings or Settings()).to_c()
+    rate = _rate_hz(input_rate)
+    xs = [np.ascontiguousarray(x) for x in signals]
+    if not xs:
+        return [], [], []
+    fmt = _fmt_of(xs[0])
+    if any(_fmt_of(x) != fmt for x in xs):
+        raise TypeError("all recordings of a batch must share one sample format")
+    ps, bpp, _pal = process_settings(contrast, percent, rotate, palette, tune, rgba)
+    pngs = png_settings(filter, matches, block_bytes, rgb_from_rgba) if png else None
+    count = len(xs)
+    caps_list = []
+    for x in xs:
+        bound = decode_len_bound(x.size, rate, settings)
+        if png:
+            caps_list.append(png_bound(2080, max(bound // 2080, 1), bpp, filter, matches, block_bytes, rgb_from_rgba))
+        else:
+            caps_list.append(bound * bpp)
+    outs = [np.empty(max(c, 1), dtype=np.uint8) for c in caps_list]
+    sig_ptrs = (C.c_void_p * count)(*[x.ctypes.data for x in xs])
+    out_ptrs = (C.c_void_p * count)(*[o.ctypes.data for o in outs])
+    lens = (C.c_uint64 * count)(*[x.size for x in xs])
+    caps = (C.c_uint64 * count)(*[o.size for o in outs])
+    nouts = (C.c_uint64 * count)()
+    infos = (_lib.CImageInfo * count)()
+    statuses = (C.c_int * count)(*([-1] * count))   # -1: not written (never "ok" unless the library says so)
+    devs = list(devices) if devices else [0]
+    dev_arr = (C.c_int * len(devs))(*devs)
+    rc = lib.apt_decode_batch_image(sig_ptrs, fmt, lens, count, rate,
+                                    C.byref(s), int(bool(sync)), C.byref(ps), C.byref(pngs) if pngs is not None else None,
+                                    out_ptrs, caps, nouts, infos, statuses, dev_arr, len(devs), int(streams_per_device))
+    if rc != _lib.OK and all(int(v) in (rc, -1) for v in statuses):
+        raise_for(rc)   # nothing decoded at all (argument errors, no device, ...): an error, not a result
+    res, inf = [], []
+    for i in range(count):
+        if statuses[i] != _lib.OK:
+            res.append(None)
+            inf.append(None)
+            continue
+        got = outs[i][: nouts[i]]
+        res.append(got.tobytes() if png else _shape(got.copy(), bpp))
+        inf.append(_info(infos[i]))
+    return res, inf, [int(v) for v in statuses]
+
+
+def png_group_plan(width, channels, heights, filter=-1, matches=True, block_bytes=65536, rgb_from_rgba=False):
+    """The layout of one batched PNG encode of images of these heights (host arithmetic, no device) ->
+    (dict of the shared buffer and grid sizes, list of dicts of each image's regions)."""
+    ps = png_settings(filter, matches, block_bytes, rgb_from_rgba)
+    hs = (C.c_uint32 * max(len(heights), 1))(*[int(h) for h in heights])
+    gi = _lib.CPngGroupInfo()
+    ims = (_lib.CPngGroupImage * max(len(heights), 1))()
+    raise_for(_lib.load().apt_png_group_plan(int(width), int(channels), C.byref(ps), hs, len(heights), C.byref(gi), ims,
+                                             len(heights)))
+    info = {n: int(getattr(gi, n)) for n, _ in _lib.CPngGroupInfo._fields_}
+    return info, [{n: int(getattr(im, n)) for n, _ in _lib.CPngGroupImage._fields_ if n != "pad"} for im in ims[: len(heights)]]
 
 
 def decode_wav_png(input_path, output_path, settings=None, sync=True, contrast=MINMAX, percent=0.98, rotate=False,

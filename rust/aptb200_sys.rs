@@ -119,6 +119,13 @@ extern "C" {
     pub fn apt_decode_png(signal: *const c_void, format: c_int, n: u64, input_rate: u32, s: *const apt_settings, sync: c_int,
                           ps: *const apt_process_settings, png: *const apt_png_settings, out: *mut u8, cap: u64,
                           nout: *mut u64, info: *mut apt_image_info, cb: apt_status_cb, user: *mut c_void) -> c_int;
+    pub fn apt_decode_batch_image(signals: *const *const c_void, format: c_int, lens: *const u64, count: c_int, input_rate: u32,
+                                  s: *const apt_settings, sync: c_int, ps: *const apt_process_settings,
+                                  png: *const apt_png_settings, outs: *const *mut u8, caps: *const u64, nouts: *mut u64,
+                                  infos: *mut apt_image_info, statuses: *mut c_int, devices: *const c_int, ndevices: c_int,
+                                  streams_per_device: c_int) -> c_int;
+    pub fn apt_png_encode_batch(pixels: *const *const u8, heights: *const u32, count: u32, width: u32, channels: c_int,
+                                ps: *const apt_png_settings, outs: *const *mut u8, caps: *const u64, nouts: *mut u64) -> c_int;
     pub fn apt_decoder_set_png_mode(dec: *mut apt_decoder, ps: *const apt_png_settings) -> c_int;
     pub fn apt_decode_wav_png(input_path: *const c_char, output_path: *const c_char, s: *const apt_settings, sync: c_int,
                               ps: *const apt_process_settings, png: *const apt_png_settings, info: *mut apt_image_info) -> c_int;

@@ -9,7 +9,7 @@ if [ ! -f "$LIB" ]; then
     mkdir -p "$(dirname "$LIB")"
     python -c "import sys; sys.path.insert(0, 'noaa-apt_b200'); import build; build.build_library(out='$LIB', extra_flags=['-DAPTB200_PNG_CHECK'])" || exit 1
 fi
-APTB200_LIB=$LIB python -m pytest -m gpu tests/test_gpu_png.py -q -p no:cacheprovider > $OUT/png_bounds_check.log 2>&1
+APTB200_LIB=$LIB python -m pytest -m gpu tests/test_gpu_png.py tests/test_gpu_batch_png.py -q -p no:cacheprovider > $OUT/png_bounds_check.log 2>&1
 echo "tests rc=$?" >> $OUT/png_bounds_check.log
 APTB200_LIB=$LIB python tools/sanitize_decode.py 1 >> $OUT/png_bounds_check.log 2>&1
 echo "sanitize_decode rc=$?" >> $OUT/png_bounds_check.log

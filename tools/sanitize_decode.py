@@ -55,3 +55,13 @@ with na.Stream(11025, na.Settings(), max_push=20000) as st:
     _rows, spng, _info = st.finish_image()
 want, _ = image.decode_png(None, na.Settings(), x, 11025, contrast=image.PERCENT, rotate=True, rgba=True, block_bytes=4096)
 print("stream png", len(spng), "bytes", "equal" if spng == want else "MISMATCH", flush=True)
+
+# Batch PNG output (DESIGN.md §11, "Batched encode"): three short recordings of different lengths, RGBA, 4 KiB blocks,
+# decoded by two decoders and encoded in groups, each file against apt_decode_png of that recording alone.
+xs = [synth.apt_signal(11025, sec, seed=4 + sec) for sec in (12, 15, 13)]
+files, _infos, sts = image.decode_batch_png(xs, 11025, contrast=image.MINMAX, rgba=True, block_bytes=4096,
+                                            streams_per_device=2)
+same = sts == [0, 0, 0] and all(
+    files[i] == image.decode_png(None, na.Settings(), x, 11025, contrast=image.MINMAX, rgba=True, block_bytes=4096)[0]
+    for i, x in enumerate(xs))
+print("batch png", [len(f or b"") for f in files], "bytes", "equal" if same else "MISMATCH", flush=True)
