@@ -485,6 +485,68 @@ int apt_stream_geometry_iq(const apt_iq_settings *iq, const apt_settings *s, int
  * (complex samples), cap in int16.  Any other layout is APT_ERR_IO. */
 int apt_wav_load_iq16(const char *path, int16_t *out, uint64_t cap, uint64_t *n, uint32_t *sample_rate);
 
+/* ------------------------------------------------------------------ I/Q input: finding the carriers */
+
+/* The averaged power spectrum of an I/Q recording (DESIGN.md §10, "Finding carriers").  With S = floor(n / nfft) whole
+ * segments and K = min(S, max_segments), segment k < K starts at sample floor(k S / K) nfft.  Each is loaded like
+ * apt_fm_demod loads it, multiplied by the periodic Hann window 0.5 - 0.5 cos(2 pi t / nfft) and transformed; psd[b],
+ * b < nfft, is the average of |X|^2 over the K segments in fftshift order: bin b is (b - nfft/2) iq_rate / nfft Hz.
+ * Only the K segments cross PCIe.  The result is the same bits on every run.  *nseg receives K.  APT_ERR_BAD_ARG (NULL
+ * pointers, an unknown format, nfft not a power of two in [256, 16384], fewer than nfft samples) and APT_ERR_CAPACITY
+ * (cap < nfft) come back before any device is touched. */
+typedef struct apt_spectrum_settings {
+    uint32_t nfft;                /* power of two, 256 ... 16384 */
+    uint32_t max_segments;        /* 0: 2048 */
+} apt_spectrum_settings;
+int apt_iq_spectrum(const void *iq, int format, uint64_t n, uint32_t iq_rate, const apt_spectrum_settings *ss,
+                    float *psd, uint64_t cap, uint32_t *nseg);
+
+/* Where to look for carriers.  Zero fields take the defaults. */
+typedef struct apt_carrier_search {
+    int32_t lo_hz, hi_hz;         /* search window relative to the tuned centre; 0, 0: the whole usable band */
+    uint32_t nfft;                /* 0: smallest power of two with bin width <= 200 Hz, capped at 16384 */
+    uint32_t max_segments;        /* 0: 2048 */
+    float min_snr_db;             /* 0: 6 dB */
+} apt_carrier_search;
+typedef struct apt_carrier {
+    int32_t offset_hz;            /* round(centre_hz); ready for apt_iq_settings.offset_hz */
+    float centre_hz, snr_db;
+    float apt_score;              /* fraction of the demodulated audio's power between 300 Hz and 4.8 kHz */
+    int is_apt;                   /* apt_score >= 0.5 */
+} apt_carrier;
+/* Carriers in an I/Q recording: the spectrum above; the noise floor, the median of psd over the window; the band power
+ * E(f), the sum of psd within +-20 kHz of f; a candidate at each local maximum of E in the window (the window clipped so
+ * that |f| + s->cutout < iq_rate / 2) with snr_db = 10 log10(E / (floor bins_in_band)) >= min_snr_db; candidates taken
+ * by descending E, each one within 40 kHz of a kept one dropped; centre_hz the floor-subtracted, power-weighted centroid
+ * of the bins within +-20 kHz of the peak.  Each returned carrier is then FM-demodulated (4 s from the middle of the
+ * recording at offset_hz, s's channel filter) and the audio's spectrum gives apt_score.  out receives the carriers by
+ * descending snr_db; *count the full number: more than cap is APT_ERR_CAPACITY (out may be NULL when cap is 0).
+ * s->offset_hz is ignored.  Argument errors (as apt_iq_spectrum, the checks of apt_fm_demod_len on s, an inverted
+ * window) come back before any device is touched. */
+int apt_iq_find_carriers(const void *iq, int format, uint64_t n, const apt_iq_settings *s, const apt_carrier_search *cs,
+                         apt_carrier *out, uint32_t cap, uint32_t *count);
+/* The search of apt_iq_find_carriers alone, on a spectrum the caller has (nfft bins in apt_iq_spectrum's order): host
+ * only, no device; apt_score and is_apt are 0.  cs->nfft and cs->max_segments are not read. */
+int apt_find_carriers_psd(const float *psd, uint32_t nfft, uint32_t iq_rate, float cutout, const apt_carrier_search *cs,
+                          apt_carrier *out, uint32_t cap, uint32_t *count);
+
+/* Several channels of one recording: channel c equals apt_decode_iq with offset_hz = offsets[c], bit for bit (rows,
+ * nouts[c], statuses[c]).  Each chunk of I/Q is uploaded once and demodulated once per channel, into that channel's
+ * decoder; the channels' decodes then run side by side.  outs[c] / caps[c] as apt_decode_iq's out / cap; a cap below the
+ * bound is APT_ERR_CAPACITY for that channel alone.  Argument errors of any channel (NULL pointers, count < 1, an offset
+ * failing |offset| + cutout < iq_rate / 2, and the errors apt_decode_iq decides from lengths) come back before any device
+ * is touched, with every status set to the error.  Returns APT_OK or the first failing status. */
+int apt_decode_iq_channels(const void *iq, int format, uint64_t n, const apt_iq_settings *s, const int32_t *offsets,
+                           int count, const apt_settings *settings, int sync,
+                           float *const *outs, const uint64_t *caps, uint64_t *nouts, int *statuses);
+/* apt_iq_find_carriers, then apt_decode_iq_channels on the carriers with is_apt: found receives those carriers in
+ * apt_iq_find_carriers' order, at most cap_found of them, *nfound their number, and outs[i] / nouts[i] / statuses[i]
+ * (cap_found entries each) belong to found[i].  No APT carrier: APT_OK with *nfound = 0.  The decode's argument errors are
+ * checked before any device is touched, on offset 0. */
+int apt_decode_iq_auto(const void *iq, int format, uint64_t n, const apt_iq_settings *s, const apt_carrier_search *cs,
+                       const apt_settings *settings, int sync, apt_carrier *found, uint32_t cap_found, uint32_t *nfound,
+                       float *const *outs, const uint64_t *caps, uint64_t *nouts, int *statuses);
+
 /* ------------------------------------------------------------------ PNG output: encoding on the device */
 
 /* A deterministic PNG encoder (DESIGN.md §11; the reference's `img.save` pins no encoder, so the bytes are this project's

@@ -314,6 +314,63 @@ inline Signal decode_iq(Context &ctx, const config::Settings &settings, const vo
     out.resize(got);
     return out;
 }
+// Finding the carriers of a recording (DESIGN.md §10, "Finding carriers")
+struct Spectrum {
+    std::vector<float> psd;   // fftshifted: bin b is (b - nfft/2) iq_rate / nfft Hz
+    uint32_t segments = 0;
+};
+inline Spectrum spectrum(const void *samples, int format, uint64_t n, uint32_t iq_rate, uint32_t nfft = 16384,
+                         uint32_t max_segments = 2048) {
+    const apt_spectrum_settings ss{nfft, max_segments};
+    Spectrum out;
+    out.psd.resize(nfft);
+    err::check(apt_iq_spectrum(samples, format, n, iq_rate, &ss, out.psd.data(), out.psd.size(), &out.segments));
+    return out;
+}
+inline std::vector<apt_carrier> find_carriers(const void *samples, int format, uint64_t n, const apt_iq_settings &s,
+                                              const apt_carrier_search &cs = apt_carrier_search{}) {
+    std::vector<apt_carrier> out(s.iq_rate / 40000 + 2);   // kept carriers are more than 40 kHz apart
+    uint32_t count = 0;
+    err::check(apt_iq_find_carriers(samples, format, n, &s, &cs, out.data(), static_cast<uint32_t>(out.size()), &count));
+    out.resize(count);
+    return out;
+}
+struct Channel {
+    apt_carrier carrier;
+    int status;               // APT_OK, or the failure of this channel's decode
+    Signal rows;
+};
+// Every APT carrier decoded from one upload of the recording; a channel that fails keeps its status, the call throws
+// only for errors every channel shares.
+inline std::vector<Channel> decode_iq_auto(const config::Settings &settings, const void *samples, int format, uint64_t n,
+                                           const apt_iq_settings &s, bool sync,
+                                           const apt_carrier_search &cs = apt_carrier_search{}, uint32_t max_channels = 8) {
+    const apt_settings st = settings.to_c();
+    apt_iq_settings s0 = s;
+    s0.offset_hz = 0;
+    uint64_t len = 0, bound = 0;
+    err::check(apt_fm_demod_len(n, &s0, &len));
+    err::check(apt_decode_len_bound(len, s.audio_rate, &st, &bound));
+    const uint32_t k = max_channels ? max_channels : 1;
+    std::vector<Signal> bufs(k, Signal(bound ? bound : 1));
+    std::vector<float *> outs(k);
+    for (uint32_t i = 0; i < k; ++i) outs[i] = bufs[i].data();
+    std::vector<uint64_t> caps(k, bound ? bound : 1), nouts(k, 0);
+    std::vector<int> statuses(k, 0);
+    std::vector<apt_carrier> found(k);
+    uint32_t nfound = 0;
+    const int rc = apt_decode_iq_auto(samples, format, n, &s, &cs, &st, sync ? 1 : 0, found.data(), k, &nfound, outs.data(),
+                                      caps.data(), nouts.data(), statuses.data());
+    bool shared = rc != APT_OK;
+    for (uint32_t i = 0; i < nfound; ++i) shared = shared && statuses[i] == rc;
+    if (rc != APT_OK && (nfound == 0 || shared)) err::check(rc);
+    std::vector<Channel> out;
+    for (uint32_t i = 0; i < nfound; ++i) {
+        bufs[i].resize(statuses[i] == APT_OK ? nouts[i] : 0);
+        out.push_back(Channel{found[i], statuses[i], std::move(bufs[i])});
+    }
+    return out;
+}
 }  // namespace iq
 
 // PNG output encoded on the device (DESIGN.md §11): the file's bytes, ready to write.

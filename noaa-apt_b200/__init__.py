@@ -17,9 +17,11 @@ from .context import Context
 from .decode import (CARRIER_FREQ, FINAL_RATE, PX_PER_ROW, Decoder, Stream, decode, decode_batch, decode_len_bound,
                      find_sync, generate_sync_frame, stream_geometry, stream_geometry_iq)
 from .frequency import Freq, Rate
+from .iq import Carrier, decode_iq_auto, decode_iq_channels, find_carriers, spectrum
 
 __all__ = ["decode", "decode_batch", "decode_len_bound", "find_sync", "generate_sync_frame", "Decoder", "Stream",
-           "stream_geometry", "stream_geometry_iq",
+           "stream_geometry", "stream_geometry_iq", "spectrum", "find_carriers", "decode_iq_channels", "decode_iq_auto",
+           "Carrier",
            "Settings", "Context", "Freq", "Rate", "dsp", "filters", "err", "config", "frequency", "image", "iq", "wav",
            "FINAL_RATE", "PX_PER_ROW", "CARRIER_FREQ"]
 

@@ -90,6 +90,20 @@ class CIqSettings(C.Structure):
                 ("delta_freq", C.c_float), ("atten", C.c_float)]
 
 
+class CSpectrumSettings(C.Structure):
+    _fields_ = [("nfft", C.c_uint32), ("max_segments", C.c_uint32)]
+
+
+class CCarrierSearch(C.Structure):
+    _fields_ = [("lo_hz", C.c_int32), ("hi_hz", C.c_int32), ("nfft", C.c_uint32), ("max_segments", C.c_uint32),
+                ("min_snr_db", C.c_float)]
+
+
+class CCarrier(C.Structure):
+    _fields_ = [("offset_hz", C.c_int32), ("centre_hz", C.c_float), ("snr_db", C.c_float), ("apt_score", C.c_float),
+                ("is_apt", C.c_int)]
+
+
 class CPngSettings(C.Structure):
     _fields_ = [("filter", C.c_int), ("matches", C.c_int), ("block_bytes", C.c_uint32), ("rgb_from_rgba", C.c_int)]
 
@@ -206,6 +220,18 @@ SIGNATURES = {
     "apt_stream_geometry_iq": (C.c_int, [C.POINTER(CIqSettings), C.POINTER(CSettings), C.c_int, C.c_uint64,
                                          C.POINTER(CStreamInfo)]),
     "apt_wav_load_iq16":(C.c_int, [C.c_char_p, C.c_void_p, C.c_uint64, _u64p, C.POINTER(C.c_uint32)]),
+    "apt_iq_spectrum": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64, C.c_uint32, C.POINTER(CSpectrumSettings), C.c_void_p,
+                                  C.c_uint64, C.POINTER(C.c_uint32)]),
+    "apt_iq_find_carriers": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64, C.POINTER(CIqSettings), C.POINTER(CCarrierSearch),
+                                       C.POINTER(CCarrier), C.c_uint32, C.POINTER(C.c_uint32)]),
+    "apt_find_carriers_psd": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_float, C.POINTER(CCarrierSearch),
+                                        C.POINTER(CCarrier), C.c_uint32, C.POINTER(C.c_uint32)]),
+    "apt_decode_iq_channels": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64, C.POINTER(CIqSettings), C.POINTER(C.c_int32),
+                                         C.c_int, C.POINTER(CSettings), C.c_int, C.POINTER(C.c_void_p), _u64p, _u64p,
+                                         C.POINTER(C.c_int)]),
+    "apt_decode_iq_auto": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64, C.POINTER(CIqSettings), C.POINTER(CCarrierSearch),
+                                     C.POINTER(CSettings), C.c_int, C.POINTER(CCarrier), C.c_uint32, C.POINTER(C.c_uint32),
+                                     C.POINTER(C.c_void_p), _u64p, _u64p, C.POINTER(C.c_int)]),
     "apt_png_default_settings": (None, [C.POINTER(CPngSettings)]),
     "apt_png_bound": (C.c_int, [C.c_uint32, C.c_uint32, C.c_int, C.POINTER(CPngSettings), _u64p]),
     "apt_png_encode": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_int, C.POINTER(CPngSettings), C.c_void_p,

@@ -17,6 +17,7 @@
 #include "decoder.hpp"
 #include "filters_host.hpp"
 #include "launch.hpp"
+#include "spectrum.hpp"
 
 using namespace aptb200;
 
@@ -992,6 +993,7 @@ extern "C" void apt_cache_clear(void) {
     }
     for (auto &e : drop) apt_decoder_destroy(e.dec);
     png_stage_cache_clear();
+    spectrum_cache_clear();
 }
 
 extern "C" int apt_decode(const float *signal, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
@@ -1076,6 +1078,189 @@ extern "C" int apt_decode_iq(const void *iq, int format, uint64_t n, const apt_i
     if (use_cache) cache_put(device, rate, *s, d);
     else apt_decoder_destroy(d);
     return st;
+}
+
+extern "C" int apt_decode_iq_channels(const void *iq, int format, uint64_t n, const apt_iq_settings *is, const int32_t *offsets,
+                                      int count, const apt_settings *s, int sync, float *const *outs, const uint64_t *caps,
+                                      uint64_t *nouts, int *statuses) {
+    if (!is || !s || !offsets || !outs || !caps || !nouts || !statuses || count < 1)
+        return fail(APT_ERR_BAD_ARG, "null argument or count < 1");
+    auto fail_all = [&](int st) {
+        for (int c = 0; c < count; ++c) statuses[c] = st;
+        return st;
+    };
+    for (int c = 0; c < count; ++c) {
+        nouts[c] = 0;
+        statuses[c] = APT_ERR_CUDA;   // overwritten by the channel's own status; never left "ok" by default
+    }
+    if (n == 0 || !iq) return fail_all(fail(APT_ERR_BAD_ARG, "empty signal"));
+    if (!iq_sample_bytes(format)) return fail_all(fail(APT_ERR_BAD_ARG, "unknown I/Q sample format %d", format));
+    // every channel's argument errors before any device work, in apt_decode_iq's order
+    std::vector<IqPlan> ips(count);
+    std::vector<apt_iq_settings> iss(count, *is);
+    for (int c = 0; c < count; ++c) {
+        iss[c].offset_hz = offsets[c];
+        const int st = make_iq(iss[c], ips[c]);
+        if (st != APT_OK) return fail_all(st);
+    }
+    const uint64_t na = ips[0].out_len(n);
+    const uint32_t rate = is->audio_rate;
+    uint64_t need = 0;
+    {
+        Plan p;
+        const int st = make_plan(rate, *s, p);
+        if (st != APT_OK) return fail_all(st);
+        const uint64_t nwork = p.front.work_len(na);
+        if (nwork < 10ull * p.row)
+            return fail_all(fail(APT_ERR_TOO_SHORT, "Got less than 10 rows of samples, audio file is too short"));
+        if (sync && !p.work_multiple) return fail_all(fail(APT_ERR_WORK_RATE, "work_rate is not multiple of FINAL_RATE"));
+        need = sync ? (nwork / p.row) * kPxPerRow : plan_out_bound(p, na);
+    }
+    std::vector<int> live;
+    for (int c = 0; c < count; ++c) {
+        if (!outs[c] || caps[c] < need)
+            statuses[c] = fail(APT_ERR_CAPACITY, "output needs room for %llu floats", (unsigned long long)need);
+        else
+            live.push_back(c);
+    }
+    auto first_status = [&]() {
+        for (int c = 0; c < count; ++c)
+            if (statuses[c] != APT_OK) return statuses[c];
+        return static_cast<int>(APT_OK);
+    };
+    if (live.empty()) return first_status();
+    if (const int st = require_device(); st != APT_OK) return fail_all(st);
+    int device = 0;
+    if (cudaGetDevice(&device) != cudaSuccess) device = 0;
+    static const bool use_cache = getenv("APTB200_NO_CACHE") == nullptr;
+    // one parked decoder per live channel; the first one's stream, stager and I/Q window carry the upload
+    std::vector<apt_decoder *> decs;
+    auto park = [&]() {
+        for (apt_decoder *d : decs) {
+            cudaStreamSynchronize(d->stream);
+            if (use_cache) cache_put_multi(device, rate, *s, d);
+            else apt_decoder_destroy(d);
+        }
+        decs.clear();
+    };
+    cudaEvent_t demod_done = nullptr;
+    auto setup = [&]() -> int {
+        for (size_t k = 0; k < live.size(); ++k) {
+            apt_decoder *d = use_cache ? cache_take(device, rate, *s, na) : nullptr;
+            if (!d) {
+                const uint64_t room = use_cache ? ((na + na / 8 + (1u << 20)) & ~((1ull << 20) - 1)) : na;
+                APT_TRY(apt_decoder_create(device, rate, s, room, &d));
+            }
+            decs.push_back(d);
+            const int c = live[k];
+            APT_CUDA(cudaSetDevice(d->device));
+            if (!d->iq_tables_valid || memcmp(&d->iq_settings, &iss[c], sizeof(iss[c])) != 0) {
+                d->iq_tables_valid = false;
+                APT_TRY(d->iq_tables.upload(ips[c]));
+                d->iq_settings = iss[c];
+                d->iq_tables_valid = true;
+            }
+            if (d->audio_cap < d->max_samples) {
+                if (d->d_audio) APT_CUDA(cudaFree(d->d_audio));
+                d->d_audio = nullptr;
+                d->audio_cap = 0;
+                APT_CUDA(cudaMalloc(&d->d_audio, std::max<uint64_t>(d->max_samples, 1) * sizeof(float)));
+                d->audio_cap = d->max_samples;
+            }
+            if (!d->d_out) APT_CUDA(cudaMalloc(&d->d_out, std::max<uint64_t>(d->max_out, 1) * sizeof(float)));
+        }
+        apt_decoder *d0 = decs[0];
+        if (is_pageable(iq) && !d0->stager && !getenv("APTB200_NO_STAGER")) {
+            int threads = 8;
+            if (const char *e = getenv("APTB200_COPY_THREADS")) threads = std::max(1, atoi(e));
+            d0->own_stager.reset(new (std::nothrow) HostStager(d0->device, 16u << 20, 3, threads));
+            if (d0->own_stager && !d0->own_stager->ok()) d0->own_stager.reset();
+            d0->stager = d0->own_stager.get();
+        }
+        std::vector<const IqPlan *> pl;
+        std::vector<const IqTables *> tb;
+        std::vector<float *> au;
+        for (size_t k = 0; k < live.size(); ++k) {
+            pl.push_back(&ips[live[k]]);
+            tb.push_back(&decs[k]->iq_tables);
+            au.push_back(decs[k]->d_audio);
+        }
+        APT_TRY(iq_demod_host_multi(LaunchCtx{d0->stream, d0->sm_count}, pl.data(), tb.data(), au.data(),
+                                    static_cast<int>(live.size()), iq, format, n, d0->iq_win,
+                                    is_pageable(iq) ? d0->stager : nullptr, nullptr));
+        APT_CUDA(cudaEventCreateWithFlags(&demod_done, cudaEventDisableTiming));
+        APT_CUDA(cudaEventRecord(demod_done, d0->stream));
+        return APT_OK;
+    };
+    int st = setup();
+    if (st != APT_OK) {
+        if (demod_done) cudaEventDestroy(demod_done);
+        park();
+        for (int c : live) statuses[c] = st;
+        return st;
+    }
+    // every channel's decode on its own decoder's stream, after the demodulation; they run side by side
+    std::vector<int> submitted(live.size(), APT_OK);
+    for (size_t k = 0; k < live.size(); ++k) {
+        apt_decoder *d = decs[k];
+        submitted[k] = cudaStreamWaitEvent(d->stream, demod_done, 0) == cudaSuccess
+                           ? apt_decoder_submit_device(d, d->d_audio, APT_F32, na, sync, d->d_out, d->max_out)
+                           : fail(APT_ERR_CUDA, "cudaStreamWaitEvent failed");
+    }
+    for (size_t k = 0; k < live.size(); ++k) {
+        apt_decoder *d = decs[k];
+        const int c = live[k];
+        uint64_t produced = 0;
+        int cst = submitted[k];
+        if (cst == APT_OK) cst = apt_decoder_wait(d, &produced);
+        if (cst == APT_OK && cudaMemcpy(outs[c], d->d_out, produced * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess)
+            cst = fail(APT_ERR_CUDA, "copying the rows of channel %d failed", c);
+        if (cst == APT_OK) nouts[c] = produced;
+        statuses[c] = cst;
+    }
+    cudaEventDestroy(demod_done);
+    park();
+    return first_status();
+}
+
+extern "C" int apt_decode_iq_auto(const void *iq, int format, uint64_t n, const apt_iq_settings *is, const apt_carrier_search *cs,
+                                  const apt_settings *s, int sync, apt_carrier *found, uint32_t cap_found, uint32_t *nfound,
+                                  float *const *outs, const uint64_t *caps, uint64_t *nouts, int *statuses) {
+    if (!is || !s || !nfound || (cap_found && (!found || !outs || !caps || !nouts || !statuses)))
+        return fail(APT_ERR_BAD_ARG, "null argument");
+    *nfound = 0;
+    if (n == 0 || !iq) return fail(APT_ERR_BAD_ARG, "empty signal");
+    if (!iq_sample_bytes(format)) return fail(APT_ERR_BAD_ARG, "unknown I/Q sample format %d", format);
+    {
+        // the decode's argument errors (on offset 0) and the search's, before any device work
+        apt_iq_settings s0 = *is;
+        s0.offset_hz = 0;
+        IqPlan ip;
+        APT_TRY(make_iq(s0, ip));
+        SearchParams sp;
+        APT_TRY(make_search(cs, is->iq_rate, sp));
+        SpecPlan spec;
+        APT_TRY(make_spectrum(n, sp.nfft, sp.max_segments, spec));
+        Plan p;
+        APT_TRY(make_plan(is->audio_rate, *s, p));
+        if (p.front.work_len(ip.out_len(n)) < 10ull * p.row)
+            return fail(APT_ERR_TOO_SHORT, "Got less than 10 rows of samples, audio file is too short");
+        if (sync && !p.work_multiple) return fail(APT_ERR_WORK_RATE, "work_rate is not multiple of FINAL_RATE");
+    }
+    // kept carriers are more than 40 kHz apart inside a band narrower than iq_rate: this many always suffice
+    std::vector<apt_carrier> all(is->iq_rate / 40000 + 2);
+    uint32_t total = 0;
+    APT_TRY(apt_iq_find_carriers(iq, format, n, is, cs, all.data(), static_cast<uint32_t>(all.size()), &total));
+    std::vector<int32_t> offsets;
+    for (uint32_t i = 0; i < total && offsets.size() < cap_found; ++i)
+        if (all[i].is_apt) {
+            found[offsets.size()] = all[i];
+            offsets.push_back(all[i].offset_hz);
+        }
+    *nfound = static_cast<uint32_t>(offsets.size());
+    if (offsets.empty()) return APT_OK;
+    return apt_decode_iq_channels(iq, format, n, is, offsets.data(), static_cast<int>(offsets.size()), s, sync, outs, caps,
+                                  nouts, statuses);
 }
 
 // ============================================================================== image stage

@@ -197,6 +197,28 @@ cudaError_t HostStager::upload(void *dst, const void *src, size_t bytes, cudaStr
     return cudaSuccess;
 }
 
+cudaError_t HostStager::upload_pieces(void *dst, const void *src, const uint64_t *offsets, size_t count, size_t piece,
+                                      cudaStream_t stream) {
+    const size_t per = std::max<size_t>(chunk_ / std::max<size_t>(piece, 1), 1);
+    const size_t nr = ring_.size();
+    for (size_t p0 = 0, c = 0; p0 < count; p0 += per, ++c) {
+        const size_t np = std::min(per, count - p0), r = c % nr;
+        if (np * piece > chunk_) return cudaErrorInvalidValue;   // a piece larger than a ring buffer
+        if (used_[r]) {
+            const cudaError_t e = cudaEventSynchronize(ev_[r]);
+            if (e != cudaSuccess) return e;
+        }
+        for (size_t i = 0; i < np; ++i)
+            pool_.copy(ring_[r] + i * piece, static_cast<const char *>(src) + offsets[p0 + i], piece);
+        cudaError_t e = cudaMemcpyAsync(static_cast<char *>(dst) + p0 * piece, ring_[r], np * piece, cudaMemcpyHostToDevice, stream);
+        if (e != cudaSuccess) return e;
+        e = cudaEventRecord(ev_[r], stream);
+        if (e != cudaSuccess) return e;
+        used_[r] = true;
+    }
+    return cudaSuccess;
+}
+
 bool is_pageable(const void *p) {
     cudaPointerAttributes at{};
     if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {

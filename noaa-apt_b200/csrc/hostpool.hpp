@@ -55,6 +55,10 @@ public:
     // Enqueues the upload of `bytes` from pageable `src` to device `dst` on `stream`; returns when the last chunk has
     // been handed to the DMA engine (the caller's buffer is no longer needed after return).
     cudaError_t upload(void *dst, const void *src, size_t bytes, cudaStream_t stream);
+    // Enqueues the upload of `count` pieces of `piece` bytes, piece i read from pageable src + offsets[i], packed one after
+    // the other at device `dst`; several pieces share a ring buffer and its one DMA.  Returns as upload() does.
+    cudaError_t upload_pieces(void *dst, const void *src, const uint64_t *offsets, size_t count, size_t piece,
+                              cudaStream_t stream);
     // Copies `bytes` from pinned `src` (already filled, e.g. by a finished D2H) into pageable `dst` with the pool.
     void scatter(void *dst, const void *src, size_t bytes) { pool_.copy(dst, src, bytes); }
     size_t chunk_bytes() const { return chunk_; }

@@ -219,8 +219,17 @@ void IqWindow::release() {
 
 int iq_demod_host(const LaunchCtx &c, const IqPlan &p, const IqTables &t, const void *iq, int format, uint64_t n,
                   IqWindow &win, HostStager *stager, float *d_audio, KernelHook *hook) {
+    const IqPlan *pp = &p;
+    const IqTables *tp = &t;
+    return iq_demod_host_multi(c, &pp, &tp, &d_audio, 1, iq, format, n, win, stager, hook);
+}
+
+int iq_demod_host_multi(const LaunchCtx &c, const IqPlan *const *plans, const IqTables *const *tables,
+                        float *const *d_audio, int count, const void *iq, int format, uint64_t n, IqWindow &win,
+                        HostStager *stager, KernelHook *hook) {
     const size_t sb = iq_sample_bytes(format);
     if (!sb) return fail(APT_ERR_BAD_ARG, "unknown I/Q sample format %d", format);
+    const IqPlan &p = *plans[0];   // D and the tap count, hence the spans, are the same for every channel
     const uint64_t nout = p.out_len(n);
     const uint64_t chunk = std::min<uint64_t>(iq_chunk_samples(), std::max<uint64_t>(n, 1));
     // one chunk's window: its new samples and the halo in front of its first output
@@ -235,8 +244,11 @@ int iq_demod_host(const LaunchCtx &c, const IqPlan &p, const IqTables &t, const 
         const size_t bytes = (c_hi - xa) * sb;
         if (stager) APT_CUDA(stager->upload(win.p, src + xa * sb, bytes, c.stream));
         else APT_CUDA(cudaMemcpyAsync(win.p, src + xa * sb, bytes, cudaMemcpyHostToDevice, c.stream));
-        KernelSlot s(hook, "fm_demod");
-        APT_TRY(iq_launch(c, p, t, static_cast<const char *>(win.p) - xa * sb, xa, c_hi, format, m_done, m_b, d_audio));
+        for (int k = 0; k < count; ++k) {
+            KernelSlot s(hook, "fm_demod");
+            APT_TRY(iq_launch(c, *plans[k], *tables[k], static_cast<const char *>(win.p) - xa * sb, xa, c_hi, format, m_done,
+                              m_b, d_audio[k]));
+        }
         m_done = m_b;
     }
     return APT_OK;

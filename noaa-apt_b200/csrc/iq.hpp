@@ -73,5 +73,10 @@ struct IqWindow {
 class HostStager;
 int iq_demod_host(const LaunchCtx &c, const IqPlan &p, const IqTables &t, const void *iq, int format, uint64_t n,
                   IqWindow &win, HostStager *stager, float *d_audio, KernelHook *hook);
+// The same for `count` channels of one recording (plans that differ in offset_hz only): each chunk is uploaded once and
+// demodulated once per channel, plans[k] with tables[k] into d_audio[k].  Channel k's audio is iq_demod_host's.
+int iq_demod_host_multi(const LaunchCtx &c, const IqPlan *const *plans, const IqTables *const *tables,
+                        float *const *d_audio, int count, const void *iq, int format, uint64_t n, IqWindow &win,
+                        HostStager *stager, KernelHook *hook);
 
 }  // namespace aptb200

@@ -142,3 +142,80 @@ def apt_iq(iq_rate, seconds=None, seed=0, offset_hz=0, deviation_hz=17000.0, fmt
     if fmt == "cu8":
         return np.clip(np.rint(inter + 127.5), 0, 255).astype(np.uint8)
     return np.clip(np.rint(inter), -32768, 32767).astype(np.int16)
+
+
+_BLOCK = 1 << 16   # noise block of apt_iq_multi: sample i comes from block i // _BLOCK, whatever the chunk size
+
+
+def _noise_blocks(key, a, b):
+    """Complex standard Gaussian noise (each part N(0, 1)) for absolute sample indices [a, b), a >= 0: counter-based,
+    one Philox stream per (key, block), so any slice is the same numbers."""
+    out = np.empty(b - a, dtype=np.complex128)
+    i = a
+    while i < b:
+        blk = i // _BLOCK
+        lo, hi = i - blk * _BLOCK, min(b - blk * _BLOCK, _BLOCK)
+        v = np.random.Generator(np.random.Philox(key=[key, blk])).standard_normal((2, _BLOCK))
+        out[i - a:i - a + hi - lo] = v[0, lo:hi] + 1j * v[1, lo:hi]
+        i += hi - lo
+    return out
+
+
+def _band_taps(width_hz, iq_rate, ntaps=255):
+    """Hann-windowed sinc low-pass with cut-off width_hz / 2: the shape of an extra band."""
+    k = np.arange(ntaps) - (ntaps - 1) / 2
+    fc = 0.5 * width_hz / iq_rate
+    return 2 * fc * np.sinc(2 * fc * k) * np.hanning(ntaps + 2)[1:-1]
+
+
+def apt_iq_multi(iq_rate, seconds=None, carriers=((0, 0, 0.0, None, 60.0),), extra_bands=(), fmt="cu8", noise_rel=0.03,
+                 n_samples=None, deviation_hz=17000.0, audio_amplitude=20000.0, chunk=1 << 22):
+    """Several signals in one synthetic I/Q recording, as an SDR tuned near 137 MHz sees them.
+
+    carriers: (offset_hz, seed, doppler_hz, tca_s, width_s) per APT carrier of amplitude 1, FM-modulated like apt_iq by the
+      audio of `seed`, whose carrier frequency is offset_hz + doppler_hz * -(t - tca) / sqrt((t - tca)^2 + width^2), the
+      shape of a pass with its closest approach at tca_s (None: the middle of the recording).
+    extra_bands: (offset_hz, width_hz, rel_power) per band of Gaussian noise width_hz wide centred at offset_hz, of power
+      rel_power relative to a carrier (an LRPT-like wideband signal).
+    Complex Gaussian noise of noise_rel per part is added and the sum quantised to `fmt` as apt_iq does, scaled down by the
+    number of signals.  Every sample is a function of its index alone (the audio phase is an exact integer running sum,
+    the Doppler phase its closed-form integral, the noise counter-based per fixed block), so the output does not depend
+    on `chunk`."""
+    if n_samples is None:
+        n_samples = int(round(iq_rate * seconds))
+    nsig = len(carriers) + len(extra_bands)
+    scale = _IQ_SCALE[fmt] / max(nsig, 1)
+    out = np.empty(n_samples, dtype=np.complex128)
+    acc = [0] * len(carriers)                 # running sum of each carrier's int16 audio before the chunk
+    bands = [(_band_taps(w, iq_rate), off, p) for off, w, p in extra_bands]
+    done = 0
+    while done < n_samples:
+        m = min(chunk, n_samples - done)
+        idx = np.arange(done, done + m, dtype=np.int64)
+        t = idx / float(iq_rate)
+        y = np.zeros(m, dtype=np.complex128)
+        for c, (off, seed, dop, tca, width) in enumerate(carriers):
+            tca = 0.5 * n_samples / iq_rate if tca is None else tca
+            audio = apt_pcm16(iq_rate, seed=seed, n_samples=m, start=done, noise_sigma=0.0, chunk=chunk).astype(np.int64)
+            s_audio = acc[c] + np.cumsum(audio) - audio
+            acc[c] += int(audio.sum())
+            ph = (0.3 + 0.1 * (seed % 17)
+                  + 2.0 * np.pi * ((idx * int(off)) % iq_rate).astype(np.float64) / iq_rate
+                  + 2.0 * np.pi * deviation_hz / (audio_amplitude * iq_rate) * s_audio.astype(np.float64)
+                  - 2.0 * np.pi * dop * (np.sqrt((t - tca) ** 2 + width ** 2) - np.sqrt(tca ** 2 + width ** 2)))
+            y += np.exp(1j * ph)
+        for b, (h, off, p) in enumerate(bands):
+            raw = _noise_blocks(0x3D1 + b, done, done + m + h.size - 1)
+            shaped = np.convolve(raw, h, mode="valid") * np.sqrt(p / (2.0 * np.sum(h * h)))
+            y += shaped * np.exp(2j * np.pi * ((idx * int(off)) % iq_rate).astype(np.float64) / iq_rate)
+        if noise_rel > 0:
+            y += _noise_blocks(0x2C7, done, done + m) * noise_rel
+        out[done:done + m] = y
+        done += m
+    if fmt == "cf32":
+        return (out * scale).astype(np.complex64)
+    inter = np.empty(2 * n_samples, dtype=np.float64)
+    inter[0::2], inter[1::2] = out.real * scale, out.imag * scale
+    if fmt == "cu8":
+        return np.clip(np.rint(inter + 127.5), 0, 255).astype(np.uint8)
+    return np.clip(np.rint(inter), -32768, 32767).astype(np.int16)

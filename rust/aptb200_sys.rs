@@ -111,6 +111,20 @@ extern "C" {
     pub fn apt_stream_geometry_iq(iq: *const apt_iq_settings, s: *const apt_settings, sync: c_int, max_push: u64,
                                   info: *mut apt_stream_info) -> c_int;
     pub fn apt_wav_load_iq16(path: *const c_char, out: *mut i16, cap: u64, n: *mut u64, sample_rate: *mut u32) -> c_int;
+    // Finding the carriers of an I/Q recording (DESIGN.md §10, "Finding carriers")
+    pub fn apt_iq_spectrum(iq: *const c_void, format: c_int, n: u64, iq_rate: u32, ss: *const apt_spectrum_settings,
+                           psd: *mut c_float, cap: u64, nseg: *mut u32) -> c_int;
+    pub fn apt_iq_find_carriers(iq: *const c_void, format: c_int, n: u64, s: *const apt_iq_settings,
+                                cs: *const apt_carrier_search, out: *mut apt_carrier, cap: u32, count: *mut u32) -> c_int;
+    pub fn apt_find_carriers_psd(psd: *const c_float, nfft: u32, iq_rate: u32, cutout: c_float, cs: *const apt_carrier_search,
+                                 out: *mut apt_carrier, cap: u32, count: *mut u32) -> c_int;
+    pub fn apt_decode_iq_channels(iq: *const c_void, format: c_int, n: u64, s: *const apt_iq_settings, offsets: *const i32,
+                                  count: c_int, settings: *const apt_settings, sync: c_int, outs: *const *mut c_float,
+                                  caps: *const u64, nouts: *mut u64, statuses: *mut c_int) -> c_int;
+    pub fn apt_decode_iq_auto(iq: *const c_void, format: c_int, n: u64, s: *const apt_iq_settings,
+                              cs: *const apt_carrier_search, settings: *const apt_settings, sync: c_int,
+                              found: *mut apt_carrier, cap_found: u32, nfound: *mut u32, outs: *const *mut c_float,
+                              caps: *const u64, nouts: *mut u64, statuses: *mut c_int) -> c_int;
     // PNG output: the file's bytes encoded on the device (DESIGN.md §11)
     pub fn apt_png_default_settings(ps: *mut apt_png_settings);
     pub fn apt_png_bound(width: u32, height: u32, channels: c_int, ps: *const apt_png_settings, bytes: *mut u64) -> c_int;
@@ -150,6 +164,18 @@ pub struct apt_iq_settings {
     pub delta_freq: c_float,
     pub atten: c_float,
 }
+
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct apt_spectrum_settings { pub nfft: u32, pub max_segments: u32 }
+
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct apt_carrier_search { pub lo_hz: i32, pub hi_hz: i32, pub nfft: u32, pub max_segments: u32, pub min_snr_db: c_float }
+
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct apt_carrier { pub offset_hz: i32, pub centre_hz: c_float, pub snr_db: c_float, pub apt_score: c_float, pub is_apt: c_int }
 
 #[repr(C)]
 pub struct apt_stream { _private: [u8; 0] }
