@@ -662,6 +662,64 @@ int apt_stream_set_png_mode(apt_stream *st, const apt_png_settings *png);
 int apt_stream_finish_image(apt_stream *st, float *rows, uint64_t cap, uint64_t *nout, uint8_t *image, uint64_t image_cap,
                             uint64_t *image_n, apt_image_info *info);
 
+/* ------------------------------------------------------------------ long recordings: finding the passes */
+
+/* A recording kept in device memory (DESIGN.md §12), for finding the satellite passes in it and decoding each one without
+ * sending the samples over PCIe again.  The rule is the project's own definition:
+ *   e      the first stage of apt_decode at the work rate (resample + envelope, what apt_decoder_read_stage 0 returns);
+ *          the work rate must be a multiple of 4160 (else APT_ERR_WORK_RATE).  R = work_rate / 2 samples per image row.
+ *   q[w]   for w < W = max(0, floor(N_w / R) - 1): the Pearson correlation of e[wR, wR + R) with e[(w+1)R, (w+1)R + R);
+ *          0 when the denominator is 0 or not finite.  Near 1 during a pass, near 0 in noise.
+ *   passes the windows with q >= exit, joined into one group when fewer than max_gap windows lie between two of them; a
+ *          group is kept when some window in it has q >= enter and it spans at least min_length windows (first to last).
+ *          Group [a, b] is input samples [floor(a input_rate / 2), min(n, ceil((b + 2) input_rate / 2))).
+ * Zero fields of apt_pass_search take the defaults: enter 0.30, exit 0.15, max_gap_s 30, min_length_s 60; seconds become
+ * windows as floor(2 s).  APT_ERR_BAD_ARG unless 0 < exit <= enter <= 1 and both times are finite and >= 0. */
+typedef struct apt_pass_search {
+    float enter, exit, max_gap_s, min_length_s;
+} apt_pass_search;
+typedef struct apt_pass {
+    uint64_t start, end;          /* input samples [start, end) */
+    uint64_t first_window, windows;
+    float mean_quality, peak_quality;   /* over the pass's windows */
+} apt_pass;
+typedef struct apt_recording apt_recording;
+typedef struct apt_recording_info {
+    uint64_t samples;             /* n */
+    uint64_t work_samples;        /* N_w */
+    uint64_t windows;             /* W */
+    uint64_t device_bytes;        /* device memory the recording holds from create to destroy */
+    uint32_t input_rate, row_samples;   /* R */
+} apt_recording_info;
+
+/* Uploads n samples of `signal` (host memory, APT_F32 or APT_PCM16, kept in that format) to device `device` once, through
+ * the pinned staging ring when the buffer is pageable, and reserves everything apt_recording_quality needs.  A device
+ * allocation failure is APT_ERR_NOMEM with nothing left allocated.  Argument errors (NULL pointers, n == 0, an unknown
+ * format, the settings checks of apt_decode, a work rate that is not a multiple of 4160) come back before any device is
+ * touched. */
+int apt_recording_create(int device, const void *signal, int format, uint64_t n, uint32_t input_rate, const apt_settings *s,
+                         apt_recording **rec);
+void apt_recording_destroy(apt_recording *rec);
+int apt_recording_get_info(apt_recording *rec, apt_recording_info *info);
+/* q of the recording: the first stage runs over the resident samples in bounded chunks and k_pass_quality turns each
+ * chunk's envelope into q; only the W floats of q are copied back.  *nq receives W; q == NULL with cap == 0 counts only;
+ * cap < W is APT_ERR_CAPACITY.  The same bits on every run and for every chunk size. */
+int apt_recording_quality(apt_recording *rec, float *q, uint64_t cap, uint64_t *nq);
+/* The pass rule on q (host only, no device): out receives the passes in time order, *count their number; more than cap is
+ * APT_ERR_CAPACITY (out may be NULL when cap is 0).  n and input_rate are the recording's. */
+int apt_find_passes_quality(const float *q, uint64_t nq, uint64_t n, uint32_t input_rate, const apt_pass_search *ps,
+                            apt_pass *out, uint32_t cap, uint32_t *count);
+/* Decodes ranges[i].start .. ranges[i].end of the resident samples exactly as apt_decode / apt_decode_pcm16 (ps == NULL:
+ * f32 rows, caps in floats), apt_decode_image (ps, png == NULL) or apt_decode_png (ps and png) decode the host slice
+ * signal[start:end) with the same arguments: outs[i], nouts[i], statuses[i] and infos[i] (infos may be NULL) bit for bit.
+ * Each range is copied to a 16-byte aligned device buffer and decoded by a parked decoder; a failing range (too short, too
+ * few sync frames, capacity) leaves the others unaffected.  Only start, end of each range are read.  Argument errors (NULL
+ * pointers, a range empty or past n, the settings checks of apt_process and apt_png_encode, png without ps) come back
+ * before any device is touched with every status set.  Returns APT_OK or the first failing status. */
+int apt_recording_decode(apt_recording *rec, const apt_pass *ranges, uint32_t count, int sync,
+                         const apt_process_settings *ps, const apt_png_settings *png, void *const *outs,
+                         const uint64_t *caps, uint64_t *nouts, apt_image_info *infos, int *statuses);
+
 #ifdef __cplusplus
 }
 #endif

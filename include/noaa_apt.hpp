@@ -13,6 +13,7 @@
 // the compiled host side above the ABI; rust/ holds the equivalent Rust shim as source.
 #pragma once
 
+#include <algorithm>
 #include <cstdint>
 #include <functional>
 #include <stdexcept>
@@ -449,5 +450,90 @@ inline void decode_wav_png(const std::string &input, const std::string &output, 
     err::check(apt_decode_wav_png(input.c_str(), output.c_str(), &s, sync ? 1 : 0, &ps, &png, nullptr));
 }
 }  // namespace png
+
+// Finding the satellite passes in a long recording and decoding each one from one upload (DESIGN.md §12)
+namespace passes {
+inline std::vector<apt_pass> find_passes_quality(const std::vector<float> &q, uint64_t n, uint32_t input_rate,
+                                                 const apt_pass_search &ps = apt_pass_search{}) {
+    uint32_t count = 0;
+    const int st = apt_find_passes_quality(q.data(), q.size(), n, input_rate, &ps, nullptr, 0, &count);
+    if (st != APT_ERR_CAPACITY) err::check(st);
+    std::vector<apt_pass> out(count);
+    if (count) err::check(apt_find_passes_quality(q.data(), q.size(), n, input_rate, &ps, out.data(), count, &count));
+    return out;
+}
+struct Image {
+    int status;               // APT_OK, or the failure of this range alone
+    std::vector<uint8_t> png;
+    apt_image_info info;
+};
+// The samples (APT_F32 / APT_PCM16 host memory) uploaded once and kept on the device until the object goes away.
+class Recording {
+public:
+    Recording(const void *samples, int format, uint64_t n, Rate input_rate, const config::Settings &settings = {},
+              int device = 0)
+        : n_(n), rate_(input_rate.get_hz()), settings_(settings) {
+        const apt_settings st = settings.to_c();
+        err::check(apt_recording_create(device, samples, format, n, rate_, &st, &h_));
+    }
+    ~Recording() { apt_recording_destroy(h_); }
+    Recording(const Recording &) = delete;
+    Recording &operator=(const Recording &) = delete;
+    apt_recording_info info() const {
+        apt_recording_info i{};
+        err::check(apt_recording_get_info(h_, &i));
+        return i;
+    }
+    std::vector<float> quality() const {
+        uint64_t nq = 0;
+        err::check(apt_recording_quality(h_, nullptr, 0, &nq));
+        std::vector<float> q(nq);
+        if (nq) err::check(apt_recording_quality(h_, q.data(), q.size(), &nq));
+        return q;
+    }
+    std::vector<apt_pass> find_passes(const apt_pass_search &ps = apt_pass_search{}) const {
+        return find_passes_quality(quality(), n_, rate_, ps);
+    }
+    // Each range as apt_decode_png of the host slice; throws only for errors every range shares.
+    std::vector<Image> decode_png(const std::vector<apt_pass> &ranges, bool sync, const apt_process_settings &ps,
+                                  const apt_png_settings &png = png::default_settings()) const {
+        const uint32_t k = static_cast<uint32_t>(ranges.size());
+        std::vector<Image> out(k);
+        if (!k) return out;
+        const apt_settings st = settings_.to_c();
+        std::vector<void *> outs(k);
+        std::vector<uint64_t> caps(k), nouts(k, 0);
+        std::vector<apt_image_info> infos(k);
+        std::vector<int> statuses(k, 0);
+        for (uint32_t i = 0; i < k; ++i) {
+            uint64_t bound = 0, bytes = 0;
+            const uint64_t len = ranges[i].end > ranges[i].start ? ranges[i].end - ranges[i].start : 0;
+            err::check(apt_decode_len_bound(len, rate_, &st, &bound));
+            const uint32_t rows = static_cast<uint32_t>(std::max<uint64_t>(bound / 2080, 1));
+            err::check(apt_png_bound(2080, rows, ps.rgba ? 4 : 1, &png, &bytes));
+            out[i].png.resize(bytes ? bytes : 1);
+            outs[i] = out[i].png.data();
+            caps[i] = out[i].png.size();
+        }
+        const int rc = apt_recording_decode(h_, ranges.data(), k, sync ? 1 : 0, &ps, &png, outs.data(), caps.data(),
+                                            nouts.data(), infos.data(), statuses.data());
+        bool shared = rc != APT_OK;
+        for (uint32_t i = 0; i < k; ++i) shared = shared && statuses[i] == rc;
+        if (shared && rc == APT_ERR_BAD_ARG) err::check(rc);
+        for (uint32_t i = 0; i < k; ++i) {
+            out[i].status = statuses[i];
+            out[i].info = infos[i];
+            out[i].png.resize(statuses[i] == APT_OK ? nouts[i] : 0);
+        }
+        return out;
+    }
+
+private:
+    apt_recording *h_ = nullptr;
+    uint64_t n_;
+    uint32_t rate_;
+    config::Settings settings_;
+};
+}  // namespace passes
 
 }  // namespace noaa_apt

@@ -10,7 +10,7 @@ Mirrors the module layout of martinber/noaa-apt's hot path:
 Every compute call goes through the C ABI of libaptb200.so (include/aptb200.h) into hand-written
 sm_90a CUDA kernels.  There is no CPU path: importing works anywhere, computing needs a GPU.
 """
-from . import _lib, config, context, dsp, err, filters, frequency, image, iq, wav  # noqa: F401
+from . import _lib, config, context, dsp, err, filters, frequency, image, iq, passes, wav  # noqa: F401
 from . import decode as _decode_mod
 from .config import Settings
 from .context import Context
@@ -18,11 +18,12 @@ from .decode import (CARRIER_FREQ, FINAL_RATE, PX_PER_ROW, Decoder, Stream, deco
                      find_sync, generate_sync_frame, stream_geometry, stream_geometry_iq)
 from .frequency import Freq, Rate
 from .iq import Carrier, decode_iq_auto, decode_iq_channels, find_carriers, spectrum
+from .passes import Pass, Recording, decode_passes_png, find_passes_quality
 
 __all__ = ["decode", "decode_batch", "decode_len_bound", "find_sync", "generate_sync_frame", "Decoder", "Stream",
            "stream_geometry", "stream_geometry_iq", "spectrum", "find_carriers", "decode_iq_channels", "decode_iq_auto",
-           "Carrier",
-           "Settings", "Context", "Freq", "Rate", "dsp", "filters", "err", "config", "frequency", "image", "iq", "wav",
+           "Carrier", "Recording", "Pass", "find_passes_quality", "decode_passes_png",
+           "Settings", "Context", "Freq", "Rate", "dsp", "filters", "err", "config", "frequency", "image", "iq", "passes", "wav",
            "FINAL_RATE", "PX_PER_ROW", "CARRIER_FREQ"]
 
 

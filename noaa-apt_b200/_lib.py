@@ -118,6 +118,20 @@ class CPngGroupInfo(C.Structure):
                [(n, C.c_uint32) for n in ("rows", "spans", "blocks", "chunks")]
 
 
+class CPassSearch(C.Structure):
+    _fields_ = [("enter", C.c_float), ("exit", C.c_float), ("max_gap_s", C.c_float), ("min_length_s", C.c_float)]
+
+
+class CPass(C.Structure):
+    _fields_ = [("start", C.c_uint64), ("end", C.c_uint64), ("first_window", C.c_uint64), ("windows", C.c_uint64),
+                ("mean_quality", C.c_float), ("peak_quality", C.c_float)]
+
+
+class CRecordingInfo(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("samples", "work_samples", "windows", "device_bytes")] + \
+               [("input_rate", C.c_uint32), ("row_samples", C.c_uint32)]
+
+
 STATUS_CB = C.CFUNCTYPE(None, C.c_float, C.c_char_p, C.c_void_p)
 
 # name -> (restype, argtypes); every symbol include/aptb200.h declares.
@@ -254,6 +268,16 @@ SIGNATURES = {
     "apt_stream_set_png_mode": (C.c_int, [C.c_void_p, C.POINTER(CPngSettings)]),
     "apt_stream_finish_image": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, _u64p, C.c_void_p, C.c_uint64, _u64p,
                                           C.POINTER(CImageInfo)]),
+    "apt_recording_create": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_uint64, C.c_uint32, C.POINTER(CSettings),
+                                       C.POINTER(C.c_void_p)]),
+    "apt_recording_destroy": (None, [C.c_void_p]),
+    "apt_recording_get_info": (C.c_int, [C.c_void_p, C.POINTER(CRecordingInfo)]),
+    "apt_recording_quality": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, _u64p]),
+    "apt_find_passes_quality": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.POINTER(CPassSearch),
+                                          C.POINTER(CPass), C.c_uint32, C.POINTER(C.c_uint32)]),
+    "apt_recording_decode": (C.c_int, [C.c_void_p, C.POINTER(CPass), C.c_uint32, C.c_int, C.POINTER(CProcessSettings),
+                                       C.POINTER(CPngSettings), C.POINTER(C.c_void_p), _u64p, _u64p, C.POINTER(CImageInfo),
+                                       C.POINTER(C.c_int)]),
 }
 
 _lib = None

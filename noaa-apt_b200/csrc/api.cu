@@ -980,6 +980,20 @@ int decode_oneshot(const void *signal, int format, uint64_t n, uint32_t input_ra
 
 }  // namespace
 
+int aptb200::take_decoder(int device, uint32_t rate, const apt_settings &st, uint64_t n, apt_decoder **d) {
+    static const bool use_cache = getenv("APTB200_NO_CACHE") == nullptr;
+    *d = use_cache ? cache_take(device, rate, st, n) : nullptr;
+    if (*d) return APT_OK;
+    const uint64_t room = use_cache ? ((n + n / 8 + (1u << 20)) & ~((1ull << 20) - 1)) : n;
+    return apt_decoder_create(device, rate, &st, room, d);
+}
+
+void aptb200::park_decoder(int device, uint32_t rate, const apt_settings &st, apt_decoder *d) {
+    static const bool use_cache = getenv("APTB200_NO_CACHE") == nullptr;
+    if (use_cache) cache_put(device, rate, st, d);
+    else apt_decoder_destroy(d);
+}
+
 extern "C" int apt_bind_thread_to_device(int device) {
     if (require_device() != APT_OK) return 0;
     return bind_thread_to_device(device) ? 1 : 0;

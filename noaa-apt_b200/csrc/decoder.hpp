@@ -55,6 +55,10 @@ uint64_t plan_table_bytes(const Plan &p);
 int free_decoder_buffers(apt_decoder *d);
 // Grows the f32 copy of a PCM16 input to `alloc` samples when it holds fewer than `need`.
 int ensure_conv(apt_decoder *d, uint64_t need, uint64_t alloc);
+// The decoders apt_decode parks between calls: take_decoder hands out a parked decoder for (device, rate, settings) of at
+// least n samples, else creates one with apt_decode's head-room; park_decoder hands it back (APTB200_NO_CACHE: destroys it).
+int take_decoder(int device, uint32_t rate, const apt_settings &st, uint64_t n, apt_decoder **d);
+void park_decoder(int device, uint32_t rate, const apt_settings &st, apt_decoder *d);
 
 // Kernel accounting of a decoder: counts the launch and, when profiling, records the begin event of slot `name`;
 // returns the slot to close with prof_end (-1: none).

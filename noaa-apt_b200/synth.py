@@ -219,3 +219,71 @@ def apt_iq_multi(iq_rate, seconds=None, carriers=((0, 0, 0.0, None, 60.0),), ext
     if fmt == "cu8":
         return np.clip(np.rint(inter + 127.5), 0, 255).astype(np.uint8)
     return np.clip(np.rint(inter), -32768, 32767).astype(np.int16)
+
+
+def _real_noise(key, a, b):
+    """Real standard Gaussian noise for absolute sample indices [a, b): one Philox stream per (key, block of _BLOCK)."""
+    out = np.empty(b - a, dtype=np.float64)
+    i = a
+    while i < b:
+        blk = i // _BLOCK
+        lo, hi = i - blk * _BLOCK, min(b - blk * _BLOCK, _BLOCK)
+        out[i - a:i - a + hi - lo] = np.random.Generator(np.random.Philox(key=[key, blk])).standard_normal(_BLOCK)[lo:hi]
+        i += hi - lo
+    return out
+
+
+def _segments(rate_hz, layout):
+    """[(kind, first sample, end sample, pass seed)] of a layout of (kind, seconds[, pass seed]) entries."""
+    out, t = [], 0.0
+    for entry in layout:
+        kind, seconds = entry[0], float(entry[1])
+        if kind not in ("noise", "silence", "pass"):
+            raise ValueError(f"unknown segment kind {kind!r}")
+        a, b = int(round(t * rate_hz)), int(round((t + seconds) * rate_hz))
+        out.append((kind, a, b, int(entry[2]) if len(entry) > 2 else 0))
+        t += seconds
+    return out
+
+
+def apt_passes_len(rate_hz, layout):
+    return _segments(rate_hz, layout)[-1][2] if layout else 0
+
+
+def apt_passes_truth(rate_hz, layout, fade_s=10.0):
+    """(fade-in midpoint, fade-out midpoint) in samples of every "pass" segment of apt_passes."""
+    h = int(round(0.5 * fade_s * rate_hz))
+    return [(a + h, b - h) for kind, a, b, _ in _segments(rate_hz, layout) if kind == "pass"]
+
+
+def apt_passes(rate_hz, layout, seed=0, start=0, n_samples=None, noise_sigma=2000.0, fade_s=10.0, amplitude=20000.0):
+    """int16 samples [start, start + n) of a long recording made of segments, as a station recording all day sees it.
+
+    layout: (kind, seconds) or ("pass", seconds, pass_seed) entries, one after the other:
+      "noise"    Gaussian receiver noise of noise_sigma;
+      "silence"  exact zeros (the receiver off or squelched);
+      "pass"     the synthetic APT recording of pass_seed (apt_pcm16 without its own noise, from its first sample), its
+                 amplitude rising linearly from 0 over the first fade_s seconds and falling to 0 over the last, over the
+                 same receiver noise.
+    Every sample depends only on its index, so any slice, and so a 96 kHz x 10 h recording generated chunk by chunk,
+    gives the same numbers."""
+    segs = _segments(rate_hz, layout)
+    total = segs[-1][2] if segs else 0
+    if n_samples is None:
+        n_samples = total - start
+    if start < 0 or start + n_samples > total:
+        raise ValueError("slice outside the recording")
+    out = np.zeros(n_samples, dtype=np.float64)
+    fade = max(fade_s * rate_hz, 1.0)
+    for kind, a, b, pseed in segs:
+        lo, hi = max(a, start), min(b, start + n_samples)
+        if lo >= hi or kind == "silence":
+            continue
+        x = _real_noise(0x5A7 + seed, lo, hi) * noise_sigma if noise_sigma > 0 else np.zeros(hi - lo)
+        if kind == "pass":
+            k = np.arange(lo - a, hi - a, dtype=np.float64)
+            gain = np.clip(np.minimum(k / fade, (b - a - k) / fade), 0.0, 1.0)
+            sig = apt_pcm16(rate_hz, seed=pseed, n_samples=hi - lo, start=lo - a, noise_sigma=0.0, amplitude=amplitude)
+            x += gain * sig.astype(np.float64)
+        out[lo - start:hi - start] = x
+    return np.clip(np.rint(out), -32768, 32767).astype(np.int16)

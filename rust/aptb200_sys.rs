@@ -218,3 +218,35 @@ pub struct apt_png_settings { pub filter: c_int /* -1 adaptive, 0..4 fixed */, p
 impl Default for apt_png_settings {
     fn default() -> Self { apt_png_settings { filter: -1, matches: 1, block_bytes: 65536, rgb_from_rgba: 0 } }
 }
+
+// Long recordings: finding the passes (DESIGN.md §12)
+#[repr(C)]
+#[derive(Default, Clone, Copy, Debug)]
+pub struct apt_pass_search { pub enter: f32, pub exit: f32, pub max_gap_s: f32, pub min_length_s: f32 }   // 0: default
+
+#[repr(C)]
+#[derive(Default, Clone, Copy, Debug)]
+pub struct apt_pass { pub start: u64, pub end: u64, pub first_window: u64, pub windows: u64, pub mean_quality: f32,
+                      pub peak_quality: f32 }
+
+#[repr(C)]
+pub struct apt_recording { _private: [u8; 0] }
+
+#[repr(C)]
+#[derive(Default, Clone, Copy, Debug)]
+pub struct apt_recording_info { pub samples: u64, pub work_samples: u64, pub windows: u64, pub device_bytes: u64,
+                                pub input_rate: u32, pub row_samples: u32 }
+
+#[link(name = "aptb200")]
+extern "C" {
+    pub fn apt_recording_create(device: c_int, signal: *const c_void, format: c_int, n: u64, input_rate: u32,
+                                s: *const apt_settings, rec: *mut *mut apt_recording) -> c_int;
+    pub fn apt_recording_destroy(rec: *mut apt_recording);
+    pub fn apt_recording_get_info(rec: *mut apt_recording, info: *mut apt_recording_info) -> c_int;
+    pub fn apt_recording_quality(rec: *mut apt_recording, q: *mut f32, cap: u64, nq: *mut u64) -> c_int;
+    pub fn apt_find_passes_quality(q: *const f32, nq: u64, n: u64, input_rate: u32, ps: *const apt_pass_search,
+                                   out: *mut apt_pass, cap: u32, count: *mut u32) -> c_int;
+    pub fn apt_recording_decode(rec: *mut apt_recording, ranges: *const apt_pass, count: u32, sync: c_int,
+                                ps: *const apt_process_settings, png: *const apt_png_settings, outs: *const *mut c_void,
+                                caps: *const u64, nouts: *mut u64, infos: *mut apt_image_info, statuses: *mut c_int) -> c_int;
+}

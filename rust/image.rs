@@ -159,7 +159,7 @@ pub fn decode_to_png(
 
 /// The apt_process_settings parts of the PNG entry points: contrast mode and percent, rotation, the palette's RGB bytes
 /// (kept alive by the caller) and the tune values.
-fn png_process_parts(
+pub(crate) fn png_process_parts(
     contrast: &Contrast,
     rotate: &Rotate,
     color: Option<&ColorSettings>,
