@@ -720,6 +720,101 @@ int apt_recording_decode(apt_recording *rec, const apt_pass *ranges, uint32_t co
                          const apt_process_settings *ps, const apt_png_settings *png, void *const *outs,
                          const uint64_t *caps, uint64_t *nouts, apt_image_info *infos, int *statuses);
 
+/* ------------------------------------------------------------------ continuous feeds: watching for passes */
+
+/* The pass rule of apt_find_passes_quality fed q window by window (host only, no device; DESIGN.md §13).
+ *   APT_PASS_AOS  fires at the first window that joins the open group once the group has reached enter and spans
+ *                 min_length windows: from here on the group is certain to be kept.  pass holds the group so far, end 0.
+ *   APT_PASS_LOS  fires at the evaluation of window last + max_gap (no later window can join the group), or at finish
+ *                 (window = the number of windows fed).  pass is exactly the entry apt_find_passes_quality returns for the
+ *                 same q, mean_quality included; an LOS before finish has end = ceil((last + 2) input_rate / 2), which is
+ *                 within the recording whenever window last + max_gap exists.
+ * A group that is dropped (never reaches enter, or spans fewer than min_length windows) emits nothing.  apt_watch also
+ * emits APT_PASS_SEGMENT (apt_watch_settings).  Feeding all of q and then finishing gives the passes of
+ * apt_find_passes_quality, however q is split. */
+enum { APT_PASS_AOS = 1, APT_PASS_LOS = 2, APT_PASS_SEGMENT = 3 };
+typedef struct apt_pass_event {
+    int kind;                 /* APT_PASS_AOS, APT_PASS_LOS or APT_PASS_SEGMENT */
+    uint64_t window;          /* the window whose evaluation fired the event */
+    apt_pass pass;            /* SEGMENT: start = the new segment's first absolute sample, the rest 0 */
+} apt_pass_event;
+typedef struct apt_pass_tracker apt_pass_tracker;
+/* APT_ERR_BAD_ARG for NULL pointers, input_rate 0 and the search settings apt_find_passes_quality refuses. */
+int apt_pass_tracker_create(uint32_t input_rate, const apt_pass_search *search, apt_pass_tracker **t);
+/* The next nq windows.  events receives the events in order and *nev their number; cap < 2 * nq is APT_ERR_CAPACITY with
+ * the tracker unchanged. */
+int apt_pass_tracker_feed(apt_pass_tracker *t, const float *q, uint64_t nq, apt_pass_event *events, uint64_t cap,
+                          uint64_t *nev);
+/* The end of a recording of n input samples: the LOS of the open group, if it is kept (cap >= 1, else APT_ERR_CAPACITY
+ * with the tracker unchanged).  The tracker then starts over at window 0. */
+int apt_pass_tracker_finish(apt_pass_tracker *t, uint64_t n, apt_pass_event *events, uint64_t cap, uint64_t *nev);
+void apt_pass_tracker_destroy(apt_pass_tracker *t);
+
+/* A watcher (DESIGN.md §13): a continuous audio feed (rtl_fm, a sound card) pushed as it arrives, in fixed device memory.
+ * Each step (at most max_push samples) uploads the slice once, runs the first stage over the units that became complete
+ * and k_pass_quality over the windows whose two rows are final, feeds the new q to the pass rule, and feeds the open group
+ * from the watcher's own input window (device to device) to a streaming decoder with image / PNG output.  The callback
+ * receives the AOS of a pass and, at its LOS, the pass's decode.  For any split of the feed into pushes (F32 and PCM16 mixed),
+ * per segment: the q returned by pushes and finish, concatenated, equal apt_recording_quality of the segment's samples bit
+ * for bit; the LOS passes equal apt_find_passes_quality on them; each LOS's status, rows, info and data equal
+ * apt_recording_decode of the pass's range with the same sync, ps and png.  Statuses beyond the decode's own: a pass with
+ * more than max_rows rows is APT_ERR_CAPACITY with rows set (the watcher continues), a kept pass too short to decode is
+ * APT_ERR_TOO_SHORT.
+ * Segments: the first stage keeps work-rate indices below 2^32.  When no group is open and the segment holds at least T
+ * work samples (2^31; APTB200_WATCH_SEGMENT=n sets T), the next step first finishes the segment as apt_watch_finish does,
+ * emits APT_PASS_SEGMENT with the new segment's first absolute sample, and starts a new segment there (window indices
+ * restart at 0).  A group still open at 2T is closed as at finish.  Samples in events are absolute (since create / reset). */
+typedef struct apt_watch apt_watch;
+typedef struct apt_watch_settings {
+    int sync;
+    apt_pass_search search;            /* zero fields: the defaults of apt_find_passes_quality */
+    const apt_process_settings *ps;    /* NULL: each pass ends in its f32 rows */
+    const apt_png_settings *png;       /* with ps: each pass ends in its PNG file; NULL: in its pixels */
+    uint64_t max_rows;                 /* the longest pass that gets its image / rows; 0: 2400 */
+    uint64_t max_push;                 /* samples per internal step, as apt_stream; 0: input_rate */
+} apt_watch_settings;
+typedef struct apt_watch_event {
+    apt_pass_event ev;                 /* samples absolute since create / reset; windows those of the segment */
+    uint32_t index;                    /* pass number since create / reset */
+    int status;                        /* LOS: the pass decode's status */
+    uint64_t rows;                     /* LOS: the pass's row count */
+    apt_image_info info;               /* LOS with ps */
+    const void *data;                  /* LOS: f32 rows, pixels or PNG file; valid during the callback only */
+    uint64_t bytes;                    /* of data */
+} apt_watch_event;
+typedef struct apt_watch_info {
+    uint64_t samples_in;               /* since create / reset */
+    uint64_t segment_start;            /* absolute first sample of the current segment */
+    uint64_t windows;                  /* windows of the segment evaluated so far */
+    uint64_t passes;                   /* LOS events since create / reset */
+    uint64_t open;                     /* 1 while a group is open */
+    uint64_t device_bytes;             /* device memory held from create to destroy */
+    uint64_t max_push;
+    uint64_t latency_windows;          /* windows a push can leave unevaluated behind its last sample */
+} apt_watch_info;
+typedef void (*apt_watch_cb)(const apt_watch_event *ev, void *user);
+/* Everything (quality path, pass stream, image / PNG output) is allocated here; push, finish and reset allocate nothing.
+ * Argument errors come back before any device is touched: NULL pointers, the search settings, the settings apt_process and
+ * apt_png_encode refuse, png without ps, max_rows or max_push out of range, and the settings apt_stream_create refuses. */
+int apt_watch_create(int device, uint32_t input_rate, const apt_settings *s, const apt_watch_settings *ws, apt_watch_cb cb,
+                     void *user, apt_watch **w);
+/* The device_bytes (and max_push, latency_windows) apt_watch_create would report, on the host. */
+int apt_watch_geometry(uint32_t input_rate, const apt_settings *s, const apt_watch_settings *ws, apt_watch_info *info);
+/* The q floats a push of n samples can return at most. */
+int apt_watch_push_bound(apt_watch *w, uint64_t n, uint64_t *cap_q);
+/* n samples of the feed (APT_F32 or APT_PCM16); q receives the new windows' quality, *nq their number (cap below
+ * apt_watch_push_bound: APT_ERR_CAPACITY before any work).  Events are delivered through the callback during the call.
+ * A pass's decode status does not fail the push. */
+int apt_watch_push(apt_watch *w, const void *samples, int format, uint64_t n, float *q, uint64_t cap, uint64_t *nq);
+/* The end of the feed: the tail windows (cap: apt_watch_push_bound(w, 0)) and the LOS of a group still open (end = n).
+ * Pushing again needs apt_watch_reset. */
+int apt_watch_finish(apt_watch *w, float *q, uint64_t cap, uint64_t *nq);
+/* A new feed with the same settings and buffers. */
+int apt_watch_reset(apt_watch *w);
+int apt_watch_get_info(apt_watch *w, apt_watch_info *info);
+void apt_watch_destroy(apt_watch *w);
+/* Every call into a watcher from its own callback is APT_ERR_BAD_ARG. */
+
 #ifdef __cplusplus
 }
 #endif

@@ -15,6 +15,7 @@
 
 #include <algorithm>
 #include <cstdint>
+#include <exception>
 #include <functional>
 #include <stdexcept>
 #include <string>
@@ -533,6 +534,75 @@ private:
     uint64_t n_;
     uint32_t rate_;
     config::Settings settings_;
+};
+
+// A continuous feed watched for satellite passes (apt_watch, DESIGN.md §13).  on_event receives every AOS, SEGMENT and
+// LOS on the pushing thread; an LOS carries the pass's decode (ev.data valid during the call only).  An exception thrown
+// by on_event is kept and rethrown when the push or finish returns; it never crosses the library.
+class Watch {
+public:
+    using Callback = std::function<void(const apt_watch_event &)>;
+    Watch(Rate input_rate, Callback on_event, const apt_watch_settings &ws = apt_watch_settings{},
+          const config::Settings &settings = {}, int device = 0)
+        : cb_(std::move(on_event)) {
+        const apt_settings st = settings.to_c();
+        err::check(apt_watch_create(device, input_rate.get_hz(), &st, &ws, &Watch::trampoline, this, &h_));
+    }
+    ~Watch() { apt_watch_destroy(h_); }
+    Watch(const Watch &) = delete;
+    Watch &operator=(const Watch &) = delete;
+    // The quality of the windows that became final.
+    std::vector<float> push(const float *samples, uint64_t n) { return push_format(samples, APT_F32, n); }
+    std::vector<float> push(const int16_t *samples, uint64_t n) { return push_format(samples, APT_PCM16, n); }
+    std::vector<float> finish() {
+        std::vector<float> q(bound(0));
+        uint64_t nq = 0;
+        const int rc = apt_watch_finish(h_, q.data(), q.size(), &nq);
+        rethrow();
+        err::check(rc);
+        q.resize(nq);
+        return q;
+    }
+    void reset() { err::check(apt_watch_reset(h_)); }
+    apt_watch_info info() const {
+        apt_watch_info i{};
+        err::check(apt_watch_get_info(h_, &i));
+        return i;
+    }
+
+private:
+    static void trampoline(const apt_watch_event *ev, void *user) {
+        Watch *w = static_cast<Watch *>(user);
+        if (!w->cb_ || w->error_) return;
+        try {
+            w->cb_(*ev);
+        } catch (...) {
+            w->error_ = std::current_exception();
+        }
+    }
+    uint64_t bound(uint64_t n) {
+        uint64_t cap = 0;
+        err::check(apt_watch_push_bound(h_, n, &cap));
+        return std::max<uint64_t>(cap, 1);
+    }
+    std::vector<float> push_format(const void *samples, int format, uint64_t n) {
+        std::vector<float> q(bound(n));
+        uint64_t nq = 0;
+        const int rc = apt_watch_push(h_, samples, format, n, q.data(), q.size(), &nq);
+        rethrow();
+        err::check(rc);
+        q.resize(nq);
+        return q;
+    }
+    void rethrow() {
+        if (!error_) return;
+        std::exception_ptr e = error_;
+        error_ = nullptr;
+        std::rethrow_exception(e);
+    }
+    Callback cb_;
+    std::exception_ptr error_;
+    apt_watch *h_ = nullptr;
 };
 }  // namespace passes
 

@@ -132,7 +132,30 @@ class CRecordingInfo(C.Structure):
                [("input_rate", C.c_uint32), ("row_samples", C.c_uint32)]
 
 
+PASS_AOS, PASS_LOS, PASS_SEGMENT = 1, 2, 3
+
+
+class CPassEvent(C.Structure):
+    _fields_ = [("kind", C.c_int), ("window", C.c_uint64), ("pass_", CPass)]
+
+
+class CWatchSettings(C.Structure):
+    _fields_ = [("sync", C.c_int), ("search", CPassSearch), ("ps", C.c_void_p), ("png", C.c_void_p), ("max_rows", C.c_uint64),
+                ("max_push", C.c_uint64)]
+
+
+class CWatchEvent(C.Structure):
+    _fields_ = [("ev", CPassEvent), ("index", C.c_uint32), ("status", C.c_int), ("rows", C.c_uint64), ("info", CImageInfo),
+                ("data", C.c_void_p), ("bytes", C.c_uint64)]
+
+
+class CWatchInfo(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("samples_in", "segment_start", "windows", "passes", "open", "device_bytes",
+                                          "max_push", "latency_windows")]
+
+
 STATUS_CB = C.CFUNCTYPE(None, C.c_float, C.c_char_p, C.c_void_p)
+WATCH_CB = C.CFUNCTYPE(None, C.POINTER(CWatchEvent), C.c_void_p)
 
 # name -> (restype, argtypes); every symbol include/aptb200.h declares.
 _u64p = C.POINTER(C.c_uint64)
@@ -278,6 +301,19 @@ SIGNATURES = {
     "apt_recording_decode": (C.c_int, [C.c_void_p, C.POINTER(CPass), C.c_uint32, C.c_int, C.POINTER(CProcessSettings),
                                        C.POINTER(CPngSettings), C.POINTER(C.c_void_p), _u64p, _u64p, C.POINTER(CImageInfo),
                                        C.POINTER(C.c_int)]),
+    "apt_pass_tracker_create": (C.c_int, [C.c_uint32, C.POINTER(CPassSearch), C.POINTER(C.c_void_p)]),
+    "apt_pass_tracker_feed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(CPassEvent), C.c_uint64, _u64p]),
+    "apt_pass_tracker_finish": (C.c_int, [C.c_void_p, C.c_uint64, C.POINTER(CPassEvent), C.c_uint64, _u64p]),
+    "apt_pass_tracker_destroy": (None, [C.c_void_p]),
+    "apt_watch_create": (C.c_int, [C.c_int, C.c_uint32, C.POINTER(CSettings), C.POINTER(CWatchSettings), WATCH_CB, C.c_void_p,
+                                   C.POINTER(C.c_void_p)]),
+    "apt_watch_geometry": (C.c_int, [C.c_uint32, C.POINTER(CSettings), C.POINTER(CWatchSettings), C.POINTER(CWatchInfo)]),
+    "apt_watch_push_bound": (C.c_int, [C.c_void_p, C.c_uint64, _u64p]),
+    "apt_watch_push": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_uint64, C.c_void_p, C.c_uint64, _u64p]),
+    "apt_watch_finish": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, _u64p]),
+    "apt_watch_reset": (C.c_int, [C.c_void_p]),
+    "apt_watch_get_info": (C.c_int, [C.c_void_p, C.POINTER(CWatchInfo)]),
+    "apt_watch_destroy": (None, [C.c_void_p]),
 }
 
 _lib = None

@@ -6,6 +6,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <memory>
+#include <new>
 
 #include "common.hpp"
 #include "hostpool.hpp"
@@ -83,6 +84,12 @@ int plan_chunks(apt_recording *r, uint64_t &e_cap, uint64_t &conv_cap) {
 }
 
 }  // namespace
+
+int aptb200::launch_pass_quality(cudaStream_t s, const float *e, uint64_t w0, uint64_t count, uint32_t R, float *q) {
+    k_pass_quality<<<static_cast<unsigned>(count), kPassQualityThreads, 0, s>>>(e, w0, R, q);
+    APT_CUDA(cudaGetLastError());
+    return APT_OK;
+}
 
 int aptb200::make_pass_rule(const apt_pass_search *ps, PassRule &r) {
     r = PassRule{};
@@ -200,9 +207,7 @@ extern "C" int apt_recording_quality(apt_recording *rec, float *q, uint64_t cap,
             }
             APT_TRY(front_launch(c, f, rec->front, rec->d_sig, rec->format, conv_biased, rec->n, rec->nwork, k.u0, k.u1, true,
                                  p.cosphi2, p.sinphi, rec->d_scratch ? rec->d_scratch - k.e0 : nullptr, e, nullptr));
-            k_pass_quality<<<static_cast<unsigned>(k.w1 - k.w0), kPassQualityThreads, 0, rec->stream>>>(e, k.w0, rec->row,
-                                                                                                      rec->d_q);
-            APT_CUDA(cudaGetLastError());
+            APT_TRY(launch_pass_quality(rec->stream, e, k.w0, k.w1 - k.w0, rec->row, rec->d_q));
         }
         APT_CUDA(cudaMemcpyAsync(q, rec->d_q, rec->windows * sizeof(float), cudaMemcpyDeviceToHost, rec->stream));
         APT_CUDA(cudaStreamSynchronize(rec->stream));
@@ -220,47 +225,63 @@ extern "C" int apt_find_passes_quality(const float *q, uint64_t nq, uint64_t n, 
     if (input_rate == 0) return fail(APT_ERR_BAD_ARG, "input_rate is 0");
     PassRule rule;
     APT_TRY(make_pass_rule(ps, rule));
-    const uint64_t rate = input_rate;
     uint32_t total = 0;
-    auto close = [&](uint64_t a, uint64_t b, bool entered) {
-        const uint64_t windows = b - a + 1;
-        if (!entered || windows < rule.min_length) return;
+    auto keep = [&](const apt_pass_event &e) {
+        if (e.kind != APT_PASS_LOS) return;
         if (total < cap) {
-            double sum = 0.0;
-            float peak = q[a];
-            for (uint64_t w = a; w <= b; ++w) {
-                sum += static_cast<double>(q[w]);
-                peak = std::max(peak, q[w]);
-            }
-            apt_pass &o = out[total];
-            o.start = a * rate / 2;
-            o.end = std::min<uint64_t>(n, ((b + 2) * rate + 1) / 2);
-            o.first_window = a;
-            o.windows = windows;
-            o.mean_quality = static_cast<float>(sum / static_cast<double>(windows));
-            o.peak_quality = peak;
+            out[total] = e.pass;
+            out[total].end = std::min(out[total].end, n);
         }
         ++total;
     };
-    bool open = false, entered = false;
-    uint64_t first = 0, last = 0;
-    for (uint64_t w = 0; w < nq; ++w) {
-        if (!(q[w] >= rule.exit)) continue;
-        if (open && w - last - 1 < rule.max_gap) {
-            last = w;
-        } else {
-            if (open) close(first, last, entered);
-            open = true;
-            entered = false;
-            first = last = w;
-        }
-        entered = entered || q[w] >= rule.enter;
+    PassTracker t(rule, input_rate);
+    try {
+        for (uint64_t w = 0; w < nq; ++w) t.feed(q[w], keep);
+        t.finish(n, keep);
+    } catch (const std::bad_alloc &) {
+        return fail(APT_ERR_NOMEM, "out of host memory");
     }
-    if (open) close(first, last, entered);
     *count = total;
     if (total > cap) return fail(APT_ERR_CAPACITY, "%u passes, room for %u", total, cap);
     return APT_OK;
 }
+
+extern "C" int apt_pass_tracker_create(uint32_t input_rate, const apt_pass_search *search, apt_pass_tracker **t) {
+    if (!t) return fail(APT_ERR_BAD_ARG, "null argument");
+    *t = nullptr;
+    if (input_rate == 0) return fail(APT_ERR_BAD_ARG, "input_rate is 0");
+    PassRule rule;
+    APT_TRY(make_pass_rule(search, rule));
+    *t = new (std::nothrow) apt_pass_tracker{PassTracker(rule, input_rate)};
+    return *t ? APT_OK : fail(APT_ERR_NOMEM, "out of host memory");
+}
+
+extern "C" int apt_pass_tracker_feed(apt_pass_tracker *t, const float *q, uint64_t nq, apt_pass_event *events, uint64_t cap,
+                                     uint64_t *nev) {
+    if (!t || !nev || (nq && (!q || !events))) return fail(APT_ERR_BAD_ARG, "null argument");
+    *nev = 0;
+    if (cap < 2 * nq) return fail(APT_ERR_CAPACITY, "events needs room for %llu entries", 2ull * (unsigned long long)nq);
+    uint64_t k = 0;
+    try {
+        for (uint64_t w = 0; w < nq; ++w) t->t.feed(q[w], [&](const apt_pass_event &e) { events[k++] = e; });
+    } catch (const std::bad_alloc &) {
+        return fail(APT_ERR_NOMEM, "out of host memory");
+    }
+    *nev = k;
+    return APT_OK;
+}
+
+extern "C" int apt_pass_tracker_finish(apt_pass_tracker *t, uint64_t n, apt_pass_event *events, uint64_t cap, uint64_t *nev) {
+    if (!t || !nev) return fail(APT_ERR_BAD_ARG, "null argument");
+    *nev = 0;
+    if (!events || cap < 1) return fail(APT_ERR_CAPACITY, "events needs room for 1 entry");
+    uint64_t k = 0;
+    t->t.finish(n, [&](const apt_pass_event &e) { events[k++] = e; });
+    *nev = k;
+    return APT_OK;
+}
+
+extern "C" void apt_pass_tracker_destroy(apt_pass_tracker *t) { delete t; }
 
 extern "C" int apt_recording_decode(apt_recording *rec, const apt_pass *ranges, uint32_t count, int sync,
                                     const apt_process_settings *ps, const apt_png_settings *png, void *const *outs,

@@ -240,10 +240,16 @@ void PngWork::release() {
     cap_n = cap_n_pos = cap_blocks = cap_out = cap_img = 0;
 }
 
-size_t PngWork::device_bytes() const {
-    return cap_n + cap_n_pos * 4 + cap_blocks * (2 * (kPngLit + kPngDist) * 4 + kPngHdrWords * 4 + 4 + 4 * 8) + cap_out +
-           cap_img * (sizeof(PngCtl) + sizeof(PngImage));
+namespace {
+size_t work_bytes(u64 n, u64 n_pos, u64 blocks, u64 out, u64 img) {
+    return n + n_pos * 4 + blocks * (2 * (kPngLit + kPngDist) * 4 + kPngHdrWords * 4 + 4 + 4 * 8) + out +
+           img * (sizeof(PngCtl) + sizeof(PngImage));
 }
+}  // namespace
+
+size_t PngWork::device_bytes() const { return work_bytes(cap_n, cap_n_pos, cap_blocks, cap_out, cap_img); }
+
+size_t PngWork::bytes_for(const PngLayout &l) { return work_bytes(l.f_bytes, l.f_bytes, l.blocks, l.out_bytes, l.img.size()); }
 
 int png_encode_device(const LaunchCtx &c, const PngPlan *plans, const unsigned char *const *pixels, u32 g, PngWork &w,
                       KernelHook *hook) {

@@ -89,6 +89,7 @@ struct PngWork {
     int reserve(const PngLayout &lay);
     void release();
     size_t device_bytes() const;
+    static size_t bytes_for(const PngLayout &lay);   // device_bytes() after reserve(lay) on an empty workspace (host only)
 };
 
 // Enqueues the whole encode of `g` images (plans[k] and device pixels[k], height * width * in_ch bytes, as png_layout

@@ -18,6 +18,7 @@
 #include "decoder.hpp"
 #include "filters_host.hpp"
 #include "launch.hpp"
+#include "stream.hpp"
 
 using namespace aptb200;
 
@@ -94,7 +95,7 @@ struct ImageOut {
     PngWork png_work;                 // reserved for a max_rows image
 
     // The stage's and the image's device memory (PostBuffers::alloc and upload_palette for max_rows rows).
-    uint64_t post_bytes() const {
+    static uint64_t post_bytes(const PostPlan &plan, uint64_t max_rows) {
         return sizeof(PostCtl) + 3 * max_rows * sizeof(float) + (plan.hist ? sizeof(ProcCtl) : 0) +
                (plan.finish ? max_rows * kPxPerRow : 0) + (plan.palette ? 256 * 256 * sizeof(u32) : 0) +
                max_rows * kPxPerRow * (sizeof(float) + plan.bpp);
@@ -184,15 +185,8 @@ int reset_state(apt_stream *st) {
     return APT_OK;
 }
 
-// Moves the tail [keep, end) of a window based at `base` to its front when that does not overlap.
 int compact(apt_stream *st, float *buf, uint64_t &base, uint64_t keep, uint64_t end) {
-    keep = floor16(std::min(keep, end));
-    if (keep <= base) return APT_OK;
-    const uint64_t drop = keep - base, tail = end - keep;
-    if (tail > drop) return APT_OK;
-    if (tail) APT_CUDA(cudaMemcpyAsync(buf, buf + drop, tail * sizeof(float), cudaMemcpyDeviceToDevice, st->dec.stream));
-    base = keep;
-    return APT_OK;
+    return window_compact(st->dec.stream, buf, base, keep, end);
 }
 
 // First envelope sample a later step can still read.
@@ -246,25 +240,21 @@ int keep_rows(apt_stream *st, uint64_t first, uint64_t end, const float *src) {
     return APT_OK;
 }
 
-// The new audio of one step into the input window, from either source: audio pushes are uploaded as they are (PCM16 cast
-// into the f32 window, so pushes may mix formats); I/Q pushes are converted into the cf32 window and every audio sample
-// they complete is demodulated into the input window.  `added` receives the number of new audio samples.
-int upload(apt_stream *st, const void *host, int format, uint64_t n, uint64_t &added) {
+// The new audio of one step into the input window, from any source: audio pushes are uploaded as they are (PCM16 cast
+// into the f32 window, so pushes may mix formats), or copied device to device from f32 samples already on the device
+// (`on_device`, stream_push_device); I/Q pushes are converted into the cf32 window and every audio sample they complete is
+// demodulated into the input window.  `added` receives the number of new audio samples.
+int upload(apt_stream *st, const void *src, bool on_device, int format, uint64_t n, uint64_t &added) {
     apt_decoder &d = st->dec;
     const LaunchCtx c{d.stream, d.sm_count};
     const uint64_t off = st->samples_in - st->in_base;
     if (!st->iq) {
         if (off + n > st->g.cap_in) return fail(APT_ERR_BAD_ARG, "internal: input window overflow");
-        if (format == APT_PCM16) {
-            APT_CUDA(cudaMemcpyAsync(st->d_pcm, host, n * 2, cudaMemcpyHostToDevice, d.stream));
-            APT_TRY(launch_pcm16_to_f32(c, st->d_pcm, n, st->d_conv));
-            APT_CUDA(cudaMemcpyAsync(st->d_in + off, st->d_conv, n * 4, cudaMemcpyDeviceToDevice, d.stream));
-        } else {
-            APT_CUDA(cudaMemcpyAsync(st->d_in + off, host, n * 4, cudaMemcpyHostToDevice, d.stream));
-        }
+        APT_TRY(window_upload(c, src, on_device, format, n, st->d_pcm, st->d_conv, st->d_in + off));
         added = n;
         return APT_OK;
     }
+    const void *host = src;
     const IqPlan &q = st->iqp;
     // the cf32 window keeps what the next audio output reads; its tail moves to the front when that does not overlap
     uint64_t xa, xb;
@@ -287,7 +277,8 @@ int upload(apt_stream *st, const void *host, int format, uint64_t n, uint64_t &a
 }
 
 // One step: `n` new samples (maybe none) and, when `finish`, the end of the recording.
-int step(apt_stream *st, const void *host, int format, uint64_t n, bool finish, float *rows, uint64_t &nout, int &status) {
+int step(apt_stream *st, const void *src, bool on_device, int format, uint64_t n, bool finish, float *rows, uint64_t &nout,
+         int &status) {
     apt_decoder &d = st->dec;
     const Plan &p = d.plan;
     const Geom &g = st->g;
@@ -295,7 +286,7 @@ int step(apt_stream *st, const void *host, int format, uint64_t n, bool finish, 
     APT_TRY(compact_all(st));
     if (n) {
         uint64_t added = 0;
-        APT_TRY(upload(st, host, format, n, added));
+        APT_TRY(upload(st, src, on_device, format, n, added));
         st->samples_in += added;
     }
     const uint64_t N = st->samples_in;
@@ -305,16 +296,9 @@ int step(apt_stream *st, const void *host, int format, uint64_t n, bool finish, 
         return APT_OK;
     }
     // ---- first stage: the units whose input span is complete (all of them at the end) ----
-    const uint64_t u_hi = p.front.complete(N, nw, finish);
     const uint64_t work_before = st->work_final;
-    if (u_hi > st->units_done) {
-        const uint64_t work_hi = finish ? nw : std::min(nw, u_hi * p.front.unit_out);
-        if (work_hi - st->e_base > g.cap_e) return fail(APT_ERR_BAD_ARG, "internal: envelope window overflow");
-        APT_TRY(front_launch(c, p.front, d.front, st->d_in - st->in_base, APT_F32, nullptr, N, nw, st->units_done, u_hi, true,
-                             p.cosphi2, p.sinphi, st->d_r ? st->d_r - st->e_base : nullptr, st->d_e - st->e_base, nullptr));
-        st->units_done = u_hi;
-        st->work_final = work_hi;
-    }
+    APT_TRY(front_advance(c, p, d.front, st->d_in - st->in_base, N, finish, g.cap_e, st->d_r, st->d_e, st->e_base,
+                          st->units_done, st->work_final));
     const u32 ntaps = static_cast<u32>(p.lp.size());
     float *e = st->d_e - st->e_base;
     if (!st->sync) {   // rows r with (r+1)*row <= work_final (decode.rs:141-147)
@@ -580,7 +564,7 @@ extern "C" int apt_stream_push(apt_stream *st, const void *samples, int format, 
     int status = APT_OK;
     for (uint64_t done = 0; done < n;) {
         const uint64_t k = std::min(per_step, n - done);
-        APT_TRY(step(st, static_cast<const char *>(samples) + done * sb, format, k, false, rows, got, status));
+        APT_TRY(step(st, static_cast<const char *>(samples) + done * sb, false, format, k, false, rows, got, status));
         done += k;
     }
     if (nout) *nout = got;
@@ -597,7 +581,7 @@ extern "C" int apt_stream_finish(apt_stream *st, float *rows, uint64_t cap, uint
     APT_CUDA(cudaSetDevice(st->dec.device));
     uint64_t got = 0;
     int status = APT_OK;
-    APT_TRY(step(st, nullptr, APT_F32, 0, true, rows, got, status));
+    APT_TRY(step(st, nullptr, false, APT_F32, 0, true, rows, got, status));
     st->finished = true;
     if (nout) *nout = got;
     return status;
@@ -677,7 +661,7 @@ extern "C" int apt_stream_set_process_mode(apt_stream *st, const apt_process_set
     APT_CUDA(cudaMalloc(&o.d_rows, max_rows * kPxPerRow * sizeof(float)));
     APT_CUDA(cudaMalloc(&o.d_px, max_rows * kPxPerRow * plan.bpp));
     APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&o.h_png), sizeof(PngCtl), cudaHostAllocDefault));
-    o.bytes = o.post_bytes();
+    o.bytes = ImageOut::post_bytes(o.plan, o.max_rows);
     rollback.armed = false;
     return APT_OK;
 }
@@ -741,4 +725,79 @@ extern "C" int apt_stream_get_info(apt_stream *st, apt_stream_info *info) {
     info->max_push = st->iq ? st->iq_max_push : st->max_push;
     info->device_bytes = st->g.bytes + st->img.bytes + st->img.png_work.device_bytes();
     return APT_OK;
+}
+
+// ---- shared with the watcher (stream.hpp) ----
+
+int aptb200::window_compact(cudaStream_t s, float *buf, uint64_t &base, uint64_t keep, uint64_t end) {
+    keep = floor16(std::min(keep, end));
+    if (keep <= base) return APT_OK;
+    const uint64_t drop = keep - base, tail = end - keep;
+    if (tail > drop) return APT_OK;
+    if (tail) APT_CUDA(cudaMemcpyAsync(buf, buf + drop, tail * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    base = keep;
+    return APT_OK;
+}
+
+int aptb200::window_upload(const LaunchCtx &c, const void *src, bool on_device, int format, uint64_t n, int16_t *d_pcm,
+                           float *d_conv, float *dst) {
+    if (on_device) {
+        APT_CUDA(cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyDeviceToDevice, c.stream));
+    } else if (format == APT_PCM16) {
+        APT_CUDA(cudaMemcpyAsync(d_pcm, src, n * 2, cudaMemcpyHostToDevice, c.stream));
+        APT_TRY(launch_pcm16_to_f32(c, d_pcm, n, d_conv));
+        APT_CUDA(cudaMemcpyAsync(dst, d_conv, n * 4, cudaMemcpyDeviceToDevice, c.stream));
+    } else {
+        APT_CUDA(cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyHostToDevice, c.stream));
+    }
+    return APT_OK;
+}
+
+int aptb200::front_advance(const LaunchCtx &c, const Plan &p, const FrontTables &t, const float *in, uint64_t N, bool finish,
+                           uint64_t cap_e, float *d_r, float *d_e, uint64_t e_base, uint64_t &units_done, uint64_t &work_final) {
+    const uint64_t nw = p.front.work_len(N);
+    const uint64_t u_hi = p.front.complete(N, nw, finish);
+    if (u_hi <= units_done) return APT_OK;
+    const uint64_t work_hi = finish ? nw : std::min(nw, u_hi * p.front.unit_out);
+    if (work_hi - e_base > cap_e) return fail(APT_ERR_BAD_ARG, "internal: envelope window overflow");
+    APT_TRY(front_launch(c, p.front, t, in, APT_F32, nullptr, N, nw, units_done, u_hi, true, p.cosphi2, p.sinphi,
+                         d_r ? d_r - e_base : nullptr, d_e - e_base, nullptr));
+    units_done = u_hi;
+    work_final = work_hi;
+    return APT_OK;
+}
+
+int aptb200::stream_push_device(apt_stream *st, const float *d_src, uint64_t n, float *rows, uint64_t cap, uint64_t *nout) {
+    *nout = 0;
+    if (st->iq || st->finished) return fail(APT_ERR_BAD_ARG, "internal: device push into an I/Q or finished stream");
+    if (n == 0) return APT_OK;
+    if (st->dec.plan.front.work_len(st->samples_in + n) >= (1ull << 32))
+        return fail(APT_ERR_BAD_ARG, "recording too long: the work-rate index would pass 2^32-1");
+    const uint64_t need = rows_bound(st, n);
+    if (need && (!rows || cap < need)) return fail(APT_ERR_CAPACITY, "rows needs room for %llu floats", (unsigned long long)need);
+    uint64_t got = 0;
+    int status = APT_OK;
+    for (uint64_t done = 0; done < n;) {
+        const uint64_t k = std::min(st->max_push, n - done);
+        APT_TRY(step(st, d_src + done, true, APT_F32, k, false, rows, got, status));
+        done += k;
+    }
+    *nout = got;
+    return status;
+}
+
+cudaStream_t aptb200::stream_cuda(const apt_stream *st) { return st->dec.stream; }
+
+uint64_t aptb200::stream_rows_out(const apt_stream *st) { return st->rows_out; }
+
+uint64_t aptb200::stream_image_bytes(const PostPlan &plan, uint64_t max_rows, const apt_png_settings *png) {
+    uint64_t bytes = ImageOut::post_bytes(plan, max_rows);
+    if (png) {
+        PngPlan pp;
+        PngLayout lay;
+        if (make_png(kPxPerRow, static_cast<uint32_t>(max_rows), plan.bpp, png, pp) == APT_OK &&
+            png_layout(&pp, nullptr, 1, lay) == APT_OK)
+            bytes += PngWork::bytes_for(lay);
+    }
+    return bytes;
 }

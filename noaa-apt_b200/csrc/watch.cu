@@ -1,0 +1,495 @@
+// Watching a continuous audio feed for satellite passes (include/aptb200.h apt_watch_*, DESIGN.md §13).
+//
+// Every step (one slice of at most max_push samples) runs on one CUDA stream, the pass stream's:
+//   upload into the f32 input window -> first stage over the units whose input is complete (stream.hpp, the code the
+//   streaming decoder runs) -> k_pass_quality over the windows whose two rows are final -> the new q back to the host ->
+//   the pass rule (PassTracker) -> the open group fed device to device from the input window to the pass stream, an
+//   apt_stream with the caller's image / PNG output, which is finished at the group's LOS and reset.
+// The input window keeps what the pass stream or a later window can still read; the envelope window keeps the rows of the
+// next window.  Both are sized at create from the arguments alone.
+#include <algorithm>
+#include <cstdlib>
+#include <cstring>
+#include <memory>
+#include <new>
+#include <vector>
+
+#include "aptb200.h"
+#include "common.hpp"
+#include "decoder.hpp"
+#include "passes.hpp"
+#include "png.hpp"
+#include "post.hpp"
+#include "stream.hpp"
+
+using namespace aptb200;
+
+namespace {
+
+
+// Work samples after which a segment ends at the next step with no group open (a group still open at 2T is closed).
+uint64_t segment_length() {
+    if (const char *e = getenv("APTB200_WATCH_SEGMENT")) {
+        const uint64_t v = strtoull(e, nullptr, 10);
+        if (v > 0) return std::min<uint64_t>(v, 1ull << 31);   // 2T stays within the 2^32 work-index limit
+    }
+    return 1ull << 31;
+}
+
+// Everything apt_watch_create derives from its arguments, on the host.
+struct WatchPlan {
+    Plan p;
+    PassRule rule;
+    int sync = 0;
+    bool has_ps = false, has_png = false;
+    apt_process_settings ps{};
+    apt_png_settings png{};
+    PostPlan post;
+    uint64_t max_rows = 0, max_push = 0;
+    uint64_t cap_in = 0, cap_e = 0, q_cap = 0, out_bytes = 0, rows_cap = 0;
+    uint64_t own_bytes = 0, stream_bytes = 0, latency = 0, step_work = 0, extra_rows = 0;
+};
+
+int make_watch_plan(uint32_t input_rate, const apt_settings *s, const apt_watch_settings *ws, WatchPlan &w) {
+    if (!s || !ws) return fail(APT_ERR_BAD_ARG, "null argument");
+    APT_TRY(make_pass_rule(&ws->search, w.rule));
+    w.sync = ws->sync ? 1 : 0;
+    w.max_rows = ws->max_rows ? ws->max_rows : 2400;
+    if (w.max_rows >= (1ull << 32) / kPxPerRow)
+        return fail(APT_ERR_BAD_ARG, "max_rows %llu: image too large", (unsigned long long)w.max_rows);
+    w.max_push = ws->max_push ? ws->max_push : input_rate;
+    if (ws->png && !ws->ps) return fail(APT_ERR_BAD_ARG, "PNG output needs process settings");
+    if (ws->ps) {
+        APT_TRY(make_post(*ws->ps, w.post));
+        w.has_ps = true;
+        w.ps = *ws->ps;
+        w.out_bytes = w.max_rows * kPxPerRow * w.post.bpp;
+    }
+    if (ws->png) {
+        PngPlan pp;
+        APT_TRY(make_png(kPxPerRow, static_cast<uint32_t>(w.max_rows), w.post.bpp, ws->png, pp));
+        w.has_png = true;
+        w.png = *ws->png;
+        w.out_bytes = pp.bound;
+    }
+    apt_stream_info si{};
+    APT_TRY(apt_stream_geometry(input_rate, s, w.sync, w.max_push, &si));   // the settings the pass stream refuses
+    APT_TRY(make_plan(input_rate, *s, w.p));
+    const FrontPlan &f = w.p.front;
+    const uint64_t R = w.p.row, rate = input_rate;
+    if (w.rule.max_gap > (1ull << 32) / (rate / 2 + 1))   // the input window holds max_gap windows of samples
+        return fail(APT_ERR_BAD_ARG, "pass search: max_gap_s %g is too long for a watcher's input window", (double)ws->search.max_gap_s);
+    // input: with no group open, from the next window's first sample; with one open, from the pass stream's position, at
+    // most max_gap + 2 windows behind the next window; either way less than the first stage's unit span behind the last
+    // sample.  Compaction moves the tail only when that does not overlap, so the window holds twice that, plus one step.
+    const uint64_t t_in = (w.rule.max_gap + 4) * (rate / 2 + 1) + 2 * (f.tail() + f.unit_in) + 64;
+    const uint64_t w_new = (w.max_push + f.tail()) * f.r.l / f.r.m + 2 * f.unit_out + 64;
+    // envelope: the two rows of the next window (k_pass_quality reads nothing else) and the units of one step
+    const uint64_t t_e = 2 * R + f.unit_out + 64;
+    w.cap_in = 2 * t_in + w.max_push + 64;
+    w.cap_e = 2 * t_e + w_new + 64;
+    w.q_cap = w_new / R + 4;
+    // the pass stream's rows for one push: rows_bound is the rows of everything pushed less the rows released, and a
+    // released row lags the newest work sample by the first stage's tail, the sync template, the picker's min_distance
+    // and its latency (apt_stream_info.latency_work), and the row the next peak closes
+    w.step_work = w_new;
+    w.extra_rows = (w_new + f.tail() * f.r.l / f.r.m + f.unit_out + w.p.guard.size() + 2 * w.p.dist + si.latency_work) / R + 8;
+    w.rows_cap = (w.max_rows + w.extra_rows) * kPxPerRow;
+    w.latency = (f.tail() * f.r.l / f.r.m + f.unit_out + R - 1) / R + 2;
+    w.own_bytes = FrontTables::bytes(f) + w.cap_in * 4 + w.max_push * (2 + 4) + w.cap_e * 4 * (f.needs_scratch() ? 2 : 1) +
+                  w.q_cap * 4;
+    w.stream_bytes = si.device_bytes + (w.has_ps ? stream_image_bytes(w.post, w.max_rows, w.has_png ? &w.png : nullptr) : 0);
+    return APT_OK;
+}
+
+}  // namespace
+
+struct apt_watch {
+    WatchPlan wp;
+    int device = 0, sm_count = 0;
+    apt_watch_cb cb = nullptr;
+    void *user = nullptr;
+    apt_stream *pass = nullptr;        // the pass stream; its CUDA stream carries every step
+    cudaStream_t cs = nullptr;
+    FrontTables front;
+    float *d_in = nullptr, *d_conv = nullptr, *d_e = nullptr, *d_r = nullptr, *d_q = nullptr;
+    int16_t *d_pcm = nullptr;
+    float *h_q = nullptr, *h_rows = nullptr;   // pinned
+    std::vector<uint8_t> h_out;                // the image or PNG file of the last pass
+    uint64_t T = 1ull << 31;
+    // the feed
+    uint64_t abs_in = 0, seg_start = 0;
+    uint64_t samples_in = 0, in_base = 0, units_done = 0, work_final = 0, e_base = 0;   // of the segment
+    PassTracker tracker{PassRule{}, 1};
+    bool active = false;               // the pass stream holds the open group's samples [start_of(first), fed)
+    bool lost = false;                 // the pass stream's rows outgrew the row buffer: this pass fails, the feed goes on
+    uint64_t fed = 0;
+    uint32_t passes = 0;
+    bool finished = false, in_cb = false;
+};
+
+namespace {
+
+void free_watch(apt_watch *w) {
+    cudaSetDevice(w->device);
+    if (w->cs) cudaStreamSynchronize(w->cs);
+    for (void *p : {(void *)w->d_in, (void *)w->d_conv, (void *)w->d_e, (void *)w->d_r, (void *)w->d_q, (void *)w->d_pcm})
+        if (p) cudaFree(p);
+    for (void *p : {(void *)w->h_q, (void *)w->h_rows})
+        if (p) cudaFreeHost(p);
+    w->front.release();
+    if (w->pass) apt_stream_destroy(w->pass);
+    cudaGetLastError();
+}
+
+void clear_segment(apt_watch *w) {
+    w->samples_in = w->in_base = w->units_done = w->work_final = w->e_base = 0;
+    w->tracker = PassTracker(w->wp.rule, w->wp.p.input_rate);
+    w->active = false;
+    w->fed = 0;
+}
+
+void call(apt_watch *w, const apt_watch_event &e) {
+    if (!w->cb) return;
+    w->in_cb = true;
+    w->cb(&e, w->user);
+    w->in_cb = false;
+}
+
+// The pass stream's row buffer for its next push: rows land at their place in the pass up to max_rows; beyond, the
+// rows past max_rows overwrite each other (the pass is refused its image then).
+float *rows_at(apt_watch *w, uint64_t &cap) {
+    const uint64_t off = std::min(stream_rows_out(w->pass), w->wp.max_rows) * kPxPerRow;
+    cap = w->wp.rows_cap - off;
+    return w->h_rows + off;
+}
+
+// Feeds the pass stream the input samples [fed, to) of the segment, one max_push slice at a time.
+int feed_to(apt_watch *w, uint64_t to) {
+    if (to > w->samples_in) return fail(APT_ERR_BAD_ARG, "internal: the pass reaches past the samples pushed");
+    while (w->fed < to) {
+        if (w->fed < w->in_base) return fail(APT_ERR_BAD_ARG, "internal: the pass's samples left the input window");
+        const uint64_t k = std::min(w->wp.max_push, to - w->fed);
+        uint64_t cap = 0, nout = 0, need = 0;
+        float *rows = rows_at(w, cap);
+        APT_TRY(apt_stream_push_bound(w->pass, k, &need));
+        w->lost = w->lost || need > cap;
+        if (!w->lost) APT_TRY(stream_push_device(w->pass, w->d_in + (w->fed - w->in_base), k, rows, cap, &nout));
+        w->fed += k;
+    }
+    return APT_OK;
+}
+
+void start_pass(apt_watch *w, uint64_t first) {
+    if (w->active) return;
+    w->active = true;
+    w->lost = false;
+    w->fed = w->tracker.start_of(first);
+}
+
+// The LOS of a kept group: the pass stream is fed to the pass's end and finished, and the callback gets the result.
+int los(apt_watch *w, apt_pass_event ev) {
+    start_pass(w, ev.pass.first_window);
+    APT_TRY(feed_to(w, ev.pass.end));
+    apt_watch_event e{};
+    uint64_t cap = 0, nout = 0, need = 0;
+    float *rows = rows_at(w, cap);
+    APT_TRY(apt_stream_push_bound(w->pass, 0, &need));
+    if (w->lost || need > cap) {
+        e.status = fail(APT_ERR_CAPACITY, "the pass stream held more rows than its buffer of max_rows + %llu rows",
+                        (unsigned long long)w->wp.extra_rows);
+        e.rows = stream_rows_out(w->pass);   // the rows released before the buffer ran out
+    } else if (w->wp.has_ps) {
+        uint64_t image_n = 0;
+        e.status = apt_stream_finish_image(w->pass, rows, cap, &nout, w->h_out.data(), w->h_out.size(), &image_n, &e.info);
+        e.rows = stream_rows_out(w->pass);
+        if (e.status == APT_OK) {
+            e.data = w->h_out.data();
+            e.bytes = image_n;
+        }
+    } else {
+        e.status = apt_stream_finish(w->pass, rows, cap, &nout);
+        e.rows = stream_rows_out(w->pass);
+        if (e.status == APT_OK && e.rows > w->wp.max_rows)
+            e.status = fail(APT_ERR_CAPACITY, "the pass has %llu rows, more than max_rows %llu", (unsigned long long)e.rows,
+                            (unsigned long long)w->wp.max_rows);
+        if (e.status == APT_OK) {
+            e.data = w->h_rows;
+            e.bytes = e.rows * kPxPerRow * sizeof(float);
+        }
+    }
+    if (e.status == APT_ERR_CUDA || e.status == APT_ERR_NOMEM) return e.status;   // the device failed, not the pass
+    ev.pass.start += w->seg_start;
+    ev.pass.end += w->seg_start;
+    e.ev = ev;
+    e.index = w->passes++;
+    call(w, e);
+    w->active = false;
+    return apt_stream_reset(w->pass);
+}
+
+int on_event(apt_watch *w, const apt_pass_event &ev) {
+    if (ev.kind == APT_PASS_LOS) return los(w, ev);
+    apt_watch_event e{};
+    e.ev = ev;
+    e.ev.pass.start += w->seg_start;
+    e.index = w->passes;
+    call(w, e);
+    return APT_OK;
+}
+
+// One step: n new samples (maybe none) and, when `finish`, the end of the segment.  q receives the new windows.
+int step(apt_watch *w, const void *src, int format, uint64_t n, bool finish, float *q, uint64_t &nq) {
+    const WatchPlan &wp = w->wp;
+    const Plan &p = wp.p;
+    const LaunchCtx c{w->cs, w->sm_count};
+    const uint64_t R = p.row;
+    // ---- retention: what the first stage, the next window and the pass stream can still read ----
+    uint64_t xa, xb;
+    p.front.span(w->units_done, w->units_done + 1, ~0ull, xa, xb);
+    // a group that opens in this step starts at or after the next window's first sample, even when the last group's LOS
+    // left the pass stream's position past it
+    const uint64_t keep = std::min<uint64_t>({xa, w->tracker.start_of(w->tracker.next()), w->active ? w->fed : ~0ull});
+    APT_TRY(window_compact(w->cs, w->d_in, w->in_base, keep, w->samples_in));
+    const uint64_t e_next = w->tracker.next() * R;
+    const uint64_t ekeep = e_next;
+    uint64_t eb = w->e_base;
+    APT_TRY(window_compact(w->cs, w->d_e, eb, ekeep, w->work_final));
+    if (w->d_r && eb != w->e_base) {
+        uint64_t rb = w->e_base;
+        APT_TRY(window_compact(w->cs, w->d_r, rb, ekeep, w->work_final));
+    }
+    w->e_base = eb;
+    // ---- upload ----
+    if (n) {
+        const uint64_t off = w->samples_in - w->in_base;
+        if (off + n > wp.cap_in) return fail(APT_ERR_BAD_ARG, "internal: input window overflow");
+        APT_TRY(window_upload(c, src, false, format, n, w->d_pcm, w->d_conv, w->d_in + off));
+        w->samples_in += n;
+        w->abs_in += n;
+    }
+    // ---- first stage and q of the windows whose two rows are final ----
+    if (w->samples_in)
+        APT_TRY(front_advance(c, p, w->front, w->d_in - w->in_base, w->samples_in, finish, wp.cap_e, w->d_r, w->d_e, w->e_base,
+                              w->units_done, w->work_final));
+    const uint64_t w0 = w->tracker.next();
+    const uint64_t w1 = w->work_final / R >= 1 ? w->work_final / R - 1 : 0;
+    const uint64_t k = w1 > w0 ? w1 - w0 : 0;
+    if (k) {
+        if (k > wp.q_cap) return fail(APT_ERR_BAD_ARG, "internal: quality buffer overflow");
+        APT_TRY(launch_pass_quality(w->cs, w->d_e - w->e_base, w0, k, static_cast<uint32_t>(R), w->d_q - w0));
+        APT_CUDA(cudaMemcpyAsync(w->h_q, w->d_q, k * sizeof(float), cudaMemcpyDeviceToHost, w->cs));
+        APT_CUDA(cudaStreamSynchronize(w->cs));
+        memcpy(q + nq, w->h_q, k * sizeof(float));
+        nq += k;
+    }
+    // ---- the rule, window by window, and the pass stream ----
+    apt_pass_event evs[2];
+    int nev = 0;
+    auto collect = [&](const apt_pass_event &e) { evs[nev++] = e; };
+    for (uint64_t i = 0; i < k; ++i) {
+        nev = 0;
+        w->tracker.feed(w->h_q[i], collect);
+        if (w->tracker.open()) start_pass(w, w->tracker.first());
+        for (int j = 0; j < nev; ++j) APT_TRY(on_event(w, evs[j]));
+        if (!w->tracker.open() && w->active) {   // a dropped group
+            w->active = false;
+            APT_TRY(apt_stream_reset(w->pass));
+        }
+    }
+    if (finish) {
+        nev = 0;
+        w->tracker.finish(w->samples_in, collect);
+        for (int j = 0; j < nev; ++j) APT_TRY(on_event(w, evs[j]));
+        if (w->active) {
+            w->active = false;
+            APT_TRY(apt_stream_reset(w->pass));
+        }
+    } else if (w->active) {
+        APT_TRY(feed_to(w, w->tracker.end_of(w->tracker.last(), ~0ull)));
+    }
+    return APT_OK;
+}
+
+// A segment that is long enough ends before the next step: finished as at apt_watch_finish, then a new one starts.
+int maybe_roll(apt_watch *w, float *q, uint64_t &nq) {
+    const uint64_t nw = w->wp.p.front.work_len(w->samples_in);
+    // an open group is closed before the step that could take the segment past 2T (T <= 2^31, so work indices stay below
+    // 2^32 in the first stage and in the pass stream)
+    if (nw < w->T || (w->tracker.open() && nw + w->wp.step_work < 2 * w->T)) return APT_OK;
+    APT_TRY(step(w, nullptr, APT_F32, 0, true, q, nq));
+    const uint64_t seg_windows = w->wp.p.front.work_len(w->samples_in) / w->wp.p.row;
+    w->seg_start += w->samples_in;
+    clear_segment(w);
+    apt_watch_event e{};
+    e.ev.kind = APT_PASS_SEGMENT;
+    e.ev.window = seg_windows >= 1 ? seg_windows - 1 : 0;
+    e.ev.pass.start = w->seg_start;
+    e.index = w->passes;
+    call(w, e);
+    return APT_OK;
+}
+
+uint64_t q_bound(const apt_watch *w, uint64_t n) {
+    const Plan &p = w->wp.p;
+    const uint64_t most = p.front.work_len(w->samples_in + n) / p.row + 1;
+    const uint64_t next = w->tracker.next();
+    return (most > next ? most - next : 0) + p.front.work_len(n) / p.row + 2;   // a new segment may start inside the push
+}
+
+int reset_feed(apt_watch *w) {
+    w->abs_in = w->seg_start = 0;
+    w->passes = 0;
+    w->finished = false;
+    clear_segment(w);
+    APT_TRY(apt_stream_reset(w->pass));
+    APT_CUDA(cudaMemsetAsync(w->d_in, 0, w->wp.cap_in * sizeof(float), w->cs));
+    APT_CUDA(cudaStreamSynchronize(w->cs));
+    return APT_OK;
+}
+
+}  // namespace
+
+extern "C" int apt_watch_geometry(uint32_t input_rate, const apt_settings *s, const apt_watch_settings *ws, apt_watch_info *info) {
+    if (!info) return fail(APT_ERR_BAD_ARG, "null argument");
+    WatchPlan wp;
+    APT_TRY(make_watch_plan(input_rate, s, ws, wp));
+    *info = apt_watch_info{};
+    info->device_bytes = wp.own_bytes + wp.stream_bytes;
+    info->max_push = wp.max_push;
+    info->latency_windows = wp.latency;
+    return APT_OK;
+}
+
+extern "C" int apt_watch_create(int device, uint32_t input_rate, const apt_settings *s, const apt_watch_settings *ws,
+                                apt_watch_cb cb, void *user, apt_watch **out) {
+    if (!out) return fail(APT_ERR_BAD_ARG, "null argument");
+    *out = nullptr;
+    std::unique_ptr<apt_watch> w(new (std::nothrow) apt_watch);
+    if (!w) return fail(APT_ERR_NOMEM, "out of host memory");
+    APT_TRY(make_watch_plan(input_rate, s, ws, w->wp));
+    const WatchPlan &wp = w->wp;
+    int count = 0;
+    if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0) {
+        cudaGetLastError();
+        return fail(APT_ERR_CUDA, "no usable CUDA device; this library has no CPU fallback");
+    }
+    w->device = device;
+    w->cb = cb;
+    w->user = user;
+    w->T = segment_length();
+    struct Rollback {
+        apt_watch *w;
+        bool armed = true;
+        ~Rollback() {
+            if (armed) free_watch(w);
+        }
+    } rollback{w.get()};
+    APT_CUDA(cudaSetDevice(device));
+    APT_CUDA(cudaDeviceGetAttribute(&w->sm_count, cudaDevAttrMultiProcessorCount, device));
+    APT_TRY(apt_stream_create(device, input_rate, s, wp.sync, wp.max_push, &w->pass));
+    if (wp.has_ps) APT_TRY(apt_stream_set_process_mode(w->pass, &wp.ps, wp.max_rows));
+    if (wp.has_png) APT_TRY(apt_stream_set_png_mode(w->pass, &wp.png));
+    w->cs = stream_cuda(w->pass);
+    APT_TRY(w->front.upload(wp.p.front));
+    APT_CUDA(cudaMalloc(&w->d_in, wp.cap_in * sizeof(float)));
+    APT_CUDA(cudaMalloc(&w->d_pcm, wp.max_push * sizeof(int16_t)));
+    APT_CUDA(cudaMalloc(&w->d_conv, wp.max_push * sizeof(float)));
+    APT_CUDA(cudaMalloc(&w->d_e, wp.cap_e * sizeof(float)));
+    if (wp.p.front.needs_scratch()) APT_CUDA(cudaMalloc(&w->d_r, wp.cap_e * sizeof(float)));
+    APT_CUDA(cudaMalloc(&w->d_q, wp.q_cap * sizeof(float)));
+    APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&w->h_q), wp.q_cap * sizeof(float), cudaHostAllocDefault));
+    APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&w->h_rows), wp.rows_cap * sizeof(float), cudaHostAllocDefault));
+    try {
+        w->h_out.resize(std::max<uint64_t>(wp.out_bytes, 1));
+    } catch (const std::bad_alloc &) {
+        return fail(APT_ERR_NOMEM, "out of host memory");
+    }
+    APT_TRY(reset_feed(w.get()));
+    rollback.armed = false;
+    *out = w.release();
+    return APT_OK;
+}
+
+extern "C" void apt_watch_destroy(apt_watch *w) {
+    if (!w || w->in_cb) return;
+    free_watch(w);
+    delete w;
+}
+
+extern "C" int apt_watch_push_bound(apt_watch *w, uint64_t n, uint64_t *cap_q) {
+    if (!w || !cap_q) return fail(APT_ERR_BAD_ARG, "null argument");
+    if (w->in_cb) return fail(APT_ERR_BAD_ARG, "a watcher's callback may not call into its own watcher");
+    *cap_q = q_bound(w, n);
+    return APT_OK;
+}
+
+extern "C" int apt_watch_push(apt_watch *w, const void *samples, int format, uint64_t n, float *q, uint64_t cap, uint64_t *nq) {
+    if (nq) *nq = 0;
+    if (!w || !nq) return fail(APT_ERR_BAD_ARG, "null argument");
+    if (w->in_cb) return fail(APT_ERR_BAD_ARG, "a watcher's callback may not call into its own watcher");
+    if (w->finished) return fail(APT_ERR_BAD_ARG, "push after finish: call apt_watch_reset to start a new feed");
+    if (format != APT_F32 && format != APT_PCM16) return fail(APT_ERR_BAD_ARG, "sample format %d is not APT_F32 or APT_PCM16", format);
+    if (n == 0) return APT_OK;
+    if (!samples) return fail(APT_ERR_BAD_ARG, "null samples");
+    const uint64_t need = q_bound(w, n);
+    if (!q || cap < need) return fail(APT_ERR_CAPACITY, "q needs room for %llu floats", (unsigned long long)need);
+    APT_CUDA(cudaSetDevice(w->device));
+    const size_t sb = format == APT_PCM16 ? 2 : 4;
+    uint64_t got = 0;
+    try {   // the rule's gap buffer is the only host allocation of a step; no exception leaves the C ABI
+        for (uint64_t done = 0; done < n;) {
+            APT_TRY(maybe_roll(w, q, got));
+            const uint64_t k = std::min(w->wp.max_push, n - done);
+            APT_TRY(step(w, static_cast<const char *>(samples) + done * sb, format, k, false, q, got));
+            done += k;
+        }
+    } catch (const std::bad_alloc &) {
+        return fail(APT_ERR_NOMEM, "out of host memory");
+    }
+    *nq = got;
+    return APT_OK;
+}
+
+extern "C" int apt_watch_finish(apt_watch *w, float *q, uint64_t cap, uint64_t *nq) {
+    if (nq) *nq = 0;
+    if (!w || !nq) return fail(APT_ERR_BAD_ARG, "null argument");
+    if (w->in_cb) return fail(APT_ERR_BAD_ARG, "a watcher's callback may not call into its own watcher");
+    if (w->finished) return fail(APT_ERR_BAD_ARG, "the watcher is already finished");
+    const uint64_t need = q_bound(w, 0);
+    if (!q || cap < need) return fail(APT_ERR_CAPACITY, "q needs room for %llu floats", (unsigned long long)need);
+    APT_CUDA(cudaSetDevice(w->device));
+    uint64_t got = 0;
+    try {
+        APT_TRY(step(w, nullptr, APT_F32, 0, true, q, got));
+    } catch (const std::bad_alloc &) {
+        return fail(APT_ERR_NOMEM, "out of host memory");
+    }
+    w->finished = true;
+    *nq = got;
+    return APT_OK;
+}
+
+extern "C" int apt_watch_reset(apt_watch *w) {
+    if (!w) return fail(APT_ERR_BAD_ARG, "null argument");
+    if (w->in_cb) return fail(APT_ERR_BAD_ARG, "a watcher's callback may not call into its own watcher");
+    APT_CUDA(cudaSetDevice(w->device));
+    return reset_feed(w);
+}
+
+extern "C" int apt_watch_get_info(apt_watch *w, apt_watch_info *info) {
+    if (!w || !info) return fail(APT_ERR_BAD_ARG, "null argument");
+    if (w->in_cb) return fail(APT_ERR_BAD_ARG, "a watcher's callback may not call into its own watcher");
+    apt_stream_info si{};
+    APT_TRY(apt_stream_get_info(w->pass, &si));
+    *info = apt_watch_info{};
+    info->samples_in = w->abs_in;
+    info->segment_start = w->seg_start;
+    info->windows = w->tracker.next();
+    info->passes = w->passes;
+    info->open = w->tracker.open() ? 1 : 0;
+    info->device_bytes = w->wp.own_bytes + si.device_bytes;
+    info->max_push = w->wp.max_push;
+    info->latency_windows = w->wp.latency;
+    return APT_OK;
+}

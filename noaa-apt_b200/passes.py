@@ -182,3 +182,190 @@ def decode_passes_png(signal, input_rate, settings=None, sync=True, device=0, se
         found = rec.find_passes(**(search or {}))
         pngs, infos, _sts = rec.decode_png(found, sync, **process)
     return list(zip(found, pngs, infos))
+
+
+@dataclass
+class PassEvent:
+    """apt_pass_event: kind "aos", "los" or "segment", the window whose evaluation fired it, and the pass.  From a Watch,
+    also the pass number, and for an LOS the decode's status, row count, image info and data (f32 rows, pixels or PNG
+    bytes; None when the decode failed)."""
+    kind: str
+    window: int
+    pass_: Pass
+    index: int = 0
+    status: int = 0
+    rows: int = 0
+    info: dict = None
+    data: object = None
+
+
+_KINDS = {_lib.PASS_AOS: "aos", _lib.PASS_LOS: "los", _lib.PASS_SEGMENT: "segment"}
+
+
+def _event(ce):
+    return PassEvent(_KINDS[int(ce.kind)], int(ce.window), Pass.from_c(ce.pass_))
+
+
+class PassTracker:
+    """apt_pass_tracker: the pass rule fed q window by window (host only).  feed(q) and finish(n) return the events."""
+
+    def __init__(self, input_rate, enter=ENTER, exit=EXIT, max_gap_s=MAX_GAP_S, min_length_s=MIN_LENGTH_S):
+        self._lib = _lib.load()
+        ps = _search(enter, exit, max_gap_s, min_length_s)
+        h = C.c_void_p(None)
+        raise_for(self._lib.apt_pass_tracker_create(_rate_hz(input_rate), C.byref(ps), C.byref(h)))
+        self._h = h
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.apt_pass_tracker_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def feed(self, q):
+        x = np.ascontiguousarray(q, dtype=np.float32)
+        evs = (_lib.CPassEvent * max(2 * x.size, 1))()
+        n = C.c_uint64(0)
+        raise_for(self._lib.apt_pass_tracker_feed(self._h, x.ctypes.data if x.size else None, x.size, evs, 2 * x.size,
+                                                  C.byref(n)))
+        return [_event(evs[i]) for i in range(n.value)]
+
+    def finish(self, n):
+        evs = (_lib.CPassEvent * 1)()
+        k = C.c_uint64(0)
+        raise_for(self._lib.apt_pass_tracker_finish(self._h, int(n), evs, 1, C.byref(k)))
+        return [_event(evs[i]) for i in range(k.value)]
+
+
+def watch_settings(sync=True, search=None, ps=None, png=None, max_rows=0, max_push=0):
+    """apt_watch_settings; search: keyword arguments of find_passes_quality's rule (enter, exit, max_gap_s, min_length_s)."""
+    ws = _lib.CWatchSettings()
+    ws.sync = int(bool(sync))
+    ws.search = _search(**(search or {}))
+    ws.ps = C.addressof(ps) if ps is not None else None
+    ws.png = C.addressof(png) if png is not None else None
+    ws.max_rows, ws.max_push = int(max_rows), int(max_push)
+    return ws
+
+
+def _image_args(image_out, process):
+    """(apt_process_settings or None, bytes per pixel or None, apt_png_settings or None) for image_out None / "image" / "png"."""
+    if image_out is None:
+        return None, None, None
+    png_kw = {k: process.pop(k) for k in ("filter", "matches", "block_bytes", "rgb_from_rgba") if k in process}
+    process.setdefault("contrast", image.MINMAX)
+    ps, bpp, pal = image.process_settings(**process)
+    png = image.png_settings(**png_kw) if image_out == "png" else None
+    return (ps, pal), bpp, png
+
+
+class Watch:
+    """apt_watch (DESIGN.md §13): a continuous feed watched for satellite passes, each finished as its rows, image or PNG file.
+
+        with Watch(48000, image_out="png", contrast=image.TELEMETRY, rgba=True) as w:
+            for block in feed:                       # any sizes, float32 or int16
+                q, events = w.push(block)
+                for e in events:
+                    if e.kind == "los" and e.status == 0:
+                        open(f"pass{e.index}.png", "wb").write(e.data)
+            q, events = w.finish()
+
+    image_out None: each pass ends in its f32 rows; "image": its pixels; "png": its PNG file.  process: the keyword
+    arguments of image.decode_image / decode_png.  Events are copied out during the callback."""
+
+    def __init__(self, input_rate, settings=None, sync=True, search=None, image_out=None, max_rows=0, max_push=0, device=0,
+                 **process):
+        self._lib = _lib.load()
+        self.input_rate = _rate_hz(input_rate)
+        self.settings = settings or Settings()
+        self._ps, self._bpp, self._png = _image_args(image_out, dict(process))
+        self._ws = watch_settings(sync, search, self._ps[0] if self._ps else None, self._png, max_rows, max_push)
+        self._events = []
+        self._cb = _lib.WATCH_CB(self._on_event)
+        s = self.settings.to_c()
+        h = C.c_void_p(None)
+        raise_for(self._lib.apt_watch_create(int(device), self.input_rate, C.byref(s), C.byref(self._ws), self._cb, None,
+                                             C.byref(h)))
+        self._h = h
+
+    def _on_event(self, pev, _user):
+        e = pev.contents
+        ev = _event(e.ev)
+        ev.index, ev.status, ev.rows = int(e.index), int(e.status), int(e.rows)
+        if ev.kind == "los":
+            if self._bpp:
+                ev.info = image._info(e.info)
+            if e.data and e.bytes:
+                raw = C.string_at(e.data, int(e.bytes))
+                if self._png is not None:
+                    ev.data = raw
+                elif self._bpp:
+                    ev.data = image._shape(np.frombuffer(raw, dtype=np.uint8).copy(), self._bpp)
+                else:
+                    ev.data = np.frombuffer(raw, dtype=np.float32).copy()
+        self._events.append(ev)
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.apt_watch_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def _take(self):
+        ev, self._events = self._events, []
+        return ev
+
+    def push(self, samples):
+        """(q of the windows that became final, [PassEvent])."""
+        x = np.ascontiguousarray(samples)
+        fmt = _fmt_of(x)
+        cap = C.c_uint64(0)
+        raise_for(self._lib.apt_watch_push_bound(self._h, x.size, C.byref(cap)))
+        q = np.empty(max(cap.value, 1), dtype=np.float32)
+        nq = C.c_uint64(0)
+        rc = self._lib.apt_watch_push(self._h, x.ctypes.data if x.size else None, fmt, x.size, q.ctypes.data, q.size,
+                                      C.byref(nq))
+        ev = self._take()
+        raise_for(rc)
+        return q[: nq.value].copy(), ev
+
+    def finish(self):
+        cap = C.c_uint64(0)
+        raise_for(self._lib.apt_watch_push_bound(self._h, 0, C.byref(cap)))
+        q = np.empty(max(cap.value, 1), dtype=np.float32)
+        nq = C.c_uint64(0)
+        rc = self._lib.apt_watch_finish(self._h, q.ctypes.data, q.size, C.byref(nq))
+        ev = self._take()
+        raise_for(rc)
+        return q[: nq.value].copy(), ev
+
+    def reset(self):
+        raise_for(self._lib.apt_watch_reset(self._h))
+        self._events = []
+
+    def info(self):
+        ci = _lib.CWatchInfo()
+        raise_for(self._lib.apt_watch_get_info(self._h, C.byref(ci)))
+        return {n: int(getattr(ci, n)) for n, _ in _lib.CWatchInfo._fields_}
+
+    @property
+    def device_bytes(self):
+        return self.info()["device_bytes"]
+
+
+def watch_geometry(input_rate, settings=None, sync=True, search=None, image_out=None, max_rows=0, max_push=0, **process):
+    """apt_watch_geometry (host only): the device_bytes, max_push and latency_windows a Watch with these arguments has."""
+    ps, _bpp, png = _image_args(image_out, dict(process))
+    ws = watch_settings(sync, search, ps[0] if ps else None, png, max_rows, max_push)
+    s = (settings or Settings()).to_c()
+    ci = _lib.CWatchInfo()
+    raise_for(_lib.load().apt_watch_geometry(_rate_hz(input_rate), C.byref(s), C.byref(ws), C.byref(ci)))
+    return {n: int(getattr(ci, n)) for n, _ in _lib.CWatchInfo._fields_}

@@ -250,3 +250,55 @@ extern "C" {
                                 ps: *const apt_process_settings, png: *const apt_png_settings, outs: *const *mut c_void,
                                 caps: *const u64, nouts: *mut u64, infos: *mut apt_image_info, statuses: *mut c_int) -> c_int;
 }
+
+// Continuous feeds: watching for passes (DESIGN.md §13)
+pub const APT_PASS_AOS: c_int = 1;
+pub const APT_PASS_LOS: c_int = 2;
+pub const APT_PASS_SEGMENT: c_int = 3;
+
+#[repr(C)]
+#[derive(Default, Clone, Copy, Debug)]
+pub struct apt_pass_event { pub kind: c_int, pub window: u64, pub pass: apt_pass }
+
+#[repr(C)]
+pub struct apt_pass_tracker { _private: [u8; 0] }
+
+#[repr(C)]
+pub struct apt_watch { _private: [u8; 0] }
+
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct apt_watch_settings { pub sync: c_int, pub search: apt_pass_search, pub ps: *const apt_process_settings,
+                                pub png: *const apt_png_settings, pub max_rows: u64, pub max_push: u64 }
+
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct apt_watch_event { pub ev: apt_pass_event, pub index: u32, pub status: c_int, pub rows: u64, pub info: apt_image_info,
+                             pub data: *const c_void, pub bytes: u64 }
+
+#[repr(C)]
+#[derive(Default, Clone, Copy, Debug)]
+pub struct apt_watch_info { pub samples_in: u64, pub segment_start: u64, pub windows: u64, pub passes: u64, pub open: u64,
+                            pub device_bytes: u64, pub max_push: u64, pub latency_windows: u64 }
+
+pub type apt_watch_cb = Option<unsafe extern "C" fn(ev: *const apt_watch_event, user: *mut c_void)>;
+
+#[link(name = "aptb200")]
+extern "C" {
+    pub fn apt_pass_tracker_create(input_rate: u32, search: *const apt_pass_search, t: *mut *mut apt_pass_tracker) -> c_int;
+    pub fn apt_pass_tracker_feed(t: *mut apt_pass_tracker, q: *const f32, nq: u64, events: *mut apt_pass_event, cap: u64,
+                                 nev: *mut u64) -> c_int;
+    pub fn apt_pass_tracker_finish(t: *mut apt_pass_tracker, n: u64, events: *mut apt_pass_event, cap: u64, nev: *mut u64) -> c_int;
+    pub fn apt_pass_tracker_destroy(t: *mut apt_pass_tracker);
+    pub fn apt_watch_create(device: c_int, input_rate: u32, s: *const apt_settings, ws: *const apt_watch_settings,
+                            cb: apt_watch_cb, user: *mut c_void, w: *mut *mut apt_watch) -> c_int;
+    pub fn apt_watch_geometry(input_rate: u32, s: *const apt_settings, ws: *const apt_watch_settings,
+                              info: *mut apt_watch_info) -> c_int;
+    pub fn apt_watch_push_bound(w: *mut apt_watch, n: u64, cap_q: *mut u64) -> c_int;
+    pub fn apt_watch_push(w: *mut apt_watch, samples: *const c_void, format: c_int, n: u64, q: *mut f32, cap: u64,
+                          nq: *mut u64) -> c_int;
+    pub fn apt_watch_finish(w: *mut apt_watch, q: *mut f32, cap: u64, nq: *mut u64) -> c_int;
+    pub fn apt_watch_reset(w: *mut apt_watch) -> c_int;
+    pub fn apt_watch_get_info(w: *mut apt_watch, info: *mut apt_watch_info) -> c_int;
+    pub fn apt_watch_destroy(w: *mut apt_watch);
+}

@@ -100,3 +100,103 @@ impl Recording {
 impl Drop for Recording {
     fn drop(&mut self) { unsafe { sys::apt_recording_destroy(self.h) } }
 }
+
+/// What a `Watch` hands its closure: an AOS, a SEGMENT, or at LOS the pass's decode (`data`: the PNG file, or the f32
+/// rows as bytes without image output; `Err` the pass's own failure, e.g. more rows than `max_rows`).
+pub enum WatchEvent<'a> {
+    Aos { index: u32, pass: sys::apt_pass },
+    Los { index: u32, pass: sys::apt_pass, rows: u64, data: err::Result<&'a [u8]>, info: sys::apt_image_info },
+    Segment { start: u64 },
+}
+
+struct Handler<'f> {
+    f: Box<dyn FnMut(WatchEvent) + 'f>,
+}
+
+unsafe extern "C" fn watch_trampoline(ev: *const sys::apt_watch_event, user: *mut c_void) {
+    let h = &mut *(user as *mut Handler);
+    let e = &*ev;
+    let out = match e.ev.kind {
+        sys::APT_PASS_AOS => WatchEvent::Aos { index: e.index, pass: e.ev.pass },
+        sys::APT_PASS_SEGMENT => WatchEvent::Segment { start: e.ev.pass.start },
+        _ => WatchEvent::Los {
+            index: e.index,
+            pass: e.ev.pass,
+            rows: e.rows,
+            data: if e.status == sys::APT_OK {
+                Ok(std::slice::from_raw_parts(e.data as *const u8, e.bytes as usize))
+            } else {
+                Err(to_error(e.status))
+            },
+            info: e.info,
+        },
+    };
+    // a panic must not unwind into the library
+    let _ = std::panic::catch_unwind(std::panic::AssertUnwindSafe(|| (h.f)(out)));
+}
+
+/// A continuous feed (16-bit samples as they arrive) watched for satellite passes, each ended in its PNG file (`png`)
+/// or its f32 rows, in fixed device memory (DESIGN.md §13).  The closure runs on the pushing thread.
+pub struct Watch<'f> {
+    h: *mut sys::apt_watch,
+    handler: Box<Handler<'f>>,
+}
+
+impl<'f> Watch<'f> {
+    pub fn new(input_rate: Rate, settings: &config::Settings, search: &sys::apt_pass_search,
+               image: Option<(&sys::apt_process_settings, Option<&sys::apt_png_settings>)>, max_rows: u64, device: i32,
+               on_event: impl FnMut(WatchEvent) + 'f) -> err::Result<Watch<'f>> {
+        let s = sys::apt_settings::from(settings);
+        let ws = sys::apt_watch_settings {
+            sync: 1,
+            search: *search,
+            ps: image.map_or(ptr::null(), |(ps, _)| ps as *const _),
+            png: image.and_then(|(_, png)| png).map_or(ptr::null(), |p| p as *const _),
+            max_rows,
+            max_push: 0,
+        };
+        let mut handler = Box::new(Handler { f: Box::new(on_event) });
+        let mut h = ptr::null_mut();
+        check(unsafe { sys::apt_watch_create(device, input_rate.get_hz(), &s, &ws, Some(watch_trampoline),
+                                             &mut *handler as *mut Handler as *mut c_void, &mut h) })?;
+        Ok(Watch { h, handler })
+    }
+
+    /// The new windows' quality; events reach the closure during the call.
+    pub fn push(&mut self, pcm: &[i16]) -> err::Result<Vec<f32>> {
+        let mut cap = 0u64;
+        check(unsafe { sys::apt_watch_push_bound(self.h, pcm.len() as u64, &mut cap) })?;
+        let mut q = vec![0f32; cap.max(1) as usize];
+        let mut nq = 0u64;
+        check(unsafe { sys::apt_watch_push(self.h, pcm.as_ptr() as *const c_void, sys::APT_PCM16, pcm.len() as u64,
+                                           q.as_mut_ptr(), q.len() as u64, &mut nq) })?;
+        q.truncate(nq as usize);
+        Ok(q)
+    }
+
+    /// The end of the feed: the tail windows and the LOS of a pass still open.
+    pub fn finish(&mut self) -> err::Result<Vec<f32>> {
+        let mut cap = 0u64;
+        check(unsafe { sys::apt_watch_push_bound(self.h, 0, &mut cap) })?;
+        let mut q = vec![0f32; cap.max(1) as usize];
+        let mut nq = 0u64;
+        check(unsafe { sys::apt_watch_finish(self.h, q.as_mut_ptr(), q.len() as u64, &mut nq) })?;
+        q.truncate(nq as usize);
+        Ok(q)
+    }
+
+    pub fn reset(&mut self) -> err::Result<()> { check(unsafe { sys::apt_watch_reset(self.h) }) }
+
+    pub fn info(&self) -> err::Result<sys::apt_watch_info> {
+        let mut i = sys::apt_watch_info::default();
+        check(unsafe { sys::apt_watch_get_info(self.h, &mut i) })?;
+        Ok(i)
+    }
+}
+
+impl<'f> Drop for Watch<'f> {
+    fn drop(&mut self) {
+        unsafe { sys::apt_watch_destroy(self.h) };
+        let _ = &self.handler;   // freed after the watcher, which holds its address
+    }
+}
