@@ -64,6 +64,25 @@ LaunchCtx stage_ctx() {
     return LaunchCtx{nullptr, std::max(sms, 1)};
 }
 
+// The decoder's staging ring for pageable buffers, made on first use (make_stager: it may have none).
+void ensure_stager(apt_decoder *d) {
+    if (d->stager) return;
+    d->own_stager = make_stager(d->device);
+    d->stager = d->own_stager.get();
+}
+
+// The decode's errors that need no device, in the reference's order: the plan, fewer than 10 rows, sync without a
+// work_rate multiple of 4160.  need (optional): the floats of the rows of n samples.
+int check_decode(uint32_t rate, const apt_settings &s, uint64_t n, int sync, uint64_t *need = nullptr) {
+    Plan p;
+    APT_TRY(make_plan(rate, s, p));
+    const uint64_t nwork = p.front.work_len(n);
+    if (nwork < 10ull * p.row) return fail(APT_ERR_TOO_SHORT, "Got less than 10 rows of samples, audio file is too short");
+    if (sync && !p.work_multiple) return fail(APT_ERR_WORK_RATE, "work_rate is not multiple of FINAL_RATE");
+    if (need) *need = sync ? (nwork / p.row) * kPxPerRow : plan_out_bound(p, n);
+    return APT_OK;
+}
+
 }  // namespace
 
 int aptb200::free_decoder_buffers(apt_decoder *d) {
@@ -512,13 +531,7 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
     if (host) {
         d->job_in_pageable = is_pageable(signal);
         d->job_out_pageable = !png && !keep && is_pageable(out);   // PNG mode copies the file straight into `out` at wait()
-        if ((d->job_in_pageable || d->job_out_pageable) && !d->stager && !getenv("APTB200_NO_STAGER")) {
-            int threads = 8;
-            if (const char *e = getenv("APTB200_COPY_THREADS")) threads = std::max(1, atoi(e));
-            d->own_stager.reset(new (std::nothrow) HostStager(d->device, 16u << 20, 3, threads));
-            if (d->own_stager && !d->own_stager->ok()) d->own_stager.reset();
-            d->stager = d->own_stager.get();
-        }
+        if (d->job_in_pageable || d->job_out_pageable) ensure_stager(d);
         if (d->job_out_pageable && !d->h_out)
             APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&d->h_out), std::max<uint64_t>(d->max_out, 1) * sizeof(float),
                                    cudaHostAllocDefault));   // sized for f32 rows: also holds the u8 image
@@ -868,9 +881,6 @@ namespace {
 // decoder costs ~14 cudaMalloc + a stream + pinned staging, so finished decoders are parked here, keyed by what their plan
 // depends on, and the next call with the same (device, rate, settings) takes one over.  apt_cache_clear() frees them.
 struct CacheEntry {
-    int device;
-    uint32_t rate;
-    apt_settings st;
     apt_decoder *dec;
     uint64_t stamp;
 };
@@ -879,62 +889,70 @@ std::vector<CacheEntry> g_cache;
 uint64_t g_cache_stamp = 0;
 constexpr size_t kCacheMaxIdle = 8;
 
-bool same_settings(const apt_settings &a, const apt_settings &b) { return memcmp(&a, &b, sizeof(a)) == 0; }
-
-apt_decoder *cache_take(int device, uint32_t rate, const apt_settings &st, uint64_t n) {
-    std::lock_guard<std::mutex> lk(g_cache_mutex);
-    for (size_t i = 0; i < g_cache.size(); ++i) {
-        const CacheEntry &e = g_cache[i];
-        if (e.device == device && e.rate == rate && same_settings(e.st, st) && e.dec->max_samples >= n) {
-            apt_decoder *d = e.dec;
-            g_cache.erase(g_cache.begin() + static_cast<long>(i));
-            return d;
-        }
-    }
-    return nullptr;
+bool cache_on() {
+    static const bool on = getenv("APTB200_NO_CACHE") == nullptr;
+    return on;
 }
 
-void cache_put(int device, uint32_t rate, const apt_settings &st, apt_decoder *d) {
-    apt_decoder *victim = nullptr;
+bool same_key(const apt_decoder *d, int device, uint32_t rate, const apt_settings &st) {
+    return d->device == device && d->plan.input_rate == rate && memcmp(&d->plan.st, &st, sizeof(st)) == 0;
+}
+
+}  // namespace
+
+int aptb200::take_decoder(int device, uint32_t rate, const apt_settings &st, uint64_t n, bool headroom, apt_decoder **d) {
+    *d = nullptr;
+    if (!cache_on()) return apt_decoder_create(device, rate, &st, n, d);
     {
         std::lock_guard<std::mutex> lk(g_cache_mutex);
-        // one idle decoder per key is enough for a sequential caller: a smaller one of the same key is replaced
         for (size_t i = 0; i < g_cache.size(); ++i) {
-            CacheEntry &e = g_cache[i];
-            if (e.device == device && e.rate == rate && same_settings(e.st, st) && e.dec->max_samples <= d->max_samples) {
-                victim = e.dec;
+            if (same_key(g_cache[i].dec, device, rate, st) && g_cache[i].dec->max_samples >= n) {
+                *d = g_cache[i].dec;
                 g_cache.erase(g_cache.begin() + static_cast<long>(i));
-                break;
+                return APT_OK;
             }
         }
-        if (!victim && g_cache.size() >= kCacheMaxIdle) {
-            size_t lru = 0;
+    }
+    // head-room so that the next, slightly longer recording of a series reuses the decoder
+    const uint64_t room = headroom ? ((n + n / 8 + (1u << 20)) & ~((1ull << 20) - 1)) : n;
+    return apt_decoder_create(device, rate, &st, room, d);
+}
+
+void aptb200::park_decoder(apt_decoder *d, bool several) {
+    cudaStreamSynchronize(d->stream);
+    d->post_plan.reset();
+    d->png_active = false;
+    d->keep_image = false;
+    d->cb = nullptr;
+    d->cb_user = nullptr;
+    d->stager = d->own_stager.get();   // never keep a pointer into another decoder
+    if (!cache_on()) {
+        apt_decoder_destroy(d);
+        return;
+    }
+    apt_decoder *victim = nullptr;
+    {
+        std::lock_guard<std::mutex> lk(g_cache_mutex);
+        size_t drop = g_cache.size();
+        // one idle decoder per key is enough for a sequential caller: a smaller one of the same key is replaced
+        for (size_t i = 0; i < g_cache.size() && !several && drop == g_cache.size(); ++i)
+            if (same_key(g_cache[i].dec, d->device, d->plan.input_rate, d->plan.st) && g_cache[i].dec->max_samples <= d->max_samples)
+                drop = i;
+        if (drop == g_cache.size() && g_cache.size() >= kCacheMaxIdle) {
+            drop = 0;
             for (size_t i = 1; i < g_cache.size(); ++i)
-                if (g_cache[i].stamp < g_cache[lru].stamp) lru = i;
-            victim = g_cache[lru].dec;
-            g_cache.erase(g_cache.begin() + static_cast<long>(lru));
+                if (g_cache[i].stamp < g_cache[drop].stamp) drop = i;
         }
-        g_cache.push_back(CacheEntry{device, rate, st, d, ++g_cache_stamp});
+        if (drop < g_cache.size()) {
+            victim = g_cache[drop].dec;
+            g_cache.erase(g_cache.begin() + static_cast<long>(drop));
+        }
+        g_cache.push_back(CacheEntry{d, ++g_cache_stamp});
     }
     if (victim) apt_decoder_destroy(victim);
 }
 
-// batch feeders park all their decoders (several per key)
-void cache_put_multi(int device, uint32_t rate, const apt_settings &st, apt_decoder *d) {
-    apt_decoder *victim = nullptr;
-    {
-        std::lock_guard<std::mutex> lk(g_cache_mutex);
-        if (g_cache.size() >= kCacheMaxIdle) {
-            size_t lru = 0;
-            for (size_t i = 1; i < g_cache.size(); ++i)
-                if (g_cache[i].stamp < g_cache[lru].stamp) lru = i;
-            victim = g_cache[lru].dec;
-            g_cache.erase(g_cache.begin() + static_cast<long>(lru));
-        }
-        g_cache.push_back(CacheEntry{device, rate, st, d, ++g_cache_stamp});
-    }
-    if (victim) apt_decoder_destroy(victim);
-}
+namespace {
 
 // ps: the image of process(), else (nullptr) f32 rows; png: that image as a PNG file.
 int decode_oneshot(const void *signal, int format, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
@@ -944,24 +962,12 @@ int decode_oneshot(const void *signal, int format, uint64_t n, uint32_t input_ra
     if (!s || !nout) return fail(APT_ERR_BAD_ARG, "null argument");
     *nout = 0;
     if (n == 0 || !signal) return fail(APT_ERR_BAD_ARG, "empty signal");
-    int device = 0;
-    {
-        // errors that do not need a device come first, in the reference's order
-        Plan p;
-        APT_TRY(make_plan(input_rate, *s, p));
-        if (p.front.work_len(n) < 10ull * p.row)
-            return fail(APT_ERR_TOO_SHORT, "Got less than 10 rows of samples, audio file is too short");
-        if (sync && !p.work_multiple) return fail(APT_ERR_WORK_RATE, "work_rate is not multiple of FINAL_RATE");
-    }
+    APT_TRY(check_decode(input_rate, *s, n, sync));
     APT_TRY(require_device());
+    int device = 0;
     if (cudaGetDevice(&device) != cudaSuccess) device = 0;
-    static const bool use_cache = getenv("APTB200_NO_CACHE") == nullptr;
-    apt_decoder *d = use_cache ? cache_take(device, input_rate, *s, n) : nullptr;
-    if (!d) {
-        // head-room so that the next, slightly longer recording of a series reuses the decoder
-        const uint64_t room = use_cache ? ((n + n / 8 + (1u << 20)) & ~((1ull << 20) - 1)) : n;
-        APT_TRY(apt_decoder_create(device, input_rate, s, room, &d));
-    }
+    apt_decoder *d = nullptr;
+    APT_TRY(take_decoder(device, input_rate, *s, n, true, &d));
     d->cb = cb;
     d->cb_user = user;
     int st = ps ? apt_decoder_set_process_mode(d, ps) : APT_OK;
@@ -969,30 +975,11 @@ int decode_oneshot(const void *signal, int format, uint64_t n, uint32_t input_ra
     if (st == APT_OK) st = apt_decoder_submit_host(d, signal, format, n, sync, out, cap);
     if (st == APT_OK) st = apt_decoder_wait(d, nout);
     if (st == APT_OK && info) *info = d->last_image;
-    d->post_plan.reset();
-    d->png_active = false;
-    d->cb = nullptr;
-    d->cb_user = nullptr;
-    if (use_cache) cache_put(device, input_rate, *s, d);
-    else apt_decoder_destroy(d);
+    park_decoder(d, false);
     return st;
 }
 
 }  // namespace
-
-int aptb200::take_decoder(int device, uint32_t rate, const apt_settings &st, uint64_t n, apt_decoder **d) {
-    static const bool use_cache = getenv("APTB200_NO_CACHE") == nullptr;
-    *d = use_cache ? cache_take(device, rate, st, n) : nullptr;
-    if (*d) return APT_OK;
-    const uint64_t room = use_cache ? ((n + n / 8 + (1u << 20)) & ~((1ull << 20) - 1)) : n;
-    return apt_decoder_create(device, rate, &st, room, d);
-}
-
-void aptb200::park_decoder(int device, uint32_t rate, const apt_settings &st, apt_decoder *d) {
-    static const bool use_cache = getenv("APTB200_NO_CACHE") == nullptr;
-    if (use_cache) cache_put(device, rate, st, d);
-    else apt_decoder_destroy(d);
-}
 
 extern "C" int apt_bind_thread_to_device(int device) {
     if (require_device() != APT_OK) return 0;
@@ -1020,83 +1007,12 @@ extern "C" int apt_decode_pcm16(const int16_t *pcm, uint64_t n, uint32_t input_r
     return decode_oneshot(pcm, APT_PCM16, n, input_rate, s, sync, out, cap, nout, cb, user);
 }
 
-// apt_decode at audio_rate of the audio the FM kernel writes into the parked decoder's device input.
-extern "C" int apt_decode_iq(const void *iq, int format, uint64_t n, const apt_iq_settings *is, const apt_settings *s, int sync,
-                             float *out, uint64_t cap, uint64_t *nout, apt_status_cb cb, void *user) {
-    if (!is || !s || !nout) return fail(APT_ERR_BAD_ARG, "null argument");
-    *nout = 0;
-    if (n == 0 || !iq) return fail(APT_ERR_BAD_ARG, "empty signal");
-    if (!iq_sample_bytes(format)) return fail(APT_ERR_BAD_ARG, "unknown I/Q sample format %d", format);
-    IqPlan ip;
-    APT_TRY(make_iq(*is, ip));
-    const uint64_t na = ip.out_len(n);
-    const uint32_t rate = is->audio_rate;
-    uint64_t need = 0;
-    {
-        // errors that do not need a device come first, in decode_oneshot's order
-        Plan p;
-        APT_TRY(make_plan(rate, *s, p));
-        const uint64_t nwork = p.front.work_len(na);
-        if (nwork < 10ull * p.row) return fail(APT_ERR_TOO_SHORT, "Got less than 10 rows of samples, audio file is too short");
-        if (sync && !p.work_multiple) return fail(APT_ERR_WORK_RATE, "work_rate is not multiple of FINAL_RATE");
-        need = sync ? (nwork / p.row) * kPxPerRow : plan_out_bound(p, na);
-    }
-    if (!out || cap < need) return fail(APT_ERR_CAPACITY, "output needs room for %llu floats", (unsigned long long)need);
-    APT_TRY(require_device());
-    int device = 0;
-    if (cudaGetDevice(&device) != cudaSuccess) device = 0;
-    static const bool use_cache = getenv("APTB200_NO_CACHE") == nullptr;
-    apt_decoder *d = use_cache ? cache_take(device, rate, *s, na) : nullptr;
-    if (!d) {
-        const uint64_t room = use_cache ? ((na + na / 8 + (1u << 20)) & ~((1ull << 20) - 1)) : na;
-        APT_TRY(apt_decoder_create(device, rate, s, room, &d));
-    }
-    auto run = [&]() -> int {
-        APT_CUDA(cudaSetDevice(d->device));
-        if (!d->iq_tables_valid || memcmp(&d->iq_settings, is, sizeof(*is)) != 0) {
-            d->iq_tables_valid = false;
-            APT_TRY(d->iq_tables.upload(ip));
-            d->iq_settings = *is;
-            d->iq_tables_valid = true;
-        }
-        if (d->audio_cap < d->max_samples) {
-            if (d->d_audio) APT_CUDA(cudaFree(d->d_audio));
-            d->d_audio = nullptr;
-            d->audio_cap = 0;
-            APT_CUDA(cudaMalloc(&d->d_audio, std::max<uint64_t>(d->max_samples, 1) * sizeof(float)));
-            d->audio_cap = d->max_samples;
-        }
-        if (!d->d_out) APT_CUDA(cudaMalloc(&d->d_out, std::max<uint64_t>(d->max_out, 1) * sizeof(float)));
-        if (is_pageable(iq) && !d->stager && !getenv("APTB200_NO_STAGER")) {
-            int threads = 8;
-            if (const char *e = getenv("APTB200_COPY_THREADS")) threads = std::max(1, atoi(e));
-            d->own_stager.reset(new (std::nothrow) HostStager(d->device, 16u << 20, 3, threads));
-            if (d->own_stager && !d->own_stager->ok()) d->own_stager.reset();
-            d->stager = d->own_stager.get();
-        }
-        APT_TRY(iq_demod_host(LaunchCtx{d->stream, d->sm_count}, ip, d->iq_tables, iq, format, n, d->iq_win,
-                              is_pageable(iq) ? d->stager : nullptr, d->d_audio, nullptr));
-        APT_TRY(apt_decoder_submit_device(d, d->d_audio, APT_F32, na, sync, d->d_out, d->max_out));
-        uint64_t produced = 0;
-        APT_TRY(apt_decoder_wait(d, &produced));
-        APT_CUDA(cudaMemcpy(out, d->d_out, produced * sizeof(float), cudaMemcpyDeviceToHost));
-        *nout = produced;
-        return APT_OK;
-    };
-    d->cb = cb;
-    d->cb_user = user;
-    const int st = run();
-    if (st != APT_OK) cudaStreamSynchronize(d->stream);
-    d->cb = nullptr;
-    d->cb_user = nullptr;
-    if (use_cache) cache_put(device, rate, *s, d);
-    else apt_decoder_destroy(d);
-    return st;
-}
+namespace {
 
-extern "C" int apt_decode_iq_channels(const void *iq, int format, uint64_t n, const apt_iq_settings *is, const int32_t *offsets,
-                                      int count, const apt_settings *s, int sync, float *const *outs, const uint64_t *caps,
-                                      uint64_t *nouts, int *statuses) {
+// apt_decode_iq_channels, with a status callback for every channel's decode.
+int decode_iq_channels(const void *iq, int format, uint64_t n, const apt_iq_settings *is, const int32_t *offsets, int count,
+                       const apt_settings *s, int sync, float *const *outs, const uint64_t *caps, uint64_t *nouts,
+                       int *statuses, apt_status_cb cb, void *user) {
     if (!is || !s || !offsets || !outs || !caps || !nouts || !statuses || count < 1)
         return fail(APT_ERR_BAD_ARG, "null argument or count < 1");
     auto fail_all = [&](int st) {
@@ -1109,7 +1025,7 @@ extern "C" int apt_decode_iq_channels(const void *iq, int format, uint64_t n, co
     }
     if (n == 0 || !iq) return fail_all(fail(APT_ERR_BAD_ARG, "empty signal"));
     if (!iq_sample_bytes(format)) return fail_all(fail(APT_ERR_BAD_ARG, "unknown I/Q sample format %d", format));
-    // every channel's argument errors before any device work, in apt_decode_iq's order
+    // every channel's argument errors before any device work, in decode_oneshot's order
     std::vector<IqPlan> ips(count);
     std::vector<apt_iq_settings> iss(count, *is);
     for (int c = 0; c < count; ++c) {
@@ -1120,16 +1036,7 @@ extern "C" int apt_decode_iq_channels(const void *iq, int format, uint64_t n, co
     const uint64_t na = ips[0].out_len(n);
     const uint32_t rate = is->audio_rate;
     uint64_t need = 0;
-    {
-        Plan p;
-        const int st = make_plan(rate, *s, p);
-        if (st != APT_OK) return fail_all(st);
-        const uint64_t nwork = p.front.work_len(na);
-        if (nwork < 10ull * p.row)
-            return fail_all(fail(APT_ERR_TOO_SHORT, "Got less than 10 rows of samples, audio file is too short"));
-        if (sync && !p.work_multiple) return fail_all(fail(APT_ERR_WORK_RATE, "work_rate is not multiple of FINAL_RATE"));
-        need = sync ? (nwork / p.row) * kPxPerRow : plan_out_bound(p, na);
-    }
+    if (const int st = check_decode(rate, *s, na, sync, &need); st != APT_OK) return fail_all(st);
     std::vector<int> live;
     for (int c = 0; c < count; ++c) {
         if (!outs[c] || caps[c] < need)
@@ -1146,27 +1053,17 @@ extern "C" int apt_decode_iq_channels(const void *iq, int format, uint64_t n, co
     if (const int st = require_device(); st != APT_OK) return fail_all(st);
     int device = 0;
     if (cudaGetDevice(&device) != cudaSuccess) device = 0;
-    static const bool use_cache = getenv("APTB200_NO_CACHE") == nullptr;
     // one parked decoder per live channel; the first one's stream, stager and I/Q window carry the upload
     std::vector<apt_decoder *> decs;
-    auto park = [&]() {
-        for (apt_decoder *d : decs) {
-            cudaStreamSynchronize(d->stream);
-            if (use_cache) cache_put_multi(device, rate, *s, d);
-            else apt_decoder_destroy(d);
-        }
-        decs.clear();
-    };
+    const bool pageable = is_pageable(iq);
     cudaEvent_t demod_done = nullptr;
     auto setup = [&]() -> int {
-        for (size_t k = 0; k < live.size(); ++k) {
-            apt_decoder *d = use_cache ? cache_take(device, rate, *s, na) : nullptr;
-            if (!d) {
-                const uint64_t room = use_cache ? ((na + na / 8 + (1u << 20)) & ~((1ull << 20) - 1)) : na;
-                APT_TRY(apt_decoder_create(device, rate, s, room, &d));
-            }
+        for (int c : live) {
+            apt_decoder *d = nullptr;
+            APT_TRY(take_decoder(device, rate, *s, na, true, &d));
             decs.push_back(d);
-            const int c = live[k];
+            d->cb = cb;
+            d->cb_user = user;
             APT_CUDA(cudaSetDevice(d->device));
             if (!d->iq_tables_valid || memcmp(&d->iq_settings, &iss[c], sizeof(iss[c])) != 0) {
                 d->iq_tables_valid = false;
@@ -1184,13 +1081,7 @@ extern "C" int apt_decode_iq_channels(const void *iq, int format, uint64_t n, co
             if (!d->d_out) APT_CUDA(cudaMalloc(&d->d_out, std::max<uint64_t>(d->max_out, 1) * sizeof(float)));
         }
         apt_decoder *d0 = decs[0];
-        if (is_pageable(iq) && !d0->stager && !getenv("APTB200_NO_STAGER")) {
-            int threads = 8;
-            if (const char *e = getenv("APTB200_COPY_THREADS")) threads = std::max(1, atoi(e));
-            d0->own_stager.reset(new (std::nothrow) HostStager(d0->device, 16u << 20, 3, threads));
-            if (d0->own_stager && !d0->own_stager->ok()) d0->own_stager.reset();
-            d0->stager = d0->own_stager.get();
-        }
+        if (pageable) ensure_stager(d0);
         std::vector<const IqPlan *> pl;
         std::vector<const IqTables *> tb;
         std::vector<float *> au;
@@ -1200,41 +1091,56 @@ extern "C" int apt_decode_iq_channels(const void *iq, int format, uint64_t n, co
             au.push_back(decs[k]->d_audio);
         }
         APT_TRY(iq_demod_host_multi(LaunchCtx{d0->stream, d0->sm_count}, pl.data(), tb.data(), au.data(),
-                                    static_cast<int>(live.size()), iq, format, n, d0->iq_win,
-                                    is_pageable(iq) ? d0->stager : nullptr, nullptr));
+                                    static_cast<int>(live.size()), iq, format, n, d0->iq_win, pageable ? d0->stager : nullptr,
+                                    nullptr));
         APT_CUDA(cudaEventCreateWithFlags(&demod_done, cudaEventDisableTiming));
         APT_CUDA(cudaEventRecord(demod_done, d0->stream));
         return APT_OK;
     };
-    int st = setup();
-    if (st != APT_OK) {
-        if (demod_done) cudaEventDestroy(demod_done);
-        park();
+    const int st = setup();
+    if (st == APT_OK) {
+        // every channel's decode on its own decoder's stream, after the demodulation; they run side by side
+        std::vector<int> submitted(live.size(), APT_OK);
+        for (size_t k = 0; k < live.size(); ++k) {
+            apt_decoder *d = decs[k];
+            submitted[k] = cudaStreamWaitEvent(d->stream, demod_done, 0) == cudaSuccess
+                               ? apt_decoder_submit_device(d, d->d_audio, APT_F32, na, sync, d->d_out, d->max_out)
+                               : fail(APT_ERR_CUDA, "cudaStreamWaitEvent failed");
+        }
+        for (size_t k = 0; k < live.size(); ++k) {
+            apt_decoder *d = decs[k];
+            const int c = live[k];
+            uint64_t produced = 0;
+            int cst = submitted[k];
+            if (cst == APT_OK) cst = apt_decoder_wait(d, &produced);
+            if (cst == APT_OK && cudaMemcpy(outs[c], d->d_out, produced * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess)
+                cst = fail(APT_ERR_CUDA, "copying the rows of channel %d failed", c);
+            if (cst == APT_OK) nouts[c] = produced;
+            statuses[c] = cst;
+        }
+    } else {
         for (int c : live) statuses[c] = st;
-        return st;
     }
-    // every channel's decode on its own decoder's stream, after the demodulation; they run side by side
-    std::vector<int> submitted(live.size(), APT_OK);
-    for (size_t k = 0; k < live.size(); ++k) {
-        apt_decoder *d = decs[k];
-        submitted[k] = cudaStreamWaitEvent(d->stream, demod_done, 0) == cudaSuccess
-                           ? apt_decoder_submit_device(d, d->d_audio, APT_F32, na, sync, d->d_out, d->max_out)
-                           : fail(APT_ERR_CUDA, "cudaStreamWaitEvent failed");
-    }
-    for (size_t k = 0; k < live.size(); ++k) {
-        apt_decoder *d = decs[k];
-        const int c = live[k];
-        uint64_t produced = 0;
-        int cst = submitted[k];
-        if (cst == APT_OK) cst = apt_decoder_wait(d, &produced);
-        if (cst == APT_OK && cudaMemcpy(outs[c], d->d_out, produced * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess)
-            cst = fail(APT_ERR_CUDA, "copying the rows of channel %d failed", c);
-        if (cst == APT_OK) nouts[c] = produced;
-        statuses[c] = cst;
-    }
-    cudaEventDestroy(demod_done);
-    park();
-    return first_status();
+    if (demod_done) cudaEventDestroy(demod_done);
+    for (apt_decoder *d : decs) park_decoder(d, decs.size() > 1);
+    return st != APT_OK ? st : first_status();
+}
+
+}  // namespace
+
+// apt_decode at audio_rate of the audio the FM kernel writes into the parked decoder's device input: the one channel at
+// is->offset_hz.
+extern "C" int apt_decode_iq(const void *iq, int format, uint64_t n, const apt_iq_settings *is, const apt_settings *s, int sync,
+                             float *out, uint64_t cap, uint64_t *nout, apt_status_cb cb, void *user) {
+    if (!is || !s || !nout) return fail(APT_ERR_BAD_ARG, "null argument");
+    int status = APT_OK;
+    return decode_iq_channels(iq, format, n, is, &is->offset_hz, 1, s, sync, &out, &cap, nout, &status, cb, user);
+}
+
+extern "C" int apt_decode_iq_channels(const void *iq, int format, uint64_t n, const apt_iq_settings *is, const int32_t *offsets,
+                                      int count, const apt_settings *s, int sync, float *const *outs, const uint64_t *caps,
+                                      uint64_t *nouts, int *statuses) {
+    return decode_iq_channels(iq, format, n, is, offsets, count, s, sync, outs, caps, nouts, statuses, nullptr, nullptr);
 }
 
 extern "C" int apt_decode_iq_auto(const void *iq, int format, uint64_t n, const apt_iq_settings *is, const apt_carrier_search *cs,
@@ -1255,11 +1161,7 @@ extern "C" int apt_decode_iq_auto(const void *iq, int format, uint64_t n, const 
         APT_TRY(make_search(cs, is->iq_rate, sp));
         SpecPlan spec;
         APT_TRY(make_spectrum(n, sp.nfft, sp.max_segments, spec));
-        Plan p;
-        APT_TRY(make_plan(is->audio_rate, *s, p));
-        if (p.front.work_len(ip.out_len(n)) < 10ull * p.row)
-            return fail(APT_ERR_TOO_SHORT, "Got less than 10 rows of samples, audio file is too short");
-        if (sync && !p.work_multiple) return fail(APT_ERR_WORK_RATE, "work_rate is not multiple of FINAL_RATE");
+        APT_TRY(check_decode(is->audio_rate, *s, ip.out_len(n), sync));
     }
     // kept carriers are more than 40 kHz apart inside a band narrower than iq_rate: this many always suffice
     std::vector<apt_carrier> all(is->iq_rate / 40000 + 2);
@@ -1750,7 +1652,6 @@ int run_batch(const void *const *signals, int format, const uint64_t *lens, int 
         nouts[i] = 0;
         if (statuses) statuses[i] = APT_ERR_CUDA;      // overwritten by the job's own status; never left "ok" by default
     }
-    static const bool use_cache = getenv("APTB200_NO_CACHE") == nullptr;
     std::vector<int> local_status(count, APT_ERR_CUDA);
     std::vector<std::string> messages(ndevices);
     std::vector<int> fatal(ndevices, APT_OK);
@@ -1817,14 +1718,11 @@ int run_batch(const void *const *signals, int format, const uint64_t *lens, int 
                 if (job_of[k] < 0) { free_k = k; break; }
             if (next < count && (free_k < decs.size() || static_cast<int>(decs.size()) < streams_per_device)) {
                 if (free_k == decs.size()) {
-                    apt_decoder *d = cache_take(device, input_rate, *s, max_len);     // parked by an earlier call
-                    int st = d ? APT_OK : apt_decoder_create(device, input_rate, s, max_len, &d);
+                    apt_decoder *d = nullptr;
+                    int st = take_decoder(device, input_rate, *s, max_len, false, &d);
                     if (st == APT_OK && img) {
                         st = apt_decoder_set_process_mode(d, img->ps);
-                        if (st != APT_OK) {
-                            if (use_cache) cache_put_multi(device, input_rate, *s, d);
-                            else apt_decoder_destroy(d);
-                        }
+                        if (st != APT_OK) park_decoder(d, true);
                     }
                     if (st != APT_OK) {
                         if (decs.empty()) { fail_rest(st); continue; }
@@ -1832,18 +1730,8 @@ int run_batch(const void *const *signals, int format, const uint64_t *lens, int 
                         continue;
                     }
                     // one stager (ring + copy threads) serves all decoders of this feeder: the first decoder's own
-                    if (decs.empty()) {
-                        if (!d->own_stager) {
-                            int threads = 8;
-                            if (const char *e = getenv("APTB200_COPY_THREADS")) threads = std::max(1, atoi(e));
-                            d->own_stager.reset(new (std::nothrow) HostStager(device, 16u << 20, 3, threads));
-                            if (d->own_stager && !d->own_stager->ok()) d->own_stager.reset();
-                        }
-                        d->stager = d->own_stager.get();
-                    } else {
-                        d->stager = decs[0]->stager;
-                    }
-                    if (!img) d->post_plan.reset();
+                    if (decs.empty()) ensure_stager(d);
+                    else d->stager = decs[0]->stager;
                     d->keep_image = feed != nullptr;
                     decs.push_back(d);
                     job_of.push_back(-1);
@@ -1875,16 +1763,7 @@ int run_batch(const void *const *signals, int format, const uint64_t *lens, int 
             }
             if (feed && feed->busy()) feed->finish(reinterpret_cast<uint8_t *const *>(outs), caps, nouts, local_status);   // the pool is full
         }
-        for (auto *d : decs) {
-            d->stager = d->own_stager.get();           // nullptr unless it owns one: never keep a pointer into another decoder
-            if (img) {
-                cudaStreamSynchronize(d->stream);      // the last copy into the pool has left d_out8
-                d->post_plan.reset();
-                d->keep_image = false;
-            }
-            if (use_cache) cache_put_multi(device, input_rate, *s, d);
-            else apt_decoder_destroy(d);
-        }
+        for (auto *d : decs) park_decoder(d, true);   // drains the last copy into the PNG pool
         feed.reset();
     };
 

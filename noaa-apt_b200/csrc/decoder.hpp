@@ -55,10 +55,14 @@ uint64_t plan_table_bytes(const Plan &p);
 int free_decoder_buffers(apt_decoder *d);
 // Grows the f32 copy of a PCM16 input to `alloc` samples when it holds fewer than `need`.
 int ensure_conv(apt_decoder *d, uint64_t need, uint64_t alloc);
-// The decoders apt_decode parks between calls: take_decoder hands out a parked decoder for (device, rate, settings) of at
-// least n samples, else creates one with apt_decode's head-room; park_decoder hands it back (APTB200_NO_CACHE: destroys it).
-int take_decoder(int device, uint32_t rate, const apt_settings &st, uint64_t n, apt_decoder **d);
-void park_decoder(int device, uint32_t rate, const apt_settings &st, apt_decoder *d);
+// The decoders the convenience entry points park between calls (APTB200_NO_CACHE: none are parked).  take_decoder hands
+// out a parked decoder for (device, rate, settings) of at least n samples, else creates one of n samples, with head-room
+// for a slightly longer next recording when `headroom` and the cache is on.  park_decoder drains the decoder's stream, clears the state of
+// the call (image, process and PNG mode, keep_image, the status callback, a borrowed stager) and parks the decoder
+// under its own key, or destroys it.  `several`: keep it beside others of its key (a batch's decoders), else it
+// replaces a smaller one of the same key.
+int take_decoder(int device, uint32_t rate, const apt_settings &st, uint64_t n, bool headroom, apt_decoder **d);
+void park_decoder(apt_decoder *d, bool several);
 
 // Kernel accounting of a decoder: counts the launch and, when profiling, records the begin event of slot `name`;
 // returns the slot to close with prof_end (-1: none).

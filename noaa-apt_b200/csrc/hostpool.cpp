@@ -6,6 +6,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <new>
 #include <string>
 
 #include <sched.h>
@@ -217,6 +218,15 @@ cudaError_t HostStager::upload_pieces(void *dst, const void *src, const uint64_t
         used_[r] = true;
     }
     return cudaSuccess;
+}
+
+std::unique_ptr<HostStager> make_stager(int device) {
+    if (getenv("APTB200_NO_STAGER")) return nullptr;
+    int threads = 8;
+    if (const char *e = getenv("APTB200_COPY_THREADS")) threads = std::max(1, atoi(e));
+    std::unique_ptr<HostStager> s(new (std::nothrow) HostStager(device, 16u << 20, 3, threads));
+    if (s && !s->ok()) s.reset();
+    return s;
 }
 
 bool is_pageable(const void *p) {

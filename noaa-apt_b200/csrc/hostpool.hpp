@@ -9,6 +9,7 @@
 #include <condition_variable>
 #include <cstddef>
 #include <cstdint>
+#include <memory>
 #include <mutex>
 #include <thread>
 #include <vector>
@@ -72,6 +73,10 @@ private:
     CopyPool pool_;
     bool ok_ = false;
 };
+
+// The staging ring of every pageable-buffer upload: three 16-MiB buffers and APTB200_COPY_THREADS copy threads (8 by
+// default).  nullptr under APTB200_NO_STAGER or when the ring cannot be allocated: the caller then uses cudaMemcpyAsync.
+std::unique_ptr<HostStager> make_stager(int device);
 
 // true if `p` is ordinary pageable host memory (not pinned / registered / managed / device)
 bool is_pageable(const void *p);

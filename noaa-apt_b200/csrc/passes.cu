@@ -153,13 +153,7 @@ extern "C" int apt_recording_create(int device, const void *signal, int format, 
     APT_TRY(device_alloc(r.get(), r->d_q, r->windows));
 
     // the one upload: pageable buffers through the pinned ring and its copy threads, pinned ones straight
-    std::unique_ptr<HostStager> stager;
-    if (is_pageable(signal) && !getenv("APTB200_NO_STAGER")) {
-        int threads = 8;
-        if (const char *e = getenv("APTB200_COPY_THREADS")) threads = std::max(1, atoi(e));
-        stager.reset(new (std::nothrow) HostStager(device, 16u << 20, 3, threads));
-        if (stager && !stager->ok()) stager.reset();
-    }
+    const std::unique_ptr<HostStager> stager = is_pageable(signal) ? make_stager(device) : nullptr;
     if (stager)
         APT_CUDA(stager->upload(r->d_sig, signal, bytes, r->stream));
     else
@@ -335,18 +329,13 @@ extern "C" int apt_recording_decode(apt_recording *rec, const apt_pass *ranges, 
     apt_decoder *d = nullptr;
     void *slice = nullptr, *dout = nullptr;
     auto release = [&]() {
-        if (d) {
-            cudaStreamSynchronize(d->stream);
-            d->post_plan.reset();
-            d->png_active = false;
-            park_decoder(rec->device, p.input_rate, p.st, d);
-        }
+        if (d) park_decoder(d, false);
         if (slice) cudaFree(slice);
         if (dout) cudaFree(dout);
         cudaGetLastError();
     };
     auto setup = [&]() -> int {
-        APT_TRY(take_decoder(rec->device, p.input_rate, p.st, max_len, &d));
+        APT_TRY(take_decoder(rec->device, p.input_rate, p.st, max_len, true, &d));
         // each range starts at an arbitrary sample: the decoder gets it at the start of a fresh (256-byte aligned) buffer,
         // as apt_decode's own staging buffer, so that every first-stage kernel sees the alignment it would see there
         APT_CUDA(cudaMalloc(&slice, max_len * sb));

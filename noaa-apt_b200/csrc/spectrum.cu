@@ -287,17 +287,16 @@ int spec_finish(SpecWork &w, const SpecPlan &p, float *d_psd) {
     return APT_OK;
 }
 
-bool want_stager(const void *host) { return is_pageable(host) && !getenv("APTB200_NO_STAGER"); }
-
-int ensure_stager(SpecWork &w) {
-    if (w.stager) return APT_OK;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    int threads = 8;
-    if (const char *e = getenv("APTB200_COPY_THREADS")) threads = std::max(1, atoi(e));
-    w.stager.reset(new (std::nothrow) HostStager(dev, 16u << 20, 3, threads));
-    if (w.stager && !w.stager->ok()) w.stager.reset();
-    return APT_OK;   // without a stager the upload falls back to cudaMemcpyAsync
+// The staging ring for an upload from `host`, made on first use: nullptr for pinned input, or when there is no ring
+// (the upload is then a cudaMemcpyAsync).
+HostStager *stager_for(SpecWork &w, const void *host) {
+    if (!is_pageable(host)) return nullptr;
+    if (!w.stager) {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        w.stager = make_stager(dev);
+    }
+    return w.stager.get();
 }
 
 // The spectrum of host I/Q into w.psd: the K segments uploaded in chunks of whole segments (APTB200_IQ_CHUNK samples at
@@ -309,16 +308,15 @@ int spec_host(SpecWork &w, const SpecPlan &p, const void *iq, int format) {
     APT_TRY(spec_setup(w, p));
     APT_TRY(grow(w.psd, w.psd_cap, p.nfft));
     APT_TRY(w.seg.reserve(per * piece));
-    const bool staged = want_stager(iq);
-    if (staged) APT_TRY(ensure_stager(w));
+    HostStager *const stager = stager_for(w, iq);
     const char *src = static_cast<const char *>(iq);
     std::vector<uint64_t> offs;
     for (u64 k0 = 0; k0 < p.K; k0 += per) {
         const u64 k1 = std::min<u64>(p.K, k0 + per);
         offs.resize(k1 - k0);
         for (u64 k = k0; k < k1; ++k) offs[k - k0] = p.start(k) * sb;
-        if (staged && w.stager) {
-            APT_CUDA(w.stager->upload_pieces(w.seg.p, src, offs.data(), offs.size(), piece, w.stream));
+        if (stager) {
+            APT_CUDA(stager->upload_pieces(w.seg.p, src, offs.data(), offs.size(), piece, w.stream));
         } else {
             // pinned input: one copy per run of adjacent segments
             for (u64 i = 0; i < offs.size();) {
@@ -355,8 +353,7 @@ int apt_test(SpecWork &w, const void *iq, int format, uint64_t n, apt_iq_setting
     APT_TRY(grow(w.audio, w.audio_cap, L));
     APT_TRY(grow(w.acf, w.acf_cap, L));
     const char *src = static_cast<const char *>(iq) + xa * sb;
-    if (want_stager(iq)) APT_TRY(ensure_stager(w));
-    if (want_stager(iq) && w.stager) APT_CUDA(w.stager->upload(w.seg.p, src, (xb - xa) * sb, w.stream));
+    if (HostStager *stager = stager_for(w, iq)) APT_CUDA(stager->upload(w.seg.p, src, (xb - xa) * sb, w.stream));
     else APT_CUDA(cudaMemcpyAsync(w.seg.p, src, (xb - xa) * sb, cudaMemcpyHostToDevice, w.stream));
     const LaunchCtx c{w.stream, w.sms};
     APT_TRY(iq_launch(c, ip, w.iqt, static_cast<const char *>(w.seg.p) - xa * sb, xa, xb, format, m0, m1, w.audio - m0));

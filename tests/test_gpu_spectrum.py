@@ -115,6 +115,7 @@ def test_staging_ring_and_pinned_input(na, monkeypatch):
     pinned = torch.from_numpy(x).pin_memory()                    # one copy per run of adjacent segments: three runs
     _assert_bits(_device(na, x, nfft, ptr=pinned.data_ptr())[0], want, "pinned")
     monkeypatch.setenv("APTB200_NO_STAGER", "1")
+    na._lib.load().apt_cache_clear()                             # a fresh workspace: it gets no staging ring
     _assert_bits(_device(na, x, nfft)[0], want, "pageable without the staging ring")
 
 
