@@ -94,12 +94,9 @@ int aptb200::free_decoder_buffers(apt_decoder *d) {
         if (p) cudaFree(p);
     if (d->h_res) cudaFreeHost(d->h_res);
     if (d->h_out) cudaFreeHost(d->h_out);
-    if (d->d_out8) cudaFree(d->d_out8);
-    d->post.release();
+    d->img.release();
     d->iq_tables.release();
     d->iq_win.release();
-    d->png_work.release();
-    if (d->h_png) cudaFreeHost(d->h_png);
     if (d->d_audio) cudaFree(d->d_audio);
     d->own_stager.reset();
     for (auto e : d->ev_begin) cudaEventDestroy(e);
@@ -447,25 +444,22 @@ extern "C" void apt_decoder_destroy(apt_decoder *dec) {
 
 namespace {
 
-// Bytes of one output pixel of the job: the plan's, or an f32 row value.
-size_t out_elem(const apt_decoder *d) { return d->post_plan ? static_cast<size_t>(d->post_plan->bpp) : sizeof(float); }
-
 // The job after the rows, at submit and again after a sync redo: the image stage on the rows in d_out (its head follows
 // to the pinned copy), the SyncResult and, for host jobs, the rows or the image to the caller.
 int enqueue_job_tail(apt_decoder *d) {
-    if (d->post_plan) {
+    ImageOut &o = d->img;
+    if (o.plan.image) {
         const u32 max_rows = static_cast<u32>(std::max<uint64_t>(d->max_out / kPxPerRow, 1));
         const u32 fixed = d->job_sync ? 0u : static_cast<u32>(d->job_fixed_out / kPxPerRow);
-        unsigned char *image = d->job_host || d->job_png ? d->d_out8 : reinterpret_cast<unsigned char *>(d->job_out);
         DecoderHook hook(d);
-        APT_TRY(post_launch(LaunchCtx{d->stream, d->sm_count}, *d->post_plan, d->post, d->d_out, d->job_sync ? d->back.res : nullptr,
-                            fixed, max_rows, kPxPerRow, nullptr, image, &hook));
+        APT_TRY(o.launch(LaunchCtx{d->stream, d->sm_count}, d->d_out, d->job_sync ? d->back.res : nullptr, fixed, max_rows,
+                         d->job_host || o.plan.png ? nullptr : d->job_out, &hook));
     }
     if (d->job_sync) APT_CUDA(cudaMemcpyAsync(d->h_res, d->back.res, sizeof(SyncResult), cudaMemcpyDeviceToHost, d->stream));
     if (d->job_host && d->job_d2h_floats)
         APT_CUDA(cudaMemcpyAsync(d->job_out_pageable ? static_cast<void *>(d->h_out) : static_cast<void *>(d->job_out),
-                                 d->post_plan ? static_cast<const void *>(d->d_out8) : static_cast<const void *>(d->d_out),
-                                 d->job_d2h_floats * out_elem(d), cudaMemcpyDeviceToHost, d->stream));
+                                 o.plan.image ? static_cast<const void *>(o.px) : static_cast<const void *>(d->d_out),
+                                 o.plan.px_bytes(d->job_d2h_floats), cudaMemcpyDeviceToHost, d->stream));
     return APT_OK;
 }
 
@@ -499,29 +493,22 @@ int submit_common(apt_decoder *d, const void *signal, int format, uint64_t n, in
         return fail(APT_ERR_BAD_ARG, "work_rate %u is too high for the sync picker (min_distance %u > 16384); decode without "
                                      "sync or use a work_rate <= 37440", p.st.work_rate, p.dist);
     const uint64_t need = d->job_sync ? (nwork / p.row) * kPxPerRow : plan_out_bound(p, n);
-    const PostPlan *post = d->post_plan ? &*d->post_plan : nullptr;
+    ImageOut &o = d->img;
+    const bool post = o.plan.image;
     // cap counts bytes of an image job, floats of an f32 one; in PNG mode PNG bytes, checked at wait() once the file's
     // length is known
-    const uint64_t per_px = post ? post->bpp : 1;
-    const bool png = post && d->png_active;
-    const bool keep = post && d->keep_image && host;
-    if (png && d->png.rgb_from_rgba && per_px != 4) return fail(APT_ERR_BAD_ARG, "rgb_from_rgba needs RGBA process output");
+    const uint64_t per_px = post ? o.plan.post.bpp : 1;
+    const bool png = post && o.plan.png;
+    const bool keep = post && o.keep && host;
+    if (png && o.plan.png_s.rgb_from_rgba && per_px != 4) return fail(APT_ERR_BAD_ARG, "rgb_from_rgba needs RGBA process output");
     if (png && !out) return fail(APT_ERR_BAD_ARG, "null output");
     if (!png && !keep && (!out || cap < need * per_px))
         return fail(APT_ERR_CAPACITY, "output needs room for %llu %s", (unsigned long long)(need * per_px), post ? "bytes" : "floats");
-    d->job_png = png;
     if (post) {
         if (!p.work_multiple) return fail(APT_ERR_BAD_ARG, "the image stage needs rows of 2080 pixels (work_rate multiple of 4160)");
-        APT_TRY(d->post.alloc(*post, static_cast<u32>(std::max<uint64_t>(d->max_out / kPxPerRow, 1))));
+        APT_TRY(o.post.alloc(o.plan.post, static_cast<u32>(std::max<uint64_t>(d->max_out / kPxPerRow, 1))));
         if (!d->d_out) APT_CUDA(cudaMalloc(&d->d_out, std::max<uint64_t>(d->max_out, 1) * sizeof(float)));
-        const uint64_t out8_need = std::max<uint64_t>(d->max_out, 1) * per_px;
-        if ((host || png) && d->out8_bytes < out8_need) {
-            if (d->d_out8) APT_CUDA(cudaFree(d->d_out8));
-            d->d_out8 = nullptr;
-            d->out8_bytes = 0;
-            APT_CUDA(cudaMalloc(&d->d_out8, out8_need));
-            d->out8_bytes = out8_need;
-        }
+        if (host || png) APT_TRY(o.reserve_px(std::max<uint64_t>(d->max_out, 1) * per_px));
     }
 
     const void *dev_in = signal;
@@ -594,22 +581,14 @@ extern "C" int apt_decoder_submit_host(apt_decoder *dec, const void *signal, int
 
 namespace {
 
-// PNG mode, at wait(): encode the job's image (in d_out8) on the decoder's stream, read the file's length from the pinned
-// control block, then copy exactly that many bytes to the caller's buffer.  Two stream synchronisations.
+// PNG mode, at wait(): encode the job's image on the decoder's stream, read the file's length, then copy exactly that many
+// bytes to the caller's buffer.  Two stream synchronisations.
 int png_job(apt_decoder *d, uint64_t rows, uint64_t *bytes) {
-    PngPlan p;
-    APT_TRY(make_png(kPxPerRow, static_cast<uint32_t>(rows), d->post_plan->bpp, &d->png, p));
-    if (!d->h_png) APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&d->h_png), sizeof(PngCtl), cudaHostAllocDefault));
     DecoderHook hook(d);
-    const unsigned char *px = d->d_out8;
-    APT_TRY(png_encode_device(LaunchCtx{d->stream, d->sm_count}, &p, &px, 1, d->png_work, &hook));
-    APT_CUDA(cudaMemcpyAsync(d->h_png, d->png_work.ctl, sizeof(PngCtl), cudaMemcpyDeviceToHost, d->stream));
+    APT_TRY(d->img.encode_px(LaunchCtx{d->stream, d->sm_count}, rows, &hook));
     APT_CUDA(cudaStreamSynchronize(d->stream));
-    const uint64_t total = d->h_png->total;
-    *bytes = total;
-    if (total > d->job_cap) return fail(APT_ERR_CAPACITY, "output needs room for %llu PNG bytes", (unsigned long long)total);
-    APT_CUDA(cudaMemcpyAsync(d->job_out, d->png_work.out, total, d->job_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice,
-                             d->stream));
+    *bytes = d->img.length(0);
+    APT_TRY(d->img.copy_out(0, d->job_out, d->job_cap, d->job_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, d->stream));
     APT_CUDA(cudaStreamSynchronize(d->stream));
     return APT_OK;
 }
@@ -649,24 +628,24 @@ extern "C" int apt_decoder_wait(apt_decoder *d, uint64_t *nout) {
         }
         produced = static_cast<uint64_t>(res.n_rows) * kPxPerRow;
     }
-    const size_t elem = out_elem(d);
-    if (d->job_host && d->job_out_pageable && produced && !d->job_png) {
-        if (d->stager) d->stager->scatter(d->job_out, d->h_out, produced * elem);
-        else memcpy(d->job_out, d->h_out, produced * elem);
+    const bool png = d->img.plan.png;
+    if (d->job_host && d->job_out_pageable && produced && !png) {
+        if (d->stager) d->stager->scatter(d->job_out, d->h_out, d->img.plan.px_bytes(produced));
+        else memcpy(d->job_out, d->h_out, d->img.plan.px_bytes(produced));
     }
     if (trace)
         fprintf(stderr, "[aptb200 host] wait: stream sync %.2f ms, copy-out %.2f ms (%s)\n",
                 std::chrono::duration<double>(t_synced - t_begin).count() * 1e3,
                 std::chrono::duration<double>(std::chrono::steady_clock::now() - t_synced).count() * 1e3,
                 d->job_out_pageable ? "pageable" : "direct");
-    if (d->post_plan) {
-        d->job_status = post_result(*d->post.head, &d->last_image);
+    if (d->img.plan.image) {
+        d->job_status = post_result(*d->img.post.head, &d->img.info);
         if (d->job_status != APT_OK) return d->job_status;
     }
     d->last_rows = d->plan.work_multiple ? produced / kPxPerRow : 0;
     d->last_out = produced;
     uint64_t png_bytes = 0;
-    if (d->job_png) {
+    if (png) {
         const int st = png_job(d, produced / kPxPerRow, &png_bytes);
         if (st != APT_OK) {
             if (st == APT_ERR_CAPACITY && nout) *nout = png_bytes;
@@ -678,7 +657,7 @@ extern "C" int apt_decoder_wait(apt_decoder *d, uint64_t *nout) {
         d->kernel_ms.assign(d->ev_used, 0.f);
         for (int i = 0; i < d->ev_used; ++i) cudaEventElapsedTime(&d->kernel_ms[i], d->ev_begin[i], d->ev_end[i]);
     }
-    if (nout) *nout = d->job_png ? png_bytes : d->post_plan ? produced * d->post_plan->bpp : produced;
+    if (nout) *nout = png ? png_bytes : produced * (d->img.plan.image ? d->img.plan.post.bpp : 1);
     return APT_OK;
 }
 
@@ -686,23 +665,26 @@ extern "C" int apt_decoder_set_image_mode(apt_decoder *d, int contrast, float pe
     if (!d) return fail(APT_ERR_BAD_ARG, "null decoder");
     if (d->in_flight) return fail(APT_ERR_BAD_ARG, "decoder has a job in flight");
     if (contrast < 0) {
-        d->post_plan.reset();
-        d->png_active = false;
+        d->img.plan = OutPlan{};
         return APT_OK;
     }
     if (contrast == APT_CONTRAST_HISTOGRAM) return fail(APT_ERR_BAD_ARG, "unknown contrast mode %d", contrast);
     PostPlan plan;
     APT_TRY(make_post(image_settings(contrast, percent), plan));
-    d->post_plan = plan;
+    d->img.plan.post = plan;
+    d->img.plan.image = true;
     return APT_OK;
 }
 
 namespace {
 
-// make_post for the entry points that take the settings by pointer.
-int process_plan(const apt_process_settings *ps, PostPlan &plan) {
+// The output plan of the entry points that make an image from process settings taken by pointer: null process settings
+// are an error, and so are null PNG settings when `file`.
+int image_plan(const apt_process_settings *ps, const apt_png_settings *png, bool file, OutPlan &plan) {
     if (!ps) return fail(APT_ERR_BAD_ARG, "null process settings");
-    return make_post(*ps, plan);
+    APT_TRY(make_out_plan(ps, png, plan));
+    if (file && !png) return fail(APT_ERR_BAD_ARG, "null PNG settings");
+    return APT_OK;
 }
 
 }  // namespace
@@ -711,43 +693,30 @@ extern "C" int apt_decoder_set_process_mode(apt_decoder *d, const apt_process_se
     if (!d) return fail(APT_ERR_BAD_ARG, "null decoder");
     if (d->in_flight) return fail(APT_ERR_BAD_ARG, "decoder has a job in flight");
     if (!ps) {
-        d->post_plan.reset();
-        d->png_active = false;
+        d->img.plan = OutPlan{};
         return APT_OK;
     }
     PostPlan plan;
     APT_TRY(make_post(*ps, plan));
     if (plan.palette) {
         APT_CUDA(cudaSetDevice(d->device));
-        APT_TRY(d->post.upload_palette(ps->palette, d->stream));
+        APT_TRY(d->img.post.upload_palette(ps->palette, d->stream));
     }
-    d->post_plan = plan;
+    d->img.plan.post = plan;
+    d->img.plan.image = true;
     return APT_OK;
-}
-
-// The settings rules of PNG output for an image of `channels` channels (no device, no pixels).
-static int check_png_settings(const apt_png_settings *png, int channels) {
-    PngPlan p;
-    return make_png(kPxPerRow, 1, channels, png, p);
 }
 
 extern "C" int apt_decoder_set_png_mode(apt_decoder *d, const apt_png_settings *ps) {
     if (!d) return fail(APT_ERR_BAD_ARG, "null decoder");
     if (d->in_flight) return fail(APT_ERR_BAD_ARG, "decoder has a job in flight");
-    if (!ps) {
-        d->png_active = false;
-        return APT_OK;
-    }
-    if (!d->post_plan) return fail(APT_ERR_BAD_ARG, "PNG mode needs image or process mode");
-    APT_TRY(check_png_settings(ps, d->post_plan->bpp));
-    d->png = *ps;
-    d->png_active = true;
-    return APT_OK;
+    if (ps && !d->img.plan.image) return fail(APT_ERR_BAD_ARG, "PNG mode needs image or process mode");
+    return d->img.plan.set_png(ps);
 }
 
 extern "C" int apt_decoder_image_info(apt_decoder *d, apt_image_info *info) {
     if (!d || !info) return fail(APT_ERR_BAD_ARG, "null argument");
-    *info = d->last_image;
+    *info = d->img.info;
     return APT_OK;
 }
 
@@ -920,9 +889,8 @@ int aptb200::take_decoder(int device, uint32_t rate, const apt_settings &st, uin
 
 void aptb200::park_decoder(apt_decoder *d, bool several) {
     cudaStreamSynchronize(d->stream);
-    d->post_plan.reset();
-    d->png_active = false;
-    d->keep_image = false;
+    d->img.plan = OutPlan{};
+    d->img.keep = false;
     d->cb = nullptr;
     d->cb_user = nullptr;
     d->stager = d->own_stager.get();   // never keep a pointer into another decoder
@@ -974,7 +942,7 @@ int decode_oneshot(const void *signal, int format, uint64_t n, uint32_t input_ra
     if (st == APT_OK && png) st = apt_decoder_set_png_mode(d, png);
     if (st == APT_OK) st = apt_decoder_submit_host(d, signal, format, n, sync, out, cap);
     if (st == APT_OK) st = apt_decoder_wait(d, nout);
-    if (st == APT_OK && info) *info = d->last_image;
+    if (st == APT_OK && info) *info = d->img.info;
     park_decoder(d, false);
     return st;
 }
@@ -1194,17 +1162,16 @@ extern "C" int apt_decode_image_u8(const void *signal, int format, uint64_t n, u
 extern "C" int apt_decode_image(const void *signal, int format, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
                                 const apt_process_settings *ps, uint8_t *out, uint64_t cap, uint64_t *nout, apt_image_info *info,
                                 apt_status_cb cb, void *user) {
-    PostPlan plan;
-    APT_TRY(process_plan(ps, plan));
+    OutPlan plan;
+    APT_TRY(image_plan(ps, nullptr, false, plan));
     return decode_oneshot(signal, format, n, input_rate, s, sync, reinterpret_cast<float *>(out), cap, nout, cb, user, ps, info);
 }
 
 extern "C" int apt_decode_png(const void *signal, int format, uint64_t n, uint32_t input_rate, const apt_settings *s, int sync,
                               const apt_process_settings *ps, const apt_png_settings *png, uint8_t *out, uint64_t cap,
                               uint64_t *nout, apt_image_info *info, apt_status_cb cb, void *user) {
-    PostPlan plan;
-    APT_TRY(process_plan(ps, plan));
-    APT_TRY(check_png_settings(png, plan.bpp));
+    OutPlan plan;
+    APT_TRY(image_plan(ps, png, true, plan));
     if (!out) return fail(APT_ERR_BAD_ARG, "null output");
     return decode_oneshot(signal, format, n, input_rate, s, sync, reinterpret_cast<float *>(out), cap, nout, cb, user, ps, info, png);
 }
@@ -1212,9 +1179,8 @@ extern "C" int apt_decode_png(const void *signal, int format, uint64_t n, uint32
 extern "C" int apt_decode_wav_png(const char *input_path, const char *output_path, const apt_settings *s, int sync,
                                   const apt_process_settings *ps, const apt_png_settings *png, apt_image_info *info) {
     if (!input_path || !output_path || !s) return fail(APT_ERR_BAD_ARG, "null argument");
-    PostPlan plan;
-    APT_TRY(process_plan(ps, plan));
-    APT_TRY(check_png_settings(png, plan.bpp));
+    OutPlan plan;
+    APT_TRY(image_plan(ps, png, true, plan));
     apt_wav_info wi;
     APT_TRY(apt_wav_info_read(input_path, &wi));
     uint32_t rate = 0;
@@ -1229,11 +1195,9 @@ extern "C" int apt_decode_wav_png(const char *input_path, const char *output_pat
         x.resize(std::max<uint64_t>(wi.frames, 1));
         APT_TRY(apt_wav_load(input_path, x.data(), x.size(), &n, &rate));
     }
-    uint64_t rows_bound = 0, cap = 0;
-    APT_TRY(apt_decode_len_bound(n, rate, s, &rows_bound));
-    rows_bound = std::max<uint64_t>(rows_bound / kPxPerRow, 1);
-    if (rows_bound > 0xFFFFFFFFull) return fail(APT_ERR_BAD_ARG, "recording too long");
-    APT_TRY(apt_png_bound(kPxPerRow, static_cast<uint32_t>(rows_bound), plan.bpp, png, &cap));
+    uint64_t px_bound = 0, cap = 0;
+    APT_TRY(apt_decode_len_bound(n, rate, s, &px_bound));
+    APT_TRY(plan.bytes(px_bound, cap));
     std::vector<uint8_t> bytes(cap);
     uint64_t nout = 0;
     APT_TRY(apt_decode_png(pcm16 ? static_cast<const void *>(pcm.data()) : static_cast<const void *>(x.data()),
@@ -1313,8 +1277,9 @@ extern "C" int apt_telemetry_rows(const float *signal, uint64_t n, float *mean_a
 
 extern "C" int apt_process(const float *rows, uint64_t n, const apt_process_settings *ps, uint8_t *out, uint64_t cap,
                            uint64_t *nout, apt_image_info *info) {
-    PostPlan plan;
-    APT_TRY(process_plan(ps, plan));
+    OutPlan op;
+    APT_TRY(image_plan(ps, nullptr, false, op));
+    const PostPlan &plan = op.post;
     if (!nout) return fail(APT_ERR_BAD_ARG, "null argument");
     *nout = 0;
     if (!rows || n == 0) return fail(APT_ERR_BAD_ARG, "empty signal");   // get_min of an empty vector is an error, dsp.rs:21-25
@@ -1451,18 +1416,16 @@ namespace {
 // PngFeed.
 struct BatchImage {
     const apt_process_settings *ps;
-    int bpp;
-    const apt_png_settings *png;   // nullptr: the images go to the caller
+    OutPlan plan;                  // plan.png false: the images go to the caller
     std::vector<apt_image_info> *infos;
 };
 
-// One feeder's PNG side.  The decoders keep their images on the device (keep_image); at reap the image is copied into a
+// One feeder's PNG side.  The decoders keep their images on the device (img.keep); at reap the image is copied into a
 // free slot of a fixed pool, so the decoder takes its next recording at once.  When the encoder is idle, every ready
 // slot forms one group, encoded on the feeder's own stream after the events of the copies; the feeder reads the
 // lengths back once the encode's event has fired and copies each file to its caller.
 struct PngFeed {
-    int bpp = 1;
-    apt_png_settings png{};
+    ImageOut out;                    // plan: the batch's; work and h_ctl: the encode in flight
     u64 slot_bytes = 0;
     unsigned char *pool = nullptr;
     std::vector<int> job;            // per slot: the recording, -1 free
@@ -1473,9 +1436,6 @@ struct PngFeed {
     cudaStream_t stream = nullptr;
     cudaEvent_t done = nullptr;
     int sms = 1;
-    PngWork w;
-    PngCtl *h_ctl = nullptr;
-    size_t h_ctl_cap = 0;
     size_t max_group = SIZE_MAX;     // the largest group whose workspace could be allocated
 
     // `slots` slots of `bytes` each; fewer when the device is short of memory, at least one
@@ -1499,12 +1459,11 @@ struct PngFeed {
     }
     ~PngFeed() {
         if (stream) cudaStreamSynchronize(stream);
-        w.release();
+        out.release();
         if (pool) cudaFree(pool);
         for (auto e : ready)
             if (e) cudaEventDestroy(e);
         if (done) cudaEventDestroy(done);
-        if (h_ctl) cudaFreeHost(h_ctl);
         if (stream) cudaStreamDestroy(stream);
     }
     int free_slot() const {
@@ -1519,15 +1478,15 @@ struct PngFeed {
             if (job[k] >= 0 && !encoding[k]) return true;
         return false;
     }
-    // the image of decoder d's finished job (in d_out8) into a free slot, on the decoder's stream
+    // the image of decoder d's finished job (in its img.px) into a free slot, on the decoder's stream
     int put(apt_decoder *d, int jb, u64 bytes) {
         const int k = free_slot();
         if (k < 0) return fail(APT_ERR_CUDA, "no free slot in the PNG image pool");
         if (bytes > slot_bytes) return fail(APT_ERR_CUDA, "image of %llu bytes exceeds the pool's slots", (unsigned long long)bytes);
-        APT_CUDA(cudaMemcpyAsync(pool + k * slot_bytes, d->d_out8, bytes, cudaMemcpyDeviceToDevice, d->stream));
+        APT_CUDA(cudaMemcpyAsync(pool + k * slot_bytes, d->img.px, bytes, cudaMemcpyDeviceToDevice, d->stream));
         APT_CUDA(cudaEventRecord(ready[k], d->stream));
         job[k] = jb;
-        rows[k] = static_cast<u32>(bytes / (static_cast<u64>(kPxPerRow) * bpp));
+        rows[k] = static_cast<u32>(bytes / (static_cast<u64>(kPxPerRow) * out.plan.post.bpp));
         return APT_OK;
     }
     // one encode over every ready slot, at most max_group of them
@@ -1537,7 +1496,7 @@ struct PngFeed {
         for (size_t k = 0; k < job.size(); ++k) {
             if (job[k] < 0 || encoding[k]) continue;
             PngPlan p;
-            const int st = make_png(kPxPerRow, rows[k], bpp, &png, p);
+            const int st = out.plan.png_plan(rows[k], p);
             if (st != APT_OK) {
                 status[job[k]] = st;
                 job[k] = -1;
@@ -1563,10 +1522,10 @@ struct PngFeed {
         for (;;) {
             PngLayout lay;
             int st = png_layout(plans.data(), px.data(), static_cast<u32>(g), lay);
-            if (st == APT_OK) st = w.reserve(lay);
+            if (st == APT_OK) st = out.work.reserve(lay);
             if (st == APT_OK) break;
             cudaGetLastError();
-            w.release();
+            out.work.release();
             if (g == 1) {   // not even one image fits: that recording fails, the rest wait for the next launch
                 status[job[slots[0]]] = st;
                 job[slots[0]] = -1;
@@ -1575,19 +1534,9 @@ struct PngFeed {
             g /= 2;         // a smaller group: the rest stay ready for the next launch
             max_group = g;
         }
-        int st = png_encode_device(LaunchCtx{stream, sms}, plans.data(), px.data(), static_cast<u32>(g), w, nullptr);
-        if (st == APT_OK && h_ctl_cap < g) {
-            if (h_ctl) cudaFreeHost(h_ctl);
-            h_ctl = nullptr;
-            h_ctl_cap = 0;
-            st = cudaHostAlloc(reinterpret_cast<void **>(&h_ctl), g * sizeof(PngCtl), cudaHostAllocDefault) == cudaSuccess
-                     ? APT_OK : fail(APT_ERR_CUDA, "out of pinned host memory");
-            if (st == APT_OK) h_ctl_cap = g;
-        }
-        if (st == APT_OK)
-            st = cudaMemcpyAsync(h_ctl, w.ctl, g * sizeof(PngCtl), cudaMemcpyDeviceToHost, stream) == cudaSuccess &&
-                         cudaEventRecord(done, stream) == cudaSuccess
-                     ? APT_OK : fail(APT_ERR_CUDA, "CUDA error: %s", cudaGetErrorString(cudaGetLastError()));
+        int st = out.encode(LaunchCtx{stream, sms}, plans.data(), px.data(), static_cast<u32>(g), nullptr);
+        if (st == APT_OK && cudaEventRecord(done, stream) != cudaSuccess)
+            st = fail(APT_ERR_CUDA, "CUDA error: %s", cudaGetErrorString(cudaGetLastError()));
         if (st != APT_OK) {   // the encode itself failed: its recordings have that status
             cudaStreamSynchronize(stream);
             for (size_t i = 0; i < g; ++i) {
@@ -1608,14 +1557,8 @@ struct PngFeed {
                 status[jb] = fail(APT_ERR_CUDA, "CUDA error: %s", cudaGetErrorString(e));
                 continue;
             }
-            const uint64_t total = h_ctl[i].total;
-            nouts[jb] = total;
-            if (total > caps[jb]) {
-                status[jb] = fail(APT_ERR_CAPACITY, "output needs room for %llu PNG bytes", (unsigned long long)total);
-                continue;
-            }
-            e = cudaMemcpyAsync(outs[jb], w.out + w.lay.img[i].out, total, cudaMemcpyDeviceToHost, stream);
-            status[jb] = e == cudaSuccess ? APT_OK : fail(APT_ERR_CUDA, "CUDA error: %s", cudaGetErrorString(e));
+            nouts[jb] = out.length(static_cast<u32>(i));
+            status[jb] = out.copy_out(static_cast<u32>(i), outs[jb], caps[jb], cudaMemcpyDeviceToHost, stream);
         }
         const cudaError_t es = cudaStreamSynchronize(stream);
         for (size_t i = 0; i < group.size(); ++i) {
@@ -1635,7 +1578,7 @@ constexpr int kPngPoolSlots = 16;
 
 // One feeder thread per device: binds itself to the device's NUMA node, owns `streams_per_device` decoders and one copy
 // stager, keeps every decoder busy and reaps the jobs in the order they complete.  Nothing is shared between devices.
-// img == nullptr: f32 rows (apt_decode_batch); else process mode, and with img->png the feeder's PngFeed.
+// img == nullptr: f32 rows (apt_decode_batch); else process mode, and with img->plan.png the feeder's PngFeed.
 int run_batch(const void *const *signals, int format, const uint64_t *lens, int count, uint32_t input_rate, const apt_settings *s,
               int sync, const BatchImage *img, void *const *outs, const uint64_t *caps, uint64_t *nouts, int *statuses,
               const int *devices, int ndevices, int streams_per_device) {
@@ -1670,7 +1613,7 @@ int run_batch(const void *const *signals, int format, const uint64_t *lens, int 
             uint64_t got = 0;
             int st = apt_decoder_wait(decs[k], &got);
             const int job = job_of[k];
-            if (img && st == APT_OK) (*img->infos)[job] = decs[k]->last_image;
+            if (img && st == APT_OK) (*img->infos)[job] = decs[k]->img.info;
             if (feed && st == APT_OK) {
                 st = feed->put(decs[k], job, got);
                 got = 0;                               // the file's length comes with its encode
@@ -1686,16 +1629,15 @@ int run_batch(const void *const *signals, int format, const uint64_t *lens, int 
             messages[g] = apt_last_error();
             for (; next < count; next += ndevices) local_status[next] = st;
         };
-        if (img && img->png && next < count) {
+        if (img && img->plan.png && next < count) {
             Plan p;
             uint64_t bound = 0;
             int st = make_plan(input_rate, *s, p);
             if (st == APT_OK) st = cudaSetDevice(device) == cudaSuccess ? APT_OK : fail(APT_ERR_CUDA, "cannot select device %d", device);
             if (st == APT_OK) {
-                bound = std::max<uint64_t>(plan_out_bound(p, max_len), kPxPerRow) * img->bpp;
+                bound = img->plan.px_bytes(std::max<uint64_t>(plan_out_bound(p, max_len), kPxPerRow));
                 feed.reset(new PngFeed());
-                feed->bpp = img->bpp;
-                feed->png = *img->png;
+                feed->out.plan = img->plan;
                 st = feed->init(device, std::min(kPngPoolSlots, (count - g + ndevices - 1) / ndevices), bound);
             }
             if (st != APT_OK) {
@@ -1732,7 +1674,7 @@ int run_batch(const void *const *signals, int format, const uint64_t *lens, int 
                     // one stager (ring + copy threads) serves all decoders of this feeder: the first decoder's own
                     if (decs.empty()) ensure_stager(d);
                     else d->stager = decs[0]->stager;
-                    d->keep_image = feed != nullptr;
+                    d->img.keep = feed != nullptr;
                     decs.push_back(d);
                     job_of.push_back(-1);
                 }
@@ -1803,9 +1745,8 @@ extern "C" int apt_decode_batch_image(const void *const *signals, int format, co
                                       apt_image_info *infos, int *statuses, const int *devices, int ndevices,
                                       int streams_per_device) {
     if (!signals || !lens || !s || !outs || !caps || !nouts || count < 0) return fail(APT_ERR_BAD_ARG, "null argument");
-    PostPlan plan;
-    APT_TRY(process_plan(ps, plan));
-    if (png) APT_TRY(check_png_settings(png, plan.bpp));
+    OutPlan plan;
+    APT_TRY(image_plan(ps, png, false, plan));
     {
         Plan p;
         APT_TRY(make_plan(input_rate, *s, p));
@@ -1820,7 +1761,7 @@ extern "C" int apt_decode_batch_image(const void *const *signals, int format, co
     if (count == 0) return APT_OK;
     std::vector<apt_image_info> got(count);
     std::vector<int> st(count, APT_ERR_CUDA);
-    const BatchImage bi{ps, plan.bpp, png, &got};
+    const BatchImage bi{ps, plan, &got};
     const int rc = run_batch(signals, format, lens, count, input_rate, s, sync, &bi, reinterpret_cast<void *const *>(outs), caps,
                              nouts, st.data(), devices, ndevices, streams_per_device);
     for (int i = 0; i < count; ++i) {

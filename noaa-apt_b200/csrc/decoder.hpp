@@ -10,7 +10,6 @@
 
 #include "aptb200.h"
 #include <memory>
-#include <optional>
 
 #include "back.hpp"
 #include "filters_host.hpp"
@@ -58,7 +57,7 @@ int ensure_conv(apt_decoder *d, uint64_t need, uint64_t alloc);
 // The decoders the convenience entry points park between calls (APTB200_NO_CACHE: none are parked).  take_decoder hands
 // out a parked decoder for (device, rate, settings) of at least n samples, else creates one of n samples, with head-room
 // for a slightly longer next recording when `headroom` and the cache is on.  park_decoder drains the decoder's stream, clears the state of
-// the call (image, process and PNG mode, keep_image, the status callback, a borrowed stager) and parks the decoder
+// the call (image, process and PNG mode, img.keep, the status callback, a borrowed stager) and parks the decoder
 // under its own key, or destroys it.  `several`: keep it beside others of its key (a batch's decoders), else it
 // replaces a smaller one of the same key.
 int take_decoder(int device, uint32_t rate, const apt_settings &st, uint64_t n, bool headroom, apt_decoder **d);
@@ -115,22 +114,9 @@ struct apt_decoder {
     uint64_t job_d2h_floats = 0;   // rows copied back by the job (an upper bound when syncing: n_rows is not known yet)
     aptb200::SyncResult *h_res = nullptr;   // pinned
 
-    // image / process mode (post.hpp): the job's output is the image of the plan; no plan: f32 rows
-    std::optional<aptb200::PostPlan> post_plan;
-    aptb200::PostBuffers post;
-    unsigned char *d_out8 = nullptr;
-    uint64_t out8_bytes = 0;       // size of d_out8 (max_out, or 4 * max_out once an RGBA process job ran)
-    apt_image_info last_image{};
-    // PNG mode (apt_decoder_set_png_mode): the image of an image / process job is encoded on the device at wait(); only the
-    // PNG bytes are copied out.  The workspaces are sized at first use from the image size.
-    bool png_active = false;
-    apt_png_settings png{};
-    aptb200::PngWork png_work;
-    aptb200::PngCtl *h_png = nullptr;   // pinned copy of the encoder's control block
-    bool job_png = false;
-    // image left on the device: a host job of image / process mode keeps its image in d_out8 and copies nothing back
-    // (the batch's PNG feeder takes it from there); out and cap are not used
-    bool keep_image = false;
+    // image / process mode and PNG mode (png.hpp): img.plan.image, the job's output is the image of the plan, else f32
+    // rows.  The pixels grow on first use; in PNG mode the image is encoded at wait() and only the file is copied out.
+    aptb200::ImageOut img;
 
     // apt_decode_iq (allocated on first use): the I/Q stage's tables for iq_settings, one chunk's I/Q window and the
     // audio the FM kernel writes, which is the input of the decode job

@@ -291,17 +291,8 @@ extern "C" int apt_recording_decode(apt_recording *rec, const apt_pass *ranges, 
         if (infos) memset(&infos[i], 0, sizeof(infos[i]));
     }
     // every argument error before any device work: the settings rules of apt_process / apt_png_encode, then the ranges
-    PostPlan post;
-    if (ps) {
-        const int st = make_post(*ps, post);
-        if (st != APT_OK) return fail_all(st);
-    }
-    if (png) {
-        if (!ps) return fail_all(fail(APT_ERR_BAD_ARG, "PNG output needs process settings"));
-        PngPlan pp;
-        const int st = make_png(kPxPerRow, 1, post.bpp, png, pp);
-        if (st != APT_OK) return fail_all(st);
-    }
+    OutPlan op;
+    if (const int st = make_out_plan(ps, png, op); st != APT_OK) return fail_all(st);
     const Plan &p = rec->plan;
     const size_t sb = sample_bytes(rec->format);
     uint64_t max_len = 0, max_out = 0;
@@ -313,13 +304,8 @@ extern "C" int apt_recording_decode(apt_recording *rec, const apt_pass *ranges, 
         if (!outs[i]) return fail_all(fail(APT_ERR_BAD_ARG, "null output %u", i));
         const uint64_t len = b - a;
         const uint64_t need = sync ? (p.front.work_len(len) / p.row) * kPxPerRow : plan_out_bound(p, len);
-        uint64_t bytes = ps ? need * post.bpp : need * sizeof(float);
-        if (png) {
-            PngPlan pp;
-            const int st = make_png(kPxPerRow, static_cast<uint32_t>(std::max<uint64_t>(need / kPxPerRow, 1)), post.bpp, png, pp);
-            if (st != APT_OK) return fail_all(st);
-            bytes = pp.bound;
-        }
+        uint64_t bytes = 0;
+        if (const int st = op.bytes(need, bytes); st != APT_OK) return fail_all(st);
         max_len = std::max(max_len, len);
         max_out = std::max(max_out, bytes);
     }
@@ -361,7 +347,7 @@ extern "C" int apt_recording_decode(apt_recording *rec, const apt_pass *ranges, 
         if (st == APT_OK || (st == APT_ERR_CAPACITY && png)) nouts[i] = got;
         if (st == APT_OK && cudaMemcpy(outs[i], dout, got * elem, cudaMemcpyDeviceToHost) != cudaSuccess)
             st = fail(APT_ERR_CUDA, "copying the output of range %u failed", i);
-        if (st == APT_OK && infos && ps) infos[i] = d->last_image;
+        if (st == APT_OK && infos && ps) infos[i] = d->img.info;
         statuses[i] = st;
     }
     release();

@@ -6,6 +6,7 @@
 #include <mutex>
 
 #include "common.hpp"
+#include "decoder.hpp"
 #include "kernels_png.cuh"
 
 namespace aptb200 {
@@ -332,32 +333,120 @@ int png_encode_device(const LaunchCtx &c, const PngPlan *plans, const unsigned c
     return APT_OK;
 }
 
+int OutPlan::set_png(const apt_png_settings *ps) {
+    if (ps) {
+        PngPlan pp;
+        APT_TRY(make_png(kPxPerRow, 1, post.bpp, ps, pp));
+        png_s = *ps;
+    }
+    png = ps != nullptr;
+    return APT_OK;
+}
+
+int OutPlan::png_plan(uint64_t rows, PngPlan &pp) const {
+    if (rows > 0xFFFFFFFFull) return fail(APT_ERR_BAD_ARG, "recording too long");
+    return make_png(kPxPerRow, static_cast<uint32_t>(rows), post.bpp, &png_s, pp);
+}
+
+int OutPlan::bytes(uint64_t px, uint64_t &b) const {
+    b = px_bytes(px);
+    if (!png) return APT_OK;
+    PngPlan pp;
+    APT_TRY(png_plan(std::max<uint64_t>(px / kPxPerRow, 1), pp));
+    b = pp.bound;
+    return APT_OK;
+}
+
+int make_out_plan(const apt_process_settings *ps, const apt_png_settings *png, OutPlan &plan) {
+    plan = OutPlan{};
+    if (ps) {
+        APT_TRY(make_post(*ps, plan.post));
+        plan.image = true;
+    }
+    if (png && !ps) return fail(APT_ERR_BAD_ARG, "PNG output needs process settings");
+    return plan.set_png(png);
+}
+
+int check_room(const void *dst, uint64_t need, uint64_t cap) {
+    if (!dst || cap < need) return fail(APT_ERR_CAPACITY, "output needs room for %llu bytes", (unsigned long long)need);
+    return APT_OK;
+}
+
+int ImageOut::reserve_px(uint64_t bytes) { return grow(px, px_cap, bytes, 1); }
+
+int ImageOut::reserve_ctl(uint32_t g) {
+    if (ctl_cap >= g) return APT_OK;
+    if (h_ctl) cudaFreeHost(h_ctl);
+    h_ctl = nullptr;
+    ctl_cap = 0;
+    APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&h_ctl), g * sizeof(PngCtl), cudaHostAllocDefault));
+    ctl_cap = g;
+    return APT_OK;
+}
+
+int ImageOut::launch(const LaunchCtx &c, const float *rows, const SyncResult *res, u32 fixed_rows, u32 max_rows, void *out,
+                     KernelHook *hook) {
+    return post_launch(c, plan.post, post, rows, res, fixed_rows, max_rows, kPxPerRow, nullptr, out ? out : px, hook);
+}
+
+int ImageOut::encode(const LaunchCtx &c, const PngPlan *plans, const unsigned char *const *pixels, u32 g, KernelHook *hook) {
+    APT_TRY(reserve_ctl(g));
+    APT_TRY(png_encode_device(c, plans, pixels, g, work, hook));
+    APT_CUDA(cudaMemcpyAsync(h_ctl, work.ctl, g * sizeof(PngCtl), cudaMemcpyDeviceToHost, c.stream));
+    return APT_OK;
+}
+
+int ImageOut::encode_px(const LaunchCtx &c, uint64_t rows, KernelHook *hook) {
+    PngPlan pp;
+    APT_TRY(plan.png_plan(rows, pp));
+    const unsigned char *p = px;
+    return encode(c, &pp, &p, 1, hook);
+}
+
+int ImageOut::copy_out(u32 k, void *dst, uint64_t cap, cudaMemcpyKind kind, cudaStream_t s) const {
+    const uint64_t n = length(k);
+    APT_TRY(check_room(dst, n, cap));
+    APT_CUDA(cudaMemcpyAsync(dst, work.out + work.lay.img[k].out, n, kind, s));
+    return APT_OK;
+}
+
+uint64_t ImageOut::device_bytes(const OutPlan &p, uint64_t max_rows) {
+    const PostPlan &q = p.post;
+    uint64_t b = sizeof(PostCtl) + 3 * max_rows * sizeof(float) + (q.hist ? sizeof(ProcCtl) : 0) +
+                 (q.finish ? max_rows * kPxPerRow : 0) + (q.palette ? 256 * 256 * sizeof(u32) : 0) + max_rows * kPxPerRow * q.bpp;
+    PngPlan pp;
+    PngLayout lay;
+    if (p.png && p.png_plan(max_rows, pp) == APT_OK && png_layout(&pp, nullptr, 1, lay) == APT_OK) b += PngWork::bytes_for(lay);
+    return b;
+}
+
+void ImageOut::release() {
+    post.release();
+    work.release();
+    if (px) cudaFree(px);
+    if (h_ctl) cudaFreeHost(h_ctl);
+    px = nullptr;
+    h_ctl = nullptr;
+    px_cap = 0;
+    ctl_cap = 0;
+}
+
 }  // namespace aptb200
 
 using namespace aptb200;
 
 namespace {
 
-// apt_png_encode keeps one workspace per device (input pixels, encoder buffers, a stream, the pinned control block) for
+// apt_png_encode keeps one workspace per device (input pixels, encoder buffers, the pinned control blocks, a stream) for
 // the next call, as the one-shot decode keeps its decoders; apt_cache_clear frees them.
 constexpr int kStageDevices = 64;
 struct PngStage {
     std::mutex mu;
-    PngWork w;
-    unsigned char *px = nullptr;
-    u64 px_cap = 0;
+    ImageOut out;                    // px: the input pixels
     cudaStream_t stream = nullptr;
-    PngCtl *h_ctl = nullptr;
-    u64 h_ctl_cap = 0;
     void release() {
         if (stream) cudaStreamSynchronize(stream);
-        w.release();
-        if (px) cudaFree(px);
-        px = nullptr;
-        px_cap = 0;
-        if (h_ctl) cudaFreeHost(h_ctl);
-        h_ctl = nullptr;
-        h_ctl_cap = 0;
+        out.release();
         if (stream) cudaStreamDestroy(stream);
         stream = nullptr;
     }
@@ -455,33 +544,21 @@ extern "C" int apt_png_encode_batch(const uint8_t *const *pixels, const uint32_t
     std::lock_guard<std::mutex> lk(sg.mu);   // one encode per device at a time: they share the workspace
     auto run = [&]() -> int {
         if (!sg.stream) APT_CUDA(cudaStreamCreateWithFlags(&sg.stream, cudaStreamNonBlocking));
-        if (sg.h_ctl_cap < count) {
-            if (sg.h_ctl) cudaFreeHost(sg.h_ctl);
-            sg.h_ctl = nullptr;
-            sg.h_ctl_cap = 0;
-            APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&sg.h_ctl), count * sizeof(PngCtl), cudaHostAllocDefault));
-            sg.h_ctl_cap = count;
-        }
-        APT_TRY(grow(sg.px, sg.px_cap, in_off[count], 1));
+        APT_TRY(sg.out.reserve_px(in_off[count]));
         std::vector<const unsigned char *> px(count);
         for (uint32_t k = 0; k < count; ++k) {
-            px[k] = sg.px + in_off[k];
-            APT_CUDA(cudaMemcpyAsync(sg.px + in_off[k], pixels[k], static_cast<u64>(width) * heights[k] * channels,
+            px[k] = sg.out.px + in_off[k];
+            APT_CUDA(cudaMemcpyAsync(sg.out.px + in_off[k], pixels[k], static_cast<u64>(width) * heights[k] * channels,
                                      cudaMemcpyHostToDevice, sg.stream));
         }
-        APT_TRY(png_encode_device(LaunchCtx{sg.stream, std::max(sms, 1)}, plans.data(), px.data(), count, sg.w, nullptr));
-        APT_CUDA(cudaMemcpyAsync(sg.h_ctl, sg.w.ctl, count * sizeof(PngCtl), cudaMemcpyDeviceToHost, sg.stream));
+        APT_TRY(sg.out.encode(LaunchCtx{sg.stream, std::max(sms, 1)}, plans.data(), px.data(), count, nullptr));
         APT_CUDA(cudaStreamSynchronize(sg.stream));
         int first = APT_OK;
         for (uint32_t k = 0; k < count; ++k) {
-            const u64 total = sg.h_ctl[k].total;
-            nouts[k] = total;
-            if (total > caps[k]) {
-                const int st = fail(APT_ERR_CAPACITY, "output needs room for %llu bytes", (unsigned long long)total);
-                if (first == APT_OK) first = st;
-                continue;
-            }
-            APT_CUDA(cudaMemcpyAsync(outs[k], sg.w.out + sg.w.lay.img[k].out, total, cudaMemcpyDeviceToHost, sg.stream));
+            nouts[k] = sg.out.length(k);
+            const int st = sg.out.copy_out(k, outs[k], caps[k], cudaMemcpyDeviceToHost, sg.stream);
+            if (st == APT_ERR_CAPACITY && first == APT_OK) first = st;
+            else if (st != APT_OK && st != APT_ERR_CAPACITY) return st;
         }
         APT_CUDA(cudaStreamSynchronize(sg.stream));
         return first;

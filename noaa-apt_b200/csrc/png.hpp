@@ -1,6 +1,7 @@
 // The PNG encoder (DESIGN.md §11): filter, match candidates, greedy parse, package-merge Huffman codes, bit emission,
 // Adler-32, CRC-32 and the PNG framing, all on the device.  This module alone reads apt_png_settings: it validates them,
-// sizes the workspaces, launches the kernel sequence and leaves the file's bytes and length on the device.
+// sizes the workspaces, launches the kernel sequence and leaves the file's bytes and length on the device.  It also owns
+// image output (OutPlan, ImageOut): the output rules and sizes, the pixels, the encode, the length read-back and the copy-out.
 #pragma once
 
 #include <cstdint>
@@ -8,6 +9,7 @@
 
 #include "aptb200.h"
 #include "launch.hpp"
+#include "post.hpp"
 
 namespace aptb200 {
 
@@ -98,6 +100,63 @@ struct PngWork {
 // it starts the next one on the same workspace.
 int png_encode_device(const LaunchCtx &c, const PngPlan *plans, const unsigned char *const *pixels, u32 g, PngWork &w,
                       KernelHook *hook);
+
+// What becomes of a decoded signal (DESIGN.md §9, "Image output"): f32 rows, the image of `post`, or that image as a PNG
+// file.  Host only.
+struct OutPlan {
+    bool image = false;           // the image of `post`; false: f32 rows
+    PostPlan post;
+    bool png = false;             // the image as a PNG file of png_s
+    apt_png_settings png_s{};
+    // PNG output of the image (the settings rules for a one-row image of post.bpp channels); png == nullptr: none.
+    int set_png(const apt_png_settings *png);
+    // The encoder's plan for an image of `rows` rows.
+    int png_plan(uint64_t rows, PngPlan &pp) const;
+    // Bytes of `px` pixels: px f32 values, or px * bpp bytes of the image.
+    uint64_t px_bytes(uint64_t px) const { return px * (image ? post.bpp : sizeof(float)); }
+    // Bytes of the output of `px` pixels: px_bytes, or the PNG bound of max(px / 2080, 1) rows.
+    int bytes(uint64_t px, uint64_t &bytes) const;
+};
+
+// The output rules, host only: the process settings (ps == nullptr: f32 rows), then PNG settings (png == nullptr: none),
+// which need process settings.
+int make_out_plan(const apt_process_settings *ps, const apt_png_settings *png, OutPlan &plan);
+
+// Where an image lives after the image stage and how it reaches the caller: the stage's buffers, the pixels, the encoder's
+// workspace and the pinned copies of its control blocks.  Decoders, streams, the batch's PNG feeder and apt_png_encode_batch
+// each own one; it runs on the caller's CUDA stream.
+struct ImageOut {
+    OutPlan plan;
+    PostBuffers post;
+    unsigned char *px = nullptr;  // the image (or apt_png_encode_batch's input pixels), px_cap bytes
+    u64 px_cap = 0;
+    PngWork work;
+    PngCtl *h_ctl = nullptr;      // pinned: the control blocks of the last encode, ctl_cap of them
+    uint32_t ctl_cap = 0;
+    apt_image_info info{};        // the decoder's last image
+    bool keep = false;            // the decoder's image stays in px: nothing is copied to the caller (the batch's PNG feeder)
+
+    ~ImageOut() { release(); }
+    int reserve_px(uint64_t bytes);      // px of at least `bytes` (grown, never shrunk)
+    int reserve_ctl(uint32_t g);         // h_ctl for g encodes
+    // The image stage on rows (device) into out, or px when out is nullptr (post_launch with rows of 2080 pixels).
+    int launch(const LaunchCtx &c, const float *rows, const SyncResult *res, u32 fixed_rows, u32 max_rows, void *out,
+               KernelHook *hook);
+    // Encodes g images (as png_encode_device takes them) and reads their control blocks back, both on c.stream; length(k)
+    // is valid once the caller has synchronised with that stream.
+    int encode(const LaunchCtx &c, const PngPlan *plans, const unsigned char *const *pixels, u32 g, KernelHook *hook);
+    // encode() of the image of `rows` rows in px.
+    int encode_px(const LaunchCtx &c, uint64_t rows, KernelHook *hook);
+    uint64_t length(u32 k) const { return h_ctl[k].total; }
+    // Enqueues the copy of file k to dst, or returns APT_ERR_CAPACITY with its length when dst is null or cap too small.
+    int copy_out(u32 k, void *dst, uint64_t cap, cudaMemcpyKind kind, cudaStream_t s) const;
+    // Device bytes of post, px and work for images of up to max_rows rows of `plan` (host only).
+    static uint64_t device_bytes(const OutPlan &plan, uint64_t max_rows);
+    void release();
+};
+
+// APT_ERR_CAPACITY with the message every output path gives when dst is null or cap is below need.
+int check_room(const void *dst, uint64_t need, uint64_t cap);
 
 // Frees the per-device workspaces apt_png_encode keeps between calls (apt_cache_clear).
 void png_stage_cache_clear();

@@ -80,43 +80,6 @@ Geom make_geom(const Plan &p, int sync, uint64_t max_push) {
     return g;
 }
 
-// Image output of a stream: the rows of the pass (f32, up to max_rows) and everything the image stage and the encoder need,
-// allocated when the mode is set so that push and finish allocate nothing.
-struct ImageOut {
-    PostPlan plan;
-    uint64_t max_rows = 0;
-    PostBuffers post;
-    float *d_rows = nullptr;          // max_rows * 2080 f32: row r of the pass at r * 2080
-    unsigned char *d_px = nullptr;    // max_rows * 2080 * bpp: the image
-    PngCtl *h_png = nullptr;          // pinned copy of the encoder's control block
-    uint64_t bytes = 0;               // device bytes of the above
-    bool png = false;                 // PNG output (apt_stream_set_png_mode)
-    apt_png_settings png_settings{};
-    PngWork png_work;                 // reserved for a max_rows image
-
-    // The stage's and the image's device memory (PostBuffers::alloc and upload_palette for max_rows rows).
-    static uint64_t post_bytes(const PostPlan &plan, uint64_t max_rows) {
-        return sizeof(PostCtl) + 3 * max_rows * sizeof(float) + (plan.hist ? sizeof(ProcCtl) : 0) +
-               (plan.finish ? max_rows * kPxPerRow : 0) + (plan.palette ? 256 * 256 * sizeof(u32) : 0) +
-               max_rows * kPxPerRow * (sizeof(float) + plan.bpp);
-    }
-    void release_png() {
-        png_work.release();
-        png = false;
-    }
-    void release() {
-        release_png();
-        post.release();
-        if (d_rows) cudaFree(d_rows);
-        if (d_px) cudaFree(d_px);
-        if (h_png) cudaFreeHost(h_png);
-        d_rows = nullptr;
-        d_px = nullptr;
-        h_png = nullptr;
-        max_rows = bytes = 0;
-    }
-};
-
 }  // namespace
 
 struct apt_stream {
@@ -151,10 +114,22 @@ struct apt_stream {
     void *d_iqraw = nullptr;        // one step's pushed samples as they came
     uint64_t iq_cap = 0, iq_in = 0, iq_base = 0;
 
-    ImageOut img;                   // image output: on when img.d_rows is set
+    // image output (apt_stream_set_process_mode), on when img_rows is set: the rows of the pass (f32, up to img_max_rows, row
+    // r at r * 2080) and what becomes of them, allocated when the mode is set so that push and finish allocate nothing
+    float *img_rows = nullptr;
+    uint64_t img_max_rows = 0;
+    ImageOut img;
 };
 
 namespace {
+
+void release_image(apt_stream *st) {
+    st->img.release();
+    st->img.plan = OutPlan{};
+    if (st->img_rows) cudaFree(st->img_rows);
+    st->img_rows = nullptr;
+    st->img_max_rows = 0;
+}
 
 void free_stream(apt_stream *st) {
     cudaSetDevice(st->dec.device);
@@ -167,7 +142,7 @@ void free_stream(apt_stream *st) {
     if (st->d_iq) cudaFree(st->d_iq);
     if (st->d_iqraw) cudaFree(st->d_iqraw);
     st->iqt.release();
-    st->img.release();
+    release_image(st);
     free_decoder_buffers(&st->dec);
 }
 
@@ -233,9 +208,9 @@ void take_rows(apt_stream *st, uint64_t rel_hi, float *rows, uint64_t &nout) {
 // Image output: rows [first, end) of the pass, at `src` on the device, into the image buffer.  Rows past max_rows are left
 // out; finish_image then refuses the image (the pass has more rows than the buffer).
 int keep_rows(apt_stream *st, uint64_t first, uint64_t end, const float *src) {
-    end = std::min(end, st->img.max_rows);
+    end = std::min(end, st->img_max_rows);
     if (first >= end) return APT_OK;
-    APT_CUDA(cudaMemcpyAsync(st->img.d_rows + first * kPxPerRow, src, (end - first) * kPxPerRow * sizeof(float),
+    APT_CUDA(cudaMemcpyAsync(st->img_rows + first * kPxPerRow, src, (end - first) * kPxPerRow * sizeof(float),
                              cudaMemcpyDeviceToDevice, st->dec.stream));
     return APT_OK;
 }
@@ -307,7 +282,7 @@ int step(apt_stream *st, const void *src, bool on_device, int format, uint64_t n
             const uint64_t cnt = std::min<uint64_t>(r_hi - st->rows_out, g.gather_cap);
             APT_TRY(launch_gather_lp(c, e, st->work_final, nullptr, nullptr, static_cast<u32>(cnt), static_cast<u32>(cnt), p.row, kPxPerRow,
                                      p.dec, p.lp.data(), ntaps, st->d_rows, static_cast<u32>(st->rows_out)));
-            if (st->img.d_rows) APT_TRY(keep_rows(st, st->rows_out, st->rows_out + cnt, st->d_rows));
+            if (st->img_rows) APT_TRY(keep_rows(st, st->rows_out, st->rows_out + cnt, st->d_rows));
             APT_CUDA(cudaMemcpyAsync(st->h_rows, st->d_rows, cnt * kPxPerRow * sizeof(float), cudaMemcpyDeviceToHost, d.stream));
             APT_CUDA(cudaStreamSynchronize(d.stream));
             st->gathered = st->rows_out + cnt;
@@ -366,7 +341,7 @@ int step(apt_stream *st, const void *src, bool on_device, int format, uint64_t n
             st->positions.insert(st->positions.end(), st->run_cnt()[st->runs_seen % kRunRing], st->run_pos()[st->runs_seen % kRunRing]);
         if (st->positions.size() != cy.len) return fail(APT_ERR_BAD_ARG, "internal: peak runs and peak count disagree");
         // the round's new rows sit behind the held ones; the copy runs on the stream ahead of the next round's gather
-        if (st->img.d_rows) APT_TRY(keep_rows(st, st->gathered, cy.gathered, st->d_rows + held * kPxPerRow));
+        if (st->img_rows) APT_TRY(keep_rows(st, st->gathered, cy.gathered, st->d_rows + held * kPxPerRow));
         st->gathered = cy.gathered;
         // released: rows whose next peak exists; a failed decode (fewer than 5 peaks at the end) releases nothing more
         const bool failed = finish && cy.len < 5;
@@ -596,38 +571,29 @@ bool pushed(const apt_stream *st) { return st->samples_in || st->iq_in || st->fi
 int finish_image(apt_stream *st, uint8_t *image, uint64_t cap, uint64_t *image_n, apt_image_info *info) {
     ImageOut &o = st->img;
     const uint64_t rows = st->rows_out;
-    if (rows > o.max_rows) {
+    if (rows > st->img_max_rows) {
         if (info) {
             *info = apt_image_info{};
             info->rows = rows;
         }
         return fail(APT_ERR_CAPACITY, "the pass has %llu rows, more than the image output's max_rows %llu", (unsigned long long)rows,
-                    (unsigned long long)o.max_rows);
+                    (unsigned long long)st->img_max_rows);
     }
     apt_decoder &d = st->dec;
     const LaunchCtx c{d.stream, d.sm_count};
-    APT_TRY(post_launch(c, o.plan, o.post, o.d_rows, nullptr, static_cast<u32>(rows), static_cast<u32>(o.max_rows), kPxPerRow,
-                        nullptr, o.d_px, nullptr));
-    const uint64_t px_bytes = rows * kPxPerRow * o.plan.bpp;
-    if (o.png) {
-        PngPlan pp;
-        APT_TRY(make_png(kPxPerRow, static_cast<uint32_t>(rows), o.plan.bpp, &o.png_settings, pp));
-        const unsigned char *px = o.d_px;
-        APT_TRY(png_encode_device(c, &pp, &px, 1, o.png_work, nullptr));
-        APT_CUDA(cudaMemcpyAsync(o.h_png, o.png_work.ctl, sizeof(PngCtl), cudaMemcpyDeviceToHost, d.stream));
-    } else if (image && cap >= px_bytes) {
-        APT_CUDA(cudaMemcpyAsync(image, o.d_px, px_bytes, cudaMemcpyDeviceToHost, d.stream));
-    }
+    APT_TRY(o.launch(c, st->img_rows, nullptr, static_cast<u32>(rows), static_cast<u32>(st->img_max_rows), nullptr, nullptr));
+    const uint64_t px_bytes = o.plan.px_bytes(rows * kPxPerRow);
+    if (o.plan.png) APT_TRY(o.encode_px(c, rows, nullptr));
+    else if (image && cap >= px_bytes) APT_CUDA(cudaMemcpyAsync(image, o.px, px_bytes, cudaMemcpyDeviceToHost, d.stream));
     APT_CUDA(cudaStreamSynchronize(d.stream));
     APT_TRY(post_result(*o.post.head, info));
-    const uint64_t bytes = o.png ? o.h_png->total : px_bytes;
-    *image_n = bytes;
-    if (!image || cap < bytes)
-        return fail(APT_ERR_CAPACITY, "image needs room for %llu %s bytes", (unsigned long long)bytes, o.png ? "PNG" : "pixel");
-    if (o.png) {
-        APT_CUDA(cudaMemcpyAsync(image, o.png_work.out, bytes, cudaMemcpyDeviceToHost, d.stream));
-        APT_CUDA(cudaStreamSynchronize(d.stream));
+    if (!o.plan.png) {
+        *image_n = px_bytes;
+        return check_room(image, px_bytes, cap);
     }
+    *image_n = o.length(0);
+    APT_TRY(o.copy_out(0, image, cap, cudaMemcpyDeviceToHost, d.stream));
+    APT_CUDA(cudaStreamSynchronize(d.stream));
     return APT_OK;
 }
 
@@ -636,32 +602,31 @@ int finish_image(apt_stream *st, uint8_t *image, uint64_t cap, uint64_t *image_n
 extern "C" int apt_stream_set_process_mode(apt_stream *st, const apt_process_settings *ps, uint64_t max_rows) {
     if (!st) return fail(APT_ERR_BAD_ARG, "null stream");
     if (pushed(st)) return fail(APT_ERR_BAD_ARG, "image output is set before the first push (after create or reset)");
-    PostPlan plan;
+    OutPlan plan;
+    APT_TRY(make_out_plan(ps, nullptr, plan));
     if (ps) {
-        APT_TRY(make_post(*ps, plan));
         if (max_rows == 0) return fail(APT_ERR_BAD_ARG, "max_rows must be at least 1");
         if (max_rows >= (1ull << 32) / kPxPerRow) return fail(APT_ERR_BAD_ARG, "max_rows %llu: image too large", (unsigned long long)max_rows);
     }
     APT_CUDA(cudaSetDevice(st->dec.device));
     APT_CUDA(cudaStreamSynchronize(st->dec.stream));
-    ImageOut &o = st->img;
-    o.release();   // a new process mode also leaves PNG mode
+    release_image(st);   // a new process mode also leaves PNG mode
     if (!ps) return APT_OK;
     struct Rollback {
-        ImageOut &o;
+        apt_stream *st;
         bool armed = true;
         ~Rollback() {
-            if (armed) o.release();
+            if (armed) release_image(st);
         }
-    } rollback{o};
+    } rollback{st};
+    ImageOut &o = st->img;
     o.plan = plan;
-    o.max_rows = max_rows;
-    APT_TRY(o.post.alloc(plan, static_cast<u32>(max_rows)));
-    if (plan.palette) APT_TRY(o.post.upload_palette(ps->palette, st->dec.stream));
-    APT_CUDA(cudaMalloc(&o.d_rows, max_rows * kPxPerRow * sizeof(float)));
-    APT_CUDA(cudaMalloc(&o.d_px, max_rows * kPxPerRow * plan.bpp));
-    APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&o.h_png), sizeof(PngCtl), cudaHostAllocDefault));
-    o.bytes = ImageOut::post_bytes(o.plan, o.max_rows);
+    st->img_max_rows = max_rows;
+    APT_TRY(o.post.alloc(plan.post, static_cast<u32>(max_rows)));
+    if (plan.post.palette) APT_TRY(o.post.upload_palette(ps->palette, st->dec.stream));
+    APT_CUDA(cudaMalloc(&st->img_rows, max_rows * kPxPerRow * sizeof(float)));
+    APT_TRY(o.reserve_px(plan.px_bytes(max_rows * kPxPerRow)));
+    APT_TRY(o.reserve_ctl(1));
     rollback.armed = false;
     return APT_OK;
 }
@@ -670,24 +635,26 @@ extern "C" int apt_stream_set_png_mode(apt_stream *st, const apt_png_settings *p
     if (!st) return fail(APT_ERR_BAD_ARG, "null stream");
     if (pushed(st)) return fail(APT_ERR_BAD_ARG, "PNG output is set before the first push (after create or reset)");
     ImageOut &o = st->img;
+    OutPlan plan = o.plan;
     PngPlan pp;
     if (png) {
-        if (!o.d_rows) return fail(APT_ERR_BAD_ARG, "PNG output needs process mode (apt_stream_set_process_mode)");
-        APT_TRY(make_png(kPxPerRow, static_cast<uint32_t>(o.max_rows), o.plan.bpp, png, pp));
+        if (!st->img_rows) return fail(APT_ERR_BAD_ARG, "PNG output needs process mode (apt_stream_set_process_mode)");
+        APT_TRY(plan.set_png(png));
+        APT_TRY(plan.png_plan(st->img_max_rows, pp));
     }
     APT_CUDA(cudaSetDevice(st->dec.device));
     APT_CUDA(cudaStreamSynchronize(st->dec.stream));
-    o.release_png();
+    o.work.release();
+    o.plan.png = false;
     if (!png) return APT_OK;
     PngLayout lay;
     int rc = png_layout(&pp, nullptr, 1, lay);
-    if (rc == APT_OK) rc = o.png_work.reserve(lay);
+    if (rc == APT_OK) rc = o.work.reserve(lay);
     if (rc != APT_OK) {
-        o.release_png();
+        o.work.release();
         return rc;
     }
-    o.png_settings = *png;
-    o.png = true;
+    o.plan = plan;
     return APT_OK;
 }
 
@@ -696,7 +663,7 @@ extern "C" int apt_stream_finish_image(apt_stream *st, float *rows, uint64_t cap
     if (nout) *nout = 0;
     if (image_n) *image_n = 0;
     if (!st || !image_n) return fail(APT_ERR_BAD_ARG, "null argument");
-    if (!st->img.d_rows) return fail(APT_ERR_BAD_ARG, "the stream has no image output (apt_stream_set_process_mode)");
+    if (!st->img_rows) return fail(APT_ERR_BAD_ARG, "the stream has no image output (apt_stream_set_process_mode)");
     APT_TRY(apt_stream_finish(st, rows, cap, nout));
     return finish_image(st, image, image_cap, image_n, info);
 }
@@ -723,7 +690,7 @@ extern "C" int apt_stream_get_info(apt_stream *st, apt_stream_info *info) {
     info->peaks = st->positions.size();
     info->latency_work = st->g.latency;
     info->max_push = st->iq ? st->iq_max_push : st->max_push;
-    info->device_bytes = st->g.bytes + st->img.bytes + st->img.png_work.device_bytes();
+    info->device_bytes = st->g.bytes + (st->img_rows ? stream_image_bytes(st->img.plan, st->img_max_rows) : 0);
     return APT_OK;
 }
 
@@ -790,14 +757,6 @@ cudaStream_t aptb200::stream_cuda(const apt_stream *st) { return st->dec.stream;
 
 uint64_t aptb200::stream_rows_out(const apt_stream *st) { return st->rows_out; }
 
-uint64_t aptb200::stream_image_bytes(const PostPlan &plan, uint64_t max_rows, const apt_png_settings *png) {
-    uint64_t bytes = ImageOut::post_bytes(plan, max_rows);
-    if (png) {
-        PngPlan pp;
-        PngLayout lay;
-        if (make_png(kPxPerRow, static_cast<uint32_t>(max_rows), plan.bpp, png, pp) == APT_OK &&
-            png_layout(&pp, nullptr, 1, lay) == APT_OK)
-            bytes += PngWork::bytes_for(lay);
-    }
-    return bytes;
+uint64_t aptb200::stream_image_bytes(const OutPlan &plan, uint64_t max_rows) {
+    return max_rows * kPxPerRow * sizeof(float) + ImageOut::device_bytes(plan, max_rows);
 }

@@ -10,7 +10,7 @@
 #include "decoder.hpp"
 #include "front.hpp"
 #include "launch.hpp"
-#include "post.hpp"
+#include "png.hpp"
 
 namespace aptb200 {
 
@@ -30,7 +30,8 @@ int front_advance(const LaunchCtx &c, const Plan &p, const FrontTables &t, const
 int stream_push_device(apt_stream *st, const float *d_src, uint64_t n, float *rows, uint64_t cap, uint64_t *nout);
 cudaStream_t stream_cuda(const apt_stream *st);
 uint64_t stream_rows_out(const apt_stream *st);
-// Device bytes apt_stream_set_process_mode (and apt_stream_set_png_mode, png != NULL) allocate for max_rows rows.
-uint64_t stream_image_bytes(const PostPlan &plan, uint64_t max_rows, const apt_png_settings *png);
+// Device bytes apt_stream_set_process_mode (and apt_stream_set_png_mode, plan.png) allocate for max_rows rows: the pass's
+// rows and the ImageOut.
+uint64_t stream_image_bytes(const OutPlan &plan, uint64_t max_rows);
 
 }  // namespace aptb200

@@ -41,10 +41,8 @@ struct WatchPlan {
     Plan p;
     PassRule rule;
     int sync = 0;
-    bool has_ps = false, has_png = false;
+    OutPlan out;                       // out.image: the pass stream's process settings are ps
     apt_process_settings ps{};
-    apt_png_settings png{};
-    PostPlan post;
     uint64_t max_rows = 0, max_push = 0;
     uint64_t cap_in = 0, cap_e = 0, q_cap = 0, out_bytes = 0, rows_cap = 0;
     uint64_t own_bytes = 0, stream_bytes = 0, latency = 0, step_work = 0, extra_rows = 0;
@@ -58,20 +56,9 @@ int make_watch_plan(uint32_t input_rate, const apt_settings *s, const apt_watch_
     if (w.max_rows >= (1ull << 32) / kPxPerRow)
         return fail(APT_ERR_BAD_ARG, "max_rows %llu: image too large", (unsigned long long)w.max_rows);
     w.max_push = ws->max_push ? ws->max_push : input_rate;
-    if (ws->png && !ws->ps) return fail(APT_ERR_BAD_ARG, "PNG output needs process settings");
-    if (ws->ps) {
-        APT_TRY(make_post(*ws->ps, w.post));
-        w.has_ps = true;
-        w.ps = *ws->ps;
-        w.out_bytes = w.max_rows * kPxPerRow * w.post.bpp;
-    }
-    if (ws->png) {
-        PngPlan pp;
-        APT_TRY(make_png(kPxPerRow, static_cast<uint32_t>(w.max_rows), w.post.bpp, ws->png, pp));
-        w.has_png = true;
-        w.png = *ws->png;
-        w.out_bytes = pp.bound;
-    }
+    APT_TRY(make_out_plan(ws->ps, ws->png, w.out));
+    if (ws->ps) w.ps = *ws->ps;
+    if (w.out.image) APT_TRY(w.out.bytes(w.max_rows * kPxPerRow, w.out_bytes));
     apt_stream_info si{};
     APT_TRY(apt_stream_geometry(input_rate, s, w.sync, w.max_push, &si));   // the settings the pass stream refuses
     APT_TRY(make_plan(input_rate, *s, w.p));
@@ -98,7 +85,7 @@ int make_watch_plan(uint32_t input_rate, const apt_settings *s, const apt_watch_
     w.latency = (f.tail() * f.r.l / f.r.m + f.unit_out + R - 1) / R + 2;
     w.own_bytes = FrontTables::bytes(f) + w.cap_in * 4 + w.max_push * (2 + 4) + w.cap_e * 4 * (f.needs_scratch() ? 2 : 1) +
                   w.q_cap * 4;
-    w.stream_bytes = si.device_bytes + (w.has_ps ? stream_image_bytes(w.post, w.max_rows, w.has_png ? &w.png : nullptr) : 0);
+    w.stream_bytes = si.device_bytes + (w.out.image ? stream_image_bytes(w.out, w.max_rows) : 0);
     return APT_OK;
 }
 
@@ -199,7 +186,7 @@ int los(apt_watch *w, apt_pass_event ev) {
         e.status = fail(APT_ERR_CAPACITY, "the pass stream held more rows than its buffer of max_rows + %llu rows",
                         (unsigned long long)w->wp.extra_rows);
         e.rows = stream_rows_out(w->pass);   // the rows released before the buffer ran out
-    } else if (w->wp.has_ps) {
+    } else if (w->wp.out.image) {
         uint64_t image_n = 0;
         e.status = apt_stream_finish_image(w->pass, rows, cap, &nout, w->h_out.data(), w->h_out.size(), &image_n, &e.info);
         e.rows = stream_rows_out(w->pass);
@@ -388,8 +375,8 @@ extern "C" int apt_watch_create(int device, uint32_t input_rate, const apt_setti
     APT_CUDA(cudaSetDevice(device));
     APT_CUDA(cudaDeviceGetAttribute(&w->sm_count, cudaDevAttrMultiProcessorCount, device));
     APT_TRY(apt_stream_create(device, input_rate, s, wp.sync, wp.max_push, &w->pass));
-    if (wp.has_ps) APT_TRY(apt_stream_set_process_mode(w->pass, &wp.ps, wp.max_rows));
-    if (wp.has_png) APT_TRY(apt_stream_set_png_mode(w->pass, &wp.png));
+    if (wp.out.image) APT_TRY(apt_stream_set_process_mode(w->pass, &wp.ps, wp.max_rows));
+    if (wp.out.png) APT_TRY(apt_stream_set_png_mode(w->pass, &wp.out.png_s));
     w->cs = stream_cuda(w->pass);
     APT_TRY(w->front.upload(wp.p.front));
     APT_CUDA(cudaMalloc(&w->d_in, wp.cap_in * sizeof(float)));

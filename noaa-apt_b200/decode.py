@@ -161,12 +161,10 @@ class Decoder:
         fmt = _fmt_of(x)
         bpp = self._bpp
         if out is None:
-            if bpp and self._png:
+            if bpp:
                 from . import image
-                rows = max(self.out_bound(x.size) // PX_PER_ROW, 1)
-                out = np.empty(image.png_bound(PX_PER_ROW, rows, bpp, *self._png), dtype=np.uint8)
-            elif bpp:
-                out = np.empty(max(self.out_bound(x.size) * bpp, 1), dtype=np.uint8)
+                png = image.png_settings(*self._png) if self._png else None
+                out = np.empty(max(image.output_bytes(self.out_bound(x.size), bpp, png), 1), dtype=np.uint8)
             else:
                 out = np.empty(max(self.out_bound(x.size), 1), dtype=np.float32)
         self._keep = (x, out)
@@ -369,11 +367,8 @@ class Stream:
         from . import image
         if self._bpp is None:
             raise InvalidInput(_lib.ERR_BAD_ARG, "the stream has no image output: call set_process_mode first")
-        if self._png:
-            cap = image.png_bound(PX_PER_ROW, self._max_rows, self._bpp, *self._png)
-        else:
-            cap = self._max_rows * PX_PER_ROW * self._bpp
-        out = np.empty(max(cap, 1), dtype=np.uint8)
+        png = image.png_settings(*self._png) if self._png else None
+        out = np.empty(max(image.output_bytes(self._max_rows * PX_PER_ROW, self._bpp, png), 1), dtype=np.uint8)
         n = C.c_uint64(0)
         ci = _lib.CImageInfo()
         rows = self._rows(0, lambda o, got: self._lib.apt_stream_finish_image(self._h, o.ctypes.data, o.size, C.byref(got),

@@ -114,6 +114,16 @@ def png_bound(width, height, channels, filter=-1, matches=True, block_bytes=6553
     return b.value
 
 
+def output_bytes(pixels, bpp, png=None):
+    """Bytes the image of `pixels` decoded pixels leaves as: pixels * bpp, or with png (png_settings) the PNG bound of
+    max(pixels // 2080, 1) rows (host arithmetic, no device)."""
+    if png is None:
+        return pixels * bpp
+    b = C.c_uint64(0)
+    raise_for(_lib.load().apt_png_bound(2080, max(pixels // 2080, 1), int(bpp), C.byref(png), C.byref(b)))
+    return b.value
+
+
 def encode_png(pixels, filter=-1, matches=True, block_bytes=65536, rgb_from_rgba=False):
     """PNG file bytes of u8 pixels (h, w) grey, (h, w, 3) RGB or (h, w, 4) RGBA, encoded on the device."""
     x = np.ascontiguousarray(pixels, dtype=np.uint8)
@@ -167,9 +177,7 @@ def decode_png(context, settings, signal, input_rate, sync=True, contrast=MINMAX
     rate = _rate_hz(input_rate)
     bound = C.c_uint64(0)
     raise_for(lib.apt_decode_len_bound(x.size, rate, C.byref(s), C.byref(bound)))
-    cap = C.c_uint64(0)
-    raise_for(lib.apt_png_bound(2080, max(bound.value // 2080, 1), bpp, C.byref(png), C.byref(cap)))
-    out = np.empty(cap.value, dtype=np.uint8)
+    out = np.empty(output_bytes(bound.value, bpp, png), dtype=np.uint8)
     n = C.c_uint64(0)
     ci = _lib.CImageInfo()
 
@@ -203,13 +211,7 @@ def decode_batch_png(signals, input_rate, settings=None, sync=True, contrast=MIN
     ps, bpp, _pal = process_settings(contrast, percent, rotate, palette, tune, rgba)
     pngs = png_settings(filter, matches, block_bytes, rgb_from_rgba) if png else None
     count = len(xs)
-    caps_list = []
-    for x in xs:
-        bound = decode_len_bound(x.size, rate, settings)
-        if png:
-            caps_list.append(png_bound(2080, max(bound // 2080, 1), bpp, filter, matches, block_bytes, rgb_from_rgba))
-        else:
-            caps_list.append(bound * bpp)
+    caps_list = [output_bytes(decode_len_bound(x.size, rate, settings), bpp, pngs) for x in xs]
     outs = [np.empty(max(c, 1), dtype=np.uint8) for c in caps_list]
     sig_ptrs = (C.c_void_p * count)(*[x.ctypes.data for x in xs])
     out_ptrs = (C.c_void_p * count)(*[o.ctypes.data for o in outs])

@@ -19,7 +19,7 @@ import numpy as np
 
 from . import _lib, image
 from .config import Settings
-from .decode import PX_PER_ROW, _fmt_of, decode_len_bound
+from .decode import _fmt_of, decode_len_bound
 from .err import raise_for
 from .frequency import _rate_hz
 
@@ -124,11 +124,7 @@ class Recording:
         caps_list = []
         for p in ranges:
             bound = decode_len_bound(max(p.end - p.start, 0), self.input_rate, self.settings)
-            if png is not None:
-                caps_list.append(image.png_bound(PX_PER_ROW, max(bound // PX_PER_ROW, 1), bpp, png.filter, bool(png.matches),
-                                                 png.block_bytes, bool(png.rgb_from_rgba)))
-            else:
-                caps_list.append(bound * (bpp or 1))
+            caps_list.append(image.output_bytes(bound, bpp, png) if bpp else bound)
         dt = np.uint8 if bpp else np.float32
         outs = [np.empty(max(c, 1), dtype=dt) for c in caps_list]
         nouts = (C.c_uint64 * k)()
