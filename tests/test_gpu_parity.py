@@ -181,8 +181,9 @@ def test_decode_matches_oracle(rate, seconds):
 
 @pytest.mark.parametrize("rate,profile", [(48000, "fast"), (48000, "slow"), (96000, "slow")])
 def test_decode_other_profiles(rate, profile):
-    # 48 kHz fast: L = 26 (tiled kernel); slow: L = 13 with the large tap-stream parameter block; 96 kHz slow: the
-    # uniform-tap kernel at its shared-memory limit (13 slots, 231.8 KB)
+    # 48 kHz fast: L = 26, the tiled kernel's unrolled (3, 0, 3, 2) loop; 48 kHz slow (L/M = 13/30) and 96 kHz slow
+    # (13/60): the tiled kernel's runtime loop with one half, 14 and 28 iterations (test_gpu_resampler_exact.py pins
+    # every shape exactly)
     x = synth.apt_signal(rate, 12, seed=11)
     settings = na.Settings.profile(profile)
     os_ = oracle.default_settings()
