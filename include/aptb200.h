@@ -466,6 +466,13 @@ int apt_fm_demod_len(uint64_t n, const apt_iq_settings *s, uint64_t *nout);
 /* The stage alone: host I/Q in, host audio (f32, Hz) out; cap in floats. */
 int apt_fm_demod(const void *iq, int format, uint64_t n, const apt_iq_settings *s, float *out, uint64_t cap,
                  uint64_t *nout);
+/* Several channels of one I/Q input: outs[c] (cap floats each) receives apt_fm_demod with offset_hz = offsets[c], bit for
+ * bit, and *nout the audio length of every channel.  Each chunk of I/Q is uploaded once and demodulated for every channel in
+ * one kernel launch.  s->offset_hz is ignored.  Argument errors (NULL pointers, count outside 1..8, an offset failing
+ * |offset| + cutout < iq_rate / 2 or any other check of apt_fm_demod_len, an unknown format, and cap below the audio
+ * length: APT_ERR_CAPACITY) come back before any device is touched. */
+int apt_fm_demod_channels(const void *iq, int format, uint64_t n, const apt_iq_settings *s, const int32_t *offsets,
+                          int count, float *const *outs, uint64_t cap, uint64_t *nout);
 /* apt_decode at s->audio_rate of the audio apt_fm_demod would return, produced on the device: the I/Q is uploaded in
  * chunks and the audio never leaves the GPU.  Rows, status and sync positions equal apt_decode(apt_fm_demod(iq)).
  * cap in floats >= apt_decode_len_bound(ceil(n / D), audio_rate). */
@@ -814,6 +821,46 @@ int apt_watch_reset(apt_watch *w);
 int apt_watch_get_info(apt_watch *w, apt_watch_info *info);
 void apt_watch_destroy(apt_watch *w);
 /* Every call into a watcher from its own callback is APT_ERR_BAD_ARG. */
+
+/* An I/Q watcher (DESIGN.md §14): one SDR's continuous I/Q feed (rtl_sdr) watched on up to 8 channels at once, each
+ * channel an apt_watch on its own FM audio.  iq->offset_hz is ignored: channel c is the FM audio a_c of apt_fm_demod at
+ * offset_hz = offsets[c], at iq->audio_rate.  Each step (at most ws->max_push I/Q samples; 0: iq_rate) uploads the slice
+ * once, converts it into one cf32 window shared by the channels, demodulates every channel in one kernel launch straight
+ * into that channel's input window, and then runs each channel's apt_watch step on its new audio.  For any split of the
+ * feed into pushes (APT_CU8, APT_CS16 and APT_CF32 mixed), channel c keeps apt_watch's contract on a_c: per segment its q,
+ * its LOS passes and each LOS's status, rows, info and data equal apt_recording_quality, apt_find_passes_quality and
+ * apt_recording_decode of a_c.  Each channel has its own pass state, pass stream, segments and image / PNG output, so
+ * overlapping passes on different channels both finish.  The other fields of ws apply to every channel.
+ * Samples in events are audio samples of the channel (absolute since create / reset, as apt_watch reports them on a_c):
+ * multiply by D = iq_rate / audio_rate for I/Q samples.  Events come through the callback during push / finish: within one
+ * internal step channel 0's first, then channel 1's, and so on, each channel's in apt_watch's order; a segment roll is an
+ * internal step of its own, taken before the step that needs it.  Every call into an I/Q watcher from its own callback is
+ * APT_ERR_BAD_ARG.  Everything is allocated at create; push, finish and reset allocate nothing.  Argument errors come back
+ * before any device is touched: NULL pointers, count outside 1..8, the checks of apt_fm_demod_len at each offset, and what
+ * apt_watch_geometry refuses at audio_rate. */
+#define APT_WATCH_IQ_MAX_CHANNELS 8
+typedef struct apt_watch_iq apt_watch_iq;
+typedef void (*apt_watch_iq_cb)(int channel, const apt_watch_event *ev, void *user);
+/* device_bytes: the shared cf32 window 2 (N + 2D) + max_push + 64 complex samples (N the channel filter's taps), one step's
+ * raw samples (8 max_push bytes), the polyphase taps once and a phasor table per channel, and per channel the device_bytes
+ * of apt_watch_geometry(audio_rate, ws with max_push = max_push / D + 1).  max_push in I/Q samples, latency_windows the
+ * channel watcher's.  Host only. */
+int apt_watch_iq_geometry(const apt_iq_settings *iq, const int32_t *offsets, int count, const apt_settings *s,
+                          const apt_watch_settings *ws, apt_watch_info *info);
+int apt_watch_iq_create(int device, const apt_iq_settings *iq, const int32_t *offsets, int count, const apt_settings *s,
+                        const apt_watch_settings *ws, apt_watch_iq_cb cb, void *user, apt_watch_iq **w);
+/* The q floats a push of n I/Q samples can return at most for any one channel. */
+int apt_watch_iq_push_bound(apt_watch_iq *w, uint64_t n, uint64_t *cap_q);
+/* n I/Q samples (APT_CU8, APT_CS16 or APT_CF32; audio formats are APT_ERR_BAD_ARG).  Channel c's new q go to q + c * cap,
+ * and nq[c] (count entries) receives their number; cap below apt_watch_iq_push_bound is APT_ERR_CAPACITY before any work. */
+int apt_watch_iq_push(apt_watch_iq *w, const void *iq, int format, uint64_t n, float *q, uint64_t cap, uint64_t *nq);
+/* The end of the feed on every channel, as apt_watch_finish (cap: apt_watch_iq_push_bound(w, 0)). */
+int apt_watch_iq_finish(apt_watch_iq *w, float *q, uint64_t cap, uint64_t *nq);
+int apt_watch_iq_reset(apt_watch_iq *w);
+/* Channel `channel`'s segment_start, windows, passes, open and latency_windows; samples_in and max_push in I/Q samples;
+ * device_bytes the whole watcher's (apt_watch_iq_geometry). */
+int apt_watch_iq_get_info(apt_watch_iq *w, int channel, apt_watch_info *info);
+void apt_watch_iq_destroy(apt_watch_iq *w);
 
 #ifdef __cplusplus
 }

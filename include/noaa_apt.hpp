@@ -604,6 +604,79 @@ private:
     std::exception_ptr error_;
     apt_watch *h_ = nullptr;
 };
+
+// apt_watch_iq (DESIGN.md §14): one SDR's I/Q feed watched on up to 8 channels (offsets in Hz from the tuned centre;
+// iq.offset_hz is ignored).  Channel c behaves as a Watch on apt_fm_demod at offsets[c]; push / finish return each
+// channel's new q.  Event positions are audio samples of the channel.
+class IqWatch {
+public:
+    using Callback = std::function<void(int channel, const apt_watch_event &)>;
+    IqWatch(const apt_iq_settings &iq, const std::vector<int32_t> &offsets, Callback on_event,
+            const apt_watch_settings &ws = apt_watch_settings{}, const config::Settings &settings = {}, int device = 0)
+        : cb_(std::move(on_event)), count_(static_cast<int>(offsets.size())) {
+        const apt_settings st = settings.to_c();
+        err::check(apt_watch_iq_create(device, &iq, offsets.data(), count_, &st, &ws, &IqWatch::trampoline, this, &h_));
+    }
+    ~IqWatch() { apt_watch_iq_destroy(h_); }
+    IqWatch(const IqWatch &) = delete;
+    IqWatch &operator=(const IqWatch &) = delete;
+    // n complex samples of APT_CU8, APT_CS16 or APT_CF32 (interleaved I, Q): the q of each channel's windows that became final.
+    std::vector<std::vector<float>> push(const void *iq, int format, uint64_t n) {
+        const uint64_t cap = bound(n);
+        std::vector<float> q(cap * count_);
+        std::vector<uint64_t> nq(count_);
+        const int rc = apt_watch_iq_push(h_, iq, format, n, q.data(), cap, nq.data());
+        rethrow();
+        err::check(rc);
+        return split(q, cap, nq);
+    }
+    std::vector<std::vector<float>> finish() {
+        const uint64_t cap = bound(0);
+        std::vector<float> q(cap * count_);
+        std::vector<uint64_t> nq(count_);
+        const int rc = apt_watch_iq_finish(h_, q.data(), cap, nq.data());
+        rethrow();
+        err::check(rc);
+        return split(q, cap, nq);
+    }
+    void reset() { err::check(apt_watch_iq_reset(h_)); }
+    apt_watch_info info(int channel) const {
+        apt_watch_info i{};
+        err::check(apt_watch_iq_get_info(h_, channel, &i));
+        return i;
+    }
+
+private:
+    static void trampoline(int channel, const apt_watch_event *ev, void *user) {
+        IqWatch *w = static_cast<IqWatch *>(user);
+        if (!w->cb_ || w->error_) return;
+        try {
+            w->cb_(channel, *ev);
+        } catch (...) {
+            w->error_ = std::current_exception();
+        }
+    }
+    uint64_t bound(uint64_t n) {
+        uint64_t cap = 0;
+        err::check(apt_watch_iq_push_bound(h_, n, &cap));
+        return std::max<uint64_t>(cap, 1);
+    }
+    std::vector<std::vector<float>> split(const std::vector<float> &q, uint64_t cap, const std::vector<uint64_t> &nq) const {
+        std::vector<std::vector<float>> out(count_);
+        for (int c = 0; c < count_; ++c) out[c].assign(q.begin() + c * cap, q.begin() + c * cap + nq[c]);
+        return out;
+    }
+    void rethrow() {
+        if (!error_) return;
+        std::exception_ptr e = error_;
+        error_ = nullptr;
+        std::rethrow_exception(e);
+    }
+    Callback cb_;
+    std::exception_ptr error_;
+    int count_ = 0;
+    apt_watch_iq *h_ = nullptr;
+};
 }  // namespace passes
 
 }  // namespace noaa_apt

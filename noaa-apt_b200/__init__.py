@@ -18,11 +18,11 @@ from .decode import (CARRIER_FREQ, FINAL_RATE, PX_PER_ROW, Decoder, Stream, deco
                      find_sync, generate_sync_frame, stream_geometry, stream_geometry_iq)
 from .frequency import Freq, Rate
 from .iq import Carrier, decode_iq_auto, decode_iq_channels, find_carriers, spectrum
-from .passes import Pass, PassTracker, Recording, Watch, decode_passes_png, find_passes_quality
+from .passes import IqWatch, Pass, PassTracker, Recording, Watch, decode_passes_png, find_passes_quality
 
 __all__ = ["decode", "decode_batch", "decode_len_bound", "find_sync", "generate_sync_frame", "Decoder", "Stream",
            "stream_geometry", "stream_geometry_iq", "spectrum", "find_carriers", "decode_iq_channels", "decode_iq_auto",
-           "Carrier", "Recording", "Pass", "find_passes_quality", "decode_passes_png", "PassTracker", "Watch",
+           "Carrier", "Recording", "Pass", "find_passes_quality", "decode_passes_png", "PassTracker", "Watch", "IqWatch",
            "Settings", "Context", "Freq", "Rate", "dsp", "filters", "err", "config", "frequency", "image", "iq", "passes", "wav",
            "FINAL_RATE", "PX_PER_ROW", "CARRIER_FREQ"]
 

@@ -156,6 +156,8 @@ class CWatchInfo(C.Structure):
 
 STATUS_CB = C.CFUNCTYPE(None, C.c_float, C.c_char_p, C.c_void_p)
 WATCH_CB = C.CFUNCTYPE(None, C.POINTER(CWatchEvent), C.c_void_p)
+WATCH_IQ_CB = C.CFUNCTYPE(None, C.c_int, C.POINTER(CWatchEvent), C.c_void_p)
+WATCH_IQ_MAX_CHANNELS = 8
 
 # name -> (restype, argtypes); every symbol include/aptb200.h declares.
 _u64p = C.POINTER(C.c_uint64)
@@ -250,6 +252,8 @@ SIGNATURES = {
     "apt_iq_default_settings": (C.c_int, [C.c_uint32, C.c_int32, C.POINTER(CIqSettings)]),
     "apt_fm_demod_len": (C.c_int, [C.c_uint64, C.POINTER(CIqSettings), _u64p]),
     "apt_fm_demod": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64, C.POINTER(CIqSettings), C.c_void_p, C.c_uint64, _u64p]),
+    "apt_fm_demod_channels": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64, C.POINTER(CIqSettings), C.POINTER(C.c_int32),
+                                        C.c_int, C.POINTER(C.c_void_p), C.c_uint64, _u64p]),
     "apt_decode_iq": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64, C.POINTER(CIqSettings), C.POINTER(CSettings), C.c_int,
                                 C.c_void_p, C.c_uint64, _u64p, STATUS_CB, C.c_void_p]),
     "apt_stream_create_iq": (C.c_int, [C.c_int, C.POINTER(CIqSettings), C.POINTER(CSettings), C.c_int, C.c_uint64,
@@ -314,6 +318,16 @@ SIGNATURES = {
     "apt_watch_reset": (C.c_int, [C.c_void_p]),
     "apt_watch_get_info": (C.c_int, [C.c_void_p, C.POINTER(CWatchInfo)]),
     "apt_watch_destroy": (None, [C.c_void_p]),
+    "apt_watch_iq_geometry": (C.c_int, [C.POINTER(CIqSettings), C.POINTER(C.c_int32), C.c_int, C.POINTER(CSettings),
+                                        C.POINTER(CWatchSettings), C.POINTER(CWatchInfo)]),
+    "apt_watch_iq_create": (C.c_int, [C.c_int, C.POINTER(CIqSettings), C.POINTER(C.c_int32), C.c_int, C.POINTER(CSettings),
+                                      C.POINTER(CWatchSettings), WATCH_IQ_CB, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "apt_watch_iq_push_bound": (C.c_int, [C.c_void_p, C.c_uint64, _u64p]),
+    "apt_watch_iq_push": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_uint64, C.c_void_p, C.c_uint64, _u64p]),
+    "apt_watch_iq_finish": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, _u64p]),
+    "apt_watch_iq_reset": (C.c_int, [C.c_void_p]),
+    "apt_watch_iq_get_info": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(CWatchInfo)]),
+    "apt_watch_iq_destroy": (None, [C.c_void_p]),
 }
 
 _lib = None

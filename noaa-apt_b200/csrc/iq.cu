@@ -126,10 +126,12 @@ int iq_default_settings(uint32_t iq_rate, int32_t offset_hz, apt_iq_settings &s)
     return make_iq(s, p);
 }
 
-int IqTables::upload(const IqPlan &p) {
+int IqTables::upload(const IqPlan &p, bool taps) {
     release();
-    APT_CUDA(cudaMalloc(&hp, p.hp.size() * sizeof(float)));
-    APT_CUDA(cudaMemcpy(hp, p.hp.data(), p.hp.size() * sizeof(float), cudaMemcpyHostToDevice));
+    if (taps) {
+        APT_CUDA(cudaMalloc(&hp, p.hp.size() * sizeof(float)));
+        APT_CUDA(cudaMemcpy(hp, p.hp.data(), p.hp.size() * sizeof(float), cudaMemcpyHostToDevice));
+    }
     APT_CUDA(cudaMalloc(&W, p.W.size() * sizeof(float)));
     APT_CUDA(cudaMemcpy(W, p.W.data(), p.W.size() * sizeof(float), cudaMemcpyHostToDevice));
     return APT_OK;
@@ -150,35 +152,77 @@ int launch_fm(const LaunchCtx &c, const IqArgs &a, size_t smem, unsigned grid) {
     APT_CUDA(cudaGetLastError());
     return APT_OK;
 }
+
+// The launch data every channel of plan p shares, and the tiles outputs [m0, m1) take.
+int iq_args(const IqPlan &p, const IqTables &t, const void *in, uint64_t w_lo, uint64_t w_hi, uint64_t m0, uint64_t m1,
+            IqArgs &a, unsigned &grid) {
+    a = IqArgs{};
+    a.in = in;
+    a.w_lo = w_lo;
+    a.w_hi = w_hi;
+    a.hp = t.hp;
+    a.D = p.D;
+    a.qpad = p.qpad;
+    a.fs = p.s.iq_rate;
+    a.scale = p.scale;
+    a.m_begin = m0;
+    a.m_end = m1;
+    a.tz = p.tz;
+    a.lp16 = p.lp16;
+    a.ps = p.ps;
+    const uint64_t g = (m1 - m0 + p.tz - 2) / (p.tz - 1);
+    if (g > 0x7fffffffull) return fail(APT_ERR_BAD_ARG, "too many audio samples for one launch");
+    grid = static_cast<unsigned>(g);
+    return APT_OK;
+}
+
+template <int FMT>
+int launch_fm_channels(const LaunchCtx &c, const IqArgs &a, const IqChannels &ch, int count, size_t smem, unsigned grid) {
+    APT_CUDA(cudaFuncSetAttribute(k_fm_demod_channels<FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    k_fm_demod_channels<FMT><<<dim3(grid, static_cast<unsigned>(count)), kIqThreads, smem, c.stream>>>(a, ch);
+    APT_CUDA(cudaGetLastError());
+    return APT_OK;
+}
 }  // namespace
 
 int iq_launch(const LaunchCtx &c, const IqPlan &p, const IqTables &t, const void *in, uint64_t w_lo, uint64_t w_hi,
               int format, uint64_t m0, uint64_t m1, float *out) {
     if (m1 <= m0) return APT_OK;
-    IqArgs a{};
-    a.in = in;
-    a.w_lo = w_lo;
-    a.w_hi = w_hi;
+    IqArgs a;
+    unsigned grid = 0;
+    APT_TRY(iq_args(p, t, in, w_lo, w_hi, m0, m1, a, grid));
     a.W = reinterpret_cast<const float2 *>(t.W);
-    a.hp = t.hp;
-    a.D = p.D;
-    a.qpad = p.qpad;
-    a.fs = p.s.iq_rate;
     a.f = p.f;
     a.mix = p.f != 0;
-    a.scale = p.scale;
-    a.m_begin = m0;
-    a.m_end = m1;
     a.out = out;
-    a.tz = p.tz;
-    a.lp16 = p.lp16;
-    a.ps = p.ps;
-    const uint64_t grid = (m1 - m0 + p.tz - 2) / (p.tz - 1);
-    if (grid > 0x7fffffffull) return fail(APT_ERR_BAD_ARG, "too many audio samples for one launch");
     switch (format) {
-    case APT_CU8: return launch_fm<APT_CU8>(c, a, p.smem, static_cast<unsigned>(grid));
-    case APT_CS16: return launch_fm<APT_CS16>(c, a, p.smem, static_cast<unsigned>(grid));
-    case APT_CF32: return launch_fm<APT_CF32>(c, a, p.smem, static_cast<unsigned>(grid));
+    case APT_CU8: return launch_fm<APT_CU8>(c, a, p.smem, grid);
+    case APT_CS16: return launch_fm<APT_CS16>(c, a, p.smem, grid);
+    case APT_CF32: return launch_fm<APT_CF32>(c, a, p.smem, grid);
+    default: return fail(APT_ERR_BAD_ARG, "unknown I/Q sample format %d", format);
+    }
+}
+
+int iq_launch_channels(const LaunchCtx &c, const IqPlan *const *plans, const IqTables *const *tables, int count,
+                       const void *in, uint64_t w_lo, uint64_t w_hi, int format, uint64_t m0, uint64_t m1,
+                       float *const *outs) {
+    if (count < 1 || count > kIqMaxChannels) return fail(APT_ERR_BAD_ARG, "channel count %d outside 1..%d", count, kIqMaxChannels);
+    if (m1 <= m0) return APT_OK;
+    const IqPlan &p = *plans[0];
+    IqArgs a;
+    unsigned grid = 0;
+    APT_TRY(iq_args(p, *tables[0], in, w_lo, w_hi, m0, m1, a, grid));
+    IqChannels ch{};
+    for (int k = 0; k < count; ++k) {
+        ch.W[k] = reinterpret_cast<const float2 *>(tables[k]->W);
+        ch.out[k] = outs[k];
+        ch.f[k] = plans[k]->f;
+        ch.mix[k] = plans[k]->f != 0;
+    }
+    switch (format) {
+    case APT_CU8: return launch_fm_channels<APT_CU8>(c, a, ch, count, p.smem, grid);
+    case APT_CS16: return launch_fm_channels<APT_CS16>(c, a, ch, count, p.smem, grid);
+    case APT_CF32: return launch_fm_channels<APT_CF32>(c, a, ch, count, p.smem, grid);
     default: return fail(APT_ERR_BAD_ARG, "unknown I/Q sample format %d", format);
     }
 }
@@ -201,6 +245,39 @@ uint64_t iq_chunk_samples() {
     uint64_t chunk = 32ull << 20;
     if (const char *e = getenv("APTB200_IQ_CHUNK")) chunk = std::max<uint64_t>(strtoull(e, nullptr, 10), 1);
     return chunk;
+}
+
+int IqFeed::alloc(const IqPlan &q, uint64_t max_push) {
+    release();
+    cap = window(q, max_push);
+    APT_CUDA(cudaMalloc(&d_iq, cap * 2 * sizeof(float)));
+    APT_CUDA(cudaMalloc(&d_raw, max_push * 8));
+    return APT_OK;
+}
+
+void IqFeed::release() {
+    if (d_iq) cudaFree(d_iq);
+    if (d_raw) cudaFree(d_raw);
+    d_iq = nullptr;
+    d_raw = nullptr;
+    cap = in = base = 0;
+}
+
+int IqFeed::push(const LaunchCtx &c, const IqPlan &q, uint64_t m_next, const void *host, int format, uint64_t n) {
+    // the window keeps what audio output m_next reads; its tail moves to the front when that does not overlap
+    uint64_t xa, xb;
+    q.span(m_next, m_next + 1, ~0ull, xa, xb);
+    if (xa > base && in - xa <= xa - base) {
+        if (in > xa)
+            APT_CUDA(cudaMemcpyAsync(d_iq, d_iq + 2 * (xa - base), (in - xa) * 2 * sizeof(float), cudaMemcpyDeviceToDevice,
+                                     c.stream));
+        base = xa;
+    }
+    if (in - base + n > cap) return fail(APT_ERR_BAD_ARG, "internal: I/Q window overflow");
+    APT_CUDA(cudaMemcpyAsync(d_raw, host, n * iq_sample_bytes(format), cudaMemcpyHostToDevice, c.stream));
+    APT_TRY(iq_to_cf32(c, d_raw, format, n, d_iq + 2 * (in - base)));
+    in += n;
+    return APT_OK;
 }
 
 int IqWindow::reserve(uint64_t bytes) {
@@ -244,10 +321,10 @@ int iq_demod_host_multi(const LaunchCtx &c, const IqPlan *const *plans, const Iq
         const size_t bytes = (c_hi - xa) * sb;
         if (stager) APT_CUDA(stager->upload(win.p, src + xa * sb, bytes, c.stream));
         else APT_CUDA(cudaMemcpyAsync(win.p, src + xa * sb, bytes, cudaMemcpyHostToDevice, c.stream));
-        for (int k = 0; k < count; ++k) {
+        for (int k = 0; k < count; k += kIqMaxChannels) {   // one launch per chunk up to 8 channels
             KernelSlot s(hook, "fm_demod");
-            APT_TRY(iq_launch(c, *plans[k], *tables[k], static_cast<const char *>(win.p) - xa * sb, xa, c_hi, format, m_done,
-                              m_b, d_audio[k]));
+            APT_TRY(iq_launch_channels(c, plans + k, tables + k, std::min(count - k, kIqMaxChannels),
+                                       static_cast<const char *>(win.p) - xa * sb, xa, c_hi, format, m_done, m_b, d_audio + k));
         }
         m_done = m_b;
     }
@@ -301,5 +378,53 @@ extern "C" int apt_fm_demod(const void *iq, int format, uint64_t n, const apt_iq
     APT_CUDA(cudaMalloc(&d_audio, ny * sizeof(float)));
     APT_TRY(iq_demod_host(c, p, t, iq, format, n, win, nullptr, d_audio, nullptr));
     APT_CUDA(cudaMemcpy(out, d_audio, ny * sizeof(float), cudaMemcpyDeviceToHost));
+    return APT_OK;
+}
+
+extern "C" int apt_fm_demod_channels(const void *iq, int format, uint64_t n, const apt_iq_settings *s, const int32_t *offsets,
+                                     int count, float *const *outs, uint64_t cap, uint64_t *nout) {
+    if (!s || !nout || !offsets || !outs || (!iq && n)) return fail(APT_ERR_BAD_ARG, "null argument");
+    *nout = 0;
+    if (count < 1 || count > kIqMaxChannels) return fail(APT_ERR_BAD_ARG, "channel count %d outside 1..%d", count, kIqMaxChannels);
+    if (!iq_sample_bytes(format)) return fail(APT_ERR_BAD_ARG, "unknown I/Q sample format %d", format);
+    IqPlan p[kIqMaxChannels];
+    const IqPlan *pp[kIqMaxChannels];
+    for (int k = 0; k < count; ++k) {
+        apt_iq_settings sk = *s;
+        sk.offset_hz = offsets[k];
+        APT_TRY(make_iq(sk, p[k]));
+        pp[k] = &p[k];
+    }
+    const uint64_t ny = p[0].out_len(n);
+    *nout = ny;
+    if (ny > cap) return fail(APT_ERR_CAPACITY, "output needs %llu floats per channel", (unsigned long long)ny);
+    for (int k = 0; k < count && ny; ++k)
+        if (!outs[k]) return fail(APT_ERR_BAD_ARG, "null output of channel %d", k);
+    if (ny == 0) return APT_OK;
+    int ndev = 0, dev = 0, sms = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
+        cudaGetLastError();
+        return fail(APT_ERR_CUDA, "no usable CUDA device; this library has no CPU fallback");
+    }
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const LaunchCtx c{nullptr, std::max(sms, 1)};
+    IqTables t[kIqMaxChannels];
+    const IqTables *tp[kIqMaxChannels];
+    IqWindow win;
+    float *d_audio = nullptr;
+    struct Free {
+        float *&p;
+        ~Free() { if (p) cudaFree(p); }
+    } free_audio{d_audio};
+    float *d_out[kIqMaxChannels];
+    for (int k = 0; k < count; ++k) {
+        APT_TRY(t[k].upload(p[k]));
+        tp[k] = &t[k];
+    }
+    APT_CUDA(cudaMalloc(&d_audio, static_cast<size_t>(count) * ny * sizeof(float)));
+    for (int k = 0; k < count; ++k) d_out[k] = d_audio + static_cast<size_t>(k) * ny;
+    APT_TRY(iq_demod_host_multi(c, pp, tp, d_out, count, iq, format, n, win, nullptr, nullptr));
+    for (int k = 0; k < count; ++k) APT_CUDA(cudaMemcpy(outs[k], d_out[k], ny * sizeof(float), cudaMemcpyDeviceToHost));
     return APT_OK;
 }

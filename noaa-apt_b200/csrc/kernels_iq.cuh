@@ -55,8 +55,19 @@ __device__ __forceinline__ float2 cmul_rn(float2 a, float2 b) {
     return make_float2(__fsub_rn(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)), __fadd_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x)));
 }
 
+// The per-channel launch data of k_fm_demod_channels: channel c (blockIdx.y) mixes with W[c], f[c], mix[c] and writes out[c].
+constexpr int kIqMaxChannels = 8;
+struct IqChannels {
+    const float2 *W[kIqMaxChannels];
+    float *out[kIqMaxChannels];
+    u64 f[kIqMaxChannels];
+    int mix[kIqMaxChannels];
+};
+
+// One tile of k_fm_demod (blockIdx.x) for the channel whose phasors, offset, mix flag and output are given; every other
+// field of `a` is shared by the channels.  Both kernels run this function, so a channel's audio is the same bits in each.
 template <int FMT>
-__global__ void __launch_bounds__(kIqThreads, 2) k_fm_demod(const IqArgs a) {
+__device__ __forceinline__ void fm_demod_tile(const IqArgs &a, const float2 *W, u64 f, int mix, float *out) {
     extern __shared__ float2 sm[];
     const u32 D = a.D, qpad = a.qpad, tz = a.tz, lp16 = a.lp16, ps = a.ps;
     const u32 tid = threadIdx.x;
@@ -68,12 +79,12 @@ __global__ void __launch_bounds__(kIqThreads, 2) k_fm_demod(const IqArgs a) {
 
     // --- P[q] = exp(-2 pi j ((q B f) mod fs) / fs), evaluated in double and rounded once
     const long long qa = (i_lo < 0 ? 0 : i_lo) >> 12;
-    if (a.mix) {
+    if (mix) {
         const long long last = i_lo + static_cast<long long>(nstage) - 1;
         const u32 nq = last < 0 ? 0u : static_cast<u32>((last >> 12) - qa + 1);
         if (tid < nq) {
             const u64 q = static_cast<u64>(qa) + tid;
-            const u64 v = ((q * kIqBlock) % a.fs) * a.f % a.fs;
+            const u64 v = ((q * kIqBlock) % a.fs) * f % a.fs;
             double sv, cv;
             sincospi(-2.0 * static_cast<double>(v) / static_cast<double>(a.fs), &sv, &cv);
             P[tid] = make_float2(static_cast<float>(cv), static_cast<float>(sv));
@@ -90,8 +101,8 @@ __global__ void __launch_bounds__(kIqThreads, 2) k_fm_demod(const IqArgs a) {
             float2 x = make_float2(0.f, 0.f);
             if (i >= static_cast<long long>(a.w_lo) && i < static_cast<long long>(a.w_hi)) {
                 x = iq_load<FMT>(a.in, static_cast<u64>(i));
-                if (a.mix) {
-                    const float2 p = cmul_rn(P[(i >> 12) - qa], __ldg(a.W + (i & (kIqBlock - 1))));
+                if (mix) {
+                    const float2 p = cmul_rn(P[(i >> 12) - qa], __ldg(W + (i & (kIqBlock - 1))));
                     x = cmul_rn(x, p);
                 }
             }
@@ -170,8 +181,20 @@ __global__ void __launch_bounds__(kIqThreads, 2) k_fm_demod(const IqArgs a) {
             const float im = __fsub_rn(__fmul_rn(z1.y, z0.x), __fmul_rn(z1.x, z0.y));
             v = __fmul_rn(atan2f(im, re), a.scale);
         }
-        a.out[m] = v;
+        out[m] = v;
     }
+}
+
+template <int FMT>
+__global__ void __launch_bounds__(kIqThreads, 2) k_fm_demod(const IqArgs a) {
+    fm_demod_tile<FMT>(a, a.W, a.f, a.mix, a.out);
+}
+
+// Several channels of one I/Q window in one launch: blockIdx.y is the channel; a.W, a.f, a.mix and a.out are not read.
+template <int FMT>
+__global__ void __launch_bounds__(kIqThreads, 2) k_fm_demod_channels(const IqArgs a, const IqChannels ch) {
+    const u32 c = blockIdx.y;
+    fm_demod_tile<FMT>(a, ch.W[c], ch.f[c], ch.mix[c], ch.out[c]);
 }
 
 // The load of k_fm_demod alone: n samples of a push into the streaming decoder's cf32 window (exact for every format).

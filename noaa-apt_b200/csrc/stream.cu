@@ -104,15 +104,13 @@ struct apt_stream {
     const u32 *run_pos() const { return reinterpret_cast<const u32 *>(h_carry + sizeof(StreamCarry)); }
     const u32 *run_cnt() const { return run_pos() + kRunRing; }
 
-    // I/Q stream (apt_stream_create_iq): every push is converted into the cf32 window d_iq, which keeps the halo the next
+    // I/Q stream (apt_stream_create_iq): every push is converted into the cf32 window `feed`, which keeps the halo the next
     // audio output reads, and k_fm_demod writes the new audio into d_in; the audio counters above then count audio samples
     bool iq = false;
     uint64_t iq_max_push = 0;       // I/Q samples one step takes
     IqPlan iqp;
     IqTables iqt;
-    float *d_iq = nullptr;          // interleaved cf32, iq_cap complex samples from absolute sample iq_base
-    void *d_iqraw = nullptr;        // one step's pushed samples as they came
-    uint64_t iq_cap = 0, iq_in = 0, iq_base = 0;
+    IqFeed feed;
 
     // image output (apt_stream_set_process_mode), on when img_rows is set: the rows of the pass (f32, up to img_max_rows, row
     // r at r * 2080) and what becomes of them, allocated when the mode is set so that push and finish allocate nothing
@@ -139,8 +137,7 @@ void free_stream(apt_stream *st) {
         if (p) cudaFree(p);
     if (st->h_carry) cudaFreeHost(st->h_carry);
     if (st->h_rows) cudaFreeHost(st->h_rows);
-    if (st->d_iq) cudaFree(st->d_iq);
-    if (st->d_iqraw) cudaFree(st->d_iqraw);
+    st->feed.release();
     st->iqt.release();
     release_image(st);
     free_decoder_buffers(&st->dec);
@@ -149,7 +146,7 @@ void free_stream(apt_stream *st) {
 int reset_state(apt_stream *st) {
     st->samples_in = st->in_base = st->units_done = st->work_final = st->e_base = st->c_base = st->c_end = 0;
     st->rows_out = st->gathered = st->held_slot = st->runs_seen = 0;
-    st->iq_in = st->iq_base = 0;
+    st->feed.in = st->feed.base = 0;
     st->finished = false;
     st->positions.clear();
     APT_CUDA(cudaSetDevice(st->dec.device));
@@ -229,25 +226,12 @@ int upload(apt_stream *st, const void *src, bool on_device, int format, uint64_t
         added = n;
         return APT_OK;
     }
-    const void *host = src;
     const IqPlan &q = st->iqp;
-    // the cf32 window keeps what the next audio output reads; its tail moves to the front when that does not overlap
-    uint64_t xa, xb;
-    q.span(st->samples_in, st->samples_in + 1, ~0ull, xa, xb);
-    if (xa > st->iq_base && st->iq_in - xa <= xa - st->iq_base) {
-        if (st->iq_in > xa)
-            APT_CUDA(cudaMemcpyAsync(st->d_iq, st->d_iq + 2 * (xa - st->iq_base), (st->iq_in - xa) * 2 * sizeof(float),
-                                     cudaMemcpyDeviceToDevice, d.stream));
-        st->iq_base = xa;
-    }
-    if (st->iq_in - st->iq_base + n > st->iq_cap) return fail(APT_ERR_BAD_ARG, "internal: I/Q window overflow");
-    APT_CUDA(cudaMemcpyAsync(st->d_iqraw, host, n * iq_sample_bytes(format), cudaMemcpyHostToDevice, d.stream));
-    APT_TRY(iq_to_cf32(c, st->d_iqraw, format, n, st->d_iq + 2 * (st->iq_in - st->iq_base)));
-    st->iq_in += n;
-    const uint64_t m1 = q.out_len(st->iq_in);
+    APT_TRY(st->feed.push(c, q, st->samples_in, src, format, n));
+    const uint64_t m1 = q.out_len(st->feed.in);
     added = m1 - st->samples_in;
     if (off + added > st->g.cap_in) return fail(APT_ERR_BAD_ARG, "internal: input window overflow");
-    return iq_launch(c, q, st->iqt, st->d_iq - 2 * st->iq_base, st->iq_base, st->iq_in, APT_CF32, st->samples_in, m1,
+    return iq_launch(c, q, st->iqt, st->feed.origin(), st->feed.base, st->feed.in, APT_CF32, st->samples_in, m1,
                      st->d_in - st->in_base);
 }
 
@@ -357,7 +341,7 @@ int step(apt_stream *st, const void *src, bool on_device, int format, uint64_t n
 }
 
 // audio samples a push of n samples adds
-uint64_t audio_of(const apt_stream *st, uint64_t n) { return st->iq ? st->iqp.out_len(st->iq_in + n) - st->samples_in : n; }
+uint64_t audio_of(const apt_stream *st, uint64_t n) { return st->iq ? st->iqp.out_len(st->feed.in + n) - st->samples_in : n; }
 
 uint64_t rows_bound(const apt_stream *st, uint64_t n) {
     const uint64_t nw = st->dec.plan.front.work_len(st->samples_in + audio_of(st, n));
@@ -392,10 +376,8 @@ int check_iq_stream_args(const apt_iq_settings *is, const apt_settings *s, int s
     return check_stream_args(is->audio_rate, s, sync, audio_push, p);
 }
 
-uint64_t iq_window(const IqPlan &q, uint64_t max_push) { return 2 * (q.h.size() + 2ull * q.D) + max_push + 64; }
-
 uint64_t iq_bytes(const IqPlan &q, uint64_t max_push) {
-    return iq_window(q, max_push) * 8 + max_push * 8 + (q.hp.size() + q.W.size()) * sizeof(float);
+    return IqFeed::bytes(q, max_push) + (q.hp.size() + q.W.size()) * sizeof(float);
 }
 
 int create(int device, uint32_t input_rate, int sync, uint64_t max_push, std::unique_ptr<apt_stream> &st);
@@ -438,7 +420,6 @@ extern "C" int apt_stream_create_iq(int device, const apt_iq_settings *is, const
     APT_TRY(check_iq_stream_args(is, s, sync, max_push, st->iqp, st->dec.plan, audio_push));
     st->iq = true;
     st->iq_max_push = max_push;
-    st->iq_cap = iq_window(st->iqp, max_push);
     APT_TRY(create(device, is->audio_rate, sync, audio_push, st));
     apt_stream *raw = st.get();
     struct Rollback {
@@ -449,8 +430,7 @@ extern "C" int apt_stream_create_iq(int device, const apt_iq_settings *is, const
         }
     } rollback{raw};
     APT_TRY(raw->iqt.upload(raw->iqp));
-    APT_CUDA(cudaMalloc(&raw->d_iq, raw->iq_cap * 2 * sizeof(float)));
-    APT_CUDA(cudaMalloc(&raw->d_iqraw, max_push * 8));
+    APT_TRY(raw->feed.alloc(raw->iqp, max_push));
     raw->g.bytes += iq_bytes(raw->iqp, max_push);
     rollback.armed = false;
     *out = st.release();
@@ -564,7 +544,7 @@ extern "C" int apt_stream_finish(apt_stream *st, float *rows, uint64_t cap, uint
 
 namespace {
 
-bool pushed(const apt_stream *st) { return st->samples_in || st->iq_in || st->finished; }
+bool pushed(const apt_stream *st) { return st->samples_in || st->feed.in || st->finished; }
 
 // The image of a finished pass from the rows kept on the device: the image stage, in PNG mode the encoder, then the pixels or
 // the file to the caller.  One stream synchronisation for pixels, two for a PNG file (its length is read first).
@@ -684,7 +664,7 @@ extern "C" int apt_stream_sync_positions(apt_stream *st, uint64_t *positions, si
 
 extern "C" int apt_stream_get_info(apt_stream *st, apt_stream_info *info) {
     if (!st || !info) return fail(APT_ERR_BAD_ARG, "null argument");
-    info->samples_in = st->iq ? st->iq_in : st->samples_in;
+    info->samples_in = st->iq ? st->feed.in : st->samples_in;
     info->work_final = st->work_final;
     info->rows_out = st->rows_out;
     info->peaks = st->positions.size();

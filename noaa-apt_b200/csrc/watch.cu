@@ -7,6 +7,11 @@
 //   apt_stream with the caller's image / PNG output, which is finished at the group's LOS and reset.
 // The input window keeps what the pass stream or a later window can still read; the envelope window keeps the rows of the
 // next window.  Both are sized at create from the arguments alone.
+//
+// The I/Q watcher (apt_watch_iq_*, DESIGN.md §14) is one apt_watch per channel on that channel's FM audio.  Its step uploads
+// the I/Q slice once into a cf32 window the channels share (IqFeed, the I/Q stream's), demodulates every channel in one
+// launch straight into the channels' input windows, and then runs the rest of each channel's step (advance()).  CUDA events
+// order the shared stream after each channel's compaction and each channel's stream after the demodulation.
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -17,6 +22,7 @@
 #include "aptb200.h"
 #include "common.hpp"
 #include "decoder.hpp"
+#include "iq.hpp"
 #include "passes.hpp"
 #include "png.hpp"
 #include "post.hpp"
@@ -225,13 +231,11 @@ int on_event(apt_watch *w, const apt_pass_event &ev) {
     return APT_OK;
 }
 
-// One step: n new samples (maybe none) and, when `finish`, the end of the segment.  q receives the new windows.
-int step(apt_watch *w, const void *src, int format, uint64_t n, bool finish, float *q, uint64_t &nq) {
-    const WatchPlan &wp = w->wp;
-    const Plan &p = wp.p;
-    const LaunchCtx c{w->cs, w->sm_count};
+// The start of a step, before its new samples land in the input window: the windows keep only what the first stage, the
+// next window and the pass stream can still read.
+int prepare(apt_watch *w) {
+    const Plan &p = w->wp.p;
     const uint64_t R = p.row;
-    // ---- retention: what the first stage, the next window and the pass stream can still read ----
     uint64_t xa, xb;
     p.front.span(w->units_done, w->units_done + 1, ~0ull, xa, xb);
     // a group that opens in this step starts at or after the next window's first sample, even when the last group's LOS
@@ -247,15 +251,16 @@ int step(apt_watch *w, const void *src, int format, uint64_t n, bool finish, flo
         APT_TRY(window_compact(w->cs, w->d_r, rb, ekeep, w->work_final));
     }
     w->e_base = eb;
-    // ---- upload ----
-    if (n) {
-        const uint64_t off = w->samples_in - w->in_base;
-        if (off + n > wp.cap_in) return fail(APT_ERR_BAD_ARG, "internal: input window overflow");
-        APT_TRY(window_upload(c, src, false, format, n, w->d_pcm, w->d_conv, w->d_in + off));
-        w->samples_in += n;
-        w->abs_in += n;
-    }
-    // ---- first stage and q of the windows whose two rows are final ----
+    return APT_OK;
+}
+
+// The rest of a step, once its new samples are in the input window and counted in samples_in: the first stage, q of the
+// windows whose two rows are final (into q + nq), the rule and the pass stream; when `finish`, the end of the segment.
+int advance(apt_watch *w, bool finish, float *q, uint64_t &nq) {
+    const WatchPlan &wp = w->wp;
+    const Plan &p = wp.p;
+    const LaunchCtx c{w->cs, w->sm_count};
+    const uint64_t R = p.row;
     if (w->samples_in)
         APT_TRY(front_advance(c, p, w->front, w->d_in - w->in_base, w->samples_in, finish, wp.cap_e, w->d_r, w->d_e, w->e_base,
                               w->units_done, w->work_final));
@@ -296,6 +301,19 @@ int step(apt_watch *w, const void *src, int format, uint64_t n, bool finish, flo
         APT_TRY(feed_to(w, w->tracker.end_of(w->tracker.last(), ~0ull)));
     }
     return APT_OK;
+}
+
+// One step: n new samples (maybe none) from the host and, when `finish`, the end of the segment.  q receives the new windows.
+int step(apt_watch *w, const void *src, int format, uint64_t n, bool finish, float *q, uint64_t &nq) {
+    APT_TRY(prepare(w));
+    if (n) {
+        const uint64_t off = w->samples_in - w->in_base;
+        if (off + n > w->wp.cap_in) return fail(APT_ERR_BAD_ARG, "internal: input window overflow");
+        APT_TRY(window_upload(LaunchCtx{w->cs, w->sm_count}, src, false, format, n, w->d_pcm, w->d_conv, w->d_in + off));
+        w->samples_in += n;
+        w->abs_in += n;
+    }
+    return advance(w, finish, q, nq);
 }
 
 // A segment that is long enough ends before the next step: finished as at apt_watch_finish, then a new one starts.
@@ -478,5 +496,286 @@ extern "C" int apt_watch_get_info(apt_watch *w, apt_watch_info *info) {
     info->device_bytes = w->wp.own_bytes + si.device_bytes;
     info->max_push = w->wp.max_push;
     info->latency_windows = w->wp.latency;
+    return APT_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------- the I/Q watcher
+
+namespace {
+
+// Everything apt_watch_iq_create derives from its arguments, on the host.
+struct WatchIqPlan {
+    IqPlan q[APT_WATCH_IQ_MAX_CHANNELS];
+    int count = 0;
+    uint32_t audio_rate = 0;
+    uint64_t max_push = 0;             // I/Q samples per step
+    apt_watch_settings wsc{};          // each channel's: max_push = max_push / D + 1 audio samples
+    uint64_t shared_bytes = 0, channel_bytes = 0, latency = 0;
+};
+
+int make_watch_iq_plan(const apt_iq_settings *iq, const int32_t *offsets, int count, const apt_settings *s,
+                       const apt_watch_settings *ws, WatchIqPlan &w) {
+    if (!iq || !offsets || !s || !ws) return fail(APT_ERR_BAD_ARG, "null argument");
+    if (count < 1 || count > APT_WATCH_IQ_MAX_CHANNELS)
+        return fail(APT_ERR_BAD_ARG, "channel count %d outside 1..%d", count, APT_WATCH_IQ_MAX_CHANNELS);
+    for (int c = 0; c < count; ++c) {
+        apt_iq_settings sc = *iq;
+        sc.offset_hz = offsets[c];
+        APT_TRY(make_iq(sc, w.q[c]));
+    }
+    w.count = count;
+    w.audio_rate = iq->audio_rate;
+    w.max_push = ws->max_push ? ws->max_push : iq->iq_rate;
+    if (w.max_push > (1ull << 28)) return fail(APT_ERR_BAD_ARG, "max_push %llu outside [1, 2^28]", (unsigned long long)w.max_push);
+    w.wsc = *ws;
+    w.wsc.max_push = w.max_push / w.q[0].D + 1;   // the most audio one step of max_push I/Q samples completes
+    WatchPlan cp;
+    APT_TRY(make_watch_plan(w.audio_rate, s, &w.wsc, cp));
+    w.channel_bytes = cp.own_bytes + cp.stream_bytes;
+    w.latency = cp.latency;
+    w.shared_bytes = IqFeed::bytes(w.q[0], w.max_push) + (w.q[0].hp.size() + count * w.q[0].W.size()) * sizeof(float);
+    return APT_OK;
+}
+
+}  // namespace
+
+struct apt_watch_iq {
+    WatchIqPlan wp;
+    int device = 0, sm_count = 0;
+    apt_watch_iq_cb cb = nullptr;
+    void *user = nullptr;
+    cudaStream_t cs = nullptr;         // the shared window's upload, conversion and demodulation
+    cudaEvent_t ready[APT_WATCH_IQ_MAX_CHANNELS] = {}, audio = nullptr;
+    IqTables t[APT_WATCH_IQ_MAX_CHANNELS];   // t[0] holds the taps, every t[c] its channel's phasors
+    IqFeed feed;
+    apt_watch *ch[APT_WATCH_IQ_MAX_CHANNELS] = {};
+    struct Hop {                       // a channel watcher's callback user data
+        apt_watch_iq *w;
+        int c;
+    } hop[APT_WATCH_IQ_MAX_CHANNELS];
+    uint64_t m_done = 0;               // audio samples of every channel since create / reset
+    bool finished = false, in_cb = false;
+};
+
+namespace {
+
+void iq_event(const apt_watch_event *e, void *user) {
+    const apt_watch_iq::Hop *h = static_cast<const apt_watch_iq::Hop *>(user);
+    apt_watch_iq *w = h->w;
+    if (!w->cb) return;
+    w->in_cb = true;
+    w->cb(h->c, e, w->user);
+    w->in_cb = false;
+}
+
+void free_watch_iq(apt_watch_iq *w) {
+    cudaSetDevice(w->device);
+    if (w->cs) cudaStreamSynchronize(w->cs);
+    for (apt_watch *c : w->ch)
+        if (c) apt_watch_destroy(c);
+    w->feed.release();
+    for (IqTables &t : w->t) t.release();
+    for (cudaEvent_t e : w->ready)
+        if (e) cudaEventDestroy(e);
+    if (w->audio) cudaEventDestroy(w->audio);
+    if (w->cs) cudaStreamDestroy(w->cs);
+    cudaGetLastError();
+}
+
+// One step of n I/Q samples (at most max_push): every channel's segment roll first, then the channels' compaction, one upload
+// and conversion into the shared window, one demodulation launch into every channel's input window, and each channel's
+// advance() in channel order.  Channel c's q go to q + c * cap from got[c] on.
+int iq_step(apt_watch_iq *w, const void *src, int format, uint64_t n, float *q, uint64_t cap, uint64_t *got) {
+    const int C = w->wp.count;
+    for (int c = 0; c < C; ++c) APT_TRY(maybe_roll(w->ch[c], q + c * cap, got[c]));
+    for (int c = 0; c < C; ++c) {
+        APT_TRY(prepare(w->ch[c]));
+        APT_CUDA(cudaEventRecord(w->ready[c], w->ch[c]->cs));
+        APT_CUDA(cudaStreamWaitEvent(w->cs, w->ready[c], 0));
+    }
+    const LaunchCtx lc{w->cs, w->sm_count};
+    const IqPlan &p = w->wp.q[0];
+    APT_TRY(w->feed.push(lc, p, w->m_done, src, format, n));
+    const uint64_t m1 = p.out_len(w->feed.in), added = m1 - w->m_done;
+    const IqPlan *pl[APT_WATCH_IQ_MAX_CHANNELS];
+    const IqTables *tb[APT_WATCH_IQ_MAX_CHANNELS];
+    float *outs[APT_WATCH_IQ_MAX_CHANNELS];
+    for (int c = 0; c < C; ++c) {
+        apt_watch *a = w->ch[c];
+        if (a->samples_in - a->in_base + added > a->wp.cap_in) return fail(APT_ERR_BAD_ARG, "internal: input window overflow");
+        pl[c] = &w->wp.q[c];
+        tb[c] = &w->t[c];
+        outs[c] = a->d_in - a->in_base - a->seg_start;   // audio indices are absolute in the kernel, of the segment here
+    }
+    APT_TRY(iq_launch_channels(lc, pl, tb, C, w->feed.origin(), w->feed.base, w->feed.in, APT_CF32, w->m_done, m1, outs));
+    APT_CUDA(cudaEventRecord(w->audio, w->cs));
+    w->m_done = m1;
+    for (int c = 0; c < C; ++c) {
+        apt_watch *a = w->ch[c];
+        APT_CUDA(cudaStreamWaitEvent(a->cs, w->audio, 0));
+        a->samples_in += added;
+        a->abs_in += added;
+        APT_TRY(advance(a, false, q + c * cap, got[c]));
+    }
+    return APT_OK;
+}
+
+uint64_t iq_q_bound(const apt_watch_iq *w, uint64_t n) {
+    const uint64_t na = w->wp.q[0].out_len(w->feed.in + n) - w->m_done;
+    uint64_t b = 0;
+    for (int c = 0; c < w->wp.count; ++c) b = std::max(b, q_bound(w->ch[c], na));
+    return b;
+}
+
+int iq_guard(const apt_watch_iq *w) {
+    if (w->in_cb) return fail(APT_ERR_BAD_ARG, "an I/Q watcher's callback may not call into its own watcher");
+    return APT_OK;
+}
+
+}  // namespace
+
+extern "C" int apt_watch_iq_geometry(const apt_iq_settings *iq, const int32_t *offsets, int count, const apt_settings *s,
+                                     const apt_watch_settings *ws, apt_watch_info *info) {
+    if (!info) return fail(APT_ERR_BAD_ARG, "null argument");
+    std::unique_ptr<WatchIqPlan> wp(new (std::nothrow) WatchIqPlan);
+    if (!wp) return fail(APT_ERR_NOMEM, "out of host memory");
+    APT_TRY(make_watch_iq_plan(iq, offsets, count, s, ws, *wp));
+    *info = apt_watch_info{};
+    info->device_bytes = wp->shared_bytes + static_cast<uint64_t>(count) * wp->channel_bytes;
+    info->max_push = wp->max_push;
+    info->latency_windows = wp->latency;
+    return APT_OK;
+}
+
+extern "C" int apt_watch_iq_create(int device, const apt_iq_settings *iq, const int32_t *offsets, int count,
+                                   const apt_settings *s, const apt_watch_settings *ws, apt_watch_iq_cb cb, void *user,
+                                   apt_watch_iq **out) {
+    if (!out) return fail(APT_ERR_BAD_ARG, "null argument");
+    *out = nullptr;
+    std::unique_ptr<apt_watch_iq> w(new (std::nothrow) apt_watch_iq);
+    if (!w) return fail(APT_ERR_NOMEM, "out of host memory");
+    APT_TRY(make_watch_iq_plan(iq, offsets, count, s, ws, w->wp));
+    const WatchIqPlan &wp = w->wp;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
+        cudaGetLastError();
+        return fail(APT_ERR_CUDA, "no usable CUDA device; this library has no CPU fallback");
+    }
+    w->device = device;
+    w->cb = cb;
+    w->user = user;
+    struct Rollback {
+        apt_watch_iq *w;
+        bool armed = true;
+        ~Rollback() {
+            if (armed) free_watch_iq(w);
+        }
+    } rollback{w.get()};
+    APT_CUDA(cudaSetDevice(device));
+    APT_CUDA(cudaDeviceGetAttribute(&w->sm_count, cudaDevAttrMultiProcessorCount, device));
+    APT_CUDA(cudaStreamCreateWithFlags(&w->cs, cudaStreamNonBlocking));
+    APT_CUDA(cudaEventCreateWithFlags(&w->audio, cudaEventDisableTiming));
+    for (int c = 0; c < count; ++c) {
+        APT_CUDA(cudaEventCreateWithFlags(&w->ready[c], cudaEventDisableTiming));
+        APT_TRY(w->t[c].upload(wp.q[c], c == 0));
+    }
+    APT_TRY(w->feed.alloc(wp.q[0], wp.max_push));
+    for (int c = 0; c < count; ++c) {
+        w->hop[c] = apt_watch_iq::Hop{w.get(), c};
+        APT_TRY(apt_watch_create(device, wp.audio_rate, s, &wp.wsc, iq_event, &w->hop[c], &w->ch[c]));
+    }
+    rollback.armed = false;
+    *out = w.release();
+    return APT_OK;
+}
+
+extern "C" void apt_watch_iq_destroy(apt_watch_iq *w) {
+    if (!w || w->in_cb) return;
+    free_watch_iq(w);
+    delete w;
+}
+
+extern "C" int apt_watch_iq_push_bound(apt_watch_iq *w, uint64_t n, uint64_t *cap_q) {
+    if (!w || !cap_q) return fail(APT_ERR_BAD_ARG, "null argument");
+    APT_TRY(iq_guard(w));
+    *cap_q = iq_q_bound(w, n);
+    return APT_OK;
+}
+
+extern "C" int apt_watch_iq_push(apt_watch_iq *w, const void *iq, int format, uint64_t n, float *q, uint64_t cap, uint64_t *nq) {
+    if (!w || !nq) return fail(APT_ERR_BAD_ARG, "null argument");
+    APT_TRY(iq_guard(w));
+    for (int c = 0; c < w->wp.count; ++c) nq[c] = 0;
+    if (w->finished) return fail(APT_ERR_BAD_ARG, "push after finish: call apt_watch_iq_reset to start a new feed");
+    const size_t sb = iq_sample_bytes(format);
+    if (!sb) return fail(APT_ERR_BAD_ARG, "sample format %d is not APT_CU8, APT_CS16 or APT_CF32", format);
+    if (n == 0) return APT_OK;
+    if (!iq) return fail(APT_ERR_BAD_ARG, "null samples");
+    const uint64_t need = iq_q_bound(w, n);
+    if (!q || cap < need) return fail(APT_ERR_CAPACITY, "q needs room for %llu floats per channel", (unsigned long long)need);
+    APT_CUDA(cudaSetDevice(w->device));
+    uint64_t got[APT_WATCH_IQ_MAX_CHANNELS] = {};
+    try {   // the rules' gap buffers are the only host allocations of a step; no exception leaves the C ABI
+        for (uint64_t done = 0; done < n;) {
+            const uint64_t k = std::min(w->wp.max_push, n - done);
+            APT_TRY(iq_step(w, static_cast<const char *>(iq) + done * sb, format, k, q, cap, got));
+            done += k;
+        }
+    } catch (const std::bad_alloc &) {
+        return fail(APT_ERR_NOMEM, "out of host memory");
+    }
+    for (int c = 0; c < w->wp.count; ++c) nq[c] = got[c];
+    return APT_OK;
+}
+
+extern "C" int apt_watch_iq_finish(apt_watch_iq *w, float *q, uint64_t cap, uint64_t *nq) {
+    if (!w || !nq) return fail(APT_ERR_BAD_ARG, "null argument");
+    APT_TRY(iq_guard(w));
+    for (int c = 0; c < w->wp.count; ++c) nq[c] = 0;
+    if (w->finished) return fail(APT_ERR_BAD_ARG, "the I/Q watcher is already finished");
+    const uint64_t need = iq_q_bound(w, 0);
+    if (!q || cap < need) return fail(APT_ERR_CAPACITY, "q needs room for %llu floats per channel", (unsigned long long)need);
+    APT_CUDA(cudaSetDevice(w->device));
+    uint64_t got[APT_WATCH_IQ_MAX_CHANNELS] = {};
+    try {
+        for (int c = 0; c < w->wp.count; ++c) {
+            APT_TRY(step(w->ch[c], nullptr, APT_F32, 0, true, q + c * cap, got[c]));
+            w->ch[c]->finished = true;
+        }
+    } catch (const std::bad_alloc &) {
+        return fail(APT_ERR_NOMEM, "out of host memory");
+    }
+    w->finished = true;
+    for (int c = 0; c < w->wp.count; ++c) nq[c] = got[c];
+    return APT_OK;
+}
+
+extern "C" int apt_watch_iq_reset(apt_watch_iq *w) {
+    if (!w) return fail(APT_ERR_BAD_ARG, "null argument");
+    APT_TRY(iq_guard(w));
+    APT_CUDA(cudaSetDevice(w->device));
+    APT_CUDA(cudaStreamSynchronize(w->cs));
+    for (int c = 0; c < w->wp.count; ++c) APT_TRY(reset_feed(w->ch[c]));
+    w->feed.in = w->feed.base = 0;
+    w->m_done = 0;
+    w->finished = false;
+    return APT_OK;
+}
+
+extern "C" int apt_watch_iq_get_info(apt_watch_iq *w, int channel, apt_watch_info *info) {
+    if (!w || !info) return fail(APT_ERR_BAD_ARG, "null argument");
+    APT_TRY(iq_guard(w));
+    if (channel < 0 || channel >= w->wp.count)
+        return fail(APT_ERR_BAD_ARG, "channel %d outside 0..%d", channel, w->wp.count - 1);
+    uint64_t bytes = w->wp.shared_bytes;
+    for (int c = 0; c < w->wp.count; ++c) {
+        apt_watch_info ci{};
+        APT_TRY(apt_watch_get_info(w->ch[c], &ci));
+        bytes += ci.device_bytes;
+    }
+    APT_TRY(apt_watch_get_info(w->ch[channel], info));
+    info->samples_in = w->feed.in;
+    info->device_bytes = bytes;
+    info->max_push = w->wp.max_push;
     return APT_OK;
 }

@@ -8,6 +8,7 @@ The format comes from the array's dtype:
 
     s = IqSettings(2_400_000, offset_hz=37_000)     # audio_rate 48 kHz, channel filter 22 kHz / 8 kHz / 40 dB
     audio = fm_demod(iq, s)                         # instantaneous frequency in Hz at s.audio_rate
+    a0, a1 = fm_demod_channels(iq, s, [-400_000, 120_000])   # several channels, one launch per chunk
     rows = decode_iq(iq, s)                         # == decode(None, None, audio, s.audio_rate); the audio stays on the GPU
 
 Without knowing where the carriers are (DESIGN.md §10, "Finding carriers"):
@@ -87,6 +88,28 @@ def fm_demod(iq, settings):
     got = C.c_uint64(0)
     raise_for(_lib.load().apt_fm_demod(x.ctypes.data, fmt, n, C.byref(s), out.ctypes.data, out.size, C.byref(got)))
     return out[: got.value].copy()
+
+
+def _offsets(offsets):
+    offs = [int(o) for o in offsets]
+    return offs, (C.c_int32 * max(len(offs), 1))(*offs)
+
+
+def fm_demod_channels(iq, iq_settings, offsets):
+    """fm_demod at every offset of `offsets` (1..8 channels; iq_settings.offset_hz is ignored), demodulated together in one
+    kernel launch per chunk: [audio of channel c], each equal to fm_demod with offset_hz = offsets[c], bit for bit."""
+    x, fmt, n = iq_format(iq)
+    s = iq_settings.to_c()
+    s.offset_hz = 0   # ignored: the channels are `offsets`
+    offs, c_offs = _offsets(offsets)
+    na = C.c_uint64(0)
+    raise_for(_lib.load().apt_fm_demod_len(n, C.byref(s), C.byref(na)))
+    outs = [np.empty(max(na.value, 1), dtype=np.float32) for _ in offs]
+    ptrs = (C.c_void_p * max(len(offs), 1))(*[o.ctypes.data for o in outs])
+    got = C.c_uint64(0)
+    raise_for(_lib.load().apt_fm_demod_channels(x.ctypes.data if n else None, fmt, n, C.byref(s), c_offs, len(offs), ptrs,
+                                                na.value, C.byref(got)))
+    return [o[: got.value].copy() for o in outs]
 
 
 def decode_iq(iq, iq_settings, settings=None, sync=True, context=None):

@@ -18,6 +18,7 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import _lib, image
+from .iq import _offsets, iq_format
 from .config import Settings
 from .decode import _fmt_of, decode_len_bound
 from .err import raise_for
@@ -256,6 +257,24 @@ def _image_args(image_out, process):
     return (ps, pal), bpp, png
 
 
+def _watch_event(e, bpp, png):
+    """A PassEvent copied out of an apt_watch_event (during the callback: its data is valid only then)."""
+    ev = _event(e.ev)
+    ev.index, ev.status, ev.rows = int(e.index), int(e.status), int(e.rows)
+    if ev.kind == "los":
+        if bpp:
+            ev.info = image._info(e.info)
+        if e.data and e.bytes:
+            raw = C.string_at(e.data, int(e.bytes))
+            if png is not None:
+                ev.data = raw
+            elif bpp:
+                ev.data = image._shape(np.frombuffer(raw, dtype=np.uint8).copy(), bpp)
+            else:
+                ev.data = np.frombuffer(raw, dtype=np.float32).copy()
+    return ev
+
+
 class Watch:
     """apt_watch (DESIGN.md §13): a continuous feed watched for satellite passes, each finished as its rows, image or PNG file.
 
@@ -286,21 +305,7 @@ class Watch:
         self._h = h
 
     def _on_event(self, pev, _user):
-        e = pev.contents
-        ev = _event(e.ev)
-        ev.index, ev.status, ev.rows = int(e.index), int(e.status), int(e.rows)
-        if ev.kind == "los":
-            if self._bpp:
-                ev.info = image._info(e.info)
-            if e.data and e.bytes:
-                raw = C.string_at(e.data, int(e.bytes))
-                if self._png is not None:
-                    ev.data = raw
-                elif self._bpp:
-                    ev.data = image._shape(np.frombuffer(raw, dtype=np.uint8).copy(), self._bpp)
-                else:
-                    ev.data = np.frombuffer(raw, dtype=np.float32).copy()
-        self._events.append(ev)
+        self._events.append(_watch_event(pev.contents, self._bpp, self._png))
 
     def close(self):
         if getattr(self, "_h", None):
@@ -364,4 +369,117 @@ def watch_geometry(input_rate, settings=None, sync=True, search=None, image_out=
     s = (settings or Settings()).to_c()
     ci = _lib.CWatchInfo()
     raise_for(_lib.load().apt_watch_geometry(_rate_hz(input_rate), C.byref(s), C.byref(ws), C.byref(ci)))
+    return {n: int(getattr(ci, n)) for n, _ in _lib.CWatchInfo._fields_}
+
+
+def _iq_watch_args(iq_settings, offsets):
+    qs = iq_settings.to_c()
+    qs.offset_hz = 0   # ignored: the channels are `offsets`
+    offs, c_offs = _offsets(offsets)
+    return qs, offs, c_offs
+
+
+class IqWatch:
+    """apt_watch_iq (DESIGN.md §14): one SDR's I/Q feed watched for passes on several channels at once (1..8 offsets, Hz
+    from the tuned centre; iq_settings.offset_hz is ignored).  Channel c behaves as a Watch at iq_settings.audio_rate fed
+    fm_demod(feed, offset_hz = offsets[c]); every step demodulates all channels in one kernel launch.
+
+        s = iq.IqSettings(2_400_000)
+        with IqWatch(s, [-400_000, 120_000, 412_500], image_out="png") as w:
+            for block in feed:                       # uint8 (cu8), int16 (cs16) or complex64 / float32 (cf32)
+                qs, events = w.push(block)           # qs[c]: channel c's new q
+                for c, e in events:
+                    if e.kind == "los" and e.status == 0:
+                        open(f"ch{c}_pass{e.index}.png", "wb").write(e.data)
+            qs, events = w.finish()
+
+    Samples in events are audio samples of the channel; multiply by iq_settings.decimation for I/Q samples.  max_push
+    counts I/Q samples.  The other arguments are Watch's."""
+
+    def __init__(self, iq_settings, offsets, settings=None, sync=True, search=None, image_out=None, max_rows=0, max_push=0,
+                 device=0, **process):
+        self._lib = _lib.load()
+        self.iq_settings = iq_settings
+        self.settings = settings or Settings()
+        qs, self.offsets, c_offs = _iq_watch_args(iq_settings, offsets)
+        self._ps, self._bpp, self._png = _image_args(image_out, dict(process))
+        self._ws = watch_settings(sync, search, self._ps[0] if self._ps else None, self._png, max_rows, max_push)
+        self._events = []
+        self._cb = _lib.WATCH_IQ_CB(self._on_event)
+        s = self.settings.to_c()
+        h = C.c_void_p(None)
+        raise_for(self._lib.apt_watch_iq_create(int(device), C.byref(qs), c_offs, len(self.offsets), C.byref(s),
+                                                C.byref(self._ws), self._cb, None, C.byref(h)))
+        self._h = h
+
+    @property
+    def channels(self):
+        return len(self.offsets)
+
+    def _on_event(self, channel, pev, _user):
+        self._events.append((int(channel), _watch_event(pev.contents, self._bpp, self._png)))
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.apt_watch_iq_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def _take(self):
+        ev, self._events = self._events, []
+        return ev
+
+    def _q_buffers(self, n):
+        cap = C.c_uint64(0)
+        raise_for(self._lib.apt_watch_iq_push_bound(self._h, int(n), C.byref(cap)))
+        cap = max(cap.value, 1)
+        return np.empty((self.channels, cap), dtype=np.float32), cap, (C.c_uint64 * self.channels)()
+
+    def push(self, iq):
+        """([q of channel c's windows that became final], [(channel, PassEvent)])."""
+        x, fmt, n = iq_format(iq)
+        q, cap, nq = self._q_buffers(n)
+        rc = self._lib.apt_watch_iq_push(self._h, x.ctypes.data if n else None, fmt, n, q.ctypes.data, cap, nq)
+        ev = self._take()
+        raise_for(rc)
+        return [q[c, : nq[c]].copy() for c in range(self.channels)], ev
+
+    def finish(self):
+        q, cap, nq = self._q_buffers(0)
+        rc = self._lib.apt_watch_iq_finish(self._h, q.ctypes.data, cap, nq)
+        ev = self._take()
+        raise_for(rc)
+        return [q[c, : nq[c]].copy() for c in range(self.channels)], ev
+
+    def reset(self):
+        raise_for(self._lib.apt_watch_iq_reset(self._h))
+        self._events = []
+
+    def info(self, channel=0):
+        ci = _lib.CWatchInfo()
+        raise_for(self._lib.apt_watch_iq_get_info(self._h, int(channel), C.byref(ci)))
+        return {n: int(getattr(ci, n)) for n, _ in _lib.CWatchInfo._fields_}
+
+    @property
+    def device_bytes(self):
+        return self.info()["device_bytes"]
+
+
+def watch_iq_geometry(iq_settings, offsets, settings=None, sync=True, search=None, image_out=None, max_rows=0, max_push=0,
+                      **process):
+    """apt_watch_iq_geometry (host only): the device_bytes, max_push (I/Q samples) and latency_windows an IqWatch with these
+    arguments has."""
+    qs, offs, c_offs = _iq_watch_args(iq_settings, offsets)
+    ps, _bpp, png = _image_args(image_out, dict(process))
+    ws = watch_settings(sync, search, ps[0] if ps else None, png, max_rows, max_push)
+    s = (settings or Settings()).to_c()
+    ci = _lib.CWatchInfo()
+    raise_for(_lib.load().apt_watch_iq_geometry(C.byref(qs), c_offs, len(offs), C.byref(s), C.byref(ws), C.byref(ci)))
     return {n: int(getattr(ci, n)) for n, _ in _lib.CWatchInfo._fields_}

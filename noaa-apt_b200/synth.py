@@ -221,6 +221,70 @@ def apt_iq_multi(iq_rate, seconds=None, carriers=((0, 0, 0.0, None, 60.0),), ext
     return np.clip(np.rint(inter), -32768, 32767).astype(np.int16)
 
 
+def _iq_pass_spans(iq_rate, passes):
+    return [(int(off), int(seed), int(round(on * iq_rate)), int(round(off_s * iq_rate))) for off, seed, on, off_s in passes]
+
+
+def apt_iq_passes_truth(iq_rate, passes, fade_s=10.0):
+    """(offset_hz, fade-in midpoint, fade-out midpoint) in I/Q samples of every pass of apt_iq_passes."""
+    h = int(round(0.5 * fade_s * iq_rate))
+    return [(off, a + h, b - h) for off, _seed, a, b in _iq_pass_spans(iq_rate, passes)]
+
+
+def apt_iq_passes(iq_rate, seconds=None, passes=(), extra_bands=(), fmt="cu8", noise_rel=0.03, fade_s=10.0, n_samples=None,
+                  deviation_hz=17000.0, audio_amplitude=20000.0, chunk=1 << 22):
+    """A continuous I/Q feed of one SDR in which each satellite's carrier is on only during its own passes.
+
+    passes: (offset_hz, seed, on_s, off_s) per pass: from on_s to off_s the carrier at offset_hz carries the APT audio of
+      `seed` (from its first sample, FM-modulated as apt_iq_multi does), its amplitude rising linearly from 0 over the first
+      fade_s seconds and falling to 0 over the last; outside, the carrier is off.  Passes may overlap in time.
+    extra_bands, noise_rel, fmt: as apt_iq_multi (receiver noise everywhere, the sum scaled down by the number of distinct
+      carrier offsets plus bands).  Every sample is a function of its index alone, so the output does not depend on `chunk`."""
+    if n_samples is None:
+        n_samples = int(round(iq_rate * seconds))
+    spans = _iq_pass_spans(iq_rate, passes)
+    nsig = len({off for off, _s, _a, _b in spans}) + len(extra_bands)
+    scale = _IQ_SCALE[fmt] / max(nsig, 1)
+    out = np.empty(n_samples, dtype=np.complex128)
+    bands = [(_band_taps(w, iq_rate), off, p) for off, w, p in extra_bands]
+    fade = max(fade_s * iq_rate, 1.0)
+    acc = [0] * len(spans)                    # running sum of each pass's int16 audio before the chunk
+    done = 0
+    while done < n_samples:
+        m = min(chunk, n_samples - done)
+        idx = np.arange(done, done + m, dtype=np.int64)
+        y = np.zeros(m, dtype=np.complex128)
+        for p, (off, seed, a, b) in enumerate(spans):
+            lo, hi = max(a, done), min(b, done + m)
+            if lo >= hi:
+                continue
+            audio = apt_pcm16(iq_rate, seed=seed, n_samples=hi - lo, start=lo - a, noise_sigma=0.0, chunk=chunk).astype(np.int64)
+            s_audio = acc[p] + np.cumsum(audio) - audio
+            acc[p] += int(audio.sum())
+            k = idx[lo - done:hi - done]
+            rel = (k - a).astype(np.float64)
+            gain = np.clip(np.minimum(rel / fade, (b - a - rel) / fade), 0.0, 1.0)
+            ph = (0.3 + 0.1 * (seed % 17)
+                  + 2.0 * np.pi * ((k * off) % iq_rate).astype(np.float64) / iq_rate
+                  + 2.0 * np.pi * deviation_hz / (audio_amplitude * iq_rate) * s_audio.astype(np.float64))
+            y[lo - done:hi - done] += gain * np.exp(1j * ph)
+        for bi, (h, off, pw) in enumerate(bands):
+            raw = _noise_blocks(0x3D1 + bi, done, done + m + h.size - 1)
+            shaped = np.convolve(raw, h, mode="valid") * np.sqrt(pw / (2.0 * np.sum(h * h)))
+            y += shaped * np.exp(2j * np.pi * ((idx * int(off)) % iq_rate).astype(np.float64) / iq_rate)
+        if noise_rel > 0:
+            y += _noise_blocks(0x2C7, done, done + m) * noise_rel
+        out[done:done + m] = y
+        done += m
+    if fmt == "cf32":
+        return (out * scale).astype(np.complex64)
+    inter = np.empty(2 * n_samples, dtype=np.float64)
+    inter[0::2], inter[1::2] = out.real * scale, out.imag * scale
+    if fmt == "cu8":
+        return np.clip(np.rint(inter + 127.5), 0, 255).astype(np.uint8)
+    return np.clip(np.rint(inter), -32768, 32767).astype(np.int16)
+
+
 def _real_noise(key, a, b):
     """Real standard Gaussian noise for absolute sample indices [a, b): one Philox stream per (key, block of _BLOCK)."""
     out = np.empty(b - a, dtype=np.float64)

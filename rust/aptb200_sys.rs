@@ -282,6 +282,11 @@ pub struct apt_watch_info { pub samples_in: u64, pub segment_start: u64, pub win
                             pub device_bytes: u64, pub max_push: u64, pub latency_windows: u64 }
 
 pub type apt_watch_cb = Option<unsafe extern "C" fn(ev: *const apt_watch_event, user: *mut c_void)>;
+// One SDR's I/Q feed on several channels (DESIGN.md §14)
+pub const APT_WATCH_IQ_MAX_CHANNELS: c_int = 8;
+#[repr(C)]
+pub struct apt_watch_iq { _private: [u8; 0] }
+pub type apt_watch_iq_cb = Option<unsafe extern "C" fn(channel: c_int, ev: *const apt_watch_event, user: *mut c_void)>;
 
 #[link(name = "aptb200")]
 extern "C" {
@@ -301,4 +306,18 @@ extern "C" {
     pub fn apt_watch_reset(w: *mut apt_watch) -> c_int;
     pub fn apt_watch_get_info(w: *mut apt_watch, info: *mut apt_watch_info) -> c_int;
     pub fn apt_watch_destroy(w: *mut apt_watch);
+    pub fn apt_fm_demod_channels(iq: *const c_void, format: c_int, n: u64, s: *const apt_iq_settings, offsets: *const i32,
+                                 count: c_int, outs: *const *mut f32, cap: u64, nout: *mut u64) -> c_int;
+    pub fn apt_watch_iq_geometry(iq: *const apt_iq_settings, offsets: *const i32, count: c_int, s: *const apt_settings,
+                                 ws: *const apt_watch_settings, info: *mut apt_watch_info) -> c_int;
+    pub fn apt_watch_iq_create(device: c_int, iq: *const apt_iq_settings, offsets: *const i32, count: c_int,
+                               s: *const apt_settings, ws: *const apt_watch_settings, cb: apt_watch_iq_cb, user: *mut c_void,
+                               w: *mut *mut apt_watch_iq) -> c_int;
+    pub fn apt_watch_iq_push_bound(w: *mut apt_watch_iq, n: u64, cap_q: *mut u64) -> c_int;
+    pub fn apt_watch_iq_push(w: *mut apt_watch_iq, iq: *const c_void, format: c_int, n: u64, q: *mut f32, cap: u64,
+                             nq: *mut u64) -> c_int;
+    pub fn apt_watch_iq_finish(w: *mut apt_watch_iq, q: *mut f32, cap: u64, nq: *mut u64) -> c_int;
+    pub fn apt_watch_iq_reset(w: *mut apt_watch_iq) -> c_int;
+    pub fn apt_watch_iq_get_info(w: *mut apt_watch_iq, channel: c_int, info: *mut apt_watch_info) -> c_int;
+    pub fn apt_watch_iq_destroy(w: *mut apt_watch_iq);
 }

@@ -113,10 +113,8 @@ struct Handler<'f> {
     f: Box<dyn FnMut(WatchEvent) + 'f>,
 }
 
-unsafe extern "C" fn watch_trampoline(ev: *const sys::apt_watch_event, user: *mut c_void) {
-    let h = &mut *(user as *mut Handler);
-    let e = &*ev;
-    let out = match e.ev.kind {
+unsafe fn watch_event<'a>(e: &'a sys::apt_watch_event) -> WatchEvent<'a> {
+    match e.ev.kind {
         sys::APT_PASS_AOS => WatchEvent::Aos { index: e.index, pass: e.ev.pass },
         sys::APT_PASS_SEGMENT => WatchEvent::Segment { start: e.ev.pass.start },
         _ => WatchEvent::Los {
@@ -130,7 +128,12 @@ unsafe extern "C" fn watch_trampoline(ev: *const sys::apt_watch_event, user: *mu
             },
             info: e.info,
         },
-    };
+    }
+}
+
+unsafe extern "C" fn watch_trampoline(ev: *const sys::apt_watch_event, user: *mut c_void) {
+    let h = &mut *(user as *mut Handler);
+    let out = watch_event(&*ev);
     // a panic must not unwind into the library
     let _ = std::panic::catch_unwind(std::panic::AssertUnwindSafe(|| (h.f)(out)));
 }
@@ -197,6 +200,90 @@ impl<'f> Watch<'f> {
 impl<'f> Drop for Watch<'f> {
     fn drop(&mut self) {
         unsafe { sys::apt_watch_destroy(self.h) };
+        let _ = &self.handler;   // freed after the watcher, which holds its address
+    }
+}
+
+/// One SDR's I/Q feed (cu8 as rtl_sdr writes it) watched for passes on up to 8 channels at once (DESIGN.md §14): channel
+/// c behaves as a `Watch` on the FM audio at `offsets[c]` Hz from the tuned centre.  The closure gets the channel and the
+/// event; event positions are audio samples of the channel.
+pub struct IqWatch<'f> {
+    h: *mut sys::apt_watch_iq,
+    count: usize,
+    handler: Box<IqHandler<'f>>,
+}
+
+struct IqHandler<'f> {
+    f: Box<dyn FnMut(usize, WatchEvent) + 'f>,
+}
+
+unsafe extern "C" fn watch_iq_trampoline(channel: i32, ev: *const sys::apt_watch_event, user: *mut c_void) {
+    let h = &mut *(user as *mut IqHandler);
+    let out = watch_event(&*ev);
+    let _ = std::panic::catch_unwind(std::panic::AssertUnwindSafe(|| (h.f)(channel as usize, out)));
+}
+
+impl<'f> IqWatch<'f> {
+    pub fn new(iq: &sys::apt_iq_settings, offsets: &[i32], settings: &config::Settings, search: &sys::apt_pass_search,
+               image: Option<(&sys::apt_process_settings, Option<&sys::apt_png_settings>)>, max_rows: u64, device: i32,
+               on_event: impl FnMut(usize, WatchEvent) + 'f) -> err::Result<IqWatch<'f>> {
+        let s = sys::apt_settings::from(settings);
+        let ws = sys::apt_watch_settings {
+            sync: 1,
+            search: *search,
+            ps: image.map_or(ptr::null(), |(ps, _)| ps as *const _),
+            png: image.and_then(|(_, png)| png).map_or(ptr::null(), |p| p as *const _),
+            max_rows,
+            max_push: 0,
+        };
+        let mut handler = Box::new(IqHandler { f: Box::new(on_event) });
+        let mut h = ptr::null_mut();
+        check(unsafe { sys::apt_watch_iq_create(device, iq, offsets.as_ptr(), offsets.len() as i32, &s, &ws,
+                                                Some(watch_iq_trampoline),
+                                                &mut *handler as *mut IqHandler as *mut c_void, &mut h) })?;
+        Ok(IqWatch { h, count: offsets.len(), handler })
+    }
+
+    fn split(&self, q: Vec<f32>, cap: usize, nq: &[u64]) -> Vec<Vec<f32>> {
+        (0..self.count).map(|c| q[c * cap..c * cap + nq[c] as usize].to_vec()).collect()
+    }
+
+    /// Interleaved cu8 I/Q: each channel's new windows' quality; events reach the closure during the call.
+    pub fn push(&mut self, cu8: &[u8]) -> err::Result<Vec<Vec<f32>>> {
+        let n = (cu8.len() / 2) as u64;
+        let mut cap = 0u64;
+        check(unsafe { sys::apt_watch_iq_push_bound(self.h, n, &mut cap) })?;
+        let cap = cap.max(1) as usize;
+        let mut q = vec![0f32; cap * self.count];
+        let mut nq = vec![0u64; self.count];
+        check(unsafe { sys::apt_watch_iq_push(self.h, cu8.as_ptr() as *const c_void, sys::APT_CU8, n, q.as_mut_ptr(),
+                                              cap as u64, nq.as_mut_ptr()) })?;
+        Ok(self.split(q, cap, &nq))
+    }
+
+    /// The end of the feed on every channel.
+    pub fn finish(&mut self) -> err::Result<Vec<Vec<f32>>> {
+        let mut cap = 0u64;
+        check(unsafe { sys::apt_watch_iq_push_bound(self.h, 0, &mut cap) })?;
+        let cap = cap.max(1) as usize;
+        let mut q = vec![0f32; cap * self.count];
+        let mut nq = vec![0u64; self.count];
+        check(unsafe { sys::apt_watch_iq_finish(self.h, q.as_mut_ptr(), cap as u64, nq.as_mut_ptr()) })?;
+        Ok(self.split(q, cap, &nq))
+    }
+
+    pub fn reset(&mut self) -> err::Result<()> { check(unsafe { sys::apt_watch_iq_reset(self.h) }) }
+
+    pub fn info(&self, channel: usize) -> err::Result<sys::apt_watch_info> {
+        let mut i = sys::apt_watch_info::default();
+        check(unsafe { sys::apt_watch_iq_get_info(self.h, channel as i32, &mut i) })?;
+        Ok(i)
+    }
+}
+
+impl<'f> Drop for IqWatch<'f> {
+    fn drop(&mut self) {
+        unsafe { sys::apt_watch_iq_destroy(self.h) };
         let _ = &self.handler;   // freed after the watcher, which holds its address
     }
 }
