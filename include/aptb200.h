@@ -303,6 +303,23 @@ int apt_decoder_last_root_count(apt_decoder *dec, uint64_t *n_roots);
 /* The roots themselves, ascending (a root is a correlation index p with no larger value in (p, p + min_distance]: the
  * only places a sync position can land -- DESIGN.md "Peak picker").  Diagnostic; valid after a wait() of a sync job. */
 int apt_decoder_last_roots(apt_decoder *dec, uint64_t *roots, size_t cap, size_t *nroots);
+/* What the sync record kernel wrote for the last job, tile by tile (DESIGN.md "Peak picker"): a tile is W consecutive
+ * correlation positions (W = 1920, 1888, 1856 for pixel widths 3, 4, 5); its weak suffix records (no later position of the
+ * tile is larger) and its strict prefix records (larger than every earlier position of the tile) are (position, value)
+ * pairs, ascending.  tiles[t] receives the counts and the maximum of tile t; `records` the records of every tile in tile
+ * order, each tile's suffix list then its prefix list.  At most tiles_cap / records_cap entries are written, *ntiles and
+ * *nrecords are the totals (NULL buffers with cap 0 ask for the sizes).  Diagnostic; valid after a wait() of a sync job
+ * that ran the record kernel and did not overflow its pool, else APT_ERR_BAD_ARG. */
+typedef struct apt_tile_records {
+    uint32_t n_suffix, n_prefix;  /* record counts of the tile */
+    float max;                    /* maximum of the correlation over the tile */
+} apt_tile_records;
+typedef struct apt_record {
+    uint32_t pos;                 /* correlation index */
+    float val;                    /* correlation value */
+} apt_record;
+int apt_decoder_last_records(apt_decoder *dec, apt_tile_records *tiles, size_t tiles_cap, size_t *ntiles,
+                             apt_record *records, size_t records_cap, size_t *nrecords);
 /* Copy an intermediate signal of the last job back to the host (what Context::step would dump):
  * which = 0 "demodulation_result" input i.e. resample+envelope output, 1 "filter_result",
  * 2 "sync_correlation". */

@@ -219,6 +219,7 @@ SIGNATURES = {
     "apt_decoder_last_counts": (C.c_int, [C.c_void_p, _u64p, _u64p, _u64p]),
     "apt_decoder_last_root_count": (C.c_int, [C.c_void_p, _u64p]),
     "apt_decoder_last_roots": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, _szp]),
+    "apt_decoder_last_records": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, _szp, C.c_void_p, C.c_size_t, _szp]),
     "apt_decoder_read_stage": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_uint64, _u64p]),
     "apt_decoder_set_profiling": (C.c_int, [C.c_void_p, C.c_int]),
     "apt_decoder_kernel_count": (C.c_int, [C.c_void_p]),

@@ -753,14 +753,26 @@ extern "C" int apt_decoder_last_roots(apt_decoder *d, uint64_t *roots, size_t ca
     return back_roots(d->plan, d->back_plan, d->back, d->last_back, d->last_work, roots, cap, nroots);
 }
 
+extern "C" int apt_decoder_last_records(apt_decoder *d, apt_tile_records *tiles, size_t tiles_cap, size_t *ntiles,
+                                        apt_record *records, size_t records_cap, size_t *nrecords) {
+    if (!d || !ntiles || !nrecords) return fail(APT_ERR_BAD_ARG, "null argument");
+    *ntiles = *nrecords = 0;
+    if (d->in_flight) return fail(APT_ERR_BAD_ARG, "decoder has a job in flight");
+    if (d->last_back != BackKind::Records || !d->job_sync)
+        return fail(APT_ERR_BAD_ARG, "the last job did not run the record kernel (a Records sync job whose pool did not overflow)");
+    APT_CUDA(cudaSetDevice(d->device));
+    return back_records(d->plan, d->back_plan, d->back, d->last_work, tiles, tiles_cap, ntiles, records, records_cap, nrecords);
+}
+
 extern "C" int apt_decoder_read_stage(apt_decoder *d, int which, float *out, uint64_t cap, uint64_t *n) {
     if (!d || !n) return fail(APT_ERR_BAD_ARG, "null argument");
     APT_CUDA(cudaSetDevice(d->device));
     const float *src = nullptr;
     uint64_t len = d->last_work;
-    if (which != 0 && d->last_back == BackKind::Records && len) {   // f / corr were never written: compute them now
+    if (which != 0 && d->last_back == BackKind::Records && !d->stages_materialised && len) {
+        // f / corr were never written: compute them now (the roots and records of the job stay where they are)
         APT_TRY(back_materialise(LaunchCtx{d->stream, d->sm_count}, d->plan, d->back_plan, d->back, d->d_e, len));
-        d->last_back = BackKind::Hbm;
+        d->stages_materialised = true;
     }
     switch (which) {
     case 0: src = d->d_e; break;

@@ -264,4 +264,29 @@ int back_roots(const Plan &p, const BackPlan &bp, const BackBuffers &b, BackKind
     return APT_OK;
 }
 
+int back_records(const Plan &p, const BackPlan &bp, const BackBuffers &b, uint64_t nwork, apt_tile_records *tiles,
+                 size_t tiles_cap, size_t *ntiles, apt_record *records, size_t records_cap, size_t *nrecords) {
+    *ntiles = *nrecords = 0;
+    if (!b.desc || nwork <= p.guard.size()) return APT_OK;
+    const uint64_t ncorr = nwork - p.guard.size();
+    const u32 nt = static_cast<u32>((ncorr + bp.tile_w - 1) / bp.tile_w);
+    std::vector<TileDesc> desc(nt);
+    APT_CUDA(cudaMemcpy(desc.data(), b.desc, nt * sizeof(TileDesc), cudaMemcpyDeviceToHost));
+    size_t total = 0;
+    std::vector<Rec> tmp;
+    for (u32 k = 0; k < nt; ++k) {
+        const u32 cnt = desc[k].ns + desc[k].np;
+        if (k < tiles_cap) tiles[k] = apt_tile_records{desc[k].ns, desc[k].np, desc[k].tmax};
+        if (records && cnt && total < records_cap) {
+            tmp.resize(cnt);
+            APT_CUDA(cudaMemcpy(tmp.data(), b.pool + desc[k].off, cnt * sizeof(Rec), cudaMemcpyDeviceToHost));
+            for (u32 i = 0; i < cnt && total + i < records_cap; ++i) records[total + i] = apt_record{tmp[i].pos, tmp[i].val};
+        }
+        total += cnt;
+    }
+    *ntiles = nt;
+    *nrecords = total;
+    return APT_OK;
+}
+
 }  // namespace aptb200

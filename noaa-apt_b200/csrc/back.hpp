@@ -7,6 +7,7 @@
 #include <cstdint>
 #include <optional>
 
+#include "aptb200.h"
 #include "launch.hpp"
 
 namespace aptb200 {
@@ -80,5 +81,9 @@ int back_materialise(const LaunchCtx &c, const Plan &p, const BackPlan &bp, Back
 // The roots of the last job, ascending, in the layout of the kind that ran it.
 int back_roots(const Plan &p, const BackPlan &bp, const BackBuffers &b, BackKind ran, uint64_t nwork, uint64_t *roots,
                size_t cap, size_t *nroots);
+// The per-tile output of k_lowpass_records of the last job (a Records sync job whose pool did not overflow): counts and
+// maximum of every tile, then its records, suffix list then prefix list, in tile order (apt_decoder_last_records).
+int back_records(const Plan &p, const BackPlan &bp, const BackBuffers &b, uint64_t nwork, apt_tile_records *tiles,
+                 size_t tiles_cap, size_t *ntiles, apt_record *records, size_t records_cap, size_t *nrecords);
 
 }  // namespace aptb200

@@ -270,6 +270,7 @@ int decoder_enqueue(apt_decoder *d, const void *in, int format, uint64_t n, int 
         if (d->cb) d->cb(0.9f, "Resampling to 4160", d->cb_user);           // decode.rs:154
     }
     DecoderHook hook(d);
+    d->stages_materialised = false;
     APT_TRY(back_launch(c, p, d->back_plan, d->back, d->d_lp, d->d_one, d->d_e, nwork, sync != 0, rows_out, &hook, d->last_back));
     if (sync && d->cb) d->cb(0.9f, "Resampling to 4160", d->cb_user);
     d->job_fixed_out = sync ? 0 : plan_out_bound(p, n);

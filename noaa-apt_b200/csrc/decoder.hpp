@@ -103,8 +103,9 @@ struct apt_decoder {
     uint64_t l2_window_bytes = 0;  // bytes of d_e covered by a persisting L2 access-policy window on `stream` (0: none)
     aptb200::BackPlan back_plan;   // the back half's kind and buffer sizes
     aptb200::BackBuffers back;     // its buffers
-    aptb200::BackKind last_back = aptb200::BackKind::Generic;   // the kind that ran the last job: where its roots are, and
-                                                                  // whether its f / corr exist
+    aptb200::BackKind last_back = aptb200::BackKind::Generic;   // the kind that ran the last job: where its roots and
+                                                                  // records are, and whether it wrote f / corr
+    bool stages_materialised = false;  // f / corr of a Records job computed since by apt_decoder_read_stage
     float *d_out = nullptr;        // rows for submit_host
     // pageable host buffers (what the reference-facing apt_decode receives) go through a pinned ring + copy threads
     aptb200::HostStager *stager = nullptr;                 // the one in use (own_stager, or the batch feeder's)

@@ -7,16 +7,17 @@
 // The template is +-1 in runs of 2*PW samples (19 runs: - | (-,+) x 7 | - - - -), so the correlation is
 // computed from box sums B[n] = f[n] + ... + f[n+2*PW-1]:  corr[i] = sum_b sign_b * B[i + 2*PW*b]  -- 24 adds
 // per output instead of 114.  The summation order differs from the reference's sequential loop, i.e. the
-// values agree to fp32 rounding (~1e-7 relative), not bit for bit; the generic kernel keeps the exact order.
+// values agree to fp32 rounding (~1e-7 relative), not bit for bit; the generic kernel keeps the exact order.  f, the box
+// sums and corr are bit for bit those of k_lowpass_records (kernels_sync2.cuh), and f those of k_gather_rows_lp: the three
+// share one low-pass order, one box-sum order and one correlation order (tests/_sync_oracle.py restates them).
 //
 // Tiles start at `base` (BASED instantiations only; a multiple of 16, so every position keeps the parity and the 16-byte alignment it has with
 // base 0 and the values are those of a run from 0); there f_out == nullptr skips storing f.
 // One CTA handles 1856 consecutive positions: e tile -> f tile -> box sums -> correlation, all on fp32 register pairs
 // (fma2: two FMAs / adds):
-//   low-pass   : a thread owns 8 outputs of ONE parity (even warps the even positions, odd warps the odd ones), so
-//                that for every output the window pairs (e[2t], e[2t+1]) -- the register pairs an LDS.128 delivers --
-//                meet the tap pairs (c[j], c[j-1]) with j of a fixed parity: fma2(window pair, tap pair) with the
-//                tap pair a warp-uniform kernel-parameter operand; f = lo + hi.
+//   low-pass   : a thread owns 8 consecutive outputs (even warps the first 8 of a block of 16, odd warps the last 8),
+//                one FMA chain each, tap 0 first: a window sample broadcast into a register pair meets the tap pair
+//                (c[j], c[j+1]) of two neighbouring outputs, a warp-uniform kernel-parameter operand.
 //   box sums   : pair sums P[k] = f[2k] + f[2k+1] shared by neighbouring outputs: PW + 2 adds per two outputs.
 //   correlation: output pairs (v, v+1), v even, accumulate box pairs (B[m], B[m+1]), m even (2*PW is even), with
 //                fma2 by (+-1, +-1): 19 per output pair.
@@ -33,8 +34,6 @@
 namespace aptb200 {
 
 struct LpTaps {          // kernel parameter: warp-uniform operands
-    float2 a_even[32];   // (c[2i], c[2i-1]), c[-1] = 0      -- used by the warps that own the even positions
-    float2 a_odd[32];    // (c[2i+1], c[2i]), c[NT] = 0      -- ... the odd positions
     float2 p[64];        // p[j+1] = (c[j], c[j+1]), j = -1 .. NT-1 -- one sample x the taps of two neighbouring outputs
     float2 pd[72];       // pd[j+DEC] = (c[j], c[j+DEC]), j = -DEC .. NT-1 -- ... of two neighbouring PIXELS (DEC samples apart)
 };
@@ -43,43 +42,40 @@ constexpr int kLpTile = 1856;   // (T + 38*PW - 1) / 16 <= 128 for PW <= 5: ever
 
 __device__ __forceinline__ u32 skew(u32 n) { return n + ((n >> 5) << 2); }   // 4 floats of padding every 32
 
-// Low-pass outputs 16*blk + PAR + 2v, v < 8, from the skewed e tile into the skewed f tile.
-template <int NT, int PAR>
+// Low-pass outputs o .. o+7, o = 16*blk + 8*HALF, from the skewed e tile into the skewed f tile.  Every output is ONE
+// chain of FMAs, tap 0 first (f[o] = fma(c[NT-1], e[o-NT+1], ... fma(c[0], e[o], 0))), the order of k_lowpass_records and
+// k_gather_rows_lp: one window sample x the taps it has in two neighbouring outputs, (c[j], c[j+1]) -- a warp-uniform tap
+// pair -- into the accumulator pair of the outputs (2v, 2v+1).  j = -1 (c[-1] = 0) and the c[NT] = 0 half of j = NT-1 add
+// +0 to a chain that starts at +0, which leaves it unchanged.
+template <int NT, int HALF>
 __device__ __forceinline__ void lp_outputs(const LpTaps &taps, const float *s_e, float *s_f, u32 blk) {
     static_assert(NT % 2 == 1, "odd tap counts only (Kaiser design, filters.rs:79)");
     constexpr int EOFF = (NT - 1 + 3) / 4 * 4;     // e tile starts this many samples before the tile (multiple of 4)
-    constexpr int D = EOFF - (NT - 1);             // 0..3
-    constexpr int SH = (PAR + D) & 3;              // offset of the oldest sample in the 16-byte aligned window
-    constexpr int WB = (PAR + D) & ~3;             // 0 or 4: where the aligned window starts relative to 16*blk
-    static_assert((SH & 1) == PAR, "window parity must follow the output parity");
-    constexpr int NPAIR = (NT + 1) / 2;            // tap pairs
-    constexpr int WN = (SH + NT - 1 + 15 + 3) / 4 * 4;
-    constexpr int T0 = PAR ? (SH + NT - 2) / 2 : (SH + NT - 1) / 2;   // window pair of tap pair i for output v: T0 + v - i
-    const u32 wal = 16 * blk + WB;
-    f32x2 w2[WN / 2];
+    constexpr int WN = EOFF + 8;                   // window: s_e[o .. o + EOFF + 7] (the oldest tap needs o + EOFF - NT + 1 >= o)
+    const u32 o = 16 * blk + 8 * HALF;
+    float w[WN];
 #pragma unroll
     for (int k = 0; k < WN / 4; ++k) {
-        const float4 q = *reinterpret_cast<const float4 *>(s_e + skew(wal + 4 * k));
-        w2[2 * k] = pack2(q.x, q.y);
-        w2[2 * k + 1] = pack2(q.z, q.w);
+        const float4 q = *reinterpret_cast<const float4 *>(s_e + skew(o + 4 * k));
+        w[4 * k] = q.x; w[4 * k + 1] = q.y; w[4 * k + 2] = q.z; w[4 * k + 3] = q.w;
     }
-    const u32 o = 16 * blk + PAR;
-    f32x2 acc[8];                                  // 8 independent chains, tap pair outermost
+    f32x2 acc[4];                                  // 4 independent chain pairs, tap pair outermost
 #pragma unroll
-    for (int v = 0; v < 8; ++v) acc[v] = 0ull;
+    for (int v = 0; v < 4; ++v) acc[v] = 0ull;
 #pragma unroll
-    for (int i = 0; i < NPAIR; ++i) {
-        const float2 tp = PAR ? taps.a_odd[i] : taps.a_even[i];
-        const f32x2 t2 = pack2(tp.x, tp.y);
+    for (int j = -1; j < NT; ++j) {
+        const f32x2 t2 = pack2(taps.p[j + 1].x, taps.p[j + 1].y);   // (c[j], c[j+1]): outputs 2v and 2v+1 from sample EOFF+2v-j
 #pragma unroll
-        for (int v = 0; v < 8; ++v) acc[v] = fma2(w2[T0 + v - i], t2, acc[v]);
+        for (int v = 0; v < 4; ++v) {
+            const float x = w[EOFF + 2 * v - j];
+            acc[v] = fma2(pack2(x, x), t2, acc[v]);
+        }
     }
+    float r[8];
 #pragma unroll
-    for (int v = 0; v < 8; ++v) {
-        float lo, hi;
-        unpack2(acc[v], lo, hi);
-        s_f[skew(o + 2 * v)] = lo + hi;
-    }
+    for (int v = 0; v < 4; ++v) unpack2(acc[v], r[2 * v], r[2 * v + 1]);
+    *reinterpret_cast<float4 *>(s_f + skew(o)) = make_float4(r[0], r[1], r[2], r[3]);
+    *reinterpret_cast<float4 *>(s_f + skew(o + 4)) = make_float4(r[4], r[5], r[6], r[7]);
 }
 
 template <int NT, int PW, bool BASED>
@@ -137,7 +133,7 @@ k_lowpass_corr(const float *__restrict__ e, u64 base_arg, u64 n, u64 ncorr, cons
         }
         fetch(tile + gridDim.x);
         __syncthreads();
-        // ---- low-pass: warp pair (2h, 2h+1) owns blocks 32h .. 32h+31 of 16 positions; even warp = even positions ----
+        // ---- low-pass: warp pair (2h, 2h+1) owns blocks 32h .. 32h+31 of 16 positions; even warp = the first 8 ----
         {
             const u32 blk = (warp >> 1) * 32 + lane;
             if (blk < FNP / 16) {

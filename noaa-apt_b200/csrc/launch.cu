@@ -263,10 +263,6 @@ int launch_lowpass_corr(const LaunchCtx &c, const float *e, u64 n, const float *
     if (base % 16) return fail(APT_ERR_BAD_ARG, "low-pass/correlation: start %llu is not a multiple of 16", (unsigned long long)base);
     LpTaps t{};
     auto tap = [&](long long j) { return j >= 0 && j < static_cast<long long>(ntaps) ? taps_host[j] : 0.f; };
-    for (int i = 0; i < 32; ++i) {
-        t.a_even[i] = make_float2(tap(2 * i), tap(2 * i - 1));
-        t.a_odd[i] = make_float2(tap(2 * i + 1), tap(2 * i));
-    }
     for (int j = -1; j < 63; ++j) t.p[j + 1] = make_float2(tap(j), tap(j + 1));
     const u64 ncorr = n > 38ull * pw ? n - 38ull * pw : 0;
     const u64 ntiles = (n - base + kLpTile - 1) / kLpTile;
@@ -369,10 +365,6 @@ int launch_pick(const LaunchCtx &c, u64 ncorr, u64 nwork, u32 row, u32 dist, con
 static LpTaps make_lp_taps(const float *taps_host, u32 ntaps, int dec = 0) {
     LpTaps t{};
     auto tap = [&](long long j) { return j >= 0 && j < static_cast<long long>(ntaps) ? taps_host[j] : 0.f; };
-    for (int i = 0; i < 32; ++i) {
-        t.a_even[i] = make_float2(tap(2 * i), tap(2 * i - 1));
-        t.a_odd[i] = make_float2(tap(2 * i + 1), tap(2 * i));
-    }
     for (int j = -1; j < 63; ++j) t.p[j + 1] = make_float2(tap(j), tap(j + 1));
     for (int j = -dec; j < 72 - dec; ++j) t.pd[j + dec] = make_float2(tap(j), tap(j + dec));
     return t;

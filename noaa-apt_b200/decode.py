@@ -83,6 +83,11 @@ def decode(context, settings, signal, input_rate, sync=True):
     return out[: n.value].copy()
 
 
+# apt_tile_records and apt_record (Decoder.last_records)
+TILE_RECORDS = np.dtype([("n_suffix", "<u4"), ("n_prefix", "<u4"), ("max", "<f4")])
+RECORD = np.dtype([("pos", "<u4"), ("val", "<f4")])
+
+
 class Decoder:
     """apt_decoder: plan + device workspaces + one stream; submit()/wait() keep one job in flight."""
 
@@ -214,6 +219,20 @@ class Decoder:
         if n.value:
             raise_for(self._lib.apt_decoder_last_roots(self._h, out.ctypes.data, out.size, C.byref(n)))
         return out
+
+    def last_records(self):
+        """What the sync record kernel wrote for the last job (apt_decoder_last_records): (tiles, records), structured
+        arrays -- tiles[t] = (n_suffix, n_prefix, max) of tile t; records = (pos, val) of every tile in tile order, its
+        suffix list then its prefix list.  Raises unless the last job was a sync job that ran the record kernel and did
+        not overflow its pool."""
+        nt, nr = C.c_size_t(0), C.c_size_t(0)
+        raise_for(self._lib.apt_decoder_last_records(self._h, None, 0, C.byref(nt), None, 0, C.byref(nr)))
+        tiles = np.zeros(nt.value, dtype=TILE_RECORDS)
+        recs = np.zeros(nr.value, dtype=RECORD)
+        raise_for(self._lib.apt_decoder_last_records(self._h, tiles.ctypes.data if tiles.size else None, tiles.size,
+                                                     C.byref(nt), recs.ctypes.data if recs.size else None, recs.size,
+                                                     C.byref(nr)))
+        return tiles, recs
 
     def read_stage(self, which):
         idx = {"demodulated": 0, "filtered": 1, "correlation": 2}[which] if isinstance(which, str) else int(which)

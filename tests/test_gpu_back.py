@@ -53,7 +53,7 @@ def run(rate, settings, x, sync):
         launches = dec.launch_count - before
         slots = [name for name, _ in dec.kernel_times_ms()]
         pos = dec.last_sync() if sync else None
-        roots = dec.last_roots() if sync else None     # before read_stage: Records roots live in the per-tile layout
+        roots = dec.last_roots() if sync else None
         f = dec.read_stage("filtered")
         corr = dec.read_stage("correlation") if sync else None
     return rows, pos, roots, f, corr, slots, launches

@@ -11,6 +11,7 @@ import pytest
 import noaa_apt_b200 as na
 from noaa_apt_b200 import synth
 import oracle
+from _sync_oracle import roots_direct
 
 pytestmark = pytest.mark.gpu
 
@@ -331,19 +332,16 @@ def test_chunked_upload_of_long_recordings(rate, monkeypatch):
 
 # ------------------------------------------------------------------------------- fused sync stage
 
-def _roots_direct(corr, dist):
-    """Definition of a root: no corr[j] > corr[p] for j in (p, p + dist]."""
-    n = corr.size
-    pad = np.concatenate([corr, np.full(dist, -np.inf, np.float32)])
-    w = np.lib.stride_tricks.sliding_window_view(pad[1:], dist).max(axis=1)[:n]
-    return np.nonzero(~(w > corr))[0].astype(np.uint64)
+_roots_direct = roots_direct
 
 
 @pytest.mark.parametrize("rate,profile,seconds", [(48000, "standard", 30), (11025, "standard", 40), (48000, "fast", 16),
                                                   (48000, "slow", 16)])
 def test_fused_sync_stage_roots_match_definition(rate, profile, seconds):
     """kernels_sync2.cuh: the roots that come out of the per-tile records (f and corr never written) must be exactly the
-    roots of the correlation the legacy kernel writes (same arithmetic, bit-identical values) by the definition."""
+    roots, by the definition, of the correlation read_stage materialises with k_lowpass_corr.  The two kernels share one
+    low-pass, box-sum and correlation order, so that correlation has the record kernel's bits (test_gpu_sync_exact.py
+    compares both with the float32 restatement)."""
     x = synth.apt_signal(rate, seconds, seed=17)
     settings = na.Settings.profile(profile)
     with na.Decoder(rate, settings, max_samples=x.size) as dec:

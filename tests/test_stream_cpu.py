@@ -16,117 +16,10 @@ import noaa_apt_b200 as na
 from noaa_apt_b200 import _lib, synth
 from noaa_apt_b200.err import Error
 import oracle
+from _sync_oracle import carried_walk
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HALO = 80
-
-
-def window_max(c, d):
-    """w[p] = max(c[p+1 .. p+d]) over the given values (-inf beyond), by the van Herk / Gil-Werman block split."""
-    n = c.size
-    x = np.full(((n + 2 * d) // d + 1) * d, -np.inf, dtype=np.float32)
-    x[: n - 1] = c[1:]
-    blocks = x.reshape(-1, d)
-    g = np.maximum.accumulate(blocks, axis=1).ravel()
-    h = np.maximum.accumulate(blocks[:, ::-1], axis=1)[:, ::-1].ravel()
-    p = np.arange(n)
-    return np.maximum(h[p], g[p + d - 1])
-
-
-def carried_walk(corr, work_rate, splits, on_step=None, run_cap=256, gather_cap=8):
-    """Positions the stream decides when corr becomes final on [0, c) for c in splits, then at the end.
-
-    Pending peaks are (position, count) runs in a ring of run_cap entries; each round walks as far as it can, lists at
-    most gather_cap rows whose envelope is final, and another round follows only if it can make progress (as in
-    k_stream_sync).  on_step(c_end, peaks, state) sees the state after each step."""
-    pw = work_rate // 4160
-    row = 2080 * pw
-    D = row * 8 // 10
-    G = 38 * pw
-    ncorr = corr.size
-    st = dict(decided=0, seed_state=0, seed=None, s=0, length=0, gathered=0, used=0, rounds=0)
-    roots = []
-    runs = []            # pending runs [position, count], oldest first
-    peaks = []           # every peak pushed, expanded
-
-    def first_root(x):
-        i = int(np.searchsorted(roots, x, side="left"))
-        return roots[i] if i < len(roots) else None
-
-    for c_end in list(splits) + [None]:
-        finish = c_end is None
-        lim = ncorr if finish else c_end
-        dec_hi = ncorr if finish else max(c_end - D, 0)
-        wf = ncorr + G if finish else c_end + G
-        if dec_hi > st["decided"]:
-            d0 = st["decided"]
-            vis = corr[d0:lim]                                 # the windows of [d0, dec_hi), clipped at lim
-            w = window_max(vis, D)
-            p = np.arange(dec_hi - d0)
-            roots.extend((d0 + p[~(w[p] > vis[p])]).tolist())
-            st["decided"] = dec_hi
-        if st["seed_state"] == 0 and (finish or c_end > D):
-            hit = np.nonzero(corr[: min(D + 1, lim)] > 0)[0]
-            st["seed"] = int(hit[0]) if hit.size else None
-            st["seed_state"] = 1
-        while True:
-            st["rounds"] += 1
-            ring_full = False
-
-            def push(pos, count):
-                nonlocal ring_full
-                if len(runs) >= run_cap:
-                    ring_full = True
-                    return False
-                runs.append([pos, count])
-                peaks.extend([pos] * count)
-                st["length"] += count
-                return True
-
-            if st["seed_state"] == 1:
-                p0 = 0 if st["seed"] is None else first_root(st["seed"])
-                if p0 is not None and push(p0, 1):
-                    st["s"] = max(p0 + D + 1, 2 * row)
-                    st["seed_state"] = 2
-            if st["seed_state"] == 2:
-                s = st["s"]
-                while s < lim:
-                    target = s // row
-                    if st["length"] + 1 < target and not push(s, target - 1 - st["length"]):
-                        break
-                    r = first_root(s)
-                    if r is None or not push(r, 1):
-                        break
-                    s = max(r + D + 1, row * (s // row + 1))
-                st["s"] = s
-            n = st["length"]
-            k_end = (n - 1 if n else 0) if finish else n
-            failed = finish and n < 5
-            ng, list_full = 0, False
-            while not failed and st["gathered"] < k_end and runs:
-                if runs[0][0] + row >= wf:
-                    break
-                if ng == gather_cap:
-                    list_full = True
-                    break
-                ng += 1
-                st["gathered"] += 1
-                st["used"] += 1
-                if st["used"] == runs[0][1]:
-                    runs.pop(0)
-                    st["used"] = 0
-            dropped = False
-            if finish and ring_full and runs and runs[0][0] + row >= wf:
-                runs.clear()
-                st["used"] = 0
-                dropped = True
-            if not (list_full or (ring_full and (ng > 0 or dropped))):
-                break
-        st["pending_runs"] = len(runs)
-        st["first_pending"] = runs[0][0] if runs else None
-        if on_step is not None and not finish:
-            on_step(c_end, list(peaks), dict(st))
-    return np.array(peaks, dtype=np.uint64)
 
 
 def correlation(x, rate):
