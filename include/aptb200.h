@@ -480,7 +480,8 @@ int apt_iq_default_settings(uint32_t iq_rate, int32_t offset_hz, apt_iq_settings
  * cutout > 0, delta_freq > 0, atten > 8, cutout < audio_rate / 2, |offset_hz| + cutout < iq_rate / 2 and the channel
  * filter has at most 8191 taps. */
 int apt_fm_demod_len(uint64_t n, const apt_iq_settings *s, uint64_t *nout);
-/* The stage alone: host I/Q in, host audio (f32, Hz) out; cap in floats. */
+/* The stage alone: host I/Q in, host audio (f32, Hz) out; cap in floats.  A cf32 sample with a NaN or Inf component (or
+ * one whose mixed value overflows) counts as 0 + 0j, so the audio is the same bits whatever the chunk size. */
 int apt_fm_demod(const void *iq, int format, uint64_t n, const apt_iq_settings *s, float *out, uint64_t cap,
                  uint64_t *nout);
 /* Several channels of one I/Q input: outs[c] (cap floats each) receives apt_fm_demod with offset_hz = offsets[c], bit for

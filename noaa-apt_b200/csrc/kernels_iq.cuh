@@ -8,7 +8,8 @@
 // 512 FMAs (a 16 x 16 register-blocked convolution), so shared memory supplies one sample per 16 FMAs.  Each plane is
 // stored as 16 sub-planes (u mod 16) so that the lanes of a warp read consecutive words.
 // Every output sums planes r = p, p + P, ... per partition p, q descending within each 16-tap block, then the partitions
-// p = 0..P-1 in order: the same sequence for every output, wherever the tile, chunk or launch boundaries fall.
+// p = 0..P-1 in order: the same sequence for every output, wherever the tile, chunk or launch boundaries fall.  A sample
+// with a non-finite component after the mix is staged as 0, so the zero-padded taps never turn it into a NaN.
 #pragma once
 
 #include <cstdint>
@@ -105,6 +106,9 @@ __device__ __forceinline__ void fm_demod_tile(const IqArgs &a, const float2 *W, 
                     const float2 p = cmul_rn(P[(i >> 12) - qa], __ldg(W + (i & (kIqBlock - 1))));
                     x = cmul_rn(x, p);
                 }
+                // a NaN or Inf would reach the outputs whose zero-padded taps cover it, and whether those read it
+                // depends on where the chunk window starts: staged as 0, every FMA with a zero tap is exact
+                if (!isfinite(x.x) || !isfinite(x.y)) x = make_float2(0.f, 0.f);
             }
             const u32 r = D - 1 - o;
             sm[static_cast<size_t>(r) * ps + (u & 15) * lp16 + (u >> 4)] = x;
