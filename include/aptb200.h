@@ -288,6 +288,32 @@ int apt_decoder_set_image_mode(apt_decoder *dec, int contrast, float percent);
  * `cap` and *nout count bytes (rows*2080*(rgba ? 4 : 1)).  The palette is copied to the device here, once.  NULL switches
  * back to f32 rows; apt_decoder_set_image_mode also leaves process mode. */
 int apt_decoder_set_process_mode(apt_decoder *dec, const apt_process_settings *ps);
+/* Sync mode of a decoder (DESIGN.md "Tracked sync").  Applies to every later submit with sync != 0, in every output
+ * mode (rows, image, process, PNG); the default is APT_SYNC_PEAKS.
+ *   APT_SYNC_PEAKS  the reference's picker (decode.rs:204-263), what `sync` means everywhere else.
+ *   APT_SYNC_TRACK  tracked sync: the row period P = work_rate / 2 followed through the whole pass.  On the reference's
+ *                   correlation c[0 .. ncorr), ncorr = N_w - template length:
+ *     1. block k = [kP, min((k+1)P, ncorr)); m_k and the population deviation s_k of c over the block in double, each
+ *        rounded once to float; z[i] = (c[i] - m_k) / s_k in float (z = 0 when s_k is 0 or not finite);
+ *     2. S[i] = z[i] for i < P + delta, else S[i] = z[i] + max over d = -delta..delta of (S[i-P-d] - float(lambda d^2)),
+ *        ties to the smaller |d|, then the negative d; before block k >= 2 the maximum S of block k-1 is subtracted from
+ *        every S of blocks k-1 and k-2 (constant across every comparison, so no choice changes in exact arithmetic);
+ *     3. from the argmax of S over [max(0, ncorr - P), ncorr) (first index on ties) walk back i <- i - P - d(i) while
+ *        i >= P + delta; these indices, ascending, are the sync positions (apt_decoder_last_sync);
+ *     4. rows as decode.rs:120-132 (every position but the last with p + row < N_w), at most floor(N_w / row) of them;
+ *        fewer than 5 positions is APT_ERR_FEW_SYNC_FRAMES.
+ *   Streams, watchers, batches and the one-shot entry points always use APT_SYNC_PEAKS. */
+typedef enum apt_sync_mode { APT_SYNC_PEAKS = 0, APT_SYNC_TRACK = 1 } apt_sync_mode;
+typedef struct apt_track_settings {
+    uint32_t delta;   /* largest change of the row period between two rows, in work-rate samples: 1..8 */
+    float lambda;     /* penalty per squared sample of change: finite, >= 0 */
+} apt_track_settings;
+/* delta 2, lambda 0.25. */
+void apt_default_track_settings(apt_track_settings *ts);
+/* ts == NULL takes the defaults.  Bad settings, an unknown mode, a job in flight or a decoder that cannot sync are
+ * APT_ERR_BAD_ARG before any device is touched.  APT_SYNC_TRACK allocates the correlation, the per-index choices and room
+ * for the positions once; APT_SYNC_PEAKS keeps them for a later switch back. */
+int apt_decoder_set_sync_mode(apt_decoder *dec, int mode, const apt_track_settings *ts);
 /* Contrast bounds / telemetry of the last image job (after apt_decoder_wait). */
 int apt_decoder_image_info(apt_decoder *dec, apt_image_info *info);
 /* 1 if the decoder's job has finished (apt_decoder_wait will not block) or none is in flight, else 0. */

@@ -193,6 +193,27 @@ inline Signal decode(Context &ctx, const config::Settings &settings, const Signa
     return out;
 }
 
+// decode() with tracked sync (aptb200.h apt_decoder_set_sync_mode, DESIGN.md "Tracked sync") on a decoder of its own
+// on device 0; track == nullptr takes the defaults (delta 2, lambda 0.25).
+inline Signal decode_tracked(const config::Settings &settings, const Signal &signal, Rate input_rate,
+                             const apt_track_settings *track = nullptr) {
+    const apt_settings s = settings.to_c();
+    uint64_t bound = 0, n = 0;
+    err::check(apt_decode_len_bound(signal.size(), input_rate.get_hz(), &s, &bound));
+    apt_decoder *dec = nullptr;
+    err::check(apt_decoder_create(0, input_rate.get_hz(), &s, signal.size(), &dec));
+    struct Guard {
+        apt_decoder *d;
+        ~Guard() { apt_decoder_destroy(d); }
+    } guard{dec};
+    Signal out(bound ? bound : 1);
+    err::check(apt_decoder_set_sync_mode(dec, APT_SYNC_TRACK, track));
+    err::check(apt_decoder_submit_host(dec, signal.data(), APT_F32, signal.size(), 1, out.data(), out.size()));
+    err::check(apt_decoder_wait(dec, &n));
+    out.resize(n);
+    return out;
+}
+
 // decode::find_sync, decode.rs:204-263 (private in the crate; exposed for tests)
 inline std::vector<uint64_t> find_sync(Context &, const Signal &signal, Rate work_rate) {
     std::vector<uint64_t> pos(signal.size() / 64 + 8);

@@ -104,6 +104,10 @@ class CCarrier(C.Structure):
                 ("is_apt", C.c_int)]
 
 
+class CTrackSettings(C.Structure):
+    _fields_ = [("delta", C.c_uint32), ("lambda_", C.c_float)]
+
+
 class CPngSettings(C.Structure):
     _fields_ = [("filter", C.c_int), ("matches", C.c_int), ("block_bytes", C.c_uint32), ("rgb_from_rgba", C.c_int)]
 
@@ -162,6 +166,8 @@ WATCH_IQ_MAX_CHANNELS = 8
 # name -> (restype, argtypes); every symbol include/aptb200.h declares.
 _u64p = C.POINTER(C.c_uint64)
 _szp = C.POINTER(C.c_size_t)
+
+SYNC_PEAKS, SYNC_TRACK = 0, 1   # apt_sync_mode
 SIGNATURES = {
     "apt_strerror": (C.c_char_p, [C.c_int]),
     "apt_last_error": (C.c_char_p, []),
@@ -207,6 +213,8 @@ SIGNATURES = {
     "apt_decoder_set_image_mode": (C.c_int, [C.c_void_p, C.c_int, C.c_float]),
     "apt_decoder_set_process_mode": (C.c_int, [C.c_void_p, C.POINTER(CProcessSettings)]),
     "apt_decoder_image_info": (C.c_int, [C.c_void_p, C.POINTER(CImageInfo)]),
+    "apt_default_track_settings": (None, [C.POINTER(CTrackSettings)]),
+    "apt_decoder_set_sync_mode": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(CTrackSettings)]),
     "apt_decoder_create": (C.c_int, [C.c_int, C.c_uint32, C.POINTER(CSettings), C.c_uint64, C.POINTER(C.c_void_p)]),
     "apt_decoder_destroy": (None, [C.c_void_p]),
     "apt_decoder_submit_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_uint64, C.c_int, C.c_void_p, C.c_uint64]),

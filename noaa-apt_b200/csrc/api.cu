@@ -714,6 +714,25 @@ extern "C" int apt_decoder_set_png_mode(apt_decoder *d, const apt_png_settings *
     return d->img.plan.set_png(ps);
 }
 
+extern "C" void apt_default_track_settings(apt_track_settings *ts) {
+    if (ts) *ts = apt_track_settings{2, 0.25f};
+}
+
+extern "C" int apt_decoder_set_sync_mode(apt_decoder *d, int mode, const apt_track_settings *ts) {
+    if (mode != APT_SYNC_PEAKS && mode != APT_SYNC_TRACK) return fail(APT_ERR_BAD_ARG, "unknown sync mode %d", mode);
+    apt_track_settings t;
+    apt_default_track_settings(&t);
+    if (ts) t = *ts;
+    if (mode == APT_SYNC_TRACK) APT_TRY(track_settings_check(t));
+    if (!d) return fail(APT_ERR_BAD_ARG, "null decoder");
+    if (d->in_flight) return fail(APT_ERR_BAD_ARG, "decoder has a job in flight");
+    if (mode == APT_SYNC_PEAKS) return back_set_track(d->plan, d->back_plan, d->back, nullptr);
+    if (!d->back_plan.can_sync)
+        return fail(APT_ERR_BAD_ARG, "tracked sync needs a decoder that can sync (work rate a multiple of 4160, at most 37440)");
+    APT_CUDA(cudaSetDevice(d->device));
+    return back_set_track(d->plan, d->back_plan, d->back, &t);
+}
+
 extern "C" int apt_decoder_image_info(apt_decoder *d, apt_image_info *info) {
     if (!d || !info) return fail(APT_ERR_BAD_ARG, "null argument");
     *info = d->img.info;

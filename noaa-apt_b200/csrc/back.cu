@@ -2,6 +2,7 @@
 #include "back.hpp"
 
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <vector>
@@ -76,6 +77,7 @@ int BackBuffers::alloc(const Plan &p, const BackPlan &bp) {
         APT_CUDA(cudaMemcpy(guard, p.guard.data(), p.guard.size(), cudaMemcpyHostToDevice));
         APT_CUDA(cudaMalloc(&root_count, static_cast<size_t>(count_blocks) * sizeof(u32)));
         APT_CUDA(cudaMalloc(&pos, static_cast<size_t>(bp.max_positions) * sizeof(u32)));
+        pos_cap = bp.max_positions;
         APT_CUDA(cudaMalloc(&pick_mem, pick_scratch_bytes(count_blocks, bp.max_positions, bp.pick_cap)));
         pick = pick_scratch_carve(pick_mem, count_blocks, bp.max_positions, bp.pick_cap);
         APT_CUDA(cudaMemset(pick.ticket, 0, 8));
@@ -96,10 +98,30 @@ int BackBuffers::ensure_hbm(const Plan &p, const BackPlan &bp) {
     return APT_OK;
 }
 
+int BackBuffers::ensure_track(const Plan &p, const BackPlan &bp) {
+    if (!f) APT_CUDA(cudaMalloc(&f, std::max<uint64_t>(bp.max_work, 1) * sizeof(float)));
+    if (!corr) APT_CUDA(cudaMalloc(&corr, bp.max_corr * sizeof(float)));
+    if (!track_back) APT_CUDA(cudaMalloc(&track_back, bp.max_corr));
+    if (!track_end) APT_CUDA(cudaMalloc(&track_end, sizeof(u32)));
+    const u32 cap = track_positions_cap(bp.max_corr, p.row);
+    if (pos_cap < cap) {
+        APT_CUDA(cudaFree(pos));
+        pos = nullptr;
+        pos_cap = 0;
+        APT_CUDA(cudaMalloc(&pos, static_cast<size_t>(cap) * sizeof(u32)));
+        pos_cap = cap;
+    }
+    return APT_OK;
+}
+
 void BackBuffers::release() {
     for (void *q : {(void *)res, (void *)guard, (void *)pos, (void *)root_count, pick_mem, (void *)ctl, (void *)desc,
-                    (void *)pool, (void *)roots, (void *)tile_base, (void *)by_id, (void *)f, (void *)corr, (void *)root_list})
+                    (void *)pool, (void *)roots, (void *)tile_base, (void *)by_id, (void *)f, (void *)corr, (void *)root_list,
+                    (void *)track_back, (void *)track_end})
         if (q) cudaFree(q);
+    track_back = nullptr;
+    track_end = nullptr;
+    pos_cap = 0;
     res = nullptr;
     guard = nullptr;
     pos = root_count = roots = tile_base = by_id = root_list = nullptr;
@@ -172,6 +194,36 @@ int launch_hbm(const LaunchCtx &c, const Plan &p, const BackPlan &bp, BackBuffer
     return launch_polyphase(c, b.f, APT_F32, alen, one, p.last.l, p.last.m, 0, 0, nout, false, 0.f, 1.f, rows);
 }
 
+// Track: f and corr in HBM, the tracked path over corr, rows from f at its positions.
+int launch_track(const LaunchCtx &c, const Plan &p, const BackPlan &bp, BackBuffers &b, const float *lp, const float *e,
+                 uint64_t nwork, float *rows, KernelHook *hook) {
+    const u32 ntaps = static_cast<u32>(p.lp.size());
+    const u32 glen = static_cast<u32>(p.guard.size());
+    const uint64_t ncorr = nwork - glen;
+    if (bp.kind == BackKind::Generic) {
+        {
+            KernelSlot s(hook, "lowpass");
+            APT_TRY(launch_fir_decimate(c, e, APT_F32, lp, ntaps, 1, nwork, b.f));
+        }
+        KernelSlot s(hook, "sync_correlation");
+        APT_TRY(launch_corr(c, b.f, ncorr, b.guard, glen, b.corr));
+    } else {
+        KernelSlot s(hook, "lowpass_correlation");
+        APT_TRY(launch_lowpass_corr(c, e, nwork, p.lp.data(), ntaps, p.dec, b.f, b.corr));
+    }
+    {
+        KernelSlot s(hook, "sync_track");
+        APT_TRY(launch_sync_track(c, b.corr, ncorr, p.row, bp.track->delta, bp.track->lambda, b.track_back, b.track_end));
+    }
+    {
+        KernelSlot s(hook, "sync_backtrack");
+        APT_TRY(launch_track_back(c, b.track_back, b.track_end, ncorr, nwork, p.row, bp.track->delta, b.pos, b.pos_cap, b.res));
+    }
+    KernelSlot s(hook, "gather_rows");
+    const u32 max_rows = static_cast<u32>(std::min<uint64_t>(nwork / p.row + 1, 1u << 30));
+    return launch_gather(c, b.f, b.pos, b.res, 0, max_rows, p.row, kPxPerRow, p.dec, rows);
+}
+
 // Records: f and corr stay on chip; records -> roots -> orbit -> rows straight from the envelope.
 int launch_records(const LaunchCtx &c, const Plan &p, const BackPlan &bp, BackBuffers &b, const float *e, uint64_t nwork,
                    bool sync, float *rows, KernelHook *hook) {
@@ -210,6 +262,10 @@ int launch_records(const LaunchCtx &c, const Plan &p, const BackPlan &bp, BackBu
 
 int back_launch(const LaunchCtx &c, const Plan &p, const BackPlan &bp, BackBuffers &b, const float *lp, const float *one,
                 const float *e, uint64_t nwork, bool sync, float *rows, KernelHook *hook, BackKind &ran) {
+    if (sync && bp.track) {
+        ran = BackKind::Track;
+        return launch_track(c, p, bp, b, lp, e, nwork, rows, hook);
+    }
     ran = bp.kind;
     if (bp.kind == BackKind::Records) return launch_records(c, p, bp, b, e, nwork, sync, rows, hook);
     return launch_hbm(c, p, bp, b, bp.kind, lp, one, e, nwork, sync, rows, hook);
@@ -220,6 +276,24 @@ int back_redo(const LaunchCtx &c, const Plan &p, const BackPlan &bp, BackBuffers
     ran = BackKind::Hbm;
     APT_CUDA(cudaMemsetAsync(b.res, 0, sizeof(SyncResult), c.stream));
     return launch_hbm(c, p, bp, b, BackKind::Hbm, nullptr, nullptr, e, nwork, true, rows, hook);
+}
+
+int track_settings_check(const apt_track_settings &ts) {
+    if (ts.delta < 1 || ts.delta > kTrackMaxDelta)
+        return fail(APT_ERR_BAD_ARG, "tracked sync: delta %u is outside 1..%u", ts.delta, kTrackMaxDelta);
+    if (!std::isfinite(ts.lambda) || ts.lambda < 0.f)
+        return fail(APT_ERR_BAD_ARG, "tracked sync: lambda must be finite and >= 0");
+    return APT_OK;
+}
+
+int back_set_track(const Plan &p, BackPlan &bp, BackBuffers &b, const apt_track_settings *ts) {
+    if (!ts) {
+        bp.track.reset();
+        return APT_OK;
+    }
+    APT_TRY(b.ensure_track(p, bp));
+    bp.track = TrackPlan{ts->delta, ts->lambda};
+    return APT_OK;
 }
 
 int back_find_sync(const LaunchCtx &c, const Plan &p, const BackPlan &bp, BackBuffers &b, uint64_t nwork) {
@@ -238,6 +312,7 @@ int back_roots(const Plan &p, const BackPlan &bp, const BackBuffers &b, BackKind
     *nroots = 0;
     if (!b.root_count || nwork <= p.guard.size()) return APT_OK;
     const uint64_t ncorr = nwork - p.guard.size();
+    if (ran == BackKind::Track) return APT_OK;   // the tracked path has no roots
     const bool tiles = ran == BackKind::Records;
     const u32 block = tiles ? bp.tile_w : p.dist;
     const u32 nb = static_cast<u32>((ncorr + block - 1) / block);

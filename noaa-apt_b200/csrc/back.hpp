@@ -21,7 +21,16 @@ enum class BackKind {
                // k_lowpass_corr writes f only); the redo after a record-pool overflow, and every job under APTB200_LEGACY_SYNC=1
     Generic,   // any low-pass in the reference's summation order: k_fir_decimate_generic -> k_corr_generic -> k_roots -> walk ->
                // k_gather_rows, or final_resample when the work rate is not a multiple of 4160; APTB200_GENERIC_LOWPASS=1
+    Track,     // a sync job of a decoder in APT_SYNC_TRACK mode: f and corr as Hbm (Generic: as Generic) -> k_sync_track ->
+               // k_track_back -> k_gather_rows; no roots
 };
+
+// Tracked-sync settings of a decoder (apt_decoder_set_sync_mode), checked by track_settings_check.
+struct TrackPlan {
+    u32 delta = 2;
+    float lambda = 0.25f;
+};
+int track_settings_check(const apt_track_settings &ts);
 
 // The Records and Hbm kernels exist for the plan's low-pass (the standard, fast and slow profiles).
 bool back_fused(const Plan &p);
@@ -36,6 +45,7 @@ struct BackPlan {
     u32 max_positions = 0;         // sync positions
     u32 tile_w = 0, max_tiles = 0, pool_cap = 0, pool_region = 0;   // Records: tiles and record pool
     u32 pick_cap = 0;              // candidates of the parallel walks
+    std::optional<TrackPlan> track;   // sync jobs run the tracked sync (set by back_set_track)
 
     // Unless forced: the whole-GPU walk when the device is otherwise idle, the 8-SM cluster walk when other jobs are in flight.
     Walk walk_for(const LaunchCtx &c) const { return walk ? *walk : c.busy ? Walk::Cluster : Walk::Grid; }
@@ -57,14 +67,22 @@ struct BackBuffers {
     u32 *tile_base = nullptr, *by_id = nullptr;    // dense root ids: first id of tile t, position by id
     float *f = nullptr, *corr = nullptr;           // Hbm / Generic, allocated on first use when the kind is Records
     u32 *root_list = nullptr;                      // roots of block b at root_list + b * min_distance
+    u32 pos_cap = 0;                               // entries of pos
+    int8_t *track_back = nullptr;                  // Track: the chosen d of every correlation index
+    u32 *track_end = nullptr;                      // Track: the index the walk back starts from
 
     BackBuffers() = default;
     BackBuffers(const BackBuffers &) = delete;
     ~BackBuffers() { release(); }
     int alloc(const Plan &p, const BackPlan &bp);      // everything but f / corr / root_list of the Records kind
     int ensure_hbm(const Plan &p, const BackPlan &bp); // f, corr and the per-block root lists
+    int ensure_track(const Plan &p, const BackPlan &bp);   // f, corr, back, end and room for the tracked positions
     void release();
 };
+
+// The sync mode of later sync jobs: the reference's picker (ts == nullptr) or tracked sync with *ts (already checked);
+// tracked sync allocates its buffers here.  Needs bp.can_sync.
+int back_set_track(const Plan &p, BackPlan &bp, BackBuffers &b, const apt_track_settings *ts);
 
 // Enqueues the back half of one job: the envelope e (nwork samples) -> rows, with the plan's kind.  lp and one are the
 // device copies of the low-pass taps and of the one-tap NoFilter (Generic).  `ran` is the kind whose buffers now hold the

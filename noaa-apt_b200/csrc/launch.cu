@@ -16,6 +16,7 @@
 #include "kernels_sync.cuh"
 #include "kernels_sync2.cuh"
 #include "kernels_stream.cuh"
+#include "kernels_track.cuh"
 #include "kernels_ut.cuh"
 
 namespace aptb200 {
@@ -478,6 +479,70 @@ int launch_gather(const LaunchCtx &c, const float *f, const u32 *positions, cons
     if (max_rows == 0) return APT_OK;
     const unsigned grid = std::min<unsigned>(max_rows, static_cast<unsigned>(c.sm_count) * 16);
     k_gather_rows<<<grid, 256, 0, c.stream>>>(f, positions, result, fixed_rows, row, px, dec, out);
+    APT_CUDA(cudaGetLastError());
+    return APT_OK;
+}
+
+u32 track_cluster() {
+    static const u32 cs = [] {
+        const char *e = getenv("APTB200_TRACK_CLUSTER");
+        const u32 v = e ? static_cast<u32>(strtoul(e, nullptr, 10)) : 8u;
+        return v == 4 || v == 16 ? v : 8u;
+    }();
+    return cs;
+}
+
+template <u32 CS>
+static int launch_sync_track_cs(const LaunchCtx &c, const TrackArgs &a) {
+    const u32 w = (a.row + CS - 1) / CS;
+    const size_t smem = (4ull * w + 2 * kTrackMaxDelta) * sizeof(float);
+    // the attribute is set once per device, so to what the longest row needs
+    const size_t smem_max = (4ull * ((kTrackMaxRow + CS - 1) / CS) + 2 * kTrackMaxDelta) * sizeof(float);
+    static std::atomic<signed char> attr[kMaxDevices];
+    if (!smem_attr_once(attr, k_sync_track<CS>, smem_max))
+        return fail(APT_ERR_CUDA, "k_sync_track: %zu bytes of shared memory refused", smem_max);
+    if (CS > 8) APT_CUDA(cudaFuncSetAttribute(k_sync_track<CS>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(CS);
+    cfg.blockDim = dim3(kTrackThreads);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = c.stream;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = CS;
+    at[0].val.clusterDim.y = 1;
+    at[0].val.clusterDim.z = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    APT_CUDA(cudaLaunchKernelEx(&cfg, k_sync_track<CS>, a));
+    return APT_OK;
+}
+
+int launch_sync_track(const LaunchCtx &c, const float *corr, u64 ncorr, u32 row, u32 delta, float lambda, int8_t *back,
+                      u32 *end) {
+    if (delta < 1 || delta > kTrackMaxDelta || row > kTrackMaxRow || row < 2 * kTrackMaxDelta * 16 || ncorr == 0)
+        return fail(APT_ERR_BAD_ARG, "tracked sync: delta %u / row %u out of range", delta, row);
+    TrackArgs a{};
+    a.corr = corr;
+    a.ncorr = ncorr;
+    a.row = row;
+    a.delta = delta;
+    for (int d = -static_cast<int>(delta); d <= static_cast<int>(delta); ++d)
+        a.pen[delta + d] = lambda * static_cast<float>(d * d);
+    a.back = back;
+    a.end = end;
+    switch (track_cluster()) {
+    case 4: return launch_sync_track_cs<4>(c, a);
+    case 16: return launch_sync_track_cs<16>(c, a);
+    default: return launch_sync_track_cs<8>(c, a);
+    }
+}
+
+u32 track_positions_cap(u64 ncorr, u32 row) { return static_cast<u32>(ncorr / (row - kTrackMaxDelta) + 2); }
+
+int launch_track_back(const LaunchCtx &c, const int8_t *back, const u32 *end, u64 ncorr, u64 nwork, u32 row, u32 delta,
+                      u32 *positions, u32 cap, SyncResult *result) {
+    k_track_back<<<1, kTrackThreads, 0, c.stream>>>(back, end, ncorr, nwork, row, delta, positions, cap, result);
     APT_CUDA(cudaGetLastError());
     return APT_OK;
 }

@@ -238,6 +238,18 @@ PickScratch pick_scratch_carve(void *base, u32 max_blocks, u32 max_positions, u3
 int launch_gather(const LaunchCtx &c, const float *f, const u32 *positions, const SyncResult *result,
                   u32 fixed_rows, u32 max_rows, u32 row, u32 px, u32 dec, float *out);
 
+// Tracked sync (kernels_track.cuh) on the correlation corr[0 .. ncorr): back[i] for every index and the end index.  One
+// cluster of track_cluster() CTAs (8; APTB200_TRACK_CLUSTER=4|16 for timing).  delta in 1..8, row in 256..20480.
+constexpr u32 kTrackMaxDelta = 8;
+u32 track_cluster();
+int launch_sync_track(const LaunchCtx &c, const float *corr, u64 ncorr, u32 row, u32 delta, float lambda, int8_t *back,
+                      u32 *end);
+// Positions of a tracked path of ncorr indices can number at most this (rows of at least row - 8 samples).
+u32 track_positions_cap(u64 ncorr, u32 row);
+// The walk back from *end: positions ascending, SyncResult as the peak pickers leave it (n_peaks, n_rows, status).
+int launch_track_back(const LaunchCtx &c, const int8_t *back, const u32 *end, u64 ncorr, u64 nwork, u32 row, u32 delta,
+                      u32 *positions, u32 cap, SyncResult *result);
+
 // Called around every kernel of a stage (profiling events and launch counting of a decoder).
 struct KernelHook {
     virtual void begin(const char *name) = 0;

@@ -61,9 +61,15 @@ def decode(context, settings, signal, input_rate, sync=True):
     """noaa_apt::decode (decode.rs:43-162): Signal at input_rate -> rows*2080 f32 pixels.
 
     `signal` may also be the int16 PCM of the WAV (the `as f32` cast of wav.rs:37 is then done
-    on the device)."""
-    lib = _lib.load()
+    on the device).  sync="track" decodes with tracked sync (Decoder.set_sync_mode) through a decoder of its own."""
     x = np.ascontiguousarray(signal)
+    if isinstance(sync, str):
+        if sync != "track":
+            raise ValueError(f"unknown sync mode {sync!r}: True, False or 'track'")
+        with Decoder(input_rate, settings, max_samples=x.size) as dec:
+            dec.set_sync_mode("track")
+            return dec.decode(x, sync=True)
+    lib = _lib.load()
     fmt = _fmt_of(x)
     s = (settings or Settings()).to_c()
     rate = _rate_hz(input_rate)
@@ -153,6 +159,15 @@ class Decoder:
         ps = image.png_settings(filter, matches, block_bytes, rgb_from_rgba)
         raise_for(self._lib.apt_decoder_set_png_mode(self._h, C.byref(ps)))
         self._png = (filter, matches, block_bytes, rgb_from_rgba)
+
+    def set_sync_mode(self, mode="peaks", delta=2, lam=0.25):
+        """Sync mode of the following sync jobs: "peaks" (the reference's picker, the default) or "track" (tracked sync
+        with `delta` samples of period change per row and penalty `lam` per squared sample, DESIGN.md "Tracked sync")."""
+        modes = {"peaks": _lib.SYNC_PEAKS, "track": _lib.SYNC_TRACK}
+        if mode not in modes:
+            raise ValueError(f"unknown sync mode {mode!r}: 'peaks' or 'track'")
+        ts = _lib.CTrackSettings(int(delta), float(lam)) if mode == "track" else None
+        raise_for(self._lib.apt_decoder_set_sync_mode(self._h, modes[mode], C.byref(ts) if ts is not None else None))
 
     def image_info(self):
         from . import image

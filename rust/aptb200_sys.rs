@@ -141,6 +141,14 @@ extern "C" {
     pub fn apt_png_encode_batch(pixels: *const *const u8, heights: *const u32, count: u32, width: u32, channels: c_int,
                                 ps: *const apt_png_settings, outs: *const *mut u8, caps: *const u64, nouts: *mut u64) -> c_int;
     pub fn apt_decoder_set_png_mode(dec: *mut apt_decoder, ps: *const apt_png_settings) -> c_int;
+    pub fn apt_decoder_create(device: c_int, input_rate: u32, s: *const apt_settings, max_samples: u64,
+                              dec: *mut *mut apt_decoder) -> c_int;
+    pub fn apt_decoder_destroy(dec: *mut apt_decoder);
+    pub fn apt_decoder_submit_host(dec: *mut apt_decoder, signal: *const c_void, format: c_int, n: u64, sync: c_int,
+                                   out: *mut f32, cap: u64) -> c_int;
+    pub fn apt_decoder_wait(dec: *mut apt_decoder, nout: *mut u64) -> c_int;
+    pub fn apt_default_track_settings(ts: *mut apt_track_settings);
+    pub fn apt_decoder_set_sync_mode(dec: *mut apt_decoder, mode: c_int, ts: *const apt_track_settings) -> c_int;
     pub fn apt_decode_wav_png(input_path: *const c_char, output_path: *const c_char, s: *const apt_settings, sync: c_int,
                               ps: *const apt_process_settings, png: *const apt_png_settings, info: *mut apt_image_info) -> c_int;
     // image output of a stream: the pass ends in its processed image or PNG file (DESIGN.md §9)
@@ -209,6 +217,13 @@ pub struct apt_process_settings { pub contrast: c_int, pub percent: c_float, pub
 
 #[repr(C)]
 pub struct apt_decoder { _private: [u8; 0] }
+
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct apt_track_settings { pub delta: u32, pub lambda: f32 }
+/// apt_sync_mode (apt_decoder_set_sync_mode)
+pub const APT_SYNC_PEAKS: c_int = 0;
+pub const APT_SYNC_TRACK: c_int = 1;
 
 #[repr(C)]
 #[derive(Clone, Copy)]

@@ -67,3 +67,55 @@ pub fn decode(
     out.truncate(n as usize);
     Ok(out)
 }
+
+/// `decode` with tracked sync (DESIGN.md "Tracked sync", `apt_decoder_set_sync_mode`): the row period followed through
+/// the whole pass instead of the reference's per-row maximum.  `track` = (delta, lambda); `None` takes the defaults
+/// (2, 0.25).  Runs on a decoder of its own on device 0.
+pub fn decode_tracked(
+    settings: &config::Settings,
+    signal: &Signal,
+    input_rate: Rate,
+    track: Option<(u32, f32)>,
+) -> err::Result<Signal> {
+    let s = sys::apt_settings {
+        work_rate: settings.work_rate,
+        resample_atten: settings.resample_atten,
+        resample_delta_freq: settings.resample_delta_freq,
+        resample_cutout: settings.resample_cutout,
+        demodulation_atten: settings.demodulation_atten,
+    };
+    let mut ts = sys::apt_track_settings { delta: 0, lambda: 0.0 };
+    unsafe { sys::apt_default_track_settings(&mut ts) };
+    if let Some((delta, lambda)) = track {
+        ts = sys::apt_track_settings { delta, lambda };
+    }
+    let mut bound: u64 = 0;
+    let st = unsafe { sys::apt_decode_len_bound(signal.len() as u64, input_rate.get_hz(), &s, &mut bound) };
+    if st != sys::APT_OK {
+        return Err(to_error(st));
+    }
+    let mut dec: *mut sys::apt_decoder = std::ptr::null_mut();
+    let st = unsafe { sys::apt_decoder_create(0, input_rate.get_hz(), &s, signal.len() as u64, &mut dec) };
+    if st != sys::APT_OK {
+        return Err(to_error(st));
+    }
+    let mut out: Signal = vec![0_f32; bound.max(1) as usize];
+    let mut n: u64 = 0;
+    let st = unsafe {
+        let mut st = sys::apt_decoder_set_sync_mode(dec, sys::APT_SYNC_TRACK, &ts);
+        if st == sys::APT_OK {
+            st = sys::apt_decoder_submit_host(dec, signal.as_ptr() as *const c_void, sys::APT_F32, signal.len() as u64, 1,
+                                              out.as_mut_ptr(), out.len() as u64);
+        }
+        if st == sys::APT_OK {
+            st = sys::apt_decoder_wait(dec, &mut n);
+        }
+        sys::apt_decoder_destroy(dec);
+        st
+    };
+    if st != sys::APT_OK {
+        return Err(to_error(st));
+    }
+    out.truncate(n as usize);
+    Ok(out)
+}
