@@ -177,7 +177,8 @@ int apt_wav_load_pcm16(const char *path, int16_t *out, uint64_t cap, uint64_t *n
 /* 16-bit mono PCM file, what resample.rs:53-66 writes. */
 int apt_wav_write_i16(const char *path, const int16_t *samples, uint64_t n, uint32_t sample_rate);
 /* wav::write_wav's conversion for 16-bit files -- wav.rs:71-85: (sample / max * 32767.0) as i16 with max = dsp::get_max,
- * on the device; bit-identical to the reference given the same signal. */
+ * on the device; bit-identical to the reference given the same signal.  max is sample 0 if that is NaN, else the first
+ * non-NaN sample equal to the largest value (-0.0 == +0.0: the first zero wins).  n < 2^32. */
 int apt_quantize_i16(const float *signal, uint64_t n, int16_t *out);
 /* resample::resample -- resample.rs:17-71: load WAV, dsp::resample (Lowpass, atten dB, delta_w in pi rad/sample) on the
  * GPU, normalise + quantise on the GPU, write a 16-bit WAV.  (The modification-time copy of resample.rs:30,68 is file
@@ -217,7 +218,10 @@ int apt_decode_image_u8(const void *signal, int format, uint64_t n, uint32_t inp
 /* Stage entry points on host buffers (rows = decode()'s output, n = rows*2080 values). */
 /* noaa_apt::map_signal_u8 -- noaa_apt.rs:249-259. */
 int apt_map_signal_u8(const float *signal, uint64_t n, float low, float high, uint8_t *out);
-/* Contrast bounds of an image: MinMax / misc::percent / telemetry (info receives bounds, wedges, frame row). */
+/* Contrast bounds of an image: MinMax / misc::percent / telemetry (info receives bounds, wedges, frame row).  Min and max
+ * (MinMax, and Percent's range) are dsp::get_min / get_max's: pixel 0 for both if it is NaN; otherwise the first non-NaN
+ * pixel equal to the smallest (largest) value, with its own bits (-0.0 == +0.0: the first zero wins).  NaN pixels map
+ * to 0.  Fewer than 2^32 pixels. */
 int apt_contrast_bounds(const float *signal, uint64_t n, int contrast, float percent, apt_image_info *info);
 /* telemetry.rs:147-170: per-row means of the two telemetry bands and their pooled variance (n / 2080 values each). */
 int apt_telemetry_rows(const float *signal, uint64_t n, float *mean_a, float *mean_b, float *variance);

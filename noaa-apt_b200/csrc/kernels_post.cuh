@@ -8,7 +8,10 @@
 //   grey histogram equalisation                 processing.rs:87-103, imageext.rs:23-46, :95-119
 //   processing::false_color                     processing.rs:108-157
 //   processing::rotate (Rotate::Yes)            processing.rs:21-37
-// Given the same f32 rows these kernels reproduce the reference's u8 / RGBA image and contrast bounds bit for bit.
+// Given the same f32 rows these kernels reproduce the reference's u8 / RGBA image and contrast bounds bit for bit,
+// non-finite pixels and signed zeros included.  Min / max follow dsp::get_min / get_max, a walk from pixel 0 with strict
+// `<` / `>`: if pixel 0 is NaN both are pixel 0; otherwise the minimum is the pixel of lowest index among the non-NaN
+// pixels that compare == to the smallest value (-0.0 == +0.0), with its own bits, and the maximum likewise.
 #pragma once
 
 #include <cstdint>
@@ -23,13 +26,10 @@ __device__ const float kTelemetryPattern[25] = {31.f, 63.f, 95.f, 127.f, 159.f, 
                                                 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f,
                                                 31.f, 63.f, 95.f, 127.f, 159.f, 191.f, 224.f, 255.f, 0.f};
 
-// monotone map float -> u32 so that integer atomicMin / atomicMax order floats
+// monotone map float -> u32 of the non-NaN floats, -0.0 folded onto +0.0 so that the two zeros tie
 __device__ __forceinline__ u32 float_key(float v) {
-    const u32 b = __float_as_uint(v);
+    const u32 b = __float_as_uint(v == 0.f ? 0.f : v);
     return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float key_float(u32 k) {
-    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
 
 __device__ __forceinline__ u32 post_rows(const PostCtl *ctl, const SyncResult *result, u32 fixed_rows) {
@@ -37,20 +37,32 @@ __device__ __forceinline__ u32 post_rows(const PostCtl *ctl, const SyncResult *r
     return result ? (result->status == 0 ? result->n_rows : 0u) : fixed_rows;
 }
 
-// min / max of the image (any order gives the same values) and, per row, the telemetry band means and their pooled
-// variance in the reference's sequential order (telemetry.rs:147-170): bands at pixels 994..1037 and 2034..2077.
+// (min, max) of the n pixels from what k_post_stats left in ctl: pixel 0 when it is NaN, else the winning pixels' values
+__device__ __forceinline__ float2 post_minmax(const float *rows, u64 n, const PostCtl *ctl) {
+    if (n == 0) return make_float2(0.f, 0.f);
+    const float x0 = rows[0];
+    if (x0 != x0) return make_float2(x0, x0);
+    return make_float2(rows[static_cast<u32>(~ctl->nmin_at)], rows[~static_cast<u32>(ctl->max_at)]);
+}
+
+// min / max of the image as the pixel index that wins them (first wins among ties: the thread's pixels come in
+// ascending index, the cross-thread reduction takes the lower index on equal keys; NaN pixels take no part) and, per
+// row, the telemetry band means and their pooled variance in the reference's sequential order (telemetry.rs:147-170):
+// bands at pixels 994..1037 and 2034..2077.  Pixel indices fit in u32 (post_launch checks).
 __global__ void __launch_bounds__(256)
 k_post_stats(const float *__restrict__ rows, const SyncResult *__restrict__ result, u32 fixed_rows, u32 px, PostCtl *__restrict__ ctl,
              float *__restrict__ mean_a, float *__restrict__ mean_b, float *__restrict__ variance) {
-    __shared__ u32 s_min[8], s_max[8];
+    __shared__ u64 s_min[8], s_max[8];
     const u32 n_rows = post_rows(ctl, result, fixed_rows);
-    u32 kmin = 0xFFFFFFFFu, kmax = 0u;
+    u32 kmin = 0xFFFFFFFFu, imin = 0xFFFFFFFFu, kmax = 0u, imax = 0xFFFFFFFFu;   // no key of a non-NaN float is 0 or ~0
     for (u32 r = blockIdx.x; r < n_rows; r += gridDim.x) {
         const float *line = rows + static_cast<u64>(r) * px;
         for (u32 c = threadIdx.x; c < px; c += blockDim.x) {
-            const u32 k = float_key(line[c]);
-            kmin = min(kmin, k);
-            kmax = max(kmax, k);
+            const float v = line[c];
+            if (v != v) continue;
+            const u32 k = float_key(v);
+            if (k < kmin) { kmin = k; imin = r * px + c; }
+            if (k > kmax) { kmax = k; imax = r * px + c; }
         }
         if (threadIdx.x < 2 && px >= 2078 && mean_a != nullptr) {
             const float *band = line + (threadIdx.x == 0 ? 994 : 2034);
@@ -67,17 +79,19 @@ k_post_stats(const float *__restrict__ rows, const SyncResult *__restrict__ resu
             if (threadIdx.x == 0) variance[r] = __fdiv_rn(__fadd_rn(var, other), 88.f);
         }
     }
+    // key << 32 | index ordered by min, key << 32 | ~index by max: equal keys go to the lower index either way
+    u64 cmin = (static_cast<u64>(kmin) << 32) | imin, cmax = (static_cast<u64>(kmax) << 32) | ~imax;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
-        kmin = min(kmin, __shfl_xor_sync(0xffffffffu, kmin, o));
-        kmax = max(kmax, __shfl_xor_sync(0xffffffffu, kmax, o));
+        cmin = min(cmin, __shfl_xor_sync(0xffffffffu, cmin, o));
+        cmax = max(cmax, __shfl_xor_sync(0xffffffffu, cmax, o));
     }
-    if ((threadIdx.x & 31) == 0) { s_min[threadIdx.x >> 5] = kmin; s_max[threadIdx.x >> 5] = kmax; }
+    if ((threadIdx.x & 31) == 0) { s_min[threadIdx.x >> 5] = cmin; s_max[threadIdx.x >> 5] = cmax; }
     __syncthreads();
     if (threadIdx.x == 0) {
-        for (int w = 1; w < 8; ++w) { kmin = min(kmin, s_min[w]); kmax = max(kmax, s_max[w]); }
-        atomicMax(&ctl->nmin_key, ~kmin);                          // zero-initialised control block: keep ~min as a maximum
-        atomicMax(&ctl->max_key, kmax);
+        for (int w = 1; w < 8; ++w) { cmin = min(cmin, s_min[w]); cmax = max(cmax, s_max[w]); }
+        atomicMax(&ctl->nmin_at, ~cmin);                           // zero-initialised control block: keep ~min as a maximum
+        atomicMax(&ctl->max_at, cmax);
     }
 }
 
@@ -88,7 +102,8 @@ k_post_histogram(const float *__restrict__ rows, const SyncResult *__restrict__ 
     for (u32 i = threadIdx.x; i < 1000; i += blockDim.x) s_b[i] = 0;
     __syncthreads();
     const u64 n = static_cast<u64>(post_rows(ctl, result, fixed_rows)) * px;
-    const float mn = key_float(~ctl->nmin_key), mx = key_float(ctl->max_key);
+    const float2 m = post_minmax(rows, n, ctl);
+    const float mn = m.x, mx = m.y;
     const float range = __fsub_rn(mx, mn);
     for (u64 i = static_cast<u64>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<u64>(gridDim.x) * blockDim.x) {
         const float t = truncf(__fmul_rn(__fdiv_rn(__fsub_rn(rows[i], mn), range), 1000.f));
@@ -106,14 +121,16 @@ k_post_histogram(const float *__restrict__ rows, const SyncResult *__restrict__ 
 //   mode 2  Telemetry  telemetry.rs:172-228 frame search (first-wins strict maximum of the quality), :30-66 wedge values,
 //                      low = wedge 9, high = wedge 8 averaged over both channels (noaa_apt.rs:143-149)
 __global__ void __launch_bounds__(1024)
-k_post_bounds(int mode, float percent, const SyncResult *__restrict__ result, u32 fixed_rows, u32 px, PostCtl *__restrict__ ctl,
-              const float *__restrict__ mean_a, const float *__restrict__ mean_b, const float *__restrict__ variance) {
+k_post_bounds(int mode, float percent, const float *__restrict__ rows, const SyncResult *__restrict__ result, u32 fixed_rows, u32 px,
+              PostCtl *__restrict__ ctl, const float *__restrict__ mean_a, const float *__restrict__ mean_b,
+              const float *__restrict__ variance) {
     __shared__ u32 s_scan[1024];
     __shared__ float s_q[1024];
     __shared__ u32 s_i[1024];
     const u32 tid = threadIdx.x;
     const u32 n_rows = post_rows(ctl, result, fixed_rows);
-    const float mn = key_float(~ctl->nmin_key), mx = key_float(ctl->max_key);
+    const float2 m = post_minmax(rows, static_cast<u64>(n_rows) * px, ctl);
+    const float mn = m.x, mx = m.y;
     if (tid == 0) {
         ctl->rows = n_rows;
         ctl->low = mn;
@@ -385,10 +402,10 @@ k_post_finish(const unsigned char *__restrict__ grey, const PostCtl *__restrict_
 }
 
 // wav.rs:71-85 for 16-bit files: (sample / max * 32767.0) as i16 -- `as` truncates toward zero, saturates, NaN -> 0.
-// The maximum arrives as the float key that k_post_stats leaves in ctl->max_key.
+// The maximum is dsp::get_max as k_post_stats leaves it in ctl (post_minmax).
 __global__ void __launch_bounds__(256)
 k_quantize_i16(const float *__restrict__ x, u64 n, const PostCtl *__restrict__ ctl, short *__restrict__ out) {
-    const float mx = key_float(ctl->max_key);
+    const float mx = post_minmax(x, n, ctl).y;
     for (u64 i = static_cast<u64>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<u64>(gridDim.x) * blockDim.x) {
         const float v = __fmul_rn(__fdiv_rn(x[i], mx), 32767.f);
         short q;

@@ -46,7 +46,7 @@ struct Rec {
 };
 // Control / result block of the image stage (kernels_post.cuh); zeroed at the start of a job.
 struct PostCtl {
-    u32 nmin_key, max_key;   // ~key(min) and key(max) of the image under the monotone float -> u32 map
+    u64 nmin_at, max_at;     // ~(key(min) << 32 | index) and key(max) << 32 | ~index: the pixels that win min / max
     u32 rows;                // image rows
     u32 status;              // 0 ok; 1 empty image; 2 percent: no low bucket; 3 too short for telemetry; 4 frame runs off the image
     float low, high;         // contrast bounds

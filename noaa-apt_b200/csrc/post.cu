@@ -73,6 +73,10 @@ int post_launch(const LaunchCtx &c, const PostPlan &p, PostBuffers &b, const flo
     const unsigned wide = static_cast<unsigned>(c.sm_count) * 8;
     float *tel_a = b.tel, *tel_b = b.tel + max_rows, *tel_v = b.tel + 2 * static_cast<size_t>(max_rows);
     if (!bounds_dev) {
+        // k_post_stats names the min / max pixels by u32 index: the decoder's rows stay below 2^32 work-rate samples, a
+        // stream's or watch's max_rows below 2^32 / 2080, apt_process and apt_quantize_i16 refuse larger inputs
+        if (static_cast<u64>(max_rows) * px >= (1ull << 32))
+            return fail(APT_ERR_BAD_ARG, "image stage: %u rows of %u pixels reach 2^32 pixels", max_rows, px);
         const int bounds_mode = p.hist ? APT_CONTRAST_MINMAX : p.s.contrast;   // Contrast::Histogram takes the MinMax bounds,
                                                                                 // noaa_apt.rs:158-163
         APT_CUDA(cudaMemsetAsync(b.ctl, 0, sizeof(PostCtl), c.stream));
@@ -88,7 +92,8 @@ int post_launch(const LaunchCtx &c, const PostPlan &p, PostBuffers &b, const flo
         }
         {
             KernelSlot s(hook, "post_bounds");
-            k_post_bounds<<<1, 1024, 0, c.stream>>>(bounds_mode, p.s.percent, result, fixed_rows, px, b.ctl, tel_a, tel_b, tel_v);
+            k_post_bounds<<<1, 1024, 0, c.stream>>>(bounds_mode, p.s.percent, rows, result, fixed_rows, px, b.ctl, tel_a, tel_b,
+                                                   tel_v);
         }
     }
     if (out) {
