@@ -1,10 +1,11 @@
-// First stage of decode(): kernel choice, device tables, unit geometry and launch (front.hpp).
+// First stage of decode(): kernel choice, device tables, unit geometry and launch, and its streamed windows (front.hpp).
 #include "front.hpp"
 
 #include <algorithm>
 #include <cstdlib>
 
 #include "common.hpp"
+#include "decoder.hpp"
 
 namespace aptb200 {
 
@@ -135,6 +136,81 @@ int front_launch(const LaunchCtx &c, const FrontPlan &f, const FrontTables &t, c
                                    envelope, cosphi2, sinphi, out);
     return launch_polyphase(c, in, format, n, t.h, f.r.l, f.r.m, f.off2, u0 * f.unit_out, std::min(nwork, u1 * f.unit_out),
                             envelope, cosphi2, sinphi, out);
+}
+
+int window_compact(cudaStream_t s, float *buf, uint64_t &base, uint64_t keep, uint64_t end) {
+    keep = std::min(keep, end) & ~static_cast<uint64_t>(15);
+    if (keep <= base) return APT_OK;
+    const uint64_t drop = keep - base, tail = end - keep;
+    if (tail > drop) return APT_OK;
+    if (tail) APT_CUDA(cudaMemcpyAsync(buf, buf + drop, tail * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    base = keep;
+    return APT_OK;
+}
+
+int FrontWindow::alloc(const FrontPlan &f, uint64_t cap_in, uint64_t cap_e, uint64_t max_push) {
+    this->cap_in = cap_in, this->cap_e = cap_e, this->max_push = max_push;
+    APT_CUDA(cudaMalloc(&d_in, cap_in * sizeof(float)));
+    APT_CUDA(cudaMalloc(&d_pcm, max_push * sizeof(int16_t)));
+    APT_CUDA(cudaMalloc(&d_conv, max_push * sizeof(float)));
+    APT_CUDA(cudaMalloc(&d_e, cap_e * sizeof(float)));
+    if (f.needs_scratch()) APT_CUDA(cudaMalloc(&d_r, cap_e * sizeof(float)));
+    return APT_OK;
+}
+
+void FrontWindow::release() {
+    for (void *p : {(void *)d_in, (void *)d_pcm, (void *)d_conv, (void *)d_e, (void *)d_r})
+        if (p) cudaFree(p);
+    d_in = d_conv = d_e = d_r = nullptr;
+    d_pcm = nullptr;
+}
+
+int FrontWindow::zero_input(cudaStream_t s) const {
+    APT_CUDA(cudaMemsetAsync(d_in, 0, cap_in * sizeof(float), s));
+    return APT_OK;
+}
+
+int FrontWindow::compact(cudaStream_t s, const FrontPlan &f, uint64_t keep_in, uint64_t keep_e) {
+    uint64_t xa, xb, eb = e_base, rb = e_base;
+    f.span(units_done, units_done + 1, ~0ull, xa, xb);
+    APT_TRY(window_compact(s, d_in, in_base, std::min(keep_in, xa), samples_in));
+    APT_TRY(window_compact(s, d_e, eb, keep_e, work_final));
+    if (d_r && eb != e_base) APT_TRY(window_compact(s, d_r, rb, keep_e, work_final));
+    e_base = eb;
+    return APT_OK;
+}
+
+int FrontWindow::room(uint64_t n) const {
+    if (samples_in - in_base + n > cap_in) return fail(APT_ERR_BAD_ARG, "internal: input window overflow");
+    return APT_OK;
+}
+
+int FrontWindow::push(const LaunchCtx &c, const void *src, bool on_device, int format, uint64_t n) {
+    APT_TRY(room(n));
+    float *dst = d_in + (samples_in - in_base);
+    if (on_device) {
+        APT_CUDA(cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyDeviceToDevice, c.stream));
+    } else if (format == APT_PCM16) {
+        APT_CUDA(cudaMemcpyAsync(d_pcm, src, n * 2, cudaMemcpyHostToDevice, c.stream));
+        APT_TRY(launch_pcm16_to_f32(c, d_pcm, n, d_conv));
+        APT_CUDA(cudaMemcpyAsync(dst, d_conv, n * 4, cudaMemcpyDeviceToDevice, c.stream));
+    } else {
+        APT_CUDA(cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyHostToDevice, c.stream));
+    }
+    commit(n);
+    return APT_OK;
+}
+
+int FrontWindow::advance(const LaunchCtx &c, const Plan &p, const FrontTables &t, bool finish) {
+    const uint64_t nw = p.front.work_len(samples_in), u_hi = p.front.complete(samples_in, nw, finish);
+    if (u_hi <= units_done) return APT_OK;
+    const uint64_t work_hi = finish ? nw : std::min(nw, u_hi * p.front.unit_out);
+    if (work_hi - e_base > cap_e) return fail(APT_ERR_BAD_ARG, "internal: envelope window overflow");
+    APT_TRY(front_launch(c, p.front, t, in_origin(), APT_F32, nullptr, samples_in, nw, units_done, u_hi, true, p.cosphi2,
+                         p.sinphi, d_r ? d_r - e_base : nullptr, d_e - e_base, nullptr));
+    units_done = u_hi;
+    work_final = work_hi;
+    return APT_OK;
 }
 
 }  // namespace aptb200

@@ -84,4 +84,43 @@ int front_launch(const LaunchCtx &c, const FrontPlan &f, const FrontTables &t, c
                  uint64_t n, uint64_t nwork, uint64_t u0, uint64_t u1, bool envelope, float cosphi2, float sinphi,
                  float *scratch, float *out, KernelHook *hook);
 
+// Moves the tail [keep, end) of a window based at `base` to its front when that does not overlap (keep is floored to a
+// multiple of 16, so the window keeps its alignment).
+int window_compact(cudaStream_t s, float *buf, uint64_t &base, uint64_t keep, uint64_t end);
+
+struct Plan;   // decoder.hpp
+
+// The streamed first stage of the stream and the watcher: the f32 input window ([in_base, samples_in)), the envelope
+// window ([e_base, work_final), with the decimating kind's scratch d_r) and the units done; the caller sizes and trims both.
+struct FrontWindow {
+    float *d_in = nullptr, *d_conv = nullptr, *d_e = nullptr, *d_r = nullptr;   // d_conv: a PCM16 push (d_pcm) as f32
+    int16_t *d_pcm = nullptr;
+    uint64_t cap_in = 0, cap_e = 0, max_push = 0;
+    uint64_t samples_in = 0, in_base = 0, units_done = 0, work_final = 0, e_base = 0;
+    FrontWindow() = default;
+    FrontWindow(const FrontWindow &) = delete;
+    ~FrontWindow() { release(); }
+    // envelope outputs one step of max_push samples can finalise (finish: the units the input tail still held)
+    static uint64_t step_outputs(const FrontPlan &f, uint64_t max_push) {
+        return (max_push + f.tail()) * f.r.l / f.r.m + 2 * f.unit_out + 64;
+    }
+    static uint64_t bytes(const FrontPlan &f, uint64_t cap_in, uint64_t cap_e, uint64_t max_push) {   // what alloc() takes
+        return cap_in * 4 + max_push * (2 + 4) + cap_e * 4 * (f.needs_scratch() ? 2 : 1);
+    }
+    int alloc(const FrontPlan &f, uint64_t cap_in, uint64_t cap_e, uint64_t max_push);
+    void release();
+    void clear() { samples_in = in_base = units_done = work_final = e_base = 0; }
+    int zero_input(cudaStream_t s) const;   // at create and reset, not at a watcher's segment roll
+    // input from min(keep_in, the next unit's first sample), envelope from keep_e (d_r follows only when d_e moves)
+    int compact(cudaStream_t s, const FrontPlan &f, uint64_t keep_in, uint64_t keep_e);
+    // n host samples (f32, or PCM16 cast through d_pcm and d_conv, so pushes may mix formats) or n f32 device samples
+    int push(const LaunchCtx &c, const void *src, bool on_device, int format, uint64_t n);
+    // audio written into the window on the device: room(n) checks that n samples fit, commit(n) counts them
+    float *in_origin() const { return d_in - in_base; }   // the address input sample 0 would have
+    int room(uint64_t n) const;
+    void commit(uint64_t n) { samples_in += n; }
+    int advance(const LaunchCtx &c, const Plan &p, const FrontTables &t, bool finish);   // the units now complete (all at finish)
+    const float *e_origin() const { return d_e - e_base; }   // the address envelope sample 0 would have
+};
+
 }  // namespace aptb200

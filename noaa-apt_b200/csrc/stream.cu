@@ -61,8 +61,7 @@ Geom make_geom(const Plan &p, int sync, uint64_t max_push) {
     g.row = p.row;
     // input tail: from the next unit's first sample to the end of what was pushed (less than one unit span)
     const uint64_t t_in = f.tail();
-    // envelope outputs one step can finalise (finish: the units the input tail still held)
-    const uint64_t w_new = (max_push + t_in) * f.r.l / f.r.m + 2 * f.unit_out + 64;
+    const uint64_t w_new = FrontWindow::step_outputs(f, max_push);
     // envelope tail: a pending row (< row + 1 before work_final) or a pending peak (>= decided >= c_end - D), plus the
     // low-pass halo and the 16-sample alignment of the window start
     const uint64_t t_e = g.row + g.D + g.G + kHalo + 64;
@@ -74,7 +73,7 @@ Geom make_geom(const Plan &p, int sync, uint64_t max_push) {
     g.gather_cap = w_new / g.row + 4;
     g.latency = sync ? g.D + 1 : 0;
     const uint64_t rows_floats = (g.gather_cap + 1) * kPxPerRow;
-    g.bytes = plan_table_bytes(p) + g.cap_in * 4 + max_push * (2 + 4) + g.cap_e * 4 * (f.needs_scratch() ? 2 : 1) +
+    g.bytes = plan_table_bytes(p) + FrontWindow::bytes(f, g.cap_in, g.cap_e, max_push) +
               (sync ? g.cap_c * 4 + g.root_cap * 4 + kRunRing * 8 + sizeof(StreamCarry) : sizeof(StreamCarry)) +
               g.gather_cap * 4 + rows_floats * 4;
     return g;
@@ -85,16 +84,15 @@ Geom make_geom(const Plan &p, int sync, uint64_t max_push) {
 struct apt_stream {
     apt_decoder dec;                // plan, device, CUDA stream and filter tables (the other members stay unused)
     int sync = 0;
-    uint64_t max_push = 0;
     Geom g;
-    float *d_in = nullptr, *d_conv = nullptr, *d_e = nullptr, *d_r = nullptr, *d_corr = nullptr, *d_rows = nullptr;
-    int16_t *d_pcm = nullptr;
+    FrontWindow win;                // input and envelope windows and the first stage's progress (max_push audio samples)
+    float *d_corr = nullptr, *d_rows = nullptr;
     u32 *d_roots = nullptr, *d_gpos = nullptr;
     char *d_carry = nullptr;        // StreamCarry, then the run ring (kRunRing positions, kRunRing counts)
     char *h_carry = nullptr;        // pinned copy of the same
     float *h_rows = nullptr;        // pinned rows of one round
     // recording state
-    uint64_t samples_in = 0, in_base = 0, units_done = 0, work_final = 0, e_base = 0, c_base = 0, c_end = 0;
+    uint64_t c_base = 0, c_end = 0;
     uint64_t rows_out = 0, gathered = 0, held_slot = 0;
     bool finished = false;
     std::vector<uint64_t> positions;
@@ -105,7 +103,7 @@ struct apt_stream {
     const u32 *run_cnt() const { return run_pos() + kRunRing; }
 
     // I/Q stream (apt_stream_create_iq): every push is converted into the cf32 window `feed`, which keeps the halo the next
-    // audio output reads, and k_fm_demod writes the new audio into d_in; the audio counters above then count audio samples
+    // audio output reads, and k_fm_demod writes the new audio into the input window, whose counters then count audio samples
     bool iq = false;
     uint64_t iq_max_push = 0;       // I/Q samples one step takes
     IqPlan iqp;
@@ -132,8 +130,8 @@ void release_image(apt_stream *st) {
 void free_stream(apt_stream *st) {
     cudaSetDevice(st->dec.device);
     if (st->dec.stream) cudaStreamSynchronize(st->dec.stream);
-    for (void *p : {(void *)st->d_in, (void *)st->d_conv, (void *)st->d_e, (void *)st->d_r, (void *)st->d_corr,
-                    (void *)st->d_rows, (void *)st->d_pcm, (void *)st->d_roots, (void *)st->d_gpos, (void *)st->d_carry})
+    st->win.release();
+    for (void *p : {(void *)st->d_corr, (void *)st->d_rows, (void *)st->d_roots, (void *)st->d_gpos, (void *)st->d_carry})
         if (p) cudaFree(p);
     if (st->h_carry) cudaFreeHost(st->h_carry);
     if (st->h_rows) cudaFreeHost(st->h_rows);
@@ -144,21 +142,17 @@ void free_stream(apt_stream *st) {
 }
 
 int reset_state(apt_stream *st) {
-    st->samples_in = st->in_base = st->units_done = st->work_final = st->e_base = st->c_base = st->c_end = 0;
-    st->rows_out = st->gathered = st->held_slot = st->runs_seen = 0;
+    st->win.clear();
+    st->c_base = st->c_end = st->rows_out = st->gathered = st->held_slot = st->runs_seen = 0;
     st->feed.in = st->feed.base = 0;
     st->finished = false;
     st->positions.clear();
     APT_CUDA(cudaSetDevice(st->dec.device));
     APT_CUDA(cudaMemsetAsync(st->d_carry, 0, sizeof(StreamCarry), st->dec.stream));
-    APT_CUDA(cudaMemsetAsync(st->d_in, 0, st->g.cap_in * sizeof(float), st->dec.stream));
+    APT_TRY(st->win.zero_input(st->dec.stream));
     APT_CUDA(cudaStreamSynchronize(st->dec.stream));
     memset(st->h_carry, 0, sizeof(StreamCarry));
     return APT_OK;
-}
-
-int compact(apt_stream *st, float *buf, uint64_t &base, uint64_t keep, uint64_t end) {
-    return window_compact(st->dec.stream, buf, base, keep, end);
 }
 
 // First envelope sample a later step can still read.
@@ -173,21 +167,11 @@ uint64_t envelope_keep(const apt_stream *st) {
 }
 
 int compact_all(apt_stream *st) {
-    uint64_t xa, xb;
-    st->dec.plan.front.span(st->units_done, st->units_done + 1, ~0ull, xa, xb);
-    APT_TRY(compact(st, st->d_in, st->in_base, xa, st->samples_in));
     const uint64_t ek = envelope_keep(st);
-    const uint64_t ekeep = ek > kHalo ? ek - kHalo : 0;
-    uint64_t eb = st->e_base;
-    APT_TRY(compact(st, st->d_e, eb, ekeep, st->work_final));
-    if (st->d_r && eb != st->e_base) {
-        uint64_t rb = st->e_base;
-        APT_TRY(compact(st, st->d_r, rb, ekeep, st->work_final));
-    }
-    st->e_base = eb;
+    APT_TRY(st->win.compact(st->dec.stream, st->dec.plan.front, ~0ull, ek > kHalo ? ek - kHalo : 0));
     if (st->sync) {
         const StreamCarry &cy = st->carry();
-        APT_TRY(compact(st, st->d_corr, st->c_base, cy.seed_state == 0 ? 0 : cy.decided, st->c_end));
+        APT_TRY(window_compact(st->dec.stream, st->d_corr, st->c_base, cy.seed_state == 0 ? 0 : cy.decided, st->c_end));
     }
     return APT_OK;
 }
@@ -212,27 +196,19 @@ int keep_rows(apt_stream *st, uint64_t first, uint64_t end, const float *src) {
     return APT_OK;
 }
 
-// The new audio of one step into the input window, from any source: audio pushes are uploaded as they are (PCM16 cast
-// into the f32 window, so pushes may mix formats), or copied device to device from f32 samples already on the device
-// (`on_device`, stream_push_device); I/Q pushes are converted into the cf32 window and every audio sample they complete is
-// demodulated into the input window.  `added` receives the number of new audio samples.
-int upload(apt_stream *st, const void *src, bool on_device, int format, uint64_t n, uint64_t &added) {
-    apt_decoder &d = st->dec;
-    const LaunchCtx c{d.stream, d.sm_count};
-    const uint64_t off = st->samples_in - st->in_base;
-    if (!st->iq) {
-        if (off + n > st->g.cap_in) return fail(APT_ERR_BAD_ARG, "internal: input window overflow");
-        APT_TRY(window_upload(c, src, on_device, format, n, st->d_pcm, st->d_conv, st->d_in + off));
-        added = n;
-        return APT_OK;
-    }
+// The new audio of one step into the input window: audio pushes from the host or (`on_device`, stream_push_device) from
+// the device; I/Q pushes are converted into the cf32 window and every audio sample they complete is demodulated into it.
+int upload(apt_stream *st, const void *src, bool on_device, int format, uint64_t n) {
+    const LaunchCtx c{st->dec.stream, st->dec.sm_count};
+    if (!st->iq) return st->win.push(c, src, on_device, format, n);
     const IqPlan &q = st->iqp;
-    APT_TRY(st->feed.push(c, q, st->samples_in, src, format, n));
-    const uint64_t m1 = q.out_len(st->feed.in);
-    added = m1 - st->samples_in;
-    if (off + added > st->g.cap_in) return fail(APT_ERR_BAD_ARG, "internal: input window overflow");
-    return iq_launch(c, q, st->iqt, st->feed.origin(), st->feed.base, st->feed.in, APT_CF32, st->samples_in, m1,
-                     st->d_in - st->in_base);
+    APT_TRY(st->feed.push(c, q, st->win.samples_in, src, format, n));
+    const uint64_t m1 = q.out_len(st->feed.in), added = m1 - st->win.samples_in;
+    APT_TRY(st->win.room(added));
+    APT_TRY(iq_launch(c, q, st->iqt, st->feed.origin(), st->feed.base, st->feed.in, APT_CF32, st->win.samples_in, m1,
+                      st->win.in_origin()));
+    st->win.commit(added);
+    return APT_OK;
 }
 
 // One step: `n` new samples (maybe none) and, when `finish`, the end of the recording.
@@ -243,28 +219,23 @@ int step(apt_stream *st, const void *src, bool on_device, int format, uint64_t n
     const Geom &g = st->g;
     const LaunchCtx c{d.stream, d.sm_count};
     APT_TRY(compact_all(st));
-    if (n) {
-        uint64_t added = 0;
-        APT_TRY(upload(st, src, on_device, format, n, added));
-        st->samples_in += added;
-    }
-    const uint64_t N = st->samples_in;
-    const uint64_t nw = p.front.work_len(N);
+    if (n) APT_TRY(upload(st, src, on_device, format, n));
+    const uint64_t nw = p.front.work_len(st->win.samples_in);
     if (finish && nw < 10ull * p.row) {    // decode.rs:79-83
         status = fail(APT_ERR_TOO_SHORT, "Got less than 10 rows of samples, audio file is too short");
         return APT_OK;
     }
     // ---- first stage: the units whose input span is complete (all of them at the end) ----
-    const uint64_t work_before = st->work_final;
-    APT_TRY(front_advance(c, p, d.front, st->d_in - st->in_base, N, finish, g.cap_e, st->d_r, st->d_e, st->e_base,
-                          st->units_done, st->work_final));
+    const uint64_t work_before = st->win.work_final;
+    APT_TRY(st->win.advance(c, p, d.front, finish));
+    const uint64_t work_final = st->win.work_final;
     const u32 ntaps = static_cast<u32>(p.lp.size());
-    float *e = st->d_e - st->e_base;
+    const float *e = st->win.e_origin();
     if (!st->sync) {   // rows r with (r+1)*row <= work_final (decode.rs:141-147)
-        const uint64_t r_hi = st->work_final / p.row;
+        const uint64_t r_hi = work_final / p.row;
         while (st->rows_out < r_hi) {
             const uint64_t cnt = std::min<uint64_t>(r_hi - st->rows_out, g.gather_cap);
-            APT_TRY(launch_gather_lp(c, e, st->work_final, nullptr, nullptr, static_cast<u32>(cnt), static_cast<u32>(cnt), p.row, kPxPerRow,
+            APT_TRY(launch_gather_lp(c, e, work_final, nullptr, nullptr, static_cast<u32>(cnt), static_cast<u32>(cnt), p.row, kPxPerRow,
                                      p.dec, p.lp.data(), ntaps, st->d_rows, static_cast<u32>(st->rows_out)));
             if (st->img_rows) APT_TRY(keep_rows(st, st->rows_out, st->rows_out + cnt, st->d_rows));
             APT_CUDA(cudaMemcpyAsync(st->h_rows, st->d_rows, cnt * kPxPerRow * sizeof(float), cudaMemcpyDeviceToHost, d.stream));
@@ -275,13 +246,13 @@ int step(apt_stream *st, const void *src, bool on_device, int format, uint64_t n
         return APT_OK;
     }
     // ---- low-pass + correlation of the newly final range ----
-    const uint64_t c_new = finish ? nw - g.G : (st->work_final > g.G ? st->work_final - g.G : 0);
-    if (!finish && c_new <= st->c_end && st->work_final == work_before) return APT_OK;   // nothing became final
+    const uint64_t c_new = finish ? nw - g.G : (work_final > g.G ? work_final - g.G : 0);
+    if (!finish && c_new <= st->c_end && work_final == work_before) return APT_OK;   // nothing became final
     if (c_new > st->c_end) {
         const uint64_t lp_base = floor16(st->c_end);
-        if (c_new - st->c_base > g.cap_c || (lp_base >= kHalo && lp_base - kHalo < st->e_base))
+        if (c_new - st->c_base > g.cap_c || (lp_base >= kHalo && lp_base - kHalo < st->win.e_base))
             return fail(APT_ERR_BAD_ARG, "internal: correlation window overflow");
-        APT_TRY(launch_lowpass_corr(c, e, st->work_final, p.lp.data(), ntaps, p.dec, nullptr, st->d_corr - st->c_base, lp_base));
+        APT_TRY(launch_lowpass_corr(c, e, work_final, p.lp.data(), ntaps, p.dec, nullptr, st->d_corr - st->c_base, lp_base));
         st->c_end = c_new;
     }
     // ---- picker + gather, in rounds until the walk has gone as far as the final data allow ----
@@ -298,7 +269,7 @@ int step(apt_stream *st, const void *src, bool on_device, int format, uint64_t n
         a.corr = st->d_corr - st->c_base;
         a.c_end = st->c_end;
         a.ncorr = st->c_end;
-        a.work_final = st->work_final;
+        a.work_final = work_final;
         a.finish = finish ? 1 : 0;
         a.row = p.row;
         a.dist = p.dist;
@@ -311,7 +282,7 @@ int step(apt_stream *st, const void *src, bool on_device, int format, uint64_t n
         a.gpos = st->d_gpos;
         a.carry = dcy;
         APT_TRY(launch_stream_sync(c, a));
-        APT_TRY(launch_gather_lp(c, e, st->work_final, st->d_gpos, &dcy->gres, 0, static_cast<u32>(g.gather_cap), p.row, kPxPerRow,
+        APT_TRY(launch_gather_lp(c, e, work_final, st->d_gpos, &dcy->gres, 0, static_cast<u32>(g.gather_cap), p.row, kPxPerRow,
                                  p.dec, p.lp.data(), ntaps, st->d_rows + held * kPxPerRow, static_cast<u32>(st->gathered)));
         APT_CUDA(cudaMemcpyAsync(st->h_carry, st->d_carry, carry_bytes, cudaMemcpyDeviceToHost, d.stream));
         APT_CUDA(cudaMemcpyAsync(st->h_rows, st->d_rows, (held + g.gather_cap) * kPxPerRow * sizeof(float), cudaMemcpyDeviceToHost,
@@ -341,10 +312,10 @@ int step(apt_stream *st, const void *src, bool on_device, int format, uint64_t n
 }
 
 // audio samples a push of n samples adds
-uint64_t audio_of(const apt_stream *st, uint64_t n) { return st->iq ? st->iqp.out_len(st->feed.in + n) - st->samples_in : n; }
+uint64_t audio_of(const apt_stream *st, uint64_t n) { return st->iq ? st->iqp.out_len(st->feed.in + n) - st->win.samples_in : n; }
 
 uint64_t rows_bound(const apt_stream *st, uint64_t n) {
-    const uint64_t nw = st->dec.plan.front.work_len(st->samples_in + audio_of(st, n));
+    const uint64_t nw = st->dec.plan.front.work_len(st->win.samples_in + audio_of(st, n));
     const uint64_t most = nw / st->g.row + 1;
     return most > st->rows_out ? (most - st->rows_out) * kPxPerRow : 0;
 }
@@ -448,7 +419,6 @@ int create(int device, uint32_t input_rate, int sync, uint64_t max_push, std::un
     }
     const Plan &p = st->dec.plan;
     st->sync = sync ? 1 : 0;
-    st->max_push = max_push;
     st->g = make_geom(p, st->sync, max_push);
     const Geom &g = st->g;
     apt_decoder &d = st->dec;
@@ -465,11 +435,7 @@ int create(int device, uint32_t input_rate, int sync, uint64_t max_push, std::un
     APT_CUDA(cudaStreamCreateWithFlags(&d.stream, cudaStreamNonBlocking));
     APT_TRY(upload_plan(&d));
     const uint64_t rows_floats = (g.gather_cap + 1) * kPxPerRow;
-    APT_CUDA(cudaMalloc(&st->d_in, g.cap_in * sizeof(float)));
-    APT_CUDA(cudaMalloc(&st->d_pcm, max_push * sizeof(int16_t)));
-    APT_CUDA(cudaMalloc(&st->d_conv, max_push * sizeof(float)));
-    APT_CUDA(cudaMalloc(&st->d_e, g.cap_e * sizeof(float)));
-    if (p.front.needs_scratch()) APT_CUDA(cudaMalloc(&st->d_r, g.cap_e * sizeof(float)));
+    APT_TRY(st->win.alloc(p.front, g.cap_in, g.cap_e, max_push));
     const size_t carry_bytes = sizeof(StreamCarry) + (st->sync ? 2 * kRunRing * sizeof(u32) : 0);
     APT_CUDA(cudaMalloc(&st->d_carry, carry_bytes));
     if (st->sync) {
@@ -508,14 +474,14 @@ extern "C" int apt_stream_push(apt_stream *st, const void *samples, int format, 
                     st->iq ? "APT_CU8, APT_CS16 or APT_CF32" : "APT_F32 or APT_PCM16");
     if (n == 0) return APT_OK;
     if (!samples) return fail(APT_ERR_BAD_ARG, "null samples");
-    if (st->dec.plan.front.work_len(st->samples_in + audio_of(st, n)) >= (1ull << 32))
+    if (st->dec.plan.front.work_len(st->win.samples_in + audio_of(st, n)) >= (1ull << 32))
         return fail(APT_ERR_BAD_ARG, "recording too long: the work-rate index would pass 2^32-1");
     const uint64_t need = rows_bound(st, n);
     if (need && (!rows || cap < need)) return fail(APT_ERR_CAPACITY, "rows needs room for %llu floats", (unsigned long long)need);
     APT_CUDA(cudaSetDevice(st->dec.device));
     uint64_t got = 0;
     const size_t sb = st->iq ? iq_sample_bytes(format) : format == APT_PCM16 ? 2 : 4;
-    const uint64_t per_step = st->iq ? st->iq_max_push : st->max_push;
+    const uint64_t per_step = st->iq ? st->iq_max_push : st->win.max_push;
     int status = APT_OK;
     for (uint64_t done = 0; done < n;) {
         const uint64_t k = std::min(per_step, n - done);
@@ -530,7 +496,7 @@ extern "C" int apt_stream_finish(apt_stream *st, float *rows, uint64_t cap, uint
     if (nout) *nout = 0;
     if (!st) return fail(APT_ERR_BAD_ARG, "null stream");
     if (st->finished) return fail(APT_ERR_BAD_ARG, "the stream is already finished");
-    if (st->samples_in == 0) return fail(APT_ERR_BAD_ARG, "empty signal");   // signal[0] panics in demodulate, dsp.rs:367
+    if (st->win.samples_in == 0) return fail(APT_ERR_BAD_ARG, "empty signal");   // signal[0] panics in demodulate, dsp.rs:367
     const uint64_t need = rows_bound(st, 0);
     if (need && (!rows || cap < need)) return fail(APT_ERR_CAPACITY, "rows needs room for %llu floats", (unsigned long long)need);
     APT_CUDA(cudaSetDevice(st->dec.device));
@@ -544,7 +510,7 @@ extern "C" int apt_stream_finish(apt_stream *st, float *rows, uint64_t cap, uint
 
 namespace {
 
-bool pushed(const apt_stream *st) { return st->samples_in || st->feed.in || st->finished; }
+bool pushed(const apt_stream *st) { return st->win.samples_in || st->feed.in || st->finished; }
 
 // The image of a finished pass from the rows kept on the device: the image stage, in PNG mode the encoder, then the pixels or
 // the file to the caller.  One stream synchronisation for pixels, two for a PNG file (its length is read first).
@@ -664,68 +630,30 @@ extern "C" int apt_stream_sync_positions(apt_stream *st, uint64_t *positions, si
 
 extern "C" int apt_stream_get_info(apt_stream *st, apt_stream_info *info) {
     if (!st || !info) return fail(APT_ERR_BAD_ARG, "null argument");
-    info->samples_in = st->iq ? st->feed.in : st->samples_in;
-    info->work_final = st->work_final;
+    info->samples_in = st->iq ? st->feed.in : st->win.samples_in;
+    info->work_final = st->win.work_final;
     info->rows_out = st->rows_out;
     info->peaks = st->positions.size();
     info->latency_work = st->g.latency;
-    info->max_push = st->iq ? st->iq_max_push : st->max_push;
+    info->max_push = st->iq ? st->iq_max_push : st->win.max_push;
     info->device_bytes = st->g.bytes + (st->img_rows ? stream_image_bytes(st->img.plan, st->img_max_rows) : 0);
     return APT_OK;
 }
 
-// ---- shared with the watcher (stream.hpp) ----
-
-int aptb200::window_compact(cudaStream_t s, float *buf, uint64_t &base, uint64_t keep, uint64_t end) {
-    keep = floor16(std::min(keep, end));
-    if (keep <= base) return APT_OK;
-    const uint64_t drop = keep - base, tail = end - keep;
-    if (tail > drop) return APT_OK;
-    if (tail) APT_CUDA(cudaMemcpyAsync(buf, buf + drop, tail * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    base = keep;
-    return APT_OK;
-}
-
-int aptb200::window_upload(const LaunchCtx &c, const void *src, bool on_device, int format, uint64_t n, int16_t *d_pcm,
-                           float *d_conv, float *dst) {
-    if (on_device) {
-        APT_CUDA(cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyDeviceToDevice, c.stream));
-    } else if (format == APT_PCM16) {
-        APT_CUDA(cudaMemcpyAsync(d_pcm, src, n * 2, cudaMemcpyHostToDevice, c.stream));
-        APT_TRY(launch_pcm16_to_f32(c, d_pcm, n, d_conv));
-        APT_CUDA(cudaMemcpyAsync(dst, d_conv, n * 4, cudaMemcpyDeviceToDevice, c.stream));
-    } else {
-        APT_CUDA(cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyHostToDevice, c.stream));
-    }
-    return APT_OK;
-}
-
-int aptb200::front_advance(const LaunchCtx &c, const Plan &p, const FrontTables &t, const float *in, uint64_t N, bool finish,
-                           uint64_t cap_e, float *d_r, float *d_e, uint64_t e_base, uint64_t &units_done, uint64_t &work_final) {
-    const uint64_t nw = p.front.work_len(N);
-    const uint64_t u_hi = p.front.complete(N, nw, finish);
-    if (u_hi <= units_done) return APT_OK;
-    const uint64_t work_hi = finish ? nw : std::min(nw, u_hi * p.front.unit_out);
-    if (work_hi - e_base > cap_e) return fail(APT_ERR_BAD_ARG, "internal: envelope window overflow");
-    APT_TRY(front_launch(c, p.front, t, in, APT_F32, nullptr, N, nw, units_done, u_hi, true, p.cosphi2, p.sinphi,
-                         d_r ? d_r - e_base : nullptr, d_e - e_base, nullptr));
-    units_done = u_hi;
-    work_final = work_hi;
-    return APT_OK;
-}
+// ---- used by the watcher (stream.hpp) ----
 
 int aptb200::stream_push_device(apt_stream *st, const float *d_src, uint64_t n, float *rows, uint64_t cap, uint64_t *nout) {
     *nout = 0;
     if (st->iq || st->finished) return fail(APT_ERR_BAD_ARG, "internal: device push into an I/Q or finished stream");
     if (n == 0) return APT_OK;
-    if (st->dec.plan.front.work_len(st->samples_in + n) >= (1ull << 32))
+    if (st->dec.plan.front.work_len(st->win.samples_in + n) >= (1ull << 32))
         return fail(APT_ERR_BAD_ARG, "recording too long: the work-rate index would pass 2^32-1");
     const uint64_t need = rows_bound(st, n);
     if (need && (!rows || cap < need)) return fail(APT_ERR_CAPACITY, "rows needs room for %llu floats", (unsigned long long)need);
     uint64_t got = 0;
     int status = APT_OK;
     for (uint64_t done = 0; done < n;) {
-        const uint64_t k = std::min(st->max_push, n - done);
+        const uint64_t k = std::min(st->win.max_push, n - done);
         APT_TRY(step(st, d_src + done, true, APT_F32, k, false, rows, got, status));
         done += k;
     }

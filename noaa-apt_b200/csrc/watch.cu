@@ -1,8 +1,8 @@
 // Watching a continuous audio feed for satellite passes (include/aptb200.h apt_watch_*, DESIGN.md §13).
 //
 // Every step (one slice of at most max_push samples) runs on one CUDA stream, the pass stream's:
-//   upload into the f32 input window -> first stage over the units whose input is complete (stream.hpp, the code the
-//   streaming decoder runs) -> k_pass_quality over the windows whose two rows are final -> the new q back to the host ->
+//   upload into the f32 input window -> first stage over the units whose input is complete (FrontWindow, front.hpp, as
+//   in the streaming decoder) -> k_pass_quality over the windows whose two rows are final -> the new q back to the host ->
 //   the pass rule (PassTracker) -> the open group fed device to device from the input window to the pass stream, an
 //   apt_stream with the caller's image / PNG output, which is finished at the group's LOS and reset.
 // The input window keeps what the pass stream or a later window can still read; the envelope window keeps the rows of the
@@ -76,7 +76,7 @@ int make_watch_plan(uint32_t input_rate, const apt_settings *s, const apt_watch_
     // most max_gap + 2 windows behind the next window; either way less than the first stage's unit span behind the last
     // sample.  Compaction moves the tail only when that does not overlap, so the window holds twice that, plus one step.
     const uint64_t t_in = (w.rule.max_gap + 4) * (rate / 2 + 1) + 2 * (f.tail() + f.unit_in) + 64;
-    const uint64_t w_new = (w.max_push + f.tail()) * f.r.l / f.r.m + 2 * f.unit_out + 64;
+    const uint64_t w_new = FrontWindow::step_outputs(f, w.max_push);
     // envelope: the two rows of the next window (k_pass_quality reads nothing else) and the units of one step
     const uint64_t t_e = 2 * R + f.unit_out + 64;
     w.cap_in = 2 * t_in + w.max_push + 64;
@@ -89,8 +89,7 @@ int make_watch_plan(uint32_t input_rate, const apt_settings *s, const apt_watch_
     w.extra_rows = (w_new + f.tail() * f.r.l / f.r.m + f.unit_out + w.p.guard.size() + 2 * w.p.dist + si.latency_work) / R + 8;
     w.rows_cap = (w.max_rows + w.extra_rows) * kPxPerRow;
     w.latency = (f.tail() * f.r.l / f.r.m + f.unit_out + R - 1) / R + 2;
-    w.own_bytes = FrontTables::bytes(f) + w.cap_in * 4 + w.max_push * (2 + 4) + w.cap_e * 4 * (f.needs_scratch() ? 2 : 1) +
-                  w.q_cap * 4;
+    w.own_bytes = FrontTables::bytes(f) + FrontWindow::bytes(f, w.cap_in, w.cap_e, w.max_push) + w.q_cap * 4;
     w.stream_bytes = si.device_bytes + (w.out.image ? stream_image_bytes(w.out, w.max_rows) : 0);
     return APT_OK;
 }
@@ -105,14 +104,13 @@ struct apt_watch {
     apt_stream *pass = nullptr;        // the pass stream; its CUDA stream carries every step
     cudaStream_t cs = nullptr;
     FrontTables front;
-    float *d_in = nullptr, *d_conv = nullptr, *d_e = nullptr, *d_r = nullptr, *d_q = nullptr;
-    int16_t *d_pcm = nullptr;
+    FrontWindow win;                   // the segment's input and envelope windows and first-stage progress
+    float *d_q = nullptr;
     float *h_q = nullptr, *h_rows = nullptr;   // pinned
     std::vector<uint8_t> h_out;                // the image or PNG file of the last pass
     uint64_t T = 1ull << 31;
     // the feed
-    uint64_t abs_in = 0, seg_start = 0;
-    uint64_t samples_in = 0, in_base = 0, units_done = 0, work_final = 0, e_base = 0;   // of the segment
+    uint64_t seg_start = 0;            // the segment's first sample; the feed holds seg_start + win.samples_in
     PassTracker tracker{PassRule{}, 1};
     bool active = false;               // the pass stream holds the open group's samples [start_of(first), fed)
     bool lost = false;                 // the pass stream's rows outgrew the row buffer: this pass fails, the feed goes on
@@ -126,8 +124,8 @@ namespace {
 void free_watch(apt_watch *w) {
     cudaSetDevice(w->device);
     if (w->cs) cudaStreamSynchronize(w->cs);
-    for (void *p : {(void *)w->d_in, (void *)w->d_conv, (void *)w->d_e, (void *)w->d_r, (void *)w->d_q, (void *)w->d_pcm})
-        if (p) cudaFree(p);
+    w->win.release();
+    if (w->d_q) cudaFree(w->d_q);
     for (void *p : {(void *)w->h_q, (void *)w->h_rows})
         if (p) cudaFreeHost(p);
     w->front.release();
@@ -136,7 +134,7 @@ void free_watch(apt_watch *w) {
 }
 
 void clear_segment(apt_watch *w) {
-    w->samples_in = w->in_base = w->units_done = w->work_final = w->e_base = 0;
+    w->win.clear();
     w->tracker = PassTracker(w->wp.rule, w->wp.p.input_rate);
     w->active = false;
     w->fed = 0;
@@ -159,15 +157,15 @@ float *rows_at(apt_watch *w, uint64_t &cap) {
 
 // Feeds the pass stream the input samples [fed, to) of the segment, one max_push slice at a time.
 int feed_to(apt_watch *w, uint64_t to) {
-    if (to > w->samples_in) return fail(APT_ERR_BAD_ARG, "internal: the pass reaches past the samples pushed");
+    if (to > w->win.samples_in) return fail(APT_ERR_BAD_ARG, "internal: the pass reaches past the samples pushed");
     while (w->fed < to) {
-        if (w->fed < w->in_base) return fail(APT_ERR_BAD_ARG, "internal: the pass's samples left the input window");
+        if (w->fed < w->win.in_base) return fail(APT_ERR_BAD_ARG, "internal: the pass's samples left the input window");
         const uint64_t k = std::min(w->wp.max_push, to - w->fed);
         uint64_t cap = 0, nout = 0, need = 0;
         float *rows = rows_at(w, cap);
         APT_TRY(apt_stream_push_bound(w->pass, k, &need));
         w->lost = w->lost || need > cap;
-        if (!w->lost) APT_TRY(stream_push_device(w->pass, w->d_in + (w->fed - w->in_base), k, rows, cap, &nout));
+        if (!w->lost) APT_TRY(stream_push_device(w->pass, w->win.in_origin() + w->fed, k, rows, cap, &nout));
         w->fed += k;
     }
     return APT_OK;
@@ -234,24 +232,10 @@ int on_event(apt_watch *w, const apt_pass_event &ev) {
 // The start of a step, before its new samples land in the input window: the windows keep only what the first stage, the
 // next window and the pass stream can still read.
 int prepare(apt_watch *w) {
-    const Plan &p = w->wp.p;
-    const uint64_t R = p.row;
-    uint64_t xa, xb;
-    p.front.span(w->units_done, w->units_done + 1, ~0ull, xa, xb);
     // a group that opens in this step starts at or after the next window's first sample, even when the last group's LOS
     // left the pass stream's position past it
-    const uint64_t keep = std::min<uint64_t>({xa, w->tracker.start_of(w->tracker.next()), w->active ? w->fed : ~0ull});
-    APT_TRY(window_compact(w->cs, w->d_in, w->in_base, keep, w->samples_in));
-    const uint64_t e_next = w->tracker.next() * R;
-    const uint64_t ekeep = e_next;
-    uint64_t eb = w->e_base;
-    APT_TRY(window_compact(w->cs, w->d_e, eb, ekeep, w->work_final));
-    if (w->d_r && eb != w->e_base) {
-        uint64_t rb = w->e_base;
-        APT_TRY(window_compact(w->cs, w->d_r, rb, ekeep, w->work_final));
-    }
-    w->e_base = eb;
-    return APT_OK;
+    const uint64_t keep_in = std::min<uint64_t>(w->tracker.start_of(w->tracker.next()), w->active ? w->fed : ~0ull);
+    return w->win.compact(w->cs, w->wp.p.front, keep_in, w->tracker.next() * w->wp.p.row);
 }
 
 // The rest of a step, once its new samples are in the input window and counted in samples_in: the first stage, q of the
@@ -261,15 +245,13 @@ int advance(apt_watch *w, bool finish, float *q, uint64_t &nq) {
     const Plan &p = wp.p;
     const LaunchCtx c{w->cs, w->sm_count};
     const uint64_t R = p.row;
-    if (w->samples_in)
-        APT_TRY(front_advance(c, p, w->front, w->d_in - w->in_base, w->samples_in, finish, wp.cap_e, w->d_r, w->d_e, w->e_base,
-                              w->units_done, w->work_final));
+    if (w->win.samples_in) APT_TRY(w->win.advance(c, p, w->front, finish));
     const uint64_t w0 = w->tracker.next();
-    const uint64_t w1 = w->work_final / R >= 1 ? w->work_final / R - 1 : 0;
+    const uint64_t w1 = w->win.work_final / R >= 1 ? w->win.work_final / R - 1 : 0;
     const uint64_t k = w1 > w0 ? w1 - w0 : 0;
     if (k) {
         if (k > wp.q_cap) return fail(APT_ERR_BAD_ARG, "internal: quality buffer overflow");
-        APT_TRY(launch_pass_quality(w->cs, w->d_e - w->e_base, w0, k, static_cast<uint32_t>(R), w->d_q - w0));
+        APT_TRY(launch_pass_quality(w->cs, w->win.e_origin(), w0, k, static_cast<uint32_t>(R), w->d_q - w0));
         APT_CUDA(cudaMemcpyAsync(w->h_q, w->d_q, k * sizeof(float), cudaMemcpyDeviceToHost, w->cs));
         APT_CUDA(cudaStreamSynchronize(w->cs));
         memcpy(q + nq, w->h_q, k * sizeof(float));
@@ -291,7 +273,7 @@ int advance(apt_watch *w, bool finish, float *q, uint64_t &nq) {
     }
     if (finish) {
         nev = 0;
-        w->tracker.finish(w->samples_in, collect);
+        w->tracker.finish(w->win.samples_in, collect);
         for (int j = 0; j < nev; ++j) APT_TRY(on_event(w, evs[j]));
         if (w->active) {
             w->active = false;
@@ -306,25 +288,19 @@ int advance(apt_watch *w, bool finish, float *q, uint64_t &nq) {
 // One step: n new samples (maybe none) from the host and, when `finish`, the end of the segment.  q receives the new windows.
 int step(apt_watch *w, const void *src, int format, uint64_t n, bool finish, float *q, uint64_t &nq) {
     APT_TRY(prepare(w));
-    if (n) {
-        const uint64_t off = w->samples_in - w->in_base;
-        if (off + n > w->wp.cap_in) return fail(APT_ERR_BAD_ARG, "internal: input window overflow");
-        APT_TRY(window_upload(LaunchCtx{w->cs, w->sm_count}, src, false, format, n, w->d_pcm, w->d_conv, w->d_in + off));
-        w->samples_in += n;
-        w->abs_in += n;
-    }
+    if (n) APT_TRY(w->win.push(LaunchCtx{w->cs, w->sm_count}, src, false, format, n));
     return advance(w, finish, q, nq);
 }
 
 // A segment that is long enough ends before the next step: finished as at apt_watch_finish, then a new one starts.
 int maybe_roll(apt_watch *w, float *q, uint64_t &nq) {
-    const uint64_t nw = w->wp.p.front.work_len(w->samples_in);
+    const uint64_t nw = w->wp.p.front.work_len(w->win.samples_in);
     // an open group is closed before the step that could take the segment past 2T (T <= 2^31, so work indices stay below
     // 2^32 in the first stage and in the pass stream)
     if (nw < w->T || (w->tracker.open() && nw + w->wp.step_work < 2 * w->T)) return APT_OK;
     APT_TRY(step(w, nullptr, APT_F32, 0, true, q, nq));
-    const uint64_t seg_windows = w->wp.p.front.work_len(w->samples_in) / w->wp.p.row;
-    w->seg_start += w->samples_in;
+    const uint64_t seg_windows = w->wp.p.front.work_len(w->win.samples_in) / w->wp.p.row;
+    w->seg_start += w->win.samples_in;
     clear_segment(w);
     apt_watch_event e{};
     e.ev.kind = APT_PASS_SEGMENT;
@@ -337,18 +313,18 @@ int maybe_roll(apt_watch *w, float *q, uint64_t &nq) {
 
 uint64_t q_bound(const apt_watch *w, uint64_t n) {
     const Plan &p = w->wp.p;
-    const uint64_t most = p.front.work_len(w->samples_in + n) / p.row + 1;
+    const uint64_t most = p.front.work_len(w->win.samples_in + n) / p.row + 1;
     const uint64_t next = w->tracker.next();
     return (most > next ? most - next : 0) + p.front.work_len(n) / p.row + 2;   // a new segment may start inside the push
 }
 
 int reset_feed(apt_watch *w) {
-    w->abs_in = w->seg_start = 0;
+    w->seg_start = 0;
     w->passes = 0;
     w->finished = false;
     clear_segment(w);
     APT_TRY(apt_stream_reset(w->pass));
-    APT_CUDA(cudaMemsetAsync(w->d_in, 0, w->wp.cap_in * sizeof(float), w->cs));
+    APT_TRY(w->win.zero_input(w->cs));
     APT_CUDA(cudaStreamSynchronize(w->cs));
     return APT_OK;
 }
@@ -397,11 +373,7 @@ extern "C" int apt_watch_create(int device, uint32_t input_rate, const apt_setti
     if (wp.out.png) APT_TRY(apt_stream_set_png_mode(w->pass, &wp.out.png_s));
     w->cs = stream_cuda(w->pass);
     APT_TRY(w->front.upload(wp.p.front));
-    APT_CUDA(cudaMalloc(&w->d_in, wp.cap_in * sizeof(float)));
-    APT_CUDA(cudaMalloc(&w->d_pcm, wp.max_push * sizeof(int16_t)));
-    APT_CUDA(cudaMalloc(&w->d_conv, wp.max_push * sizeof(float)));
-    APT_CUDA(cudaMalloc(&w->d_e, wp.cap_e * sizeof(float)));
-    if (wp.p.front.needs_scratch()) APT_CUDA(cudaMalloc(&w->d_r, wp.cap_e * sizeof(float)));
+    APT_TRY(w->win.alloc(wp.p.front, wp.cap_in, wp.cap_e, wp.max_push));
     APT_CUDA(cudaMalloc(&w->d_q, wp.q_cap * sizeof(float)));
     APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&w->h_q), wp.q_cap * sizeof(float), cudaHostAllocDefault));
     APT_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&w->h_rows), wp.rows_cap * sizeof(float), cudaHostAllocDefault));
@@ -488,7 +460,7 @@ extern "C" int apt_watch_get_info(apt_watch *w, apt_watch_info *info) {
     apt_stream_info si{};
     APT_TRY(apt_stream_get_info(w->pass, &si));
     *info = apt_watch_info{};
-    info->samples_in = w->abs_in;
+    info->samples_in = w->seg_start + w->win.samples_in;
     info->segment_start = w->seg_start;
     info->windows = w->tracker.next();
     info->passes = w->passes;
@@ -602,10 +574,10 @@ int iq_step(apt_watch_iq *w, const void *src, int format, uint64_t n, float *q, 
     float *outs[APT_WATCH_IQ_MAX_CHANNELS];
     for (int c = 0; c < C; ++c) {
         apt_watch *a = w->ch[c];
-        if (a->samples_in - a->in_base + added > a->wp.cap_in) return fail(APT_ERR_BAD_ARG, "internal: input window overflow");
+        APT_TRY(a->win.room(added));
         pl[c] = &w->wp.q[c];
         tb[c] = &w->t[c];
-        outs[c] = a->d_in - a->in_base - a->seg_start;   // audio indices are absolute in the kernel, of the segment here
+        outs[c] = a->win.in_origin() - a->seg_start;   // audio indices are absolute in the kernel, of the segment here
     }
     APT_TRY(iq_launch_channels(lc, pl, tb, C, w->feed.origin(), w->feed.base, w->feed.in, APT_CF32, w->m_done, m1, outs));
     APT_CUDA(cudaEventRecord(w->audio, w->cs));
@@ -613,8 +585,7 @@ int iq_step(apt_watch_iq *w, const void *src, int format, uint64_t n, float *q, 
     for (int c = 0; c < C; ++c) {
         apt_watch *a = w->ch[c];
         APT_CUDA(cudaStreamWaitEvent(a->cs, w->audio, 0));
-        a->samples_in += added;
-        a->abs_in += added;
+        a->win.commit(added);
         APT_TRY(advance(a, false, q + c * cap, got[c]));
     }
     return APT_OK;

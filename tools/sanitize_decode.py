@@ -65,3 +65,43 @@ same = sts == [0, 0, 0] and all(
     files[i] == image.decode_png(None, na.Settings(), x, 11025, contrast=image.MINMAX, rgba=True, block_bytes=4096)[0]
     for i, x in enumerate(xs))
 print("batch png", [len(f or b"") for f in files], "bytes", "equal" if same else "MISMATCH", flush=True)
+
+# The streamed first stage (FrontWindow, front.hpp) with the decimate kind, the only one with the scratch window d_r beside
+# the envelope window: a 24 960 Hz stream and an audio watcher, each pushed in uneven pieces so that every window compacts,
+# against apt_decode of the whole recording and the recording path (apt_recording_quality / _find_passes / _decode).
+x = synth.apt_signal(24960, 14, seed=5)
+pieces = [7001, 13, 30011, 1, 24960]
+with na.Stream(24960, max_push=20000) as st:
+    rows, at, i = [], 0, 0
+    while at < x.size:
+        rows.append(st.push(x[at:at + pieces[i % len(pieces)]]))
+        at += pieces[i % len(pieces)]
+        i += 1
+    rows.append(st.finish())
+got = np.concatenate(rows).ravel()
+want = na.decode(None, na.Settings(), x, 24960, True)
+print("stream 24960", got.size // 2080, "rows", "equal" if np.array_equal(got.view(np.uint32), want.view(np.uint32))
+      else "MISMATCH", flush=True)
+
+search = dict(max_gap_s=5.0, min_length_s=20.0)
+x = synth.apt_passes(24960, [("noise", 6), ("pass", 40, 5), ("noise", 12)], seed=6)
+with na.Watch(24960, search=search, max_push=12480) as w:
+    qs, evs, at, i = [], [], 0, 0
+    while at < x.size:
+        q, e = w.push(x[at:at + pieces[i % len(pieces)]])
+        qs.append(q)
+        evs += e
+        at += pieces[i % len(pieces)]
+        i += 1
+    q, e = w.finish()
+    qs.append(q)
+    evs += e
+with na.Recording(x, 24960) as rec:
+    q_ref = rec.quality()
+    found = na.find_passes_quality(q_ref, x.size, 24960, **search)
+    data, sts = rec.decode(found, True)
+los = [e for e in evs if e.kind == "los"]
+same = np.array_equal(np.concatenate(qs).view(np.uint32), q_ref.view(np.uint32)) and [e.pass_ for e in los] == found and \
+    all(e.status == s and (s != 0 or np.array_equal(e.data.view(np.uint32), d.view(np.uint32)))
+        for e, s, d in zip(los, sts, data))
+print("watch 24960", len(found), "passes", "equal" if same and found else "MISMATCH", flush=True)
